@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the B200-native Unicorn per-frame hot path (contract: see the task statement / DESIGN.md §Measurement).
+"""Benchmark of the H100-native Unicorn per-frame hot path (DESIGN.md §Measurement).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--size H W]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--size H W] [--dump-outputs DIR]
 
 A step = one steady-state SOT frame (BASELINE.json configs[1]: unicorn_track_large, 800x1280): backbone+neck ->
 deformable interaction -> 2x embedding upsample -> fused correlation/propagation -> head -> NMS, on synthetic video
@@ -9,6 +9,8 @@ with seeded random weights.  `value` = frames/s with frames resident in HBM (CUD
 `e2e` = frames/s through UnicornSOTTrack.track_tensor with pinned HOST frames (H2D + D2H inside the timed region).
 `--impl reference` times the reference algorithm's CPU restatement (oracle/, validated against the real reference)
 on the host cores for the same workload.
+`--dump-outputs DIR` writes what the timed (pipelined) path computed for its last step as DIR/<name>.npy: the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -33,7 +35,8 @@ def peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sus=p.get("bf16_tflops_sustained", p["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- upper bounds, not measured rates
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -103,17 +106,25 @@ def run_reference(args):
     cores = host_threads()
     torch.set_num_threads(cores)
     H, W = args.size
-    steps, warm = min(args.steps, 6), min(args.warmup, 1)
+    steps, warm = args.steps, args.warmup
     sd = make_state_dict(args.config, 0)
-    frames, boxes = make_video(steps + warm + 1, H, W, seed=0)
+    n_frames = min(steps + warm, 16)  # the frames of the sequence are reused cyclically past 16, like the GPU arm
+    frames, boxes = make_video(n_frames + 1, H, W, seed=0)
     o = orc.SOTOracle(sd, args.config)
     o.initialize(frames[0:1], boxes[0, 0])
+    frame = lambda i: frames[1 + i % n_frames:2 + i % n_frames]  # noqa: E731
     for i in range(warm):
-        o.track(frames[1 + i:2 + i])
+        o.track(frame(i))
     t0 = time.perf_counter()
     for i in range(steps):
-        o.track(frames[1 + warm + i:2 + warm + i])
+        st = {}
+        dets = o.track(frame(warm + i), st)
     dt = time.perf_counter() - t0
+    if args.dump_outputs and steps > 0:
+        n = 0 if dets is None else int(dets.shape[0])
+        save_arrays(args.dump_outputs, {"dets": (dets[:min(n, 3)] if n else torch.zeros(0, 7)).float(),
+                                        "count": torch.tensor([n], dtype=torch.float64), "head": st["head"].float(),
+                                        "priors": st["coarse"].float()})
     fps = steps / dt
     print(json.dumps({
         "impl": "reference", "metric": "frames/sec", "value": fps, "unit": "frames/s", "n_gpus": args.gpus, "steps": steps,
@@ -290,15 +301,24 @@ def extra_workloads(dev, rank, world, K, sync_all, save_tuning=None):
     return out
 
 
-def roofline_inputs():
-    """Per-launch DRAM traffic of the kernels quoted below, from the committed ncu captures of the CURRENT kernels
-    (profiles/r2_roofline_inputs.json, written by tools/make_roofline_inputs.py from profiles/r2_ncu_*.csv)."""
-    path = os.path.join(ROOT, "profiles", "r2_roofline_inputs.json")
-    return json.load(open(path)) if os.path.exists(path) else {"kernels": {}}
-
-
 def pk_burst():
     return peaks()["tf_burst"]
+
+
+def dump_outputs(d, c, max_inst):
+    """What the caller of the timed path receives for the frame (the detections and their count, UnicornSOTTrack.collect), plus
+    the head output and the propagated label map they are computed from, as float32 / float64 .npy files (< 1 MB at 800x1280)."""
+    torch.cuda.synchronize()
+    n = int(c.ws.count.item())
+    save_arrays(d, {"dets": c.ws.dets[:min(n, max_inst)].float(), "count": torch.tensor([n], dtype=torch.float64),
+                    "head": c.last["head"].float(), "priors": c.last["priors"][0].float()})
+
+
+def save_arrays(d, arrays):
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), t.detach().cpu().numpy())
 
 
 def main():
@@ -313,6 +333,7 @@ def main():
     ap.add_argument("--depth", type=int, default=3, help="frames in flight of the headline measurement (>= 2; the sequential numbers are always reported too)")
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[2] (MOT 1536x2048) and configs[3] (VOS mask) workloads")
     ap.add_argument("--save-tuning", default=None, help="directory: write every engine's per-layer N-tile table (with UC_NO_TUNED=1: fresh autotuning)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.size is None:
         args.size = (320, 320) if "tiny" in args.config else (800, 1280)
@@ -398,6 +419,8 @@ def main():
         return pipe, e0.elapsed_time(e1) / 1e3
     D = max(2, args.depth)
     pipe, dt_dev_pipe = measure_pipe(D)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pipe._ctxs[(K - 1) % D], pipe.max_inst)
     dt_dev_pipe3 = measure_pipe(D + 1)[1]
     # ---------------- end to end through the public API with pinned host frames, driven by the product's multi-GPU module:
     # one sequence per rank (parallel.shard_sequences), start barrier, wall clock of the slowest rank, one all_gather of the
@@ -444,10 +467,9 @@ def main():
         torch.cuda.synchronize()
         ts.append(a.elapsed_time(b) / 1e3)
     t_corr = sorted(ts)[len(ts) // 2]
-    # ---------------- dominant kernel: conv_gemm on the two stage-3 pointwise GEMM shapes (54 of the 172 conv launches of
-    # a frame, 37 % of its device time), timed the way the frame runs them: kernel nodes of a CUDA graph, CUDA events.
+    # ---------------- dominant kernel: conv_gemm on the two stage-3 pointwise GEMM shapes (the 27 blocks of ConvNeXt-L stage 3
+    # run them 54 times a frame), timed the way the frame runs them: kernel nodes of a CUDA graph, CUDA events.
     conv_roof = dw_roof = mlp_roof = None
-    RI = roofline_inputs()
     if "large" in args.config and (H, W) == (800, 1280):
         xs = torch.randn(1, 50, 80, 768, device=dev).bfloat16()
         w1 = ops.pack_conv_weight(torch.randn(3072, 768, 1, 1, device=dev) / 768 ** 0.5)
@@ -477,12 +499,9 @@ def main():
         fl = 2 * 2.0 * 4000 * 768 * 3072
         conv_roof = {"bound": "tensor", "achieved": fl / t_pair / 1e12, "peak": pk_burst(), "unit": "TFLOP/s",
                      "frac": fl / t_pair / 1e12 / pk_burst(), "us_per_launch": t_pair * 1e6 / 2,
-                     "traffic": RI["kernels"].get("r2_ncu_conv_s3pw2", {}).get("dram_bytes"),
-                     "traffic_note": "dram__bytes_read + write of the pwconv2 launch (conv_gemm_kernel<192,7,2>), ncu --set full, cold L2: A 24.6 + W 4.7 + residual "
-                                     "6.1 MB = the algorithmic bytes; profiles/r2_ncu_conv_gn.csv (pwconv1: r2_ncu_conv_s3pw1, 10.9 MB = A 6.1 + W 4.7)",
                      "kernel": "uc::conv_gemm_kernel, ConvNeXt-L stage-3 pwconv1 (768->3072, GELU) + pwconv2 (3072->768, layer-scale + residual), "
                                "M = 4000 pixels, CUDA-graph nodes",
-                     "peak_source": "measured bf16_tflops (burst)"}
+                     "peak_source": peaks()["src"] + " bf16"}
 
         # ---- the two other hand-written hot kernels of a ConvNeXt block on its stage-1 shape: the tensor-core depthwise 7x7 and the fused
         # LayerNorm + MLP (CUDA-graph nodes, 10 launches per replay; the 49 MB working set stays L2 resident like inside the frame)
@@ -508,26 +527,22 @@ def main():
         t_dw = graph_time(lambda: ops.dwconv7_mma(x1, qt, out=y1))
         dw_bytes = 4.0 * M1 * C1  # read + write the bf16 map once
         dw_roof = {"bound": "hbm", "achieved": dw_bytes / t_dw / 1e9, "peak": peaks()["hbm"], "unit": "GB/s", "frac": dw_bytes / t_dw / 1e9 / peaks()["hbm"],
-                   "us_per_launch": t_dw * 1e6, "traffic": RI["kernels"].get("r2_ncu_dwmma_s1", {}).get("dram_bytes"),
+                   "us_per_launch": t_dw * 1e6,
                    "kernel": "uc::dwconv7_mma_kernel<4> (depthwise 7x7 as Toeplitz blocks on mma.sync), ConvNeXt-L stage 1: 200x320x192, static item schedule",
-                   "note": "algorithmic bytes (49 MB: the map read and written once) over the launch time; the kernel is bound by shared-memory wavefronts "
-                           "(ldmatrix), not by HBM — DESIGN.md 4.3", "peak_source": "measured hbm_gbs"}
+                   "note": "algorithmic bytes (49 MB: the map read and written once) over the launch time", "peak_source": peaks()["src"] + " hbm"}
         w1f = ops.pack_conv_weight(torch.randn(4 * C1, C1, 1, 1, device=dev) / C1 ** 0.5)
         w2s = ops.pack_conv_weight(torch.randn(C1, 4 * C1, 1, 1, device=dev) / (4 * C1) ** 0.5)
         c1v, b2v, gmv = torch.randn(4 * C1, device=dev), torch.randn(C1, device=dev), torch.randn(C1, device=dev) * 0.1
         t_mlp = graph_time(lambda: ops.convnext_mlp(y1.view(-1, C1), w1f, c1v, w2s, b2v, gmv, x1.view(-1, C1)))
         fl_mlp = 2 * 2.0 * M1 * C1 * 4 * C1
         mlp_roof = {"bound": "tensor", "achieved": fl_mlp / t_mlp / 1e12, "peak": pk_burst(), "unit": "TFLOP/s", "frac": fl_mlp / t_mlp / 1e12 / pk_burst(),
-                    "us_per_launch": t_mlp * 1e6, "traffic": RI["kernels"].get("r2_ncu_mlp_s1", {}).get("dram_bytes"),
+                    "us_per_launch": t_mlp * 1e6,
                     "kernel": "uc::convnext_mlp_kernel<192> (LayerNorm + pwconv1 + GELU + pwconv2 + layer scale + residual), ConvNeXt-L stage 1: M = 64000 pixels",
-                    "note": "the GELU of the 64000 x 768 hidden activations (2 MUFU operations per element, 16 per clock and SM) bounds this kernel at "
-                            "~26 us, not the tensor pipe; the separate kernels it replaces take 120 us (profiles/r2_mlp_fused_microbench.txt)",
-                    "peak_source": "measured bf16_tflops (burst)"}
+                    "peak_source": peaks()["src"] + " bf16"}
 
-    extra = {} if args.no_extra else extra_workloads(dev, rank, world, max(8, min(K, 24)), sync_all, args.save_tuning if rank == 0 else None)
+    extra = {} if args.no_extra else extra_workloads(dev, rank, world, K, sync_all, args.save_tuning if rank == 0 else None)
     if args.save_tuning and rank == 0:
         eng.save_tuning(os.path.join(args.save_tuning, f"{args.config}.json"))
-    RI_frame = RI.get("frame", {})
     if world > 1:
         t = torch.tensor([dt_dev, dt_e2e, dt_dev_pipe, dt_e2e_pipe, dt_dev_pipe3] + [v for k in sorted(extra) for v in (extra[k]["_dt_dev"], extra[k]["_dt_e2e"])], device=dev, dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -550,18 +565,17 @@ def main():
         "dtype": "bf16", "data": "synthetic",
         "config": {"workload": f"{args.config} SOT steady-state frame {H}x{W}, 1 object (BASELINE configs[1])",
                    "parallelism": f"dp{world} (one sequence per GPU, no data-path collective)",
-                   "l2": "per-frame working set (0.52 GB bf16 weights + activations) exceeds the 126 MB L2; a different frame every step",
+                   "l2": "per-frame working set (0.52 GB bf16 weights + activations) exceeds the 50 MB L2; a different frame every step",
                    "weights": "seeded random init (unicorn_b200.weights.make_state_dict)", "cuda_graph": True,
                    "frames_in_flight": D, "frames_in_flight_note": "independent frames of one sequence on separate streams / engine contexts; "
                                                                 "ms_per_step = timed region / steps; per-frame latency is the `sequential` entry's",
                    "input": "uint8 HWC BGR frames (3.07 MB H2D per frame); float conversion fused into the stem kernel"},
         "roofline": {"bound": "tensor", "achieved": ach, "peak": pk["tf_sus"], "unit": "TFLOP/s", "frac": ach / pk["tf_sus"],
-                     "traffic": RI_frame.get("dram_bytes"), "traffic_note": RI_frame.get("note"),
                      "kernel": "whole-frame CUDA graph (1997 GFLOP algorithmic per 800x1280 frame, SURVEY §8d)",
                      "peak_source": pk["src"] + " bf16_tflops_sustained"},
         "roofline_conv": conv_roof,
         "roofline_dwconv": dw_roof, "roofline_mlp": mlp_roof,
-        "roofline_corr": {"bound": "tensor", "traffic": RI["kernels"].get("r2_ncu_corr", {}).get("dram_bytes"),
+        "roofline_corr": {"bound": "tensor",
                           "hbm_note": "the fused kernel moves only its algorithmic 8.26 MB (the 16000^2 similarity matrix never leaves the SM), so it is bound "
                                       "by the tensor / MUFU / issue pipes, not by HBM: hbm_frac is reported because BASELINE.json's metric asks for it, it is not a "
                                       "utilisation target", "achieved": CORR_GFLOP(n_pos) / t_corr / 1e3, "peak": pk["tf_burst"], "unit": "TFLOP/s",

@@ -1,10 +1,10 @@
-/* unicorn_b200 — C ABI of the B200-native Unicorn per-frame inference hot path.
+/* unicorn_b200 — C ABI of the H100-native Unicorn per-frame inference hot path.
  *
  * Every entry point takes plain device pointers, sizes and a CUDA stream (passed as void* so the header
  * needs no CUDA include).  No entry point allocates, synchronises or keeps state between calls (apart from
  * a lazily resolved driver entry point), so all of them are CUDA-graph capturable.  All return 0 on success
  * and a negative UC_E* / positive cudaError_t code otherwise; uc_last_error() gives the text.
- * There is NO CPU fallback: on a machine without an sm_100 device every launch returns an error.
+ * There is NO CPU fallback: on a machine without an sm_90 device every launch returns an error.
  *
  * Reference interfaces replaced (paths relative to MasterBin-IIAU/Unicorn):
  *   uc_msda_forward_*      unicorn/models/ops/src/ms_deform_attn.h:20-39  (ms_deform_attn_forward)
@@ -38,7 +38,7 @@ extern "C" {
 #define UC_OK 0
 #define UC_EINVAL (-1)   /* bad argument (shape / alignment / dtype) */
 #define UC_EDRIVER (-2)  /* driver entry point (cuTensorMapEncodeTiled) unavailable */
-#define UC_ENODEV (-3)   /* no sm_100 device */
+#define UC_ENODEV (-3)   /* no sm_90 device */
 
 /* dtypes of activation tensors */
 #define UC_BF16 0
@@ -54,10 +54,10 @@ extern "C" {
 
 UC_API const char* uc_last_error(void);
 UC_API int uc_version(void);
-/* 0 if the current device is sm_100 and the driver entry points resolve, else a UC_E* code */
+/* 0 if the current device is sm_90 and the driver entry points resolve, else a UC_E* code */
 UC_API int uc_check_device(void);
 
-/* Dense convolution / linear layer as an implicit GEMM on tcgen05 tensor cores (TMA-fed, TMEM accumulators).
+/* Dense convolution / linear layer as an implicit GEMM on wgmma tensor cores (TMA-fed, register accumulators).
  *   x : NHWC activations, 16-bit (bf16 or f16 per x_dtype), pixel stride ldx elements (ldx >= Cin, ldx % 8 == 0)
  *   w : packed weights [Cout][KH*KW][Cin] in the same 16-bit type as x (K-major)
  *   y : NHWC output, pixel stride ldy, dtype y_dtype; y = act(conv(x) + bias) ; then y = res + gamma * y if given
@@ -80,8 +80,8 @@ typedef struct UcConv2d {
   void* y;
   int ldy;
   int y_dtype;
-  int block_n; /* 0 = auto; else force the N tile (16,32,64,96,128,192,256); +1000 (1128,1192,1256) = the
-                  cta_group::2 variant: an SM pair computes a 256 x N tile with one pair-MMA stream */
+  int block_n; /* 0 = auto; else force the N tile (16,32,64,96,128,192,256); +1000 (1128,1192,1256) = the 2-CTA
+                  cluster variant: two CTAs with consecutive M tiles share one weight stream (TMA multicast) */
   /* Optional GroupNorm statistics of the (pre-activation) output, accumulated per (image, group):
    * gn_stats[b][g] = {sum, sumsq} as int64 fixed point (value * 2^22; integer atomics => order independent,
    * bit-reproducible); must be zeroed by the caller; NULL = off.  Consumed by uc_groupnorm_apply. */
@@ -173,7 +173,7 @@ UC_API int uc_nhwc_to_nchw_f32(const void* src, int lds, float* dst, int B, int 
 UC_API int uc_msda_forward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
                                const float* sampling_loc, const float* attn_weight, int B, int S, int M, int D, int L,
                                int Lq, int P, float* out, void* stream);
-/* Fused form used by the B200 path (B=1, head dim 32): value bf16 [S, M*32]; offlog f32 [Lq, ld] = raw
+/* Fused form used by the H100 path (B=1, head dim 32): value bf16 [S, M*32]; offlog f32 [Lq, ld] = raw
  * sampling_offsets (M*L*P*2) followed by attention logits (M*L*P); queries = concatenated level grids;
  * level_hw host int[2L] (h,w).  out bf16 [Lq, M*32]. */
 UC_API int uc_msda_fused_bf16(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw,

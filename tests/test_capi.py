@@ -1,5 +1,5 @@
 """The C-ABI library loads without a GPU, exports every symbol include/unicorn_b200.h declares, and the product path
-fails loudly (no CPU / PyTorch fallback) when there is no sm_100 device."""
+fails loudly (no CPU / PyTorch fallback) when there is no sm_90 device."""
 import ctypes
 import os
 import re

@@ -1,4 +1,4 @@
-"""uc_conv2d (tcgen05 implicit GEMM) against torch fp32 conv2d on the same bf16-rounded operands."""
+"""uc_conv2d (wgmma implicit GEMM) against torch fp32 conv2d on the same bf16-rounded operands."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -31,6 +31,9 @@ for bn in (1128, 1192, 1256):
 CASES.append(("mc_conv3x3_gn", 1, 26, 40, 256, 256, 3, 1, 1, {"block_n": 1256, "gn": 16}))
 CASES.append(("mc_res_gamma", 1, 1, 777, 768, 192, 1, 1, 0, {"block_n": 1192, "bias": True, "gamma": True, "res": True}))
 CASES.append(("mc_conv3x3_s2", 1, 50, 80, 384, 384, 3, 2, 1, {"block_n": 1128}))
+# the fp16 operand path of the explicit N tiles, on a partial last M tile
+for bn in (128, 192, 256, 1256):
+    CASES.append((f"f16_bn{bn}_gelu", 1, 1, 1150, 320, 768, 1, 1, 0, {"block_n": bn, "bias": True, "act": "gelu", "f16": True}))
 
 
 def _act(x, name):
@@ -94,7 +97,7 @@ def test_conv(case):
 
 
 def test_gelu_epilogue_whole_range():
-    """The GELU of the epilogue (uc_epilogue.cuh: x * sigmoid(x * P(x^2)) on packed fp32 pairs) over the whole range a pre-activation can
+    """The GELU of the epilogue (uc_epilogue.cuh: x * sigmoid(x * P(x^2)) on fp32 pairs) over the whole range a pre-activation can
     take, including values whose exponentials saturate or overflow: a 1x1 conv with the identity as weight and the test values as
     bias.  fp32 output against torch's exact GELU."""
     from unicorn_b200 import ops

@@ -125,7 +125,7 @@ def test_cuda_graph_replay_matches_eager(setup):
 def test_reference_api_facade(setup):
     """unicorn_b200.compat.model: the reference's stage-by-stage calling convention (unicorn_sot.py:78-109 written out with
     model(..., mode=...) calls, NCHW fp32 tensors and the plain torch mm + softmax(dim=0) correlation of the reference) on
-    the B200 engine; same tolerances as the fused driver, and seq_dict must survive copy.deepcopy (mot_evaluator.py:1015)."""
+    the H100 engine; same tolerances as the fused driver, and seq_dict must survive copy.deepcopy (mot_evaluator.py:1015)."""
     import copy
     import torch.nn.functional as F
     from unicorn_b200.compat.model import UnicornB200Model, postprocess

@@ -1,4 +1,4 @@
-"""`mode="whole"` (SURVEY §8 a13: unicorn/models/unicorn.py:133-139 — zero priors, MOT prediction set) on the B200 engine against
+"""`mode="whole"` (SURVEY §8 a13: unicorn/models/unicorn.py:133-139 — zero priors, MOT prediction set) on the H100 engine against
 the outputs of the UNMODIFIED reference (tests/golden/whole_tiny_320.npz, written by tests/golden/make_golden_whole.py), for the
 plain model (MOT detector) and the mask model (MOTS detector: controllers + mask branch).
 

@@ -1,4 +1,4 @@
-"""Frames/s of the other BASELINE.json workloads on ONE B200 (bench.py is the contract line for configs[1]):
+"""Frames/s of the other BASELINE.json workloads on ONE H100 (bench.py measures configs[1]):
   mot : configs[2] — ConvNeXt-L MOT detector + embedding path at 1536x2048 (mode="whole", NMS, embedding sampling), then
         (a) the QDTrack association of the reference's MOT evaluator on the model's own detections and
         (b) ByteTrack association on 100 synthetic objects per frame (random weights give few detections of their own).

@@ -1,4 +1,7 @@
-"""Run init + N eager (non-graph) SOT frames of a config; used under ncu to list per-kernel device times."""
+"""Run init + N eager (non-graph) SOT frames of a config, then print where the device time of one more frame goes: per-kernel
+device time from torch.profiler (CUDA activities), grouped by kernel name, largest first.
+
+usage: profile_frame.py [config] [frames] [tuning table to save]"""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,6 +25,16 @@ for i in range(nfr):
     ops.CONV_TRACE = [] if i == nfr - 1 else None
     trk.track_tensor(frames[1 + i:2 + i])
     print("frame", i, "launches", _lib.LAUNCHES - l0)
+from torch.profiler import ProfilerActivity, profile
+torch.cuda.synchronize()
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    trk.track_tensor(frames[1:2])
+    torch.cuda.synchronize()
+rows = [(e.key, e.count, e.device_time_total) for e in prof.key_averages() if e.device_time_total > 0]
+total = sum(r[2] for r in rows)
+print(f"{torch.cuda.get_device_name()}: device time of one eager {H}x{W} frame {total / 1e3:.2f} ms in {sum(r[1] for r in rows)} kernels")
+for key, n, us in sorted(rows, key=lambda r: -r[2])[:20]:
+    print(f"{us / 1e3:8.3f} ms {100 * us / total:5.1f} % {n:5d}x  {key[:110]}")
 if os.environ.get("UC_CONV_TRACE"):
     import json
     json.dump(ops.CONV_TRACE, open(os.environ["UC_CONV_TRACE"], "w"))

@@ -1,2 +1,2 @@
-"""unicorn_b200 — B200-native (sm_100a) implementation of Unicorn's per-frame inference hot path."""
+"""unicorn_b200 — H100-native (sm_90a) implementation of Unicorn's per-frame inference hot path."""
 __version__ = "0.1.0"

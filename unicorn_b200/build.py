@@ -1,4 +1,4 @@
-"""Build libunicorn_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Build libunicorn_b200.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
 No torch extension machinery: the library has a plain C ABI (include/unicorn_b200.h) and is loaded with ctypes.
 nvcc cross-compiles without a GPU, so this runs in the CPU-only build container.
@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libunicorn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -50,7 +50,7 @@ def build_lib(force=False, verbose=False):
         for l in logs:
             print(l)
     if jobs or force or _stale(LIB, objs):
-        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

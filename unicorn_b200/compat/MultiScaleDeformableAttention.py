@@ -2,7 +2,7 @@
 (unicorn/models/ops/src/vision.cpp:13-16; imported at unicorn/models/ops/functions/ms_deform_attn_func.py:18).
 
 Put this directory on sys.path (or call unicorn_b200.compat.install()) and the reference's `MSDeformAttnFunction`
-runs unmodified on the sm_100a kernel `uc_msda_forward_f32`.  Same contract as the reference op
+runs unmodified on the sm_90a kernel `uc_msda_forward_f32`.  Same contract as the reference op
 (ops/src/cuda/ms_deform_attn_cuda.cu:20-80): contiguous CUDA tensors, value [B,S,M,D], spatial_shapes [L,2] int64,
 level_start_index [L] int64, sampling_loc [B,Lq,M,L,P,2], attn_weight [B,Lq,M,L,P]; returns a new [B,Lq,M*D] tensor.
 CPU tensors raise (the reference's CPU stub also only raises, ops/src/cpu/ms_deform_attn_cpu.cpp:17-40)."""

@@ -1,6 +1,6 @@
 """Reference-shaped facade over UnicornEngine: the call conventions the reference's drivers use on `Unicorn`
 (unicorn/models/unicorn.py:60-139; SURVEY.md 8b "Python model API to keep"), with the reference's tensor formats at the
-boundary (NCHW fp32 in, NCHW fp32 out) so that `unicorn_sot.py` / `unicorn_vos.py` / `mot_evaluator.py`-style code runs on the B200
+boundary (NCHW fp32 in, NCHW fp32 out) so that `unicorn_sot.py` / `unicorn_vos.py` / `mot_evaluator.py`-style code runs on the H100
 path unchanged:
 
     model = get_exp("exps/default/unicorn_track_large", None).get_model(load_pretrain=False)   # unicorn_b200/shim/unicorn/exp
@@ -21,7 +21,7 @@ numbers).  `seq_dict` holds plain tensors (keys feat, pos, h, w) and survives co
 fused fast paths (correlation without the N x N matrix, CUDA-graph frames) live in the driver classes
 (unicorn_b200.sot / mot / vos / mots), which is where a per-frame loop should go; this class is the drop-in for code that calls
 the model stage by stage.  There is no CPU path: the engine is built by `.cuda()` / `.to("cuda")` (or by the constructor when a
-state_dict is given) and raises without an sm_100 GPU; tensors must be CUDA tensors on the engine's device."""
+state_dict is given) and raises without an sm_90 GPU; tensors must be CUDA tensors on the engine's device."""
 import collections
 import math
 
@@ -118,7 +118,7 @@ class UnicornB200Model:
             self._device = device if not isinstance(device, int) else f"cuda:{device}"
         self._on_gpu = True
         if self.engine is None and self._sd is not None:
-            self.engine = UnicornEngine(self._sd, self.cfg_name, device=self._device)  # raises without an sm_100 GPU: no CPU fallback
+            self.engine = UnicornEngine(self._sd, self.cfg_name, device=self._device)  # raises without an sm_90 GPU: no CPU fallback
         return self
 
     def to(self, device=None, *a, **k):

@@ -91,7 +91,7 @@ int num_sms() {
   if (!n) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, cur_device()) != cudaSuccess) {
       cudaGetLastError();
-      n = 148;
+      n = 132;
     }
   }
   return n;
@@ -105,8 +105,9 @@ extern "C" int uc_check_device(void) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) { cudaGetLastError(); return uc::set_error(UC_ENODEV, "no CUDA device: %s", cudaGetErrorString(e)); }
-  int major = 0;
+  int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return uc::set_error(UC_ENODEV, "device compute capability %d.x is not sm_100", major);
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) return uc::set_error(UC_ENODEV, "device compute capability %d.%d is not sm_90", major, minor);
   return uc::ensure_driver();
 }

@@ -1,16 +1,22 @@
-// Implicit-GEMM convolution / linear layer on Blackwell tensor cores.
+// Implicit-GEMM convolution / linear layer on Hopper tensor cores (wgmma).
 //
 //   D[pixel, cout] = sum_{tap, cin} X[pixel + tap, cin] * W[cout, tap, cin]
 //
 // One CTA computes a 128-pixel x BLOCK_N-channel output tile.  The 128 pixels are a tile_w x tile_h patch of
 // the NHWC output map; for every filter tap the TMA engine fetches the shifted tile_w x tile_h x 64-channel
 // box of the input straight into 128B-swizzled shared memory (out-of-bounds coordinates are zero-filled by
-// the hardware, which is the convolution's zero padding), so no im2col buffer ever exists.  A single elected
-// thread issues tcgen05.mma (UMMA 128 x BLOCK_N x 16, bf16/fp16 in, fp32 accumulate in a double-buffered TMEM
-// accumulator); sixteen epilogue warps read the accumulator back with tcgen05.ld and apply bias / activation /
-// layer-scale+residual, and optionally accumulate GroupNorm statistics, before 256-bit (one L2 sector per lane) stores.
+// the hardware, which is the convolution's zero padding), so no im2col buffer ever exists.  Two consumer
+// warpgroups own 64 pixels each and issue wgmma m64 x BLOCK_N x 16 (bf16/fp16 in, fp32 accumulate in registers)
+// on the shared stage; when a tile's K loop is done they apply bias / activation / layer-scale+residual, and
+// optionally accumulate GroupNorm statistics, straight from the accumulator registers, while the producer is
+// already filling the ring with the next tile's boxes.
 //
-// Warp roles (576 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..17 = epilogue.
+// CLUSTER = 2 (block_n 1128 / 1192 / 1256): two CTAs of a thread-block cluster take consecutive M tiles of the same N tile.
+// Each loads its own activation box and HALF of the weight box, multicast by TMA into the same stage of both CTAs, so the
+// weights of a tile are read from L2 once per pair; a stage is refilled when the consumers of BOTH CTAs have released it
+// (remote mbarrier arrives).
+//
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one warp), warpgroups 1-2 = MMA + epilogue.
 // Reference call sites replaced: see include/unicorn_b200.h (uc_conv2d).
 #include <algorithm>
 #include <stdlib.h>
@@ -25,8 +31,8 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 16-bit elements -> 128-byte rows
 constexpr int kMaxTaps = 9;
 constexpr int kABytes = kBlockM * kBlockK * 2;
-constexpr int kConvEpiWarps = 16;                       // four per TMEM lane quadrant
-constexpr int kConvThreads = (2 + kConvEpiWarps) * 32;  // warp 0 TMA, warp 1 MMA, then the epilogue warps
+constexpr int kConvConsumers = 2;                       // warpgroups of 64 pixels
+constexpr int kConvThreads = (1 + kConvConsumers) * 128;
 constexpr int kGnMaxLocal = 64;                         // GroupNorm groups per N tile (tile width 256 / group size >= 4)
 constexpr int kGnSmemBytes = 2 * kGnMaxLocal * 2 * 8;   // two tile parities x {sum, sumsq} int64
 
@@ -37,21 +43,18 @@ struct ConvTap {
 struct alignas(64) ConvKernelParams {
   CUtensorMap tmA[4];
   CUtensorMap tmB;
-  CUtensorMap tmBh;  // half-height weight box for the 2-CTA multicast variant
+  CUtensorMap tmBh;  // half-height weight box of the cluster variant
   ConvTap taps[kMaxTaps];
   int ntaps, kchunks;
   int n_tiles, m_tiles;
   int tile_w, tile_h, tiles_w, tiles_h;
   int Wo, Ho, B, Cout;
-  uint32_t idesc;
   const float* bias;
   const float* gamma;
   const void* res;
   int ldres;
   void* y;
   int ldy, y_dtype, act;
-  int wide_store, wide_res;  // 256-bit stores / residual loads possible (32-byte aligned rows)
-  int debug;  // tools only (UC_CONV_DEBUG): 1 = no MMA (operand feed rate alone), 2 = no TMA loads (MMA + epilogue alone)
   const long long* row_stats;  // LayerNorm folded into this 1x1 conv: per input pixel {sum, sumsq} (fixed point 2^22) ...
   const float* col_s;          // ... column sums of the folded weights, channel count and epsilon of the LayerNorm
   float row_inv, row_eps;  // row_inv = 1 / (2^22 * Cin)
@@ -59,98 +62,53 @@ struct alignas(64) ConvKernelParams {
   int gn_groups, gn_gs;  // gs = Cout / groups
 };
 
-// GroupNorm partial sums of one epilogue item (this warp's 32 rows x ncols columns starting at channel cbase), added to the
-// CTA's shared-memory accumulators of the current tile (fixed point, integer adds: order independent).  g0 = first group of
-// the N tile (an N tile never splits a group).
-__device__ __forceinline__ void gn_partial_sums(const float (&f)[16], const ConvKernelParams& p, int cbase, int ncols, bool valid,
-                                             int lane, unsigned long long* acc_tile, int g0) {
-  int c = 0;
-#pragma unroll 1
-  while (c < ncols) {
-    const int g = (cbase + c) / p.gn_gs;
-    const int end = min(ncols, (g + 1) * p.gn_gs - cbase);
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float x = (valid && j >= c && j < end) ? f[j] : 0.f;
-      s1 += x;
-      s2 = fmaf(x, x, s2);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    }
-    if (lane == 0) {
-      atomicAdd(acc_tile + (g - g0) * 2, static_cast<unsigned long long>(__float2ll_rn(s1 * kGnFixedScale)));
-      atomicAdd(acc_tile + (g - g0) * 2 + 1, static_cast<unsigned long long>(__float2ll_rn(s2 * kGnFixedScale)));
-    }
-    c = end;
-  }
-}
-
-// Persistent kernel: grid = min(#tiles, resident CTAs); every CTA walks tiles tile = blockIdx.x + i * gridDim.x (N tile
-// fastest, so CTAs running side by side share the activation tile in L2).  The TMEM accumulator is double buffered:
-// the MMA warp fills accumulator (i+1)&1 while the epilogue warps drain accumulator i&1.
-// CLUSTER = 2 is the cta_group::2 variant: two CTAs (a cluster = one TPC's SM pair) with consecutive M tiles and the same N
-// tile compute a 256 x BLOCK_N tile with ONE pair-MMA stream issued by the leader CTA.  Each CTA stages its own 128 rows
-// of A and only HALF of the weight box (BLOCK_N/2 rows): shared-memory traffic per MAC (TMA writes + MMA operand reads,
-// which is what bounds the single-CTA kernel on K-deep layers) drops by a third.  Barriers: the leader's full[stage]
-// collects the bytes of all four loads; one tcgen05.commit.cta_group::2 multicast releases the stage / publishes the
-// accumulator in both CTAs; the peer's epilogue warps hand their accumulator back with remote arrives on the leader.
-template <int BLOCK_N, int STAGES, int CLUSTER>
+// Persistent kernel: grid = min(#tiles, SMs); every CTA (pair) walks work items item = blockIdx.x / CLUSTER + i * gridDim.x / CLUSTER
+// (N tile fastest, so CTAs running side by side share the activation tile in L2); item = (N tile, group of CLUSTER M tiles).
+template <int BLOCK_N, int STAGES, bool F16, int CLUSTER>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
-  constexpr int B_BYTES = (BLOCK_N / CLUSTER) * kBlockK * 2;  // per-CTA weight bytes per stage
-  constexpr uint32_t ACC_COLS = BLOCK_N <= 32 ? 32 : BLOCK_N <= 64 ? 64 : BLOCK_N <= 128 ? 128 : 256;
-  constexpr uint32_t TMEM_COLS = 2 * ACC_COLS;
+  constexpr int B_BYTES = BLOCK_N * kBlockK * 2;
+  constexpr int NACC = BLOCK_N / 2;  // accumulator registers per thread: m64 x BLOCK_N over 128 threads
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = sA + STAGES * kABytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tmem_full = empty + STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  // per-CTA GroupNorm accumulators (fixed point): the epilogue warps add into shared memory, ONE global atomic per group and
-  // tile follows — the short-K GN convs were bound by ~36k global atomics on the 32 addresses of an image (DESIGN.md 9.1d)
+  // per-CTA GroupNorm accumulators (fixed point): the epilogue adds into shared memory, ONE global atomic per group and tile
+  // follows (the short-K GN convs are otherwise bound by global atomics on the few addresses of an image)
   unsigned long long* gn_acc = reinterpret_cast<unsigned long long*>(smem + STAGES * (kABytes + B_BYTES) + 256);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kiters = p.ntaps * p.kchunks;
   const int crank = CLUSTER > 1 ? static_cast<int>(cluster_ctarank()) : 0;
-  // work items: (N tile, group of CLUSTER consecutive M tiles); this CTA takes M tile group*CLUSTER + crank
   const int num_items = p.n_tiles * ((p.m_tiles + CLUSTER - 1) / CLUSTER);
   const int item0 = blockIdx.x / CLUSTER, item_step = gridDim.x / CLUSTER;
+  // releases stage s: in the cluster variant the peer's producer multicasts into this CTA's stage too, so both CTAs' rings hear it
+  auto release = [&](int s) {
+    mbar_arrive(&empty[s]);
+    if (CLUSTER > 1) mbar_arrive_remote(&empty[s], static_cast<uint32_t>(crank ^ 1));
+  };
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmA[0]);
     prefetch_tmap(&p.tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kConvEpiWarps * CLUSTER);  // pair mode: the peer's epilogue warps arrive remotely
+      mbar_init(&empty[i], kConvConsumers * CLUSTER);
     }
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < 2 * kGnMaxLocal * 2; i += kConvThreads) gn_acc[i] = 0ull;
-  if (warp == 1) {
-    if (CLUSTER > 1) { tmem_alloc_2sm(tmem_slot, TMEM_COLS); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CLUSTER > 1) cluster_sync_all();  // the peer's barriers must be initialised before anything is multicast to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the
-  // tail of the previous kernel in the stream; global memory is touched only after it has completed.
+  if (CLUSTER > 1) cluster_sync_all();  // the peer's barriers are initialised before anything is multicast / arrived to them
+  // Programmatic dependent launch: the set-up above overlapped the tail of the previous kernel in the stream; global memory
+  // is touched only after it has completed.
   pdl_wait();
   pdl_launch_dependents();
 
+  if (wg == 0) {
+    regs_dealloc<40>();
+  }
   if (warp == 0) {
     // ---------------- TMA producer: the whole warp walks the loop (converged), one elected lane issues
     int stage = 0, phase = 0;
@@ -164,313 +122,213 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         for (int kc = 0; kc < p.kchunks; ++kc) {
           mbar_wait(&empty[stage], phase ^ 1);
           if (elect_one()) {
-            if (CLUSTER > 1 && p.debug == 2) {
-              if (crank == 0) mbar_arrive(&full[stage]);
-            } else if (CLUSTER > 1) {
-              // the leader arms its barrier for the bytes of both CTAs; the peer's loads are credited to it as well
-              if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2 * (kABytes + B_BYTES));
-              tma_load_4d_2sm(sA + stage * kABytes, &p.tmA[tp.map], &full[stage], kc * kBlockK, ow0 + tp.dw, oh0 + tp.dh, b);
-              tma_load_3d_2sm(sB + stage * B_BYTES, &p.tmBh, &full[stage], kc * kBlockK, tp.tap, n0 + crank * (BLOCK_N / 2));
-            } else if (p.debug == 2) {
-              mbar_arrive(&full[stage]);
-            } else {
-              mbar_arrive_expect_tx(&full[stage], kABytes + B_BYTES);
-              tma_load_4d(sA + stage * kABytes, &p.tmA[tp.map], &full[stage], kc * kBlockK, ow0 + tp.dw, oh0 + tp.dh, b);
+            mbar_arrive_expect_tx(&full[stage], kABytes + B_BYTES);  // cluster variant: own A + both multicast weight halves
+            tma_load_4d(sA + stage * kABytes, &p.tmA[tp.map], &full[stage], kc * kBlockK, ow0 + tp.dw, oh0 + tp.dh, b);
+            if (CLUSTER > 1)
+              tma_load_3d_mc(sB + stage * B_BYTES + crank * (B_BYTES / 2), &p.tmBh, &full[stage], kc * kBlockK, tp.tap,
+                             n0 + crank * (BLOCK_N / 2), static_cast<uint16_t>(0x3));
+            else
               tma_load_3d(sB + stage * B_BYTES, &p.tmB, &full[stage], kc * kBlockK, tp.tap, n0);
-            }
           }
           __syncwarp();
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer (pair mode: leader CTA only): converged warp, one elected lane issues.
-    // Shared-memory descriptors are built once per stage: inside the K loop only their start-address field advances.
-    if (crank == 0) {
-      const uint32_t idesc = p.idesc;
-      const uint64_t a_desc0 = umma_desc_sw128(smem_u32(sA)), b_desc0 = umma_desc_sw128(smem_u32(sB));
-      int stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (int item = item0; item < num_items; item += item_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-        for (int it = 0; it < kiters; ++it) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          if (CLUSTER == 1 && p.debug == 1) {
-            if (elect_one()) {
-              mbar_arrive(&empty[stage]);
-              if (it == kiters - 1) mbar_arrive(&tmem_full[acc]);
-            }
-          } else if (elect_one()) {
-            // descriptor start address is in 16-byte units: stage offsets and the 32-byte K step are plain adds
-            const uint64_t a_desc = a_desc0 + static_cast<uint64_t>((stage * kABytes) >> 4);
-            const uint64_t b_desc = b_desc0 + static_cast<uint64_t>((stage * B_BYTES) >> 4);
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-              if (CLUSTER > 1) umma_f16_2sm(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (it | k) != 0 ? 1u : 0u);
-              else umma_f16(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (it | k) != 0 ? 1u : 0u);
-            }
-            // frees this smem stage (in both CTAs of the pair) when the MMAs above have read it
-            if (CLUSTER > 1) umma_commit_2sm_mc(&empty[stage], static_cast<uint16_t>(0x3));
-            else umma_commit(&empty[stage]);
-            if (it == kiters - 1) {  // accumulator complete (in both CTAs' tensor memory)
-              if (CLUSTER > 1) umma_commit_2sm_mc(&tmem_full[acc], static_cast<uint16_t>(0x3));
-              else umma_commit(&tmem_full[acc]);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    // ---------------- epilogue: TMEM -> registers -> fused math -> NHWC global
-    // 16 warps = 4 TMEM lane quadrants (q = warp % 4, fixed by the hardware) x 4 column groups (cg).  Work item = 32 rows x 16
-    // channels: warp (q, cg) owns rows 32q..32q+31 and the channels 64 rd + 16 cg of round rd, so the warps are balanced for
-    // every N tile.  A lane holds 16 consecutive channels of one pixel = 32 bytes of bf16 = exactly one L2 sector, written
-    // with ONE 256-bit store (no partial sectors, no staging buffer, no barrier): the warps are completely independent and
-    // drift apart, which is what hides the TMEM / L2 / MUFU latencies of one another.
-    const int q = warp & 3;
-    const int cg = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    const int wi = row % p.tile_w, hi = row / p.tile_w;
-    const bool f16 = p.y_dtype == UC_F16;
-    constexpr int ROUNDS = (BLOCK_N + 63) / 64;
-    int acc = 0, acc_phase = 0, gpar = 0;
+  } else if (wg > 0) {
+    regs_alloc<232>();
+    // ---------------- consumers: warpgroup c = pixels 64c .. 64c+63 of the tile.  Accumulator fragment of thread (warp w of the
+    // warpgroup, lane = 4 g + t): rows r0 = 16 w + g and r0 + 8; registers 4i, 4i+1 = row r0, columns 8i + 2t, 8i + 2t + 1;
+    // registers 4i+2, 4i+3 = row r0 + 8, same columns.
+    const int c = wg - 1, ct = threadIdx.x - 128;
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = c * 64 + (warp & 3) * 16 + g;
+    const bool f16o = p.y_dtype == UC_F16;
+    const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(sA + c * 64 * 128)), b_desc0 = wgmma_desc_sw128(smem_u32(sB));
+    int stage = 0, phase = 0, gpar = 0;
+    float acc[NACC];
     for (int item = item0; item < num_items; item += item_step) {
       const int n0 = (item % p.n_tiles) * BLOCK_N;
       const int mt = (item / p.n_tiles) * CLUSTER + crank;
+      const bool tile_ok = mt < p.m_tiles;  // false: padding tile of an odd pair
       const int ow0 = (mt % p.tiles_w) * p.tile_w, oh0 = ((mt / p.tiles_w) % p.tiles_h) * p.tile_h;
       const int b = mt / (p.tiles_w * p.tiles_h);
-      const int ow = ow0 + wi, oh = oh0 + hi;
-      const bool tile_ok = mt < p.m_tiles;  // false: padding tile of an odd pair
-      const bool valid = (ow < p.Wo) && (oh < p.Ho) && tile_ok;
-      const size_t pix = (static_cast<size_t>(b) * p.Ho + oh) * p.Wo + ow;
-      const int limit = min(BLOCK_N, p.Cout - n0);  // valid columns of this tile (multiple of 8)
-      // LayerNorm folded into the GEMM: y = rstd * (W' x) - rstd * mu * colsum(W') + c ; (mu, rstd) of this lane's pixel
-      float r_rstd = 1.f, r_murstd = 0.f;
-      if (p.row_stats && valid) {  // one 128-bit load; fp32 is enough here (|mu| <~ 10 sigma for a ConvNeXt block's depthwise output)
-        const longlong2 st = __ldg(reinterpret_cast<const longlong2*>(p.row_stats) + pix);
-        const float mu = static_cast<float>(st.x) * p.row_inv;
-        const float var = fmaxf(fmaf(-mu, mu, static_cast<float>(st.y) * p.row_inv), 0.f);
-        r_rstd = rsqrtf(var + p.row_eps);
-        r_murstd = mu * r_rstd;
+      // ---- K loop: one wgmma group per stage in flight; a stage is released once the group after it has been issued
+      int prev_stage = -1;
+      for (int it = 0; it < kiters; ++it) {
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        const uint64_t a_desc = a_desc0 + static_cast<uint64_t>((stage * kABytes) >> 4);
+        const uint64_t b_desc = b_desc0 + static_cast<uint64_t>((stage * B_BYTES) >> 4);
+  #pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) wgmma_ss<BLOCK_N, F16>(acc, a_desc + 2 * k, b_desc + 2 * k, (it | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && ct % 128 == 0) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      // this warp's last round with columns to read: the accumulator is handed back to the MMA warp right after it
-      const int last_rd = (limit - 1 - cg * 16) >= 0 ? min(ROUNDS - 1, (limit - 1 - cg * 16) / 64) : -1;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_acc = tmem_base + acc * ACC_COLS + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-      for (int rd = 0; rd <= last_rd; ++rd) {
-        const int c0 = rd * 64 + cg * 16;
-        const int cbase = n0 + c0;
-        const int ncols = min(16, limit - c0);  // 8 or 16
-        uint32_t v[16];
-        tmem_ld_32x16(t_acc + c0, v);
-        float4 bb[4];
-        if (p.bias) {  // in flight together with the TMEM load
-#pragma unroll
-          for (int j = 0; j < 4; ++j) bb[j] = (4 * j < ncols) ? __ldg(reinterpret_cast<const float4*>(p.bias + cbase) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) bb[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev_stage >= 0 && ct % 128 == 0) release(prev_stage);
+
+      // ---- epilogue straight from the accumulator registers
+      const int limit = min(BLOCK_N, p.Cout - n0);  // valid columns of this tile (multiple of 8)
+      size_t pix[2];
+      bool valid[2];
+      float r_rstd[2] = {1.f, 1.f}, r_murstd[2] = {0.f, 0.f};
+  #pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        const int ow = ow0 + row % p.tile_w, oh = oh0 + row / p.tile_w;
+        valid[h] = (ow < p.Wo) && (oh < p.Ho) && tile_ok;
+        pix[h] = (static_cast<size_t>(b) * p.Ho + oh) * p.Wo + ow;
+        // LayerNorm folded into the GEMM: y = rstd * (W' x) - rstd * mu * colsum(W') + c ; (mu, rstd) of this row's pixel
+        if (p.row_stats && valid[h]) {  // fp32 is enough here (|mu| <~ 10 sigma for a ConvNeXt block's depthwise output)
+          const longlong2 st = __ldg(reinterpret_cast<const longlong2*>(p.row_stats) + pix[h]);
+          const float mu = static_cast<float>(st.x) * p.row_inv;
+          const float var = fmaxf(fmaf(-mu, mu, static_cast<float>(st.y) * p.row_inv), 0.f);
+          r_rstd[h] = rsqrtf(var + p.row_eps);
+          r_murstd[h] = mu * r_rstd[h];
         }
-        uint32_t rw[8];
-        const bool has_res = p.res && valid;
-        if (has_res) {  // residual: the same 32-byte sector of the shortcut tensor
-          const uint16_t* r = reinterpret_cast<const uint16_t*>(p.res) + pix * p.ldres + cbase;
-          if (p.wide_res && ncols == 16) {
-            ldg_v8(r, rw);
+      }
+      // GroupNorm partial sums: per thread and column parity j, summed over the chunks of one group, then over the 16 rows of the
+      // warp (shuffles) and added to the CTA's shared-memory slots by lanes 0..3 (fixed point, integer adds: order independent)
+      unsigned long long* gacc = gn_acc + gpar * (kGnMaxLocal * 2);
+      const int g0 = p.gn_stats ? n0 / p.gn_gs : 0;
+      float gs1[2] = {0.f, 0.f}, gs2[2] = {0.f, 0.f};
+      int gcur[2] = {-1, -1};
+      auto gn_flush = [&]() {
+  #pragma unroll
+        for (int j = 0; j < 2; ++j) {
+  #pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            gs1[j] += __shfl_xor_sync(0xffffffffu, gs1[j], o);
+            gs2[j] += __shfl_xor_sync(0xffffffffu, gs2[j], o);
+          }
+          if (g == 0 && gcur[j] >= 0) {
+            atomicAdd(gacc + (gcur[j] - g0) * 2, static_cast<unsigned long long>(__float2ll_rn(gs1[j] * kGnFixedScale)));
+            atomicAdd(gacc + (gcur[j] - g0) * 2 + 1, static_cast<unsigned long long>(__float2ll_rn(gs2[j] * kGnFixedScale)));
+          }
+          gs1[j] = gs2[j] = 0.f;
+          gcur[j] = -1;
+        }
+      };
+  #pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        if (8 * i >= limit) break;  // warp-uniform
+        const int cbase = n0 + 8 * i + 2 * t;
+        const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + cbase)) : make_float2(0.f, 0.f);
+        f32x2 hv[2];
+  #pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const f32x2 v = pk2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          if (p.row_stats) {
+            const float2 cs = __ldg(reinterpret_cast<const float2*>(p.col_s + cbase));
+            const f32x2 nm = pk2(-r_murstd[h], -r_murstd[h]);
+            hv[h] = fma2(v, pk2(r_rstd[h], r_rstd[h]), fma2(nm, pk2(cs.x, cs.y), pk2(bb.x, bb.y)));
           } else {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              uint4 rv = make_uint4(0, 0, 0, 0);
-              if (8 * j < ncols) rv = __ldg(reinterpret_cast<const uint4*>(r) + j);
-              rw[4 * j] = rv.x; rw[4 * j + 1] = rv.y; rw[4 * j + 2] = rv.z; rw[4 * j + 3] = rv.w;
-            }
+            hv[h] = add2(v, pk2(bb.x, bb.y));
           }
         }
-        tmem_ld_wait();
-        if (rd == last_rd) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (CLUSTER > 1 && crank != 0) mbar_arrive_remote(&tmem_empty[acc], 0);
-            else mbar_arrive(&tmem_empty[acc]);
+        if (p.gn_stats) {
+          const int ga = cbase / p.gn_gs, gb = (cbase + 1) / p.gn_gs;
+          if (__any_sync(0xffffffffu, (gcur[0] >= 0 && gcur[0] != ga) || (gcur[1] >= 0 && gcur[1] != gb))) gn_flush();
+          gcur[0] = ga;
+          gcur[1] = gb;
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float x0 = valid[h] ? lo2(hv[h]) : 0.f, x1 = valid[h] ? hi2(hv[h]) : 0.f;
+            gs1[0] += x0; gs2[0] = fmaf(x0, x0, gs2[0]);
+            gs1[1] += x1; gs2[1] = fmaf(x1, x1, gs2[1]);
           }
         }
-        f32x2 h[8];
-        if (p.row_stats) {
-          const f32x2 rs = pk2(r_rstd, r_rstd), nm = pk2(-r_murstd, -r_murstd);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float4 cs = (4 * j < ncols) ? __ldg(reinterpret_cast<const float4*>(p.col_s + cbase) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-            h[2 * j] = fma2(pk2(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1])), rs, fma2(nm, pk2(cs.x, cs.y), pk2(bb[j].x, bb[j].y)));
-            h[2 * j + 1] = fma2(pk2(__uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])), rs, fma2(nm, pk2(cs.z, cs.w), pk2(bb[j].z, bb[j].w)));
+        if (p.act != UC_ACT_NONE) {
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (p.act == UC_ACT_GELU) hv[h] = gelu2(hv[h]);
+            else hv[h] = pk2(apply_act(lo2(hv[h]), p.act), apply_act(hi2(hv[h]), p.act));
           }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            h[2 * j] = add2(pk2(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1])), pk2(bb[j].x, bb[j].y));
-            h[2 * j + 1] = add2(pk2(__uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])), pk2(bb[j].z, bb[j].w));
-          }
-        }
-        if (p.act == UC_ACT_GELU && !p.gn_stats) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) h[j] = gelu2(h[j]);
-        } else if (p.gn_stats || p.act != UC_ACT_NONE) {
-          float f[16];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { f[2 * j] = lo2(h[j]); f[2 * j + 1] = hi2(h[j]); }
-          if (p.gn_stats) gn_partial_sums(f, p, cbase, ncols, valid, lane, gn_acc + gpar * (kGnMaxLocal * 2), n0 / p.gn_gs);
-          switch (p.act) {
-            case UC_ACT_RELU:
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-              break;
-            case UC_ACT_NONE: break;
-            default:
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = apply_act(f[j], p.act);
-              break;
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) h[j] = pk2(f[2 * j], f[2 * j + 1]);
         }
         if (p.gamma) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (4 * j < ncols) {
-              const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + cbase) + j);
-              h[2 * j] = mul2(h[2 * j], pk2(g.x, g.y));
-              h[2 * j + 1] = mul2(h[2 * j + 1], pk2(g.z, g.w));
-            }
-          }
+          const float2 gm = __ldg(reinterpret_cast<const float2*>(p.gamma + cbase));
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) hv[h] = mul2(hv[h], pk2(gm.x, gm.y));
         }
-        if (has_res) {
-#pragma unroll
-          for (int t = 0; t < 8; ++t) {
-            const f32x2 rr = f16 ? pk2(bits16_to_float(rw[t] & 0xffffu, UC_F16), bits16_to_float(rw[t] >> 16, UC_F16))
-                                 : pk2(bf16lo(rw[t]), bf16hi(rw[t]));
-            h[t] = add2(h[t], rr);
+  #pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!valid[h]) continue;
+          if (p.res) {
+            const uint32_t rw = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.res) + pix[h] * p.ldres + cbase));
+            hv[h] = add2(hv[h], f16o ? pk2(bits16_to_float(rw & 0xffffu, UC_F16), bits16_to_float(rw >> 16, UC_F16)) : pk2(bf16lo(rw), bf16hi(rw)));
           }
-        }
-        if (valid) {
           if (p.y_dtype == UC_F32) {
-            float* yp = reinterpret_cast<float*>(p.y) + pix * p.ldy + cbase;
-            uint32_t o[16];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { o[2 * j] = __float_as_uint(lo2(h[j])); o[2 * j + 1] = __float_as_uint(hi2(h[j])); }
-            if (p.wide_store) {
-              stg_v8(yp, o);
-              if (ncols == 16) stg_v8(yp + 8, o + 8);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                if (4 * j < ncols) *(reinterpret_cast<uint4*>(yp) + j) = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-              }
-            }
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + pix[h] * p.ldy + cbase) = hv[h];
           } else {
-            uint16_t* yp = reinterpret_cast<uint16_t*>(p.y) + pix * p.ldy + cbase;
-            uint32_t o[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = pack2_fast(lo2(h[j]), hi2(h[j]), f16);
-            if (p.wide_store && ncols == 16) {
-              stg_v8(yp, o);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                if (8 * j < ncols) *(reinterpret_cast<uint4*>(yp) + j) = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-              }
-            }
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.y) + pix[h] * p.ldy + cbase) = pack2_fast(lo2(hv[h]), hi2(hv[h]), f16o);
           }
-        }
-      }
-      if (last_rd < 0) {  // narrow or edge tile: nothing to read for this warp, still release the accumulator
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CLUSTER > 1 && crank != 0) mbar_arrive_remote(&tmem_empty[acc], 0);
-          else mbar_arrive(&tmem_empty[acc]);
         }
       }
       if (p.gn_stats) {
-        // every epilogue warp has added its partial sums of this tile: one global atomic per group, then the slots are
-        // cleared for the tile after next (the next tile uses the other parity, so no second barrier is needed)
-        asm volatile("bar.sync 1, %0;" ::"n"(kConvEpiWarps * 32) : "memory");
-        const int et = static_cast<int>(threadIdx.x) - 64;  // 0 .. 511 over the epilogue warps
+        gn_flush();
+        // every consumer thread has added its partial sums of this tile: one global atomic per group, then the slots are cleared for
+        // the tile after next (the next tile uses the other parity, so no second barrier is needed)
+        named_sync(1, kConvConsumers * 128);
         const int ng = (limit + p.gn_gs - 1) / p.gn_gs;
-        if (et < 2 * ng) {
-          unsigned long long* slot = gn_acc + gpar * (kGnMaxLocal * 2) + et;
+        if (ct < 2 * ng) {
+          unsigned long long* slot = gacc + ct;
           const unsigned long long v = *slot;
           *slot = 0ull;
           if (tile_ok && v != 0ull) {
-            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.gn_stats) +
-                                      (static_cast<size_t>(b) * p.gn_groups + n0 / p.gn_gs) * 2 + et;
+            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.gn_stats) + (static_cast<size_t>(b) * p.gn_groups + g0) * 2 + ct;
             atomicAdd(dst, v);
           }
         }
         gpar ^= 1;
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (CLUSTER > 1) cluster_sync_all();  // no CTA may exit while its peer can still signal its barriers / write its smem
-  if (warp == 1) {
-    tc_fence_after();
-    if (CLUSTER > 1) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
-  }
+  if (CLUSTER > 1) cluster_sync_all();  // no CTA exits while its peer can still multicast into it or arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------- host side
 
 template <int BLOCK_N, int STAGES, int CLUSTER>
-static int launch_conv(ConvKernelParams& p, cudaStream_t stream) {
-  constexpr int smem = STAGES * (kABytes + (BLOCK_N / CLUSTER) * kBlockK * 2) + 1024 + 256 + kGnSmemBytes;
-  static PerDeviceInt per_sm_dev;
-  int& per_sm = per_sm_dev.get();
-  auto kern = conv_gemm_kernel<BLOCK_N, STAGES, CLUSTER>;
-  if (!per_sm) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(static_cast<int>(e), "conv_gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    int n = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kConvThreads, smem);
-    if (e != cudaSuccess || n < 1) return set_error(UC_EINVAL, "conv_gemm<%d,%d>: does not fit on an SM", BLOCK_N, STAGES);
-    constexpr int acc_cols = BLOCK_N <= 32 ? 32 : BLOCK_N <= 64 ? 64 : BLOCK_N <= 128 ? 128 : 256;
-    per_sm = std::min(n, 512 / (2 * acc_cols));  // TMEM: 512 columns per SM
+static int launch_conv(ConvKernelParams& p, bool f16, cudaStream_t stream) {
+  constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2) + 1024 + 256 + kGnSmemBytes;
+  static PerDeviceFlag attr_dev;
+  bool& attr = attr_dev.get();
+  auto kern = f16 ? conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER> : conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>;
+  if (!attr) {
+    for (auto k : {conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER>, conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>}) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (e != cudaSuccess) return set_error(static_cast<int>(e), "conv_gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    }
+    attr = true;
   }
   const int items = p.n_tiles * ((p.m_tiles + CLUSTER - 1) / CLUSTER);
-  int grid = std::min(items * CLUSTER, num_sms() * per_sm);
+  int grid = std::min(items * CLUSTER, num_sms());  // one CTA per SM
   grid -= grid % CLUSTER;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kConvThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr_list[2];
   int na = 0;
   if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    attr_list[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr_list[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
   }
   if (CLUSTER > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CLUSTER;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
+    attr_list[na].id = cudaLaunchAttributeClusterDimension;
+    attr_list[na].val.clusterDim.x = CLUSTER;
+    attr_list[na].val.clusterDim.y = 1;
+    attr_list[na].val.clusterDim.z = 1;
     ++na;
   }
-  cfg.attrs = attr;
+  cfg.attrs = attr_list;
   cfg.numAttrs = na;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
   if (e != cudaSuccess) return set_error(static_cast<int>(e), "conv_gemm<%d,%d,%d> launch: %s", BLOCK_N, STAGES, CLUSTER, cudaGetErrorString(e));
@@ -581,7 +439,7 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   p.kchunks = (d->Cin + kBlockK - 1) / kBlockK;
 
   const int gn_gs = d->gn_stats ? d->Cout / d->gn_groups : 0;
-  // block_n >= 1000 selects the cta_group::2 pair variant (1128 / 1192 / 1256)
+  // block_n >= 1000 selects the 2-CTA cluster variant with weight multicast (1128 / 1192 / 1256)
   const bool cluster2 = d->block_n >= 1000;
   const int bn = cluster2 ? d->block_n - 1000 : d->block_n ? d->block_n : pick_block_n(d->Cout, m_tiles, gn_gs);
   if (bn == 0) return set_error(UC_EINVAL, "uc_conv2d: no N tile compatible with GroupNorm group size %d", gn_gs);
@@ -592,18 +450,7 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     rc = encode_tmap(&p.tmB, dt, 3, d->w, dims, strides, box);
     if (rc) return rc;
   }
-  {
-    const size_t yes = d->y_dtype == UC_F32 ? 4 : 2;
-    p.wide_store = ((d->ldy * yes) % 32 == 0) && (reinterpret_cast<uintptr_t>(d->y) % 32 == 0);
-    p.wide_res = d->res && ((d->ldres * es) % 32 == 0) && (reinterpret_cast<uintptr_t>(d->res) % 32 == 0);
-  }
   p.Cout = d->Cout;
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("UC_CONV_DEBUG"); dbg = e ? atoi(e) : 0; }
-    p.debug = dbg;
-  }
-  p.idesc = umma_idesc_f16(d->x_dtype == UC_BF16 ? 1u : 0u, kBlockM, static_cast<uint32_t>(bn));
   p.bias = d->bias; p.gamma = d->gamma; p.res = d->res; p.ldres = d->ldres;
   p.y = d->y; p.ldy = d->ldy; p.y_dtype = d->y_dtype; p.act = d->act;
   p.row_stats = static_cast<const long long*>(d->row_stats); p.col_s = d->col_s; p.row_inv = 1.f / (kGnFixedScale * static_cast<float>(d->Cin)); p.row_eps = d->row_eps;
@@ -615,28 +462,28 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     return set_error(UC_EINVAL, "uc_conv2d: N tile %d incompatible with GroupNorm group size %d", bn, p.gn_gs);
   p.n_tiles = (d->Cout + bn - 1) / bn;
   p.m_tiles = m_tiles;
+  const bool f16 = d->x_dtype == UC_F16;
   if (cluster2) {
     uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(nt), static_cast<uint64_t>(d->Cout)};
     uint64_t strides[2] = {static_cast<uint64_t>(d->Cin) * es, static_cast<uint64_t>(nt) * d->Cin * es};
     uint32_t box[3] = {static_cast<uint32_t>(kBlockK), 1, static_cast<uint32_t>(bn / 2)};
     rc = encode_tmap(&p.tmBh, dt, 3, d->w, dims, strides, box);
     if (rc) return rc;
-    p.idesc = umma_idesc_f16(d->x_dtype == UC_BF16 ? 1u : 0u, 2 * kBlockM, static_cast<uint32_t>(bn));  // UMMA M = 256
     switch (bn) {
-      case 256: return launch_conv<256, 6, 2>(p, stream);  // 6 x 32 KB ring
-      case 192: return launch_conv<192, 7, 2>(p, stream);  // 7 x 28 KB
-      case 128: return launch_conv<128, 8, 2>(p, stream);  // 8 x 24 KB
-      default: return set_error(UC_EINVAL, "uc_conv2d: the cta_group::2 variant exists for block_n 128/192/256 only");
+      case 256: return launch_conv<256, 4, 2>(p, f16, stream);
+      case 192: return launch_conv<192, 5, 2>(p, f16, stream);
+      case 128: return launch_conv<128, 6, 2>(p, f16, stream);
+      default: return set_error(UC_EINVAL, "uc_conv2d: the cluster variant exists for block_n 128/192/256 only");
     }
   }
-  switch (bn) {
-    case 256: return launch_conv<256, 4, 1>(p, stream);
-    case 192: return launch_conv<192, 5, 1>(p, stream);
-    case 128: return launch_conv<128, 6, 1>(p, stream);
-    case 96: return launch_conv<96, 6, 1>(p, stream);
-    case 64: return launch_conv<64, 8, 1>(p, stream);
-    case 32: return launch_conv<32, 8, 1>(p, stream);
-    case 16: return launch_conv<16, 8, 1>(p, stream);
+  switch (bn) {  // stage rings of 144 - 200 KB (227 KB of shared memory per block)
+    case 256: return launch_conv<256, 4, 1>(p, f16, stream);
+    case 192: return launch_conv<192, 5, 1>(p, f16, stream);
+    case 128: return launch_conv<128, 6, 1>(p, f16, stream);
+    case 96: return launch_conv<96, 6, 1>(p, f16, stream);
+    case 64: return launch_conv<64, 8, 1>(p, f16, stream);
+    case 32: return launch_conv<32, 8, 1>(p, f16, stream);
+    case 16: return launch_conv<16, 8, 1>(p, f16, stream);
     default: return set_error(UC_EINVAL, "uc_conv2d: unsupported block_n %d", bn);
   }
 }

@@ -4,13 +4,13 @@
 //
 // replaces the three materialising passes of external/lib/test/tracker/unicorn_sot.py:95-100
 // (torch.mm -> softmax(dim=0) -> values @ trans_mat; same in unicorn_vos.py:171-181): the (N_ref x N_cur) similarity
-// matrix (512 MB in fp16 at 800x1280) never leaves the SM.  Flash-attention style: one CTA owns 128 current positions
-// (rows of the TMEM accumulator), streams the reference positions in chunks of 256 through a TMA ring, computes the
-// 128x256 similarity tile with tcgen05.mma (UMMA 128x256x16) into a double-buffered TMEM accumulator (all 512 columns), and
-// sixteen softmax warps (four per TMEM lane quadrant, 64 columns each, no cross-thread reductions inside the loop) keep the
-// running max / sum / weighted label sums; one exponential in four is evaluated on the FMA pipe (the kernel is MUFU bound).
-// V has only n_obj (1..8) rows, so the P.V product is done with CUDA-core FMAs on the probabilities instead of
-// wasting an MMA tile.
+// matrix (512 MB in fp16 at 800x1280) never leaves the SM.  Flash-attention style: one CTA owns 128 current positions,
+// streams the reference positions in chunks of 128 through a TMA ring, and each of two consumer warpgroups computes the
+// 64 x 128 similarity tile of its 64 positions with wgmma (m64n128k16) into registers and keeps, per thread, the running
+// max / sum / weighted label sums of the columns it holds (no cross-thread reductions inside the loop; the four partial
+// states of a position are merged once at the end).  One exponential in four is evaluated on the FMA pipe (the softmax is
+// bound by the MUFU unit).  V has only n_obj (1..8) rows, so the P.V product is done with CUDA-core FMAs on the
+// probabilities instead of wasting an MMA tile.
 #include "uc_ptx.cuh"
 #include "uc_common.h"
 #include "../../include/unicorn_b200.h"
@@ -18,22 +18,19 @@
 namespace uc {
 
 constexpr int kCorrC = 128;       // embedding channels
-constexpr int kCorrTile = 128;    // current positions per CTA (rows of the TMEM accumulator)
-constexpr int kCorrChunk = 256;   // reference positions per MMA chunk (UMMA N = 256: half as many barrier hand-offs as 128)
-constexpr int kCorrStages = 2;    // K ring (64 KB per stage)
-constexpr int kCorrVSlots = 6;    // label-value slots, see the producer: chunk x's values may be written once every softmax warp has LOADED
-                                  // S of chunk x-4 (it may still be computing chunk x-4, but is done with x-5): >= 5 slots are needed
+constexpr int kCorrTile = 128;    // current positions per CTA (64 per consumer warpgroup)
+constexpr int kCorrChunk = 128;   // reference positions per MMA chunk (64 accumulator registers per thread)
+constexpr int kCorrStages = 4;    // K ring (32 KB per stage; the chunk's label values travel with it)
 constexpr int kCorrQBytes = kCorrTile * kCorrC * 2;    // 32 KB (two 128B-swizzled 64-channel halves)
-constexpr int kCorrKBytes = kCorrChunk * kCorrC * 2;   // 64 KB
-constexpr int kCorrSoftmaxWarps = 16;                  // 4 per TMEM lane quadrant, each owning 64 of the 256 chunk columns
-constexpr int kCorrThreads = (2 + kCorrSoftmaxWarps) * 32;
+constexpr int kCorrKBytes = kCorrChunk * kCorrC * 2;   // 32 KB
+constexpr int kCorrConsumers = 2;
+constexpr int kCorrThreads = (1 + kCorrConsumers) * 128;
 
 struct alignas(64) CorrParams {
   CUtensorMap tmQ, tmK;
   const float* V;  // [n_obj, ldv]
   float* out;      // [n_obj, ldo]
   int ldv, ldo, n_cur, n_ref, n_obj;
-  uint32_t idesc;
 };
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -55,47 +52,37 @@ __device__ __forceinline__ float poly_exp2(float x) {
   return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
 
-template <int NOBJ>
+template <int NOBJ, bool F16>
 __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_constant__ CorrParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sK = smem + kCorrQBytes;
-  float* sV = reinterpret_cast<float*>(sK + kCorrStages * kCorrKBytes);  // [kCorrVSlots][NOBJ][256]
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + kCorrVSlots * NOBJ * kCorrChunk);
+  float* sV = reinterpret_cast<float*>(sK + kCorrStages * kCorrKBytes);  // [kCorrStages][NOBJ][kCorrChunk]
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + kCorrStages * NOBJ * kCorrChunk);
   uint64_t* k_full = q_full + 1;
   uint64_t* k_empty = k_full + kCorrStages;
-  uint64_t* s_full = k_empty + kCorrStages;
-  uint64_t* s_empty = s_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int j0 = blockIdx.x * kCorrTile;
   const int nchunks = (p.n_ref + kCorrChunk - 1) / kCorrChunk;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmQ);
     prefetch_tmap(&p.tmK);
     mbar_init(q_full, 1);
-    for (int i = 0; i < kCorrStages; ++i) { mbar_init(&k_full[i], 2); mbar_init(&k_empty[i], 1); }  // full: TMA bytes + label values
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], kCorrSoftmaxWarps); }
+    // full: TMA bytes + label values; empty: one arrival per consumer WARP (every warp reads the stage's label values itself)
+    for (int i = 0; i < kCorrStages; ++i) { mbar_init(&k_full[i], 2); mbar_init(&k_empty[i], kCorrConsumers * 4); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);  // two 128 x 256 fp32 similarity buffers
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // barrier init / TMEM allocation above overlapped the previous kernel's tail
+  pdl_wait();  // barrier init above overlapped the previous kernel's tail
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    // Producer: TMA for the K chunk (one elected lane) and — all 32 lanes — the chunk's label values V[:, i0 .. i0+255] into their
-    // slot.  The producer runs up to kCorrStages chunks ahead of the MMA, so the L2 latency of these loads is never on the softmax
-    // warps' critical path (it was: they used to stage V themselves behind a 512-thread barrier every chunk).
+  if (wg == 0) {
+    if (warp != 0) return;
+    // Producer: TMA for the K chunk (one elected lane) and — all 32 lanes — the chunk's label values V[:, i0 .. i0+127] into the
+    // same stage.  The producer runs up to kCorrStages chunks ahead, so the L2 latency of these loads is off the softmax's path.
     if (elect_one()) {
       mbar_arrive_expect_tx(q_full, kCorrQBytes);
       tma_load_2d(sQ, &p.tmQ, q_full, 0, j0);
@@ -112,7 +99,7 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
         tma_load_2d(dst, &p.tmK, &k_full[stage], 0, i0);
         tma_load_2d(dst + kCorrKBytes / 2, &p.tmK, &k_full[stage], 64, i0);
       }
-      float* vb = sV + (c % kCorrVSlots) * NOBJ * kCorrChunk;
+      float* vb = sV + stage * NOBJ * kCorrChunk;
 #pragma unroll
       for (int o = 0; o < NOBJ; ++o) {
 #pragma unroll
@@ -122,162 +109,125 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
         }
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&k_full[stage]);  // release: the MMA warp acquires it, its commit publishes it to the softmax warps
+      if (lane == 0) mbar_arrive(&k_full[stage]);  // release: the consumers acquire it with their wait
       if (++stage == kCorrStages) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1) {
-    // MMA issuer: converged warp, one elected lane issues; descriptors built once, only the address field advances
-    mbar_wait(q_full, 0);
-    const uint64_t q_desc = umma_desc_sw128(smem_u32(sQ)), k_desc0 = umma_desc_sw128(smem_u32(sK));
-    const uint32_t idesc = p.idesc;
-    int stage = 0, phase = 0;
-    for (int c = 0; c < nchunks; ++c) {
-      const int buf = c & 1;
-      mbar_wait(&s_empty[buf], ((c >> 1) & 1) ^ 1);
-      mbar_wait(&k_full[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t k_desc = k_desc0 + static_cast<uint64_t>((stage * kCorrKBytes) >> 4);
+    return;
+  }
+  // ---------------- consumers: S = Q K^T, online softmax + label propagation.  Warpgroup c owns positions 64c .. 64c+63;
+  // thread (warp w, lane = 4 g + t) holds rows 16 w + g (h = 0) and + 8 (h = 1), columns 8i + 2t, 8i + 2t + 1 of the chunk.
+  // Everything is in the log2 domain: p = 2^(s*log2e - m).
+  const int c = wg - 1;
+  const int g = lane >> 2, t = lane & 3;
+  constexpr float kLog2e = 1.4426950408889634f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float acc[2][NOBJ];
 #pragma unroll
-        for (int ks = 0; ks < kCorrC / 16; ++ks) {
-          const uint64_t qo = static_cast<uint64_t>(((ks >> 2) * (kCorrQBytes / 2) + (ks & 3) * 32) >> 4);
-          const uint64_t ko = static_cast<uint64_t>(((ks >> 2) * (kCorrKBytes / 2) + (ks & 3) * 32) >> 4);
-          umma_f16(tmem_base + buf * kCorrChunk, q_desc + qo, k_desc + ko, idesc, ks != 0 ? 1u : 0u);
-        }
-        umma_commit(&k_empty[stage]);
-        umma_commit(&s_full[buf]);
-      }
-      __syncwarp();
-      if (++stage == kCorrStages) { stage = 0; phase ^= 1; }
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int o = 0; o < NOBJ; ++o) acc[h][o] = 0.f;
+  mbar_wait(q_full, 0);
+  const uint64_t q_desc = wgmma_desc_sw128(smem_u32(sQ + c * 64 * 128)), k_desc0 = wgmma_desc_sw128(smem_u32(sK));
+  int stage = 0, phase = 0;
+  for (int cc = 0; cc < nchunks; ++cc) {
+    const int i0 = cc * kCorrChunk;
+    mbar_wait(&k_full[stage], phase);
+    float s[kCorrChunk / 2];
+    wgmma_fence();
+    const uint64_t k_desc = k_desc0 + static_cast<uint64_t>((stage * kCorrKBytes) >> 4);
+#pragma unroll
+    for (int ks = 0; ks < kCorrC / 16; ++ks) {
+      const uint64_t qo = static_cast<uint64_t>(((ks >> 2) * (kCorrQBytes / 2) + (ks & 3) * 32) >> 4);
+      const uint64_t ko = static_cast<uint64_t>(((ks >> 2) * (kCorrKBytes / 2) + (ks & 3) * 32) >> 4);
+      wgmma_ss<kCorrChunk, F16>(s, q_desc + qo, k_desc + ko, ks != 0 ? 1u : 0u);
     }
-  } else {
-    // ---------------- online softmax + label propagation
-    // 16 warps: warp w owns TMEM lane quadrant (w & 3) (= 32 current positions) and columns [64*cg, 64*cg+64) of every 256-column
-    // similarity chunk, cg = (w-2)/4.  Each thread keeps a private running (max, sum, weighted label sums) for its (position,
-    // column group); the four partial states of a position are merged once at the end.  No block-level barrier inside the loop: the
-    // warps drift apart and hide one another's tcgen05.ld / MUFU latencies.  Everything is in the log2 domain: p = 2^(s*log2e - m).
-    const int q = warp & 3;
-    const int cg = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    const int j = j0 + row;
-    constexpr float kLog2e = 1.4426950408889634f;
-    constexpr int CW = kCorrChunk / 4;  // 64 columns per warp and chunk
-    float m = -INFINITY;
-    float l[4] = {0.f, 0.f, 0.f, 0.f};
-    float acc[NOBJ][2];
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    const int nvalid = min(kCorrChunk, p.n_ref - i0);
+    if (nvalid < kCorrChunk) {  // tail chunk only (uniform)
 #pragma unroll
-    for (int o = 0; o < NOBJ; ++o) acc[o][0] = acc[o][1] = 0.f;
-    for (int c = 0; c < nchunks; ++c) {
-      const int buf = c & 1;
-      const int i0 = c * kCorrChunk;
-      const float* vb = sV + (c % kCorrVSlots) * NOBJ * kCorrChunk;
-      mbar_wait(&s_full[buf], (c >> 1) & 1);
-      tc_fence_after();
-      const int nvalid = min(kCorrChunk, p.n_ref - i0);
-      const int c0 = cg * CW;
-      uint32_t v[CW];
-      {
-        const uint32_t ta = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * kCorrChunk + c0;
-        uint32_t v0[32], v1[32];
-        tmem_ld_32x32(ta, v0);
-        tmem_ld_32x32(ta + 32, v1);
-        tmem_ld_wait();
+      for (int i = 0; i < kCorrChunk / 8; ++i)
 #pragma unroll
-        for (int t = 0; t < 32; ++t) { v[t] = v0[t]; v[32 + t] = v1[t]; }
-      }
-      // this warp's only read of the S buffer is done: hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[buf]);
-      if (c0 >= nvalid) continue;  // warp-uniform: fully masked column group of the tail chunk
-      float s[CW];
+        for (int e = 0; e < 4; ++e)
+          if (8 * i + 2 * t + (e & 1) >= nvalid) s[4 * i + e] = -INFINITY;
+    }
+    const float* vb = sV + stage * NOBJ * kCorrChunk;
 #pragma unroll
-      for (int t = 0; t < CW; ++t) s[t] = __uint_as_float(v[t]);
-      if (nvalid < kCorrChunk) {  // tail chunk only (warp-uniform)
+    for (int h = 0; h < 2; ++h) {
+      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // tree maximum: no 32-deep dependent chain
 #pragma unroll
-        for (int t = 0; t < CW; ++t)
-          if (c0 + t >= nvalid) s[t] = -INFINITY;
-      }
-      float mx[8];  // tree maximum (a 64-deep dependent chain of FMNMX would sit on the critical path of every chunk)
+      for (int i = 0; i < kCorrChunk / 8; ++i) mx[i & 3] = fmaxf(mx[i & 3], fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+      const float cmax = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
+      if (cmax == -INFINITY) continue;  // every column of this thread is masked (tail chunk)
+      const float m_new = fmaxf(m[h], cmax * kLog2e);
+      if (m_new != m[h]) {  // the running maximum moves in the first few chunks only: skip the rescale otherwise
+        const float scale = fast_exp2(m[h] - m_new);
+        m[h] = m_new;
+        l[h] *= scale;
 #pragma unroll
-      for (int t = 0; t < 8; ++t) mx[t] = fmaxf(fmaxf(s[t], s[t + 8]), fmaxf(s[t + 16], s[t + 24]));
-#pragma unroll
-      for (int t = 0; t < 8; ++t) mx[t] = fmaxf(mx[t], fmaxf(fmaxf(s[t + 32], s[t + 40]), fmaxf(s[t + 48], s[t + 56])));
-      const float cmax = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])), fmaxf(fmaxf(mx[4], mx[5]), fmaxf(mx[6], mx[7])));
-      const float m_new = fmaxf(m, cmax * kLog2e);
-      if (m_new != m) {  // the running maximum moves in the first few chunks only: skip the rescale otherwise
-        const float scale = fast_exp2(m - m_new);
-        m = m_new;
-#pragma unroll
-        for (int u = 0; u < 4; ++u) l[u] *= scale;
-#pragma unroll
-        for (int o = 0; o < NOBJ; ++o) { acc[o][0] *= scale; acc[o][1] *= scale; }
+        for (int o = 0; o < NOBJ; ++o) acc[h][o] *= scale;
       }
       const float neg_m = -m_new;
 #pragma unroll
-      for (int t = 0; t < CW; t += 4) {
-        float pr[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const float x = fmaf(s[t + u], kLog2e, neg_m);  // <= 0 (-inf for masked columns -> p = 0 on both paths)
-          pr[u] = (u == 3) ? poly_exp2(x) : fast_exp2(x);
-          l[u] += pr[u];
-        }
+      for (int i = 0; i < kCorrChunk / 8; ++i) {
+        const float x0 = fmaf(s[4 * i + 2 * h], kLog2e, neg_m), x1 = fmaf(s[4 * i + 2 * h + 1], kLog2e, neg_m);  // <= 0
+        const float p0 = fast_exp2(x0), p1 = (i & 1) ? poly_exp2(x1) : fast_exp2(x1);
+        l[h] += p0 + p1;
 #pragma unroll
         for (int o = 0; o < NOBJ; ++o) {
-          const float4 vv = *reinterpret_cast<const float4*>(vb + o * kCorrChunk + c0 + t);  // same address in every lane: broadcast
-          acc[o][0] = fmaf(pr[0], vv.x, acc[o][0]); acc[o][1] = fmaf(pr[1], vv.y, acc[o][1]);
-          acc[o][0] = fmaf(pr[2], vv.z, acc[o][0]); acc[o][1] = fmaf(pr[3], vv.w, acc[o][1]);
+          const float2 vv = *reinterpret_cast<const float2*>(vb + o * kCorrChunk + 8 * i + 2 * t);
+          acc[h][o] = fmaf(p1, vv.y, fmaf(p0, vv.x, acc[h][o]));
         }
       }
     }
-    // merge the four column groups of every position (the K ring is idle now: reuse it as scratch)
-    float* part = reinterpret_cast<float*>(sK);  // [4][128][2 + NOBJ]
-    float* mine = part + (cg * kCorrTile + row) * (2 + NOBJ);
-    mine[0] = m; mine[1] = (l[0] + l[1]) + (l[2] + l[3]);
+    // K chunk and label values of this stage consumed by this warp: the label values are read with ordinary loads by every lane, so
+    // the slot may be refilled only when all lanes of all consumer warps are past their last read (a per-warpgroup release from one
+    // thread would not order the other warps' reads)
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&k_empty[stage]);
+    if (++stage == kCorrStages) { stage = 0; phase ^= 1; }
+  }
+  // merge the four partial states of every position (the 4 lanes t of a quad)
 #pragma unroll
-    for (int o = 0; o < NOBJ; ++o) mine[2 + o] = acc[o][0] + acc[o][1];
-    asm volatile("bar.sync 1, %0;" ::"n"(kCorrSoftmaxWarps * 32) : "memory");
-    if (cg == 0 && j < p.n_cur) {
-      float M = -INFINITY;
+  for (int h = 0; h < 2; ++h) {
+    float M = m[h];
+    M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, 1));
+    M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, 2));
+    const float w = fast_exp2(m[h] - M);  // a thread that saw only masked columns has m = -inf -> weight 0
+    float L = l[h] * w;
+    L += __shfl_xor_sync(0xffffffffu, L, 1);
+    L += __shfl_xor_sync(0xffffffffu, L, 2);
+    float A[NOBJ];
 #pragma unroll
-      for (int g = 0; g < 4; ++g) M = fmaxf(M, part[(g * kCorrTile + row) * (2 + NOBJ)]);
-      float L = 0.f, A[NOBJ];
-#pragma unroll
-      for (int o = 0; o < NOBJ; ++o) A[o] = 0.f;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const float* pg = part + (g * kCorrTile + row) * (2 + NOBJ);
-        const float w = fast_exp2(pg[0] - M);  // a group that saw only masked columns has m = -inf -> weight 0
-        L = fmaf(pg[1], w, L);
-#pragma unroll
-        for (int o = 0; o < NOBJ; ++o) A[o] = fmaf(pg[2 + o], w, A[o]);
-      }
+    for (int o = 0; o < NOBJ; ++o) {
+      A[o] = acc[h][o] * w;
+      A[o] += __shfl_xor_sync(0xffffffffu, A[o], 1);
+      A[o] += __shfl_xor_sync(0xffffffffu, A[o], 2);
+    }
+    const int j = j0 + c * 64 + (warp & 3) * 16 + g + 8 * h;
+    if (t == 0 && j < p.n_cur) {
       const float inv = 1.f / L;
 #pragma unroll
       for (int o = 0; o < NOBJ; ++o)
         if (o < p.n_obj) p.out[static_cast<long>(o) * p.ldo + j] = A[o] * inv;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 template <int NOBJ>
-static int launch_corr(const CorrParams& p, int grid, cudaStream_t stream) {
-  constexpr int smem = kCorrQBytes + kCorrStages * kCorrKBytes + kCorrVSlots * NOBJ * kCorrChunk * 4 + 256 + 1024;
+static int launch_corr(const CorrParams& p, bool f16, int grid, cudaStream_t stream) {
+  constexpr int smem = kCorrQBytes + kCorrStages * kCorrKBytes + kCorrStages * NOBJ * kCorrChunk * 4 + 256 + 1024;
   static PerDeviceFlag attr_dev;
   bool& attr_set = attr_dev.get();
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(corr_kernel<NOBJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(static_cast<int>(e), "corr: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    for (auto k : {corr_kernel<NOBJ, true>, corr_kernel<NOBJ, false>}) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (e != cudaSuccess) return set_error(static_cast<int>(e), "corr: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    }
     attr_set = true;
   }
-  launch_pdl(corr_kernel<NOBJ>, grid, kCorrThreads, smem, stream, p);
+  launch_pdl(f16 ? corr_kernel<NOBJ, true> : corr_kernel<NOBJ, false>, grid, kCorrThreads, smem, stream, p);
   return check_launch("uc_corr_propagate");
 }
 
@@ -313,11 +263,11 @@ extern "C" int uc_corr_propagate(const void* embed_ref, int ld_ref, int n_ref, c
     if (rc) return rc;
   }
   p.V = values; p.out = out; p.ldv = ldv; p.ldo = ldo; p.n_cur = n_cur; p.n_ref = n_ref; p.n_obj = n_obj;
-  p.idesc = umma_idesc_f16(dtype == UC_BF16 ? 1u : 0u, kCorrTile, kCorrChunk);
+  const bool f16 = dtype == UC_F16;
   const int grid = (n_cur + kCorrTile - 1) / kCorrTile;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (n_obj == 1) return launch_corr<1>(p, grid, stream);
-  if (n_obj == 2) return launch_corr<2>(p, grid, stream);
-  if (n_obj <= 4) return launch_corr<4>(p, grid, stream);
-  return launch_corr<8>(p, grid, stream);
+  if (n_obj == 1) return launch_corr<1>(p, f16, grid, stream);
+  if (n_obj == 2) return launch_corr<2>(p, f16, grid, stream);
+  if (n_obj <= 4) return launch_corr<4>(p, f16, grid, stream);
+  return launch_corr<8>(p, f16, grid, stream);
 }

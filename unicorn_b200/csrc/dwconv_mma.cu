@@ -7,8 +7,8 @@
 //     out[h, w0+n] += sum_k  X[h + kh - 3, w0 - 4 + k] * T_kh[k][n],      T_kh[k][n] = f[kh][k - n - 1]  (0 <= k-n-1 <= 6, else 0)
 //
 // i.e. one mma.sync.m16n8k16 (bf16 in, fp32 accumulate) per (channel, filter row, 16 x 8 output block): M = 16 output rows, K = a
-// 16-pixel window of one input row, N = 8 output columns; 7 MMAs per block and channel, 44 % of the issued MACs are useful, which is
-// irrelevant at 558 TFLOP/s of mma.sync (tools/ubench/mma_rate.cu) against 15.6 GFLOP of useful work.  What it needs is
+// 16-pixel window of one input row, N = 8 output columns; 7 MMAs per block and channel, 44 % of the issued MACs are useful, which matters
+// little next to the tensor-core rate of mma.sync and the 15.6 GFLOP of useful work per 800x1280 frame.  What it needs is
 //   * the input tile CHANNEL-PLANAR in shared memory ([channel][row][col], so that ldmatrix delivers A fragments).  The kernel is
 //     bound by shared-memory wavefronts (ldmatrix.x4 = 4), so a warp computes BOTH 8-column blocks of a 16-wide tile from three
 //     8-column fragment halves (ldmatrix.x4 + .x2 = 6 wavefronts per two MMAs instead of 8: the middle half is shared);
@@ -261,8 +261,7 @@ extern "C" int uc_dwconv7_mma(const void* x_bf16, const void* qtab, void* y_bf16
   const long items = static_cast<long>(p.tiles_w) * p.tiles_h * B * ((C + kMmCH - 1) / kMmCH);
   if (items > 0x7fffffffL) return set_error(UC_EINVAL, "uc_dwconv7_mma: too many tiles");
   p.n_items = static_cast<int>(items);
-  // 4 warps per item; the 8-warp variant (UC_DW_MMA_WARPS=8) was measured slower on every backbone stage of ConvNeXt-L at 800x1280 (34.0 /
-  // 20.1 / 14.0 us vs 26.4 / 15.6 / 13.2 on stages 1-3, 8.2 vs 8.6 on stage 4: profiles/r2_dwconv_mma_microbench.txt) and is kept for experiments
+  // 4 warps per item (3 CTAs per SM); the 8-warp variant (UC_DW_MMA_WARPS=8, 2 CTAs per SM) is kept for experiments
   static int forced = -1;
   if (forced < 0) { const char* e = getenv("UC_DW_MMA_WARPS"); forced = e ? atoi(e) : 0; }
   const bool wide = forced == 8;

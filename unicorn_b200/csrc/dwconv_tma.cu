@@ -8,12 +8,11 @@
 // taps; both land in one of TWO shared-memory stages and complete on that stage's mbarrier, so the box of item n+1 streams in
 // while item n is computed.  No thread computes an address or a bounds check for the staging.
 //
-// The kernel is bound by fp32 FMA issue, not by HBM (98 flop per output element, 15.6 GFLOP per 800x1280 frame; measured peak of
-// packed FFMA2 with a shared multiplier operand: 73 TFLOP/s, tools/ubench/fma_rate.cu) — and at that rate the first version also
-// saturated the shared-memory pipe (0.5 wavefronts per FFMA2).  Register blocking brings that to 0.25: 256 threads = 8 warps;
-// a warp owns an 8-pixel strip of TWO output rows, a lane one channel pair; per staged input row (14 pixels, read and converted
-// once) it issues 2 x 56 FFMA2 — with filter row kh for the upper output row and the previous filter row, kept in registers, for the
-// lower one.  Items are handed out by an atomic counter (uneven per-SM loads of a static split cost 30 % on the 50 x 80 maps).
+// The kernel is bound by fp32 FMA issue, not by HBM (98 flop per output element, 15.6 GFLOP per 800x1280 frame), and register
+// blocking keeps the shared-memory reads per FMA low: 256 threads = 8 warps; a warp owns an 8-pixel strip of TWO output rows, a lane
+// one channel pair; per staged input row (14 pixels, read and converted once) it issues 2 x 56 channel-pair FMAs (fma_pair) — with
+// filter row kh for the upper output row and the previous filter row, kept in registers, for the lower one.  Items are handed out by
+// an atomic counter (a static split gives uneven per-SM loads on small maps).
 //
 // Optional per-pixel LayerNorm statistics (sum, sum of squares over C of the STORED bf16 values, int64 fixed point 2^22, integer
 // atomics: order independent) feed the following pwconv1, which applies the normalisation in its epilogue (UcConv2d.row_stats).
@@ -135,13 +134,13 @@ __global__ void __launch_bounds__(kDwThreads, kDwCtasPerSm) dwconv7_tma_kernel(c
 #pragma unroll
         for (int kw = 0; kw < 7; ++kw)
 #pragma unroll
-          for (int q = 0; q < kDwPX; ++q) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[0][q]) : "l"(v[q + kw]), "l"(wcur[kw]));
+          for (int q = 0; q < kDwPX; ++q) fma_pair(acc[0][q], v[q + kw], wcur[kw]);
       }
       if (i > 0) {
 #pragma unroll
         for (int kw = 0; kw < 7; ++kw)
 #pragma unroll
-          for (int q = 0; q < kDwPX; ++q) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[1][q]) : "l"(v[q + kw]), "l"(wprev[kw]));
+          for (int q = 0; q < kDwPX; ++q) fma_pair(acc[1][q], v[q + kw], wprev[kw]);
       }
       if (i < 7) {
 #pragma unroll

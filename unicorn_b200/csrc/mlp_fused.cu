@@ -2,25 +2,26 @@
 //
 //     x += gamma * ( W2 . GELU( W1 . LayerNorm(t) + b1 ) + b2 )          t = depthwise-conv output, x = the block's input (shortcut)
 //
-// in ONE persistent launch for the stages whose channel count C fits a shared-memory row tile (C = 96, 192, 256, 384: stages 1-2 of
-// ConvNeXt-L, stages 1-3 of ConvNeXt-T, the attention blocks of the head; C = 256 has room for one row-tile buffer, C = 384 for one
-// row-tile buffer and one stage per weight ring only).  There the separate kernels are bound by the 4C hidden map, not by the tensor pipe: at 800x1280 /
-// ConvNeXt-L stage 1 it is 64000 x 768 x 2 B = 98 MB that pwconv1 writes to and pwconv2 reads back from HBM (69 + 40 us for 2 x 19
-// GFLOP), plus a 17 us LayerNorm pass.  Here the hidden activations never leave the SM:
+// in ONE persistent launch for C = 96, 192, 256, 384 (stages 1-2 of ConvNeXt-L, stages 1-3 of ConvNeXt-T, the attention blocks of
+// the head).  There the separate
+// kernels are bound by the 4C hidden map, which pwconv1 writes to and pwconv2 reads back from HBM, and by the LayerNorm pass; here
+// the hidden activations never leave the SM:
 //
-//   * TMA brings a 128-row x C tile of t into 128B-swizzled shared memory (K-major UMMA operand layout); the 16 compute warps
-//     LayerNorm it IN PLACE (two-pass mean / variance in fp32 over the bf16 values, like uc_layernorm; the affine part is folded into
-//     W1 / b1 by the host: W1' = W1 diag(g), b1' = b1 + W1 beta) and publish it to the tensor core with a proxy fence;
-//   * the hidden dimension is walked in chunks of 64: GEMM1 (UMMA 128 x 64 x 16, K = C) -> double-buffered TMEM accumulator -> the
-//     compute warps add b1', apply the exact GELU (uc_epilogue.cuh) and write the bf16 chunk into a double-buffered 128B-swizzled
-//     shared-memory tile -> GEMM2 (UMMA 128 x C x 16, K = 64) accumulates it into the output accumulator (TMEM columns 128..128+C);
-//     the weight chunks W1'[64 j .. 64 j + 63][:] and W2[:][64 j .. 64 j + 63] stream through two 2-stage TMA rings;
-//   * after the last chunk the compute warps read the output accumulator, add b2, multiply by the layer scale, add the shortcut
-//     (one 32-byte sector per lane) and store x in place — the same epilogue arithmetic and order as uc_conv2d's.
-//   * the MMA warp issues GEMM1 of chunk j+1 BEFORE GEMM2 of chunk j, so the tensor core works on the next chunk while the compute
-//     warps are in the GELU of the current one, and the next row tile is loaded and normalised during the second half of the current.
+//   * TMA brings a 128-row x C tile of t into 128B-swizzled shared memory (K-major wgmma operand layout); each consumer warpgroup
+//     LayerNorms its 64 rows IN PLACE (two-pass mean / variance in fp32 over the bf16 values, like uc_layernorm; the affine part is
+//     folded into W1 / b1 by the host: W1' = W1 diag(g), b1' = b1 + W1 beta) and publishes them to the tensor core with a proxy fence;
+//   * the hidden dimension is walked in chunks of 64: GEMM1 (wgmma 64 x 64 x 16, K = C, both operands in shared memory) -> registers
+//     -> + b1', exact GELU (uc_epilogue.cuh), rounded to bf16 IN REGISTERS: the fp32 accumulator fragment of GEMM1 is, pair by pair,
+//     the A-operand fragment of GEMM2 (wgmma 64 x C x 16 with A from registers, K = 64), which accumulates into the output registers;
+//     the weight chunks W1'[64 j .. 64 j + 63][:] and W2[:][64 j .. 64 j + 63] stream through two TMA rings;
+//   * C = 384: the 64 x 384 output accumulator does not fit a warpgroup's registers next to the hidden chunk, so the output columns
+//     are computed in two halves of 192, each walking all hidden chunks (GEMM1 and the GELU are evaluated twice);
+//   * after the last chunk the warpgroup adds b2 to its accumulator, multiplies by the layer scale, adds the shortcut and stores x
+//     in place — the same epilogue arithmetic and order as uc_conv2d's.
+//   * the two consumer warpgroups share the weight rings and run independently otherwise, so one is in its GELU / LayerNorm while
+//     the other keeps the tensor core busy.
 //
-// Warp roles (576 threads, 1 CTA / SM): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..17 = compute.
+// Warp roles (384 threads, 1 CTA / SM): warpgroup 0 = TMA producer (one warp), warpgroups 1-2 = rows 0-63 / 64-127 of the tile.
 #include <algorithm>
 #include "uc_ptx.cuh"
 #include "uc_common.h"
@@ -31,26 +32,23 @@ namespace uc {
 
 constexpr int kMlpRows = 128;
 constexpr int kMlpHC = 64;  // hidden chunk = one 128-byte K block of GEMM2
-constexpr int kMlpComputeWarps = 16;
-constexpr int kMlpThreads = (2 + kMlpComputeWarps) * 32;
-constexpr int kMlpGroups = 1;  // compute-warp groups taking alternate hidden chunks (2 was measured slower: 89.6 vs 78.3 us on stage 1)
-constexpr int kMlpColsPerWarp = kMlpHC / (4 / kMlpGroups);  // columns of a chunk per warp: 16 (one group) or 32
-constexpr uint32_t kMlpAcc2Col = 128;  // TMEM: columns 0..127 = the two GEMM1 accumulators, 128.. = the output accumulator
+constexpr int kMlpConsumers = 2;
+constexpr int kMlpThreads = (1 + kMlpConsumers) * 128;
 
 template <int C>
 struct MlpCfg {
   static constexpr int KB = (C + 63) / 64;              // K blocks of the row tile (the last one zero-filled past C by TMA)
   static constexpr int A_BYTES = KB * kMlpRows * 128;   // 128 rows x KB x 128 B
   static constexpr int W1_BYTES = KB * kMlpHC * 128;    // 64 hidden rows x KB x 128 B
-  static constexpr int W2_BYTES = C * 128;              // C output rows x 64 hidden (128 B)
-  static constexpr int H_BYTES = kMlpRows * 128;        // 128 rows x 64 hidden
+  static constexpr int NH = C > 256 ? 2 : 1;            // output column halves (register budget, see above)
+  static constexpr int N2 = C / NH;                     // output columns per pass
+  static constexpr int W2_BYTES = N2 * 128;             // N2 output rows x 64 hidden (128 B)
   static constexpr int NCHUNK = 4 * C / kMlpHC;
-  static constexpr int AS = C <= 192 ? 2 : 1;           // row-tile buffers and weight-ring stages: C = 256 has room for one row tile,
-  static constexpr int WS = C <= 256 ? 2 : 1;           // C = 384 for one of each (the next weight chunk is then requested when the MMAs reading this one retire)
-  static constexpr int N2S = C > 256 ? 2 : 1;           // GEMM2 is issued as N2S UMMAs of N = C / N2S <= 256 columns
-  static constexpr int N2 = C / N2S;
-  static constexpr int SMEM = AS * A_BYTES + WS * (W1_BYTES + W2_BYTES) + 2 * H_BYTES + 1024 + 512;
-  static constexpr int CPT = C / 32;                    // 16-byte chunks of a row per LayerNorm thread (4 threads per row)
+  static constexpr int STEPS = NH * NCHUNK;             // weight chunks per row tile
+  static constexpr int AS = C <= 192 ? 2 : 1;           // row-tile buffers (C >= 256 has room for one next to the weight rings)
+  static constexpr int WS = C <= 256 ? 2 : 1;           // weight-ring stages
+  static constexpr int SMEM = AS * A_BYTES + WS * (W1_BYTES + W2_BYTES) + 1024 + 512;
+  static constexpr int CPT = C / 16;                    // 16-byte chunks of a row per LayerNorm thread (2 threads per row)
 };
 
 struct alignas(64) MlpParams {
@@ -61,12 +59,10 @@ struct alignas(64) MlpParams {
   uint16_t* x;         // [M][C] shortcut in, block output out
   int M, m_tiles;
   float ln_eps;
-  uint32_t idesc1, idesc2;
 };
 
 // barrier indices
-enum { A_FULL = 0, A_READY = 2, A_EMPTY = 4, W1_FULL = 6, W1_EMPTY = 8, W2_FULL = 10, W2_EMPTY = 12, ACC1_FULL = 14, ACC1_EMPTY = 16,
-       H_FULL = 18, H_EMPTY = 20, ACC2_FULL = 22, ACC2_EMPTY = 23, MLP_NBARS = 24 };
+enum { A_FULL = 0, A_EMPTY = 2, W1_FULL = 4, W1_EMPTY = 6, W2_FULL = 8, W2_EMPTY = 10, MLP_NBARS = 12 };
 
 template <int C>
 __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __grid_constant__ MlpParams p) {
@@ -76,47 +72,33 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
   uint8_t* sA = smem;                                 // [AS][KB][128 rows][128 B]
   uint8_t* sW1 = sA + Cfg::AS * Cfg::A_BYTES;         // [WS][KB][64 rows][128 B]
   uint8_t* sW2 = sW1 + Cfg::WS * Cfg::W1_BYTES;       // [WS][C rows][128 B]
-  uint8_t* sH = sW2 + Cfg::WS * Cfg::W2_BYTES;        // [2][128 rows][128 B]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sH + 2 * Cfg::H_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + MLP_NBARS);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sW2 + Cfg::WS * Cfg::W2_BYTES);
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmA);
     prefetch_tmap(&p.tmW1);
     prefetch_tmap(&p.tmW2);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&bar[A_FULL + i], 1);
-      mbar_init(&bar[A_READY + i], kMlpComputeWarps);
-      mbar_init(&bar[A_EMPTY + i], 1);
+      mbar_init(&bar[A_EMPTY + i], kMlpConsumers);
       mbar_init(&bar[W1_FULL + i], 1);
-      mbar_init(&bar[W1_EMPTY + i], 1);
+      mbar_init(&bar[W1_EMPTY + i], kMlpConsumers);
       mbar_init(&bar[W2_FULL + i], 1);
-      mbar_init(&bar[W2_EMPTY + i], 1);
-      mbar_init(&bar[ACC1_FULL + i], 1);
-      mbar_init(&bar[ACC1_EMPTY + i], kMlpComputeWarps / kMlpGroups);  // two groups: chunk buffer i belongs to compute group i
-      mbar_init(&bar[H_FULL + i], kMlpComputeWarps / kMlpGroups);
-      mbar_init(&bar[H_EMPTY + i], 1);
+      mbar_init(&bar[W2_EMPTY + i], kMlpConsumers);
     }
-    mbar_init(&bar[ACC2_FULL], 1);
-    mbar_init(&bar[ACC2_EMPTY], kMlpComputeWarps);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
 
   const int n_local = (p.m_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);  // row tiles of this CTA
   auto tile_of = [&](int i) { return static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x); };
 
-  if (warp == 0) {
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (warp != 0) return;
     // ---------------- TMA producer
     auto load_a = [&](int i) {
       const int ab = i % Cfg::AS;
@@ -129,9 +111,9 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
       }
       __syncwarp();
     };
-    // weight chunk g: hidden rows (W1) / columns (W2) 64 (g % NCHUNK) .. + 63
-    auto load_w1 = [&](int g) {
-      const int s = g % Cfg::WS, ph = (g / Cfg::WS) & 1, j = g % Cfg::NCHUNK;
+    // weight step g: hidden rows (W1) / columns (W2) 64 j .. + 63 of output half nh
+    auto load_w = [&](int g) {
+      const int s = g % Cfg::WS, ph = (g / Cfg::WS) & 1, j = g % Cfg::NCHUNK, nh = (g / Cfg::NCHUNK) % Cfg::NH;
       mbar_wait(&bar[W1_EMPTY + s], ph ^ 1);
       if (elect_one()) {
         mbar_arrive_expect_tx(&bar[W1_FULL + s], Cfg::W1_BYTES);
@@ -140,234 +122,148 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
           tma_load_2d(sW1 + s * Cfg::W1_BYTES + kb * (kMlpHC * 128), &p.tmW1, &bar[W1_FULL + s], kb * 64, j * kMlpHC);
       }
       __syncwarp();
-    };
-    auto load_w2 = [&](int g) {
-      const int s = g % Cfg::WS, ph = (g / Cfg::WS) & 1, j = g % Cfg::NCHUNK;
       mbar_wait(&bar[W2_EMPTY + s], ph ^ 1);
       if (elect_one()) {
         mbar_arrive_expect_tx(&bar[W2_FULL + s], Cfg::W2_BYTES);
-#pragma unroll
-        for (int nh = 0; nh < Cfg::N2S; ++nh)
-          tma_load_2d(sW2 + s * Cfg::W2_BYTES + nh * (Cfg::N2 * 128), &p.tmW2, &bar[W2_FULL + s], j * kMlpHC, nh * Cfg::N2);
+        tma_load_2d(sW2 + s * Cfg::W2_BYTES, &p.tmW2, &bar[W2_FULL + s], j * kMlpHC, nh * Cfg::N2);
       }
       __syncwarp();
     };
-    const int total = n_local * Cfg::NCHUNK;
-    // one-stage rings: W1 one chunk ahead of W2 (GEMM1 of chunk g+1 is issued before GEMM2 of g, and the ring can only be refilled
-    // when its reader has retired); two-stage rings: in chunk order (measured 5 % faster there than the look-ahead order)
-    if (n_local > 0) {
-      load_a(0);
-      if (Cfg::WS == 1) load_w1(0);
-    }
+    const int total = n_local * Cfg::STEPS;
+    if (n_local > 0) load_a(0);
     for (int g = 0; g < total; ++g) {
-      if (Cfg::WS == 1) {
-        if (g + 1 < total) load_w1(g + 1);
-      } else {
-        load_w1(g);
-      }
-      load_w2(g);
-      const int i = g / Cfg::NCHUNK, j = g % Cfg::NCHUNK;
+      load_w(g);
+      const int i = g / Cfg::STEPS, r = g % Cfg::STEPS;
       // the next row tile: into the other buffer right away, or (single buffer) once the last GEMM1 of this tile has read it
-      if (j == (Cfg::AS == 2 ? 0 : Cfg::NCHUNK - 1) && i + 1 < n_local) load_a(i + 1);
+      if (r == (Cfg::AS == 2 ? 0 : Cfg::STEPS - 1) && i + 1 < n_local) load_a(i + 1);
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer: converged warp, one elected lane issues
-    const uint64_t a_desc0 = umma_desc_sw128(smem_u32(sA)), w1_desc0 = umma_desc_sw128(smem_u32(sW1));
-    const uint64_t w2_desc0 = umma_desc_sw128(smem_u32(sW2)), h_desc0 = umma_desc_sw128(smem_u32(sH));
-    const uint32_t acc2 = tmem_base + kMlpAcc2Col;
-    auto gemm2 = [&](int gg, bool first, int i) {  // output accumulator += H chunk gg . W2 chunk gg^T
-      const int s = gg & 1, ph = (gg >> 1) & 1;
-      const int ws = gg % Cfg::WS, wph = (gg / Cfg::WS) & 1;
-      mbar_wait(&bar[H_FULL + s], ph);
-      mbar_wait(&bar[W2_FULL + ws], wph);
-      if (first) mbar_wait(&bar[ACC2_EMPTY], (i & 1) ^ 1);  // the previous tile's output has been read out
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t ad = h_desc0 + static_cast<uint64_t>((s * Cfg::H_BYTES) >> 4);
-#pragma unroll
-        for (int nh = 0; nh < Cfg::N2S; ++nh) {
-          const uint64_t bd = w2_desc0 + static_cast<uint64_t>((ws * Cfg::W2_BYTES + nh * (Cfg::N2 * 128)) >> 4);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(acc2 + static_cast<uint32_t>(nh * Cfg::N2), ad + 2 * k, bd + 2 * k, p.idesc2, (first && k == 0) ? 0u : 1u);
-        }
-        umma_commit(&bar[H_EMPTY + s]);
-        umma_commit(&bar[W2_EMPTY + ws]);
-      }
-      __syncwarp();
-    };
-    int g = 0;
-    for (int i = 0; i < n_local; ++i) {
-      const int ab = i % Cfg::AS;
-      mbar_wait(&bar[A_READY + ab], (i / Cfg::AS) & 1);  // tile loaded AND normalised
-      for (int j = 0; j < Cfg::NCHUNK; ++j, ++g) {
-        const int s = g & 1, ph = (g >> 1) & 1;
-        const int ws = g % Cfg::WS, wph = (g / Cfg::WS) & 1;
-        mbar_wait(&bar[W1_FULL + ws], wph);
-        mbar_wait(&bar[ACC1_EMPTY + s], ph ^ 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t acc1 = tmem_base + static_cast<uint32_t>(s * kMlpHC);
-#pragma unroll
-          for (int kb = 0; kb < Cfg::KB; ++kb) {
-            const uint64_t ad = a_desc0 + static_cast<uint64_t>((ab * Cfg::A_BYTES + kb * (kMlpRows * 128)) >> 4);
-            const uint64_t bd = w1_desc0 + static_cast<uint64_t>((ws * Cfg::W1_BYTES + kb * (kMlpHC * 128)) >> 4);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(acc1, ad + 2 * k, bd + 2 * k, p.idesc1, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&bar[W1_EMPTY + ws]);
-          umma_commit(&bar[ACC1_FULL + s]);
-          if (j == Cfg::NCHUNK - 1) umma_commit(&bar[A_EMPTY + ab]);
-        }
-        __syncwarp();
-        if (j > 0) gemm2(g - 1, j == 1, i);
-      }
-      gemm2(g - 1, Cfg::NCHUNK == 1, i);
-      if (elect_one()) umma_commit(&bar[ACC2_FULL]);
-      __syncwarp();
-    }
-  } else {
-    // ---------------- compute warps: LayerNorm of the row tile, GELU of the hidden chunks, output epilogue
-    const int q = warp & 3;                  // TMEM lane quadrant (fixed by the hardware: warp id % 4)
-    const int cg = (warp - 2) >> 2;          // column group 0..3 of the output epilogue
-    const int grp = kMlpGroups == 2 ? (warp - 2) >> 3 : 0;  // two groups: hidden chunks with g % 2 == grp are this warp's
-    const int col0 = (kMlpGroups == 2 ? ((warp - 2) >> 2) & 1 : cg) * kMlpColsPerWarp;  // a warp = 32 rows x kMlpColsPerWarp columns of a chunk
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    // LayerNorm: thread (r, part) = 4 threads per row, adjacent lanes; part handles the 16-byte chunks part * CPT .. + CPT - 1
-    const int lt = static_cast<int>(threadIdx.x) - 64, lr = lt >> 2, lp = lt & 3;
-    auto layer_norm_tile = [&](int i) {
-      const int ab = i % Cfg::AS;
-      mbar_wait(&bar[A_FULL + ab], (i / Cfg::AS) & 1);
-      uint8_t* a = sA + ab * Cfg::A_BYTES + lr * 128;
-      // chunk gc of the row: K block gc / 8, 16-byte slot gc % 8 (swizzled with the row)
-      auto chunk_ptr = [&](int c) {
-        const int gc = lp * Cfg::CPT + c;
-        return reinterpret_cast<uint4*>(a + (gc >> 3) * (kMlpRows * 128) + (((gc & 7) ^ (lr & 7)) << 4));
-      };
-      float s1 = 0.f;
-#pragma unroll(Cfg::CPT > 6 ? 3 : Cfg::CPT)
-      for (int c = 0; c < Cfg::CPT; ++c) {
-        const uint4 v = *chunk_ptr(c);
-        s1 += (bf16lo(v.x) + bf16hi(v.x)) + (bf16lo(v.y) + bf16hi(v.y)) + (bf16lo(v.z) + bf16hi(v.z)) + (bf16lo(v.w) + bf16hi(v.w));
-      }
-      s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-      const float mean = s1 * (1.f / C);
-      float s2 = 0.f;
-#pragma unroll(Cfg::CPT > 6 ? 3 : Cfg::CPT)
-      for (int c = 0; c < Cfg::CPT; ++c) {
-        const uint4 v = *chunk_ptr(c);
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float d0 = bf16lo(w[e]) - mean, d1 = bf16hi(w[e]) - mean;
-          s2 = fmaf(d0, d0, s2);
-          s2 = fmaf(d1, d1, s2);
-        }
-      }
-      s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-      s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-      const float rstd = rsqrtf(s2 * (1.f / C) + p.ln_eps);
-#pragma unroll(Cfg::CPT > 6 ? 3 : Cfg::CPT)
-      for (int c = 0; c < Cfg::CPT; ++c) {
-        uint4* ptr = chunk_ptr(c);
-        const uint4 v = *ptr;
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-        uint32_t o[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) o[e] = pack2_fast((bf16lo(w[e]) - mean) * rstd, (bf16hi(w[e]) - mean) * rstd, false);
-        *ptr = make_uint4(o[0], o[1], o[2], o[3]);
-      }
-      fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar[A_READY + ab]);
-    };
-    if (n_local > 0) layer_norm_tile(0);
-    int g = 0;
-    for (int i = 0; i < n_local; ++i) {
-      for (int j = 0; j < Cfg::NCHUNK; ++j, ++g) {
-        const int s = g & 1, ph = (g >> 1) & 1;
-        if (kMlpGroups == 1 || s == grp) {
-          constexpr int NH = kMlpColsPerWarp / 16;
-          mbar_wait(&bar[ACC1_FULL + s], ph);
-          tc_fence_after();
-          uint32_t v[NH][16];
-#pragma unroll
-          for (int hh = 0; hh < NH; ++hh) tmem_ld_32x16(t_lane + static_cast<uint32_t>(s * kMlpHC + col0 + hh * 16), v[hh]);
-          tmem_ld_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar[ACC1_EMPTY + s]);
-          mbar_wait(&bar[H_EMPTY + s], ph ^ 1);  // GEMM2 of chunk g-2 has read this buffer (long ago)
-          uint8_t* hrow = sH + s * Cfg::H_BYTES + row * 128;
-#pragma unroll
-          for (int hh = 0; hh < NH; ++hh) {
-            const float4* bp = reinterpret_cast<const float4*>(p.c1 + j * kMlpHC + col0 + hh * 16);
-            uint32_t o[8];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const float4 bb = __ldg(bp + t);
-              const f32x2 h0 = gelu2(add2(pk2(__uint_as_float(v[hh][4 * t]), __uint_as_float(v[hh][4 * t + 1])), pk2(bb.x, bb.y)));
-              const f32x2 h1 = gelu2(add2(pk2(__uint_as_float(v[hh][4 * t + 2]), __uint_as_float(v[hh][4 * t + 3])), pk2(bb.z, bb.w)));
-              o[2 * t] = pack2_fast(lo2(h0), hi2(h0), false);
-              o[2 * t + 1] = pack2_fast(lo2(h1), hi2(h1), false);
-            }
-            const int ck = col0 / 8 + hh * 2;  // 16-byte slot of the row before the swizzle
-            *reinterpret_cast<uint4*>(hrow + ((ck ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-            *reinterpret_cast<uint4*>(hrow + (((ck + 1) ^ (row & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar[H_FULL + s]);
-        }
-        if (Cfg::AS == 2 && j == Cfg::NCHUNK / 2 - 1 && i + 1 < n_local) layer_norm_tile(i + 1);
-      }
-      if (Cfg::AS == 1 && i + 1 < n_local) layer_norm_tile(i + 1);  // single buffer: the producer refilled it after this tile's last GEMM1
-      // ---- output: x += gamma * (acc2 + b2)
-      const long grow = static_cast<long>(tile_of(i)) * kMlpRows + row;
-      const bool valid = grow < p.M;
-      mbar_wait(&bar[ACC2_FULL], i & 1);
-      tc_fence_after();
-      constexpr int ROUNDS = C / 64;  // 16 columns per warp and round, 4 column groups
-#pragma unroll 1
-      for (int rd = 0; rd < ROUNDS + (C % 64 ? 1 : 0); ++rd) {
-        const int c0 = (rd * 4 + cg) * 16;
-        const bool cols = c0 < C;  // C = 96: the last round has columns for column groups 0 and 1 only
-        uint32_t v[16], rw[8];
-        if (cols) {
-          tmem_ld_32x16(t_lane + kMlpAcc2Col + static_cast<uint32_t>(c0), v);
-          if (valid) ldg_v8(p.x + grow * C + c0, rw);
-          tmem_ld_wait();
-        }
-        if (rd == ROUNDS + (C % 64 ? 1 : 0) - 1) {  // this warp's last read of the output accumulator
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar[ACC2_EMPTY]);
-        }
-        if (cols && valid) {
-          uint32_t o[8];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(p.b2 + c0) + t), gm = __ldg(reinterpret_cast<const float4*>(p.gamma + c0) + t);
-            f32x2 h0 = add2(pk2(__uint_as_float(v[4 * t]), __uint_as_float(v[4 * t + 1])), pk2(b.x, b.y));
-            f32x2 h1 = add2(pk2(__uint_as_float(v[4 * t + 2]), __uint_as_float(v[4 * t + 3])), pk2(b.z, b.w));
-            h0 = mul2(h0, pk2(gm.x, gm.y));
-            h1 = mul2(h1, pk2(gm.z, gm.w));
-            h0 = add2(h0, pk2(bf16lo(rw[2 * t]), bf16hi(rw[2 * t])));
-            h1 = add2(h1, pk2(bf16lo(rw[2 * t + 1]), bf16hi(rw[2 * t + 1])));
-            o[2 * t] = pack2_fast(lo2(h0), hi2(h0), false);
-            o[2 * t + 1] = pack2_fast(lo2(h1), hi2(h1), false);
-          }
-          stg_v8(p.x + grow * C + c0, o);
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  regs_alloc<232>();
+  // ---------------- consumer warpgroup c: rows 64c .. 64c+63 of every row tile.  Accumulator fragment of thread (warp w of the
+  // warpgroup, lane = 4 g + t): rows 16 w + g and 16 w + g + 8, columns 8i + 2t, 8i + 2t + 1 in registers 4i .. 4i+3.
+  const int c = wg - 1, ct = threadIdx.x & 127;
+  const int g8 = lane >> 2, t = lane & 3;
+  const int rl = (warp & 3) * 16 + g8;  // first row of this thread inside the warpgroup's 64
+  // LayerNorm: 2 threads per row (adjacent lanes), part lp handles the 16-byte chunks lp * CPT .. + CPT - 1
+  const int lr = c * 64 + (ct >> 1), lp = ct & 1;
+  auto layer_norm_tile = [&](int ab) {
+    uint8_t* a = sA + ab * Cfg::A_BYTES + lr * 128;
+    // chunk gc of the row: K block gc / 8, 16-byte slot gc % 8 (swizzled with the row)
+    auto chunk_ptr = [&](int cc) {
+      const int gc = lp * Cfg::CPT + cc;
+      return reinterpret_cast<uint4*>(a + (gc >> 3) * (kMlpRows * 128) + (((gc & 7) ^ (lr & 7)) << 4));
+    };
+    float s1 = 0.f;
+#pragma unroll 4
+    for (int cc = 0; cc < Cfg::CPT; ++cc) {
+      const uint4 v = *chunk_ptr(cc);
+      s1 += (bf16lo(v.x) + bf16hi(v.x)) + (bf16lo(v.y) + bf16hi(v.y)) + (bf16lo(v.z) + bf16hi(v.z)) + (bf16lo(v.w) + bf16hi(v.w));
+    }
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+    const float mean = s1 * (1.f / C);
+    float s2 = 0.f;
+#pragma unroll 4
+    for (int cc = 0; cc < Cfg::CPT; ++cc) {
+      const uint4 v = *chunk_ptr(cc);
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float d0 = bf16lo(w[e]) - mean, d1 = bf16hi(w[e]) - mean;
+        s2 = fmaf(d0, d0, s2);
+        s2 = fmaf(d1, d1, s2);
+      }
+    }
+    s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+    const float rstd = rsqrtf(s2 * (1.f / C) + p.ln_eps);
+#pragma unroll 4
+    for (int cc = 0; cc < Cfg::CPT; ++cc) {
+      uint4* ptr = chunk_ptr(cc);
+      const uint4 v = *ptr;
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      uint32_t o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[e] = pack2_fast((bf16lo(w[e]) - mean) * rstd, (bf16hi(w[e]) - mean) * rstd, false);
+      *ptr = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+    fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
+    named_sync(1 + c, 128);
+  };
+  const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(sA + c * 64 * 128)), w1_desc0 = wgmma_desc_sw128(smem_u32(sW1));
+  const uint64_t w2_desc0 = wgmma_desc_sw128(smem_u32(sW2));
+  float acc2[Cfg::N2 / 2];
+  int g = 0;
+  for (int i = 0; i < n_local; ++i) {
+    const int ab = i % Cfg::AS;
+    mbar_wait(&bar[A_FULL + ab], (i / Cfg::AS) & 1);
+    layer_norm_tile(ab);
+#pragma unroll 1
+   for (int nh = 0; nh < Cfg::NH; ++nh) {
+    for (int j = 0; j < Cfg::NCHUNK; ++j, ++g) {
+      const int ws = g % Cfg::WS, wph = (g / Cfg::WS) & 1;
+      // ---- GEMM1: hidden chunk j of this warpgroup's 64 rows
+      float acc1[kMlpHC / 2];
+      mbar_wait(&bar[W1_FULL + ws], wph);
+      wgmma_fence();
+#pragma unroll
+      for (int kb = 0; kb < Cfg::KB; ++kb) {
+        const uint64_t ad = a_desc0 + static_cast<uint64_t>((ab * Cfg::A_BYTES + kb * (kMlpRows * 128)) >> 4);
+        const uint64_t bd = w1_desc0 + static_cast<uint64_t>((ws * Cfg::W1_BYTES + kb * (kMlpHC * 128)) >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss<kMlpHC, false>(acc1, ad + 2 * k, bd + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc1);
+      if (ct == 0) {
+        mbar_arrive(&bar[W1_EMPTY + ws]);
+        if (nh == Cfg::NH - 1 && j == Cfg::NCHUNK - 1) mbar_arrive(&bar[A_EMPTY + ab]);
+      }
+      // ---- + b1', GELU, bf16: accumulator columns 16 kk .. 16 kk + 15 are the A fragment of GEMM2's K step kk
+      uint32_t hf[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int i8 = 2 * kk + half;
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(p.c1 + j * kMlpHC + 8 * i8 + 2 * t));
+          const f32x2 h0 = gelu2(add2(pk2(acc1[4 * i8], acc1[4 * i8 + 1]), pk2(bb.x, bb.y)));
+          const f32x2 h1 = gelu2(add2(pk2(acc1[4 * i8 + 2], acc1[4 * i8 + 3]), pk2(bb.x, bb.y)));
+          hf[kk][2 * half] = pack2_fast(lo2(h0), hi2(h0), false);
+          hf[kk][2 * half + 1] = pack2_fast(lo2(h1), hi2(h1), false);
+        }
+      }
+      // ---- GEMM2: output accumulator += H chunk . W2 chunk^T
+      mbar_wait(&bar[W2_FULL + ws], wph);
+      wgmma_fence();
+      const uint64_t bd2 = w2_desc0 + static_cast<uint64_t>((ws * Cfg::W2_BYTES) >> 4);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs_bf16<Cfg::N2>(acc2, hf[kk], bd2 + 2 * kk, (j | kk) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc2);
+      if (ct == 0) mbar_arrive(&bar[W2_EMPTY + ws]);
+    }
+    // ---- output columns nh * N2 .. : x += gamma * (acc2 + b2)
+    const long grow0 = static_cast<long>(tile_of(i)) * kMlpRows + c * 64 + rl;
+#pragma unroll
+    for (int i8 = 0; i8 < Cfg::N2 / 8; ++i8) {
+      const int col = nh * Cfg::N2 + 8 * i8 + 2 * t;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.b2 + col)), gm = __ldg(reinterpret_cast<const float2*>(p.gamma + col));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long grow = grow0 + 8 * h;
+        if (grow < p.M) {
+          uint32_t* xp = reinterpret_cast<uint32_t*>(p.x + grow * C + col);
+          const uint32_t rw = *xp;
+          f32x2 v = add2(pk2(acc2[4 * i8 + 2 * h], acc2[4 * i8 + 2 * h + 1]), pk2(b.x, b.y));
+          v = mul2(v, pk2(gm.x, gm.y));
+          v = add2(v, pk2(bf16lo(rw), bf16hi(rw)));
+          *xp = pack2_fast(lo2(v), hi2(v), false);
+        }
+      }
+    }
+   }
   }
 }
 
@@ -435,7 +331,5 @@ extern "C" int uc_convnext_mlp(const void* t_bf16, const void* w1f_bf16, const f
   p.M = M;
   p.m_tiles = (M + kMlpRows - 1) / kMlpRows;
   p.ln_eps = ln_eps;
-  p.idesc1 = umma_idesc_f16(1u, kMlpRows, kMlpHC);
-  p.idesc2 = umma_idesc_f16(1u, kMlpRows, static_cast<uint32_t>(C > 256 ? C / 2 : C));
   return C == 96 ? launch_mlp<96>(p, stream) : C == 192 ? launch_mlp<192>(p, stream) : C == 256 ? launch_mlp<256>(p, stream) : launch_mlp<384>(p, stream);
 }

@@ -2,7 +2,7 @@
 //  * uc_msda_forward_f32  — drop-in for the reference operator MultiScaleDeformableAttention.ms_deform_attn_forward
 //    (unicorn/models/ops/src/ms_deform_attn.h:20-39 -> cuda/ms_deform_attn_cuda.cu:20-80 ->
 //     ms_deformable_im2col_gpu_kernel, cuda/ms_deform_im2col_cuda.cuh:237-299, bilinear :33-84).
-//  * uc_msda_fused_bf16   — the form the B200 path uses: reads the raw sampling-offset / attention-logit projection
+//  * uc_msda_fused_bf16   — the form the H100 path uses: reads the raw sampling-offset / attention-logit projection
 //    (one fused Linear), does the softmax over L*P, the reference-point arithmetic
 //    (deformable_transformer.py:141-153, ops/modules/ms_deform_attn.py:99-105) and the gather in one kernel.
 // Semantics (both): pixel coords x = loc_x*W - 0.5, y = loc_y*H - 0.5; a sample counts only if -1 < y < H and

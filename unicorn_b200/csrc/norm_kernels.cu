@@ -220,7 +220,7 @@ __global__ void __launch_bounds__(512, 2) dwconv7_tiled_kernel(const uint16_t* _
   __syncthreads();
   const int cp = threadIdx.x % PAIRS;
   const int hx = (threadIdx.x / PAIRS) & 1, r = threadIdx.x / (PAIRS * 2);
-  // accumulators and operands are (channel 2cp, channel 2cp+1) pairs: one packed fma.rn.f32x2 (Blackwell FFMA2) per tap
+  // accumulators and operands are (channel 2cp, channel 2cp+1) pairs: one fma_pair per tap
   // and pixel instead of two scalar FMAs — the kernel is instruction-issue bound.
   unsigned long long acc[PX];
   {
@@ -242,7 +242,7 @@ __global__ void __launch_bounds__(512, 2) dwconv7_tiled_kernel(const uint16_t* _
     for (int kw = 0; kw < 7; ++kw) {
       const unsigned long long wv = *reinterpret_cast<const unsigned long long*>(sw + (kh * 7 + kw) * CCH + 2 * cp);
 #pragma unroll
-      for (int p = 0; p < PX; ++p) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[p]) : "l"(v[p + kw]), "l"(wv));
+      for (int p = 0; p < PX; ++p) fma_pair(acc[p], v[p + kw], wv);
     }
   }
   float a0[PX], a1[PX];
@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(512, 2) dwconv7_tiled_kernel(const uint16_t* _
 // ConvNeXt block head (convnext.py:43-45, 48): y = LN_C(dwconv7x7(x) + bias).  One CTA owns a TW x TH pixel tile and ALL C
 // channels of it: it walks the channels in chunks of 64, staging each chunk's (TW+6) x (TH+6) halo tile and its 49 x 64
 // filter taps with cp.async (double buffered: chunk k+1 streams in while chunk k is computed), computes the depthwise
-// outputs with packed FFMA2 (channel pairs) and parks them as bf16 in a [pixels][C] shared-memory buffer; a second phase
+// outputs as channel-pair FMAs (fma_pair) and parks them as bf16 in a [pixels][C] shared-memory buffer; a second phase
 // does the (two-pass, fp32) LayerNorm of every pixel from that buffer and writes full 128-byte lines.  The intermediate
 // map never exists in global memory and the two launches of the unfused path (uc_dwconv7 + uc_layernorm) become one.
 // The rounding points are the same as the unfused path (conv output rounded to bf16 before the LayerNorm).
@@ -369,7 +369,7 @@ __global__ void __launch_bounds__(NT) dwln_kernel(const uint16_t* __restrict__ x
       for (int kw = 0; kw < 7; ++kw) {
         const unsigned long long wv = *reinterpret_cast<const unsigned long long*>(sw + (kh * 7 + kw) * CCH + 2 * cp);
 #pragma unroll
-        for (int p = 0; p < PX; ++p) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[p]) : "l"(v[p + kw]), "l"(wv));
+        for (int p = 0; p < PX; ++p) fma_pair(acc[p], v[p + kw], wv);
       }
     }
 #pragma unroll
@@ -413,7 +413,7 @@ static bool launch_dwln(const void* x, const float* w49, const float* bias, cons
   const int smem = smem_fixed + TW * TH * C * 2;
   const int tiles_w = (W + TW - 1) / TW, tiles = tiles_w * ((H + TH - 1) / TH);
   if (smem > 227 * 1024) return false;
-  if (!force && static_cast<long>(tiles) * B < 100) return false;  // too few CTAs for 148 SMs: try a smaller tile
+  if (!force && static_cast<long>(tiles) * B < 100) return false;  // too few CTAs for the SMs: try a smaller tile
   static PerDeviceInt smem_dev;
   int& smem_set = smem_dev.get();
   auto kern = dwln_kernel<TW, TH, PX, NT>;

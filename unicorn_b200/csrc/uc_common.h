@@ -78,6 +78,14 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return __bfloat16_as_ushort(__float2bfloat16_rn(lo)) | (static_cast<uint32_t>(__bfloat16_as_ushort(__float2bfloat16_rn(hi))) << 16);
 }
 
+// acc += a * b on a pair of fp32 values packed in 64 bits (low word = first element)
+__device__ __forceinline__ void fma_pair(unsigned long long& acc, unsigned long long a, unsigned long long b) {
+  const float lo = fmaf(__uint_as_float(static_cast<uint32_t>(a)), __uint_as_float(static_cast<uint32_t>(b)), __uint_as_float(static_cast<uint32_t>(acc)));
+  const float hi = fmaf(__uint_as_float(static_cast<uint32_t>(a >> 32)), __uint_as_float(static_cast<uint32_t>(b >> 32)),
+                        __uint_as_float(static_cast<uint32_t>(acc >> 32)));
+  acc = (static_cast<unsigned long long>(__float_as_uint(hi)) << 32) | __float_as_uint(lo);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

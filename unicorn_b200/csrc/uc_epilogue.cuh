@@ -1,4 +1,4 @@
-// Epilogue arithmetic shared by the tcgen05 kernels (conv_gemm.cu, mlp_fused.cu): packed fp32 pairs, activations, 16-bit packing.
+// Epilogue arithmetic shared by the wgmma kernels (conv_gemm.cu, mlp_fused.cu): fp32 pairs, activations, 16-bit packing.
 #pragma once
 #include "uc_ptx.cuh"
 #include "uc_common.h"
@@ -11,23 +11,20 @@ __device__ __forceinline__ float fast_ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// ---- packed fp32 pairs (Blackwell FFMA2 / FMUL2 / FADD2): one issue slot per two elements
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-  return (static_cast<unsigned long long>(__float_as_uint(hi)) << 32) | __float_as_uint(lo);
-}
-__device__ __forceinline__ float lo2(f32x2 v) { return __uint_as_float(static_cast<uint32_t>(v)); }
-__device__ __forceinline__ float hi2(f32x2 v) { return __uint_as_float(static_cast<uint32_t>(v >> 32)); }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+// ---- fp32 pairs: the epilogues work on the (even, odd) column pairs a thread holds in a wgmma accumulator
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ float lo2(f32x2 v) { return v.x; }
+__device__ __forceinline__ float hi2(f32x2 v) { return v.y; }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float fast_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // exact (erf) GELU, nn.GELU(), as x * sigmoid(x * P(x^2)): P is the degree-4 least-squares fit of logit(Phi(x)) / x,
 // max |error| 3.3e-6 over the whole real line (tools/fit_gelu.py; the bf16 output ulp is >= 1.5e-5 wherever |y| > 4e-3,
-// and the fit saturates correctly: y -> x for x -> +inf, y -> -0 for x -> -inf).  Per PAIR of elements: 8 packed
-// FMA-pipe instructions + 2 x (ex2, rcp) — the earlier Abramowitz-Stegun form cost ~25 issue slots per element and the
-// epilogue, not the tensor pipe, set the pace of every pwconv1 (round-1 ncu source view; DESIGN.md 4.1 history).
+// and the fit saturates correctly: y -> x for x -> +inf, y -> -0 for x -> -inf).  Per element: 8 FMA-pipe instructions
+// + (ex2, rcp), about a third of the issue slots of an Abramowitz-Stegun erf.
 __device__ __forceinline__ f32x2 gelu2(f32x2 x) {
   // coefficients pre-multiplied by -log2(e): e = 2^(x * P'(x^2)) = exp(-q(x))
   const f32x2 c0 = pk2(-2.30204844f, -2.30204844f), c1 = pk2(-0.105217814f, -0.105217814f), c2 = pk2(3.54831049e-4f, 3.54831049e-4f),

@@ -1,5 +1,6 @@
-// Hand-written sm_100a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (TMEM alloc,
-// UMMA issue, commit, TMEM load).  No CUTLASS/CuTe is included anywhere in this library.
+// Hand-written sm_90a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors, fences, commit / wait
+// groups; the mma_async wrappers themselves are generated into uc_wgmma.cuh).  No CUTLASS/CuTe is included anywhere in
+// this library.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -7,6 +8,7 @@
 #include <cuda.h>
 #include <stdint.h>
 #include <stdio.h>
+#include "uc_wgmma.cuh"
 
 namespace uc {
 
@@ -15,8 +17,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 // One lane of a fully converged warp (CUTLASS' elect_one_sync): keeps the surrounding control flow warp-uniform so that
-// ptxas can keep descriptors / barrier addresses in uniform registers instead of wrapping every UTMALDG / UTCHMMA in
-// an ELECT + R2UR + BRA.U.ANY loop (which made the MMA issue rate, not the tensor pipe, the bottleneck).
+// ptxas can keep descriptors / barrier addresses in uniform registers instead of wrapping every UTMALDG in an
+// ELECT + R2UR + BRA.U.ANY loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -111,25 +113,9 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
+// every thread of every CTA of the cluster
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// cta_group::2 loads: executed by both CTAs of a pair; the transaction bytes are credited to the mbarrier of the leader
-// CTA (the CTA-rank bit of the shared::cluster barrier address is cleared, as CUTLASS' SM100_TMA_2SM_LOAD does).
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-      "[%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
 }
 // arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
@@ -151,121 +137,36 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
-// 256-bit global accesses (sm_100+): 32 bytes per lane = one full L2 sector
-__device__ __forceinline__ void stg_v8(void* p, const uint32_t* v) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
+// ---------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int K>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void ldg_v8(const void* p, uint32_t* v) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(p));
-}
+// warpgroup register re-allocation (every warp of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barrier over `count` threads (ids 1.. ; 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// pair (cta_group::2) allocation: issued by one warp in each CTA of the pair
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::f16 covers bf16 and fp16 operands with fp32 accumulation.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Pair MMA: D[256 x N] (+)= A[256 x 16] * B[N x 16]^T, issued by the leader CTA only.  Each CTA of the pair holds its own
-// 128 rows of A and N/2 rows of B at the same shared-memory offsets; rows 0..127 of D land in the leader's TMEM, rows
-// 128..255 in the peer's.
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of cta_mask (cluster-wide stage release)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major operand tile in shared memory, rows of 128 bytes, 128B swizzle (what a TMA box with a 128-byte
-// inner extent and CU_TENSOR_MAP_SWIZZLE_128B writes).  8-row groups are 1024 B apart (SBO); LBO is unused
-// for swizzled K-major layouts (encoded 1); descriptor version 1 (Blackwell); layout type 2 = SWIZZLE_128B.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major operand tile in shared memory, rows of 128 bytes, 128B swizzle (what a TMA box with a 128-byte inner extent and
+// CU_TENSOR_MAP_SWIZZLE_128B writes; the tile starts on a 1024-byte boundary).  8-row groups are 1024 B apart (SBO); LBO
+// is unused for swizzled K-major layouts (encoded 1); layout type 1 = SWIZZLE_128B.  The start address is in 16-byte
+// units, so a 16-element K step inside the 128-byte row is +2 and a row offset r (multiple of 8) is + 8 r.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-// Instruction descriptor for kind::f16: fp32 accumulate, A/B both K-major.  fmt: 0 = fp16, 1 = bf16.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 }  // namespace uc

@@ -1,7 +1,7 @@
-"""UnicornEngine — the per-frame inference hot path as a static sequence of sm_100a kernel launches.
+"""UnicornEngine — the per-frame inference hot path as a static sequence of sm_90a kernel launches.
 
 Host-side mirror of the reference model (unicorn/models/unicorn.py `Unicorn`, backbone/yolo_pafpn_new.py,
-backbone/convnext.py, deformable_transformer.py, unicorn_head.py) with a B200-first data layout:
+backbone/convnext.py, deformable_transformer.py, unicorn_head.py) with an H100-first data layout:
 
   * activations live in HBM as NHWC bf16 (channels contiguous): LayerNorm/Linear of ConvNeXt need no permutes and
     every convolution is an implicit GEMM whose A operand is fetched by TMA boxes straight from the NHWC map;
@@ -36,7 +36,7 @@ class _ConvGN:
 
 class UnicornEngine:
     def __init__(self, state_dict, cfg_name, device="cuda", autotune=True, ln_fold=None):
-        ops._lib.check(ops._lib.lib().uc_check_device(), "uc_check_device")  # fail loudly without an sm_100 GPU
+        ops._lib.check(ops._lib.lib().uc_check_device(), "uc_check_device")  # fail loudly without an sm_90 GPU
         self.cfg_name = cfg_name
         self.cfg = CONFIGS[cfg_name]
         self.dev = torch.device(device)
@@ -203,11 +203,11 @@ class UnicornEngine:
             kw2["gn_stats"] = torch.zeros(out.shape[0], gn, 2, dtype=torch.int64, device=self.dev)
         best, best_t, times = 0, None, []
         reps = 6
-        # objective: launch time discounted by the share of the SMs the launch occupies, t * (w + (1 - w) * min(CTAs, 148) / 148) with
+        # objective: launch time discounted by the share of the SMs the launch occupies, t * (w + (1 - w) * min(CTAs, SMs) / SMs) with
         # w = UC_TUNE_SMTIME_W (default 0.5; 1 = pure latency): with several frames in flight a launch on fewer CTAs leaves SMs to the other
-        # frames' kernels.  Measured on the SOT frame (profiles/r2_autotune_objective.txt): w = 1: 288 frames/s pipelined / 224 sequential,
-        # w = 0.5: 299 / 225, w = 0: 307 / 216 — 0.5 is the largest gain that costs no latency
+        # frames' kernels
         w_lat = float(os.environ.get("UC_TUNE_SMTIME_W", "0.5"))
+        sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
         m_tiles = -(-(out.shape[0] * out.shape[1] * out.shape[2]) // 128)
         for bn in cands:
             # timed as the frame runs it: back-to-back kernel nodes of a CUDA graph (stream launches of ~20 us kernels
@@ -233,7 +233,7 @@ class UnicornEngine:
             times.append((bn, round(t * 1e3, 1)))  # us per launch
             if w_lat < 1.0 and bn:
                 ctas = m_tiles * -(-Cout // (bn % 1000))
-                t = t * (w_lat + (1.0 - w_lat) * min(ctas, 148) / 148.0)
+                t = t * (w_lat + (1.0 - w_lat) * min(ctas, sms) / sms)
             if best_t is None or t < best_t * 0.97:  # require a 3 % win to leave the earlier (heuristic-first) choice
                 best, best_t = bn, t
         if os.environ.get("UC_TUNE_LOG"):
@@ -244,8 +244,9 @@ class UnicornEngine:
         return os.path.join(os.path.dirname(os.path.abspath(__file__)), "tuned", f"{self.cfg_name}.json")
 
     def load_tuning(self, path=None):
-        """Per-layer N-tile choices measured on a B200 and committed under unicorn_b200/tuned/ (plan-time autotuning
-        fills in whatever is missing).  Returns the number of entries loaded."""
+        """Per-layer N-tile choices committed under unicorn_b200/tuned/ (measured on an H100 80GB HBM3 at a 400 W power limit;
+        plan-time autotuning fills in whatever is missing).
+        Returns the number of entries loaded."""
         import glob
         import json
         if path is None and os.environ.get("UC_NO_TUNED"):
@@ -323,14 +324,12 @@ class UnicornEngine:
     def convnext_block(self, x, bp, tag):
         """In place on x (NHWC contiguous) — convnext.py:41-54."""
         B, H, W, C = x.shape
-        # two launches: the channel-chunked tiled depthwise kernel + a row LayerNorm on the L2-resident result.  The fused
-        # one-CTA-per-pixel-tile kernel (ops.dwconv7_ln) was measured slower on every stage of ConvNeXt-L (34.6 vs 28 us on
-        # stage 3: 2.3x the instructions per output, 8 warps per SM) — see DESIGN.md 4.3.
+        # two launches: the channel-chunked tiled depthwise kernel + a row LayerNorm on the L2-resident result (the fused
+        # one-CTA-per-pixel-tile kernel ops.dwconv7_ln needs 2.3x the instructions per output).
         # The 4C hidden map of the first stages is larger than what stays in L2 next to everything else (64000 x 768 x 2 B = 98 MB in
         # stage 1): pwconv1 -> pwconv2 pays an HBM round trip for it.  Running the pair per band of rows with ONE band-sized hidden
-        # buffer (rewritten by every band, so it never leaves L2) was MEASURED SLOWER — 243.8 vs 247.5 frames/s at 800x1280 and 89.7 vs
-        # 102.5 at 1536x2048 with 32 MB bands: four times the launches on a quarter of the rows cost more than the round trip saves
-        # (profiles/README.md) — so it is off by default (UC_MLP_BAND_MB = band size limit in MB enables it).
+        # buffer (rewritten by every band, so it stays in L2) quadruples the launches on a quarter of the rows each, so it is off by
+        # default (UC_MLP_BAND_MB = band size limit in MB enables it).
         band_mb = float(os.environ.get("UC_MLP_BAND_MB", "0"))
         nb = 1
         if band_mb > 0 and B == 1:
@@ -339,8 +338,7 @@ class UnicornEngine:
                 nb += 1
         hb = H // nb
         # fused back half (csrc/mlp_fused.cu): one CTA per 128 rows.  On the head's small levels (32 and 8 row tiles at 800x1280) the launch
-        # is slower than the three separate kernels in isolation (31 vs 22 us) but occupies a fifth of their SM-time, and the levels run on
-        # parallel streams next to two more frames in flight: fusing them too is +1.8 % frames/s (286 vs 281), so there is no size gate by default
+        # occupies few SMs but the levels run on parallel streams next to other frames in flight, so there is no size gate by default
         if bp.get("fused") and (C != 256 or B * H * W >= self.mlp_min_rows):
             if self.dw_mma:
                 t = ops.dwconv7_mma(x, bp["dwm"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())

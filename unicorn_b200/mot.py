@@ -1,4 +1,4 @@
-"""MOT per-frame driver on the B200 engine — the per-frame body of MOTEvaluator.evaluate_omni
+"""MOT per-frame driver on the H100 engine — the per-frame body of MOTEvaluator.evaluate_omni
 (unicorn/evaluators/mot_evaluator.py:985-1057): `model(imgs, mode="whole")` -> postprocess -> score filter ->
 interaction with the previous frame -> embedding upsample (current frame only) -> embedding sampling at the box
 centres -> QuasiDenseEmbedTracker.match; with `assoc="byte"` the association is BYTETracker.update on the NMS output

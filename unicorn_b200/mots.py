@@ -1,5 +1,5 @@
 """MOTS per-frame driver (UNTESTED ON A GPU — written after the round-1 GPU budget was spent; see tests/test_mots_gpu.py):
-the per-frame body of MOTEvaluator.evaluate_omni_mots (unicorn/evaluators/mot_evaluator.py:776-897) on the B200 engine:
+the per-frame body of MOTEvaluator.evaluate_omni_mots (unicorn/evaluators/mot_evaluator.py:776-897) on the H100 engine:
 whole-mode detector with the CondInst controllers -> NMS -> dynamic-conv masks of the kept detections -> embedding
 sampling -> QuasiDenseEmbedTracker.match(return_index=True) -> masks of the tracked boxes in ascending-id order,
 overlap free, area filter, RLE (results.mots_frame_result)."""

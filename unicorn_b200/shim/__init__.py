@@ -1,7 +1,7 @@
 """`unicorn`-importable API shim (SURVEY.md 8b "Python model API to keep"; north_star: "keeping the unicorn.models / unicorn.tracker
 Python API surface").  Put this directory FIRST on sys.path / PYTHONPATH and the reference's per-frame driver code
 (external/lib/test/tracker/unicorn_sot.py, unicorn_vos.py, the per-frame bodies of unicorn/evaluators/mot_evaluator.py) resolves its
-`unicorn.*` imports to the B200 path instead of the reference's PyTorch modules:
+`unicorn.*` imports to the H100 path instead of the reference's PyTorch modules:
 
     import unicorn_b200.shim as shim; shim.install()        # or: PYTHONPATH=<repo>/unicorn_b200/shim
     from unicorn.exp import get_exp

@@ -34,7 +34,7 @@ class Exp:
         self.model = None
 
     def get_model(self, load_pretrain=True):
-        """exp/unicorn_track.py:115-193.  Returns the B200 model shell; weights come from load_state_dict (there is no
+        """exp/unicorn_track.py:115-193.  Returns the H100 model shell; weights come from load_state_dict (there is no
         Unicorn_outputs/<pretrain>/best_ckpt.pth lookup: pass load_pretrain=False like the reference's inference drivers)."""
         if load_pretrain:
             raise RuntimeError("get_model(load_pretrain=True) would read a COCO-pretrained checkpoint for training; the inference "

@@ -1,4 +1,4 @@
-"""SOT per-frame driver on the B200 engine — mirrors external/lib/test/tracker/unicorn_sot.py
+"""SOT per-frame driver on the H100 engine — mirrors external/lib/test/tracker/unicorn_sot.py
 (UnicornSOTTrack.initialize :39-56, track :57-77, get_det_results :78-109, PreprocessorX :111-123,
 get_label_map :128-139) with the same initialize/track protocol (external/lib/test/tracker/basetracker.py:14-20).
 

@@ -1,10 +1,10 @@
-"""ByteTrack association on the B200 path — mirrors unicorn/tracker/byte_tracker.py (BYTETracker.update :161-296,
+"""ByteTrack association on the H100 path — mirrors unicorn/tracker/byte_tracker.py (BYTETracker.update :161-296,
 STrack :13-144), unicorn/tracker/matching.py (iou_distance :73-91, fuse_score :173-180, linear_assignment :39-50)
 and unicorn/tracker/kalman_filter.py (:23-269), with the same `BYTETracker(args).update(output_results, img_info,
 img_size)` entry point used by unicorn/evaluators/mot_evaluator.py:100-245 / tools/track.py.
 
 Differences in form, not in behaviour: the Kalman state of all tracks is one struct-of-arrays updated with batched
-numpy algebra; the IoU cost matrices come from the sm_100a kernel uc_box_iou (inclusive-pixel convention of
+numpy algebra; the IoU cost matrices come from the sm_90a kernel uc_box_iou (inclusive-pixel convention of
 cython_bbox); the assignment is the same extended-cost Jonker-Volgenant problem that `lap.lapjv(extend_cost=True,
 cost_limit=t)` solves, solved with scipy's linear_sum_assignment (lap is not installed offline — optimal cost is
 identical, tie-breaking between equal-cost optima is unpinned, see DESIGN.md §5)."""

@@ -1,9 +1,9 @@
-"""Quasi-dense embedding tracker on the B200 path — same constructor and `match` signature as the reference's
+"""Quasi-dense embedding tracker on the H100 path — same constructor and `match` signature as the reference's
 unicorn/tracker/quasi_dense_embed_tracker.py (QuasiDenseEmbedTracker.match :137-212, update_memo :47-102).
 
 Everything dense lives on the device: the tracklet memo (ids, boxes, embeddings, labels, last frame, velocity) and the backdrops are
 device tensors that never travel; the pairwise IoU matrices (duplicate removal, backdrop NMS), the bi-softmax embedding similarity
-E.M^T and the greedy row-max assignment with column zeroing (:188-199) are sm_100a kernels (uc_box_iou, uc_bisoftmax, uc_qd_assign).
+E.M^T and the greedy row-max assignment with column zeroing (:188-199) are sm_90a kernels (uc_box_iou, uc_bisoftmax, uc_qd_assign).
 The host keeps the bookkeeping only (which id sits in which memo row) and reads back one small tensor per frame: the assigned
 ids, which the caller needs anyway.  Inputs may be CPU or CUDA tensors; outputs come back on the device of `bboxes`, labels in the
 caller's dtype, like the reference (which only indexes what it is given)."""

@@ -1,9 +1,9 @@
-"""VOS per-frame driver on the B200 engine — mirrors external/lib/test/tracker/unicorn_vos.py: `initialize` :43-69, `track`
+"""VOS per-frame driver on the H100 engine — mirrors external/lib/test/tracker/unicorn_vos.py: `initialize` :43-69, `track`
 :71-127 (objects of the first frame, reference groups of objects that appear later :79-84, :86-98, soft aggregation + argmax
 :105-121), `get_mask_results` :129-155 (best instance per object, mask resized to the original frame), `get_det_results`
 :157-201 (interaction, correlation, per-object prior pyramid -> mask head -> postprocess_inst).
 
-B200 restructuring, same results: one backbone pass and one mask-branch pass per frame (the reference recomputes the mask branch
+H100 restructuring, same results: one backbone pass and one mask-branch pass per frame (the reference recomputes the mask branch
 inside the head for every object); per reference group ONE fused correlation launch propagates the label maps of all its
 objects (the 16000^2 similarity matrix never exists); the resize to the original frame, the float32 background product and the
 argmax run in one kernel on the device (uc_vos_aggregate); the only per-frame host traffic is the frame in, the label map and the
