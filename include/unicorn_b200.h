@@ -62,9 +62,9 @@ UC_API int uc_check_device(void);
  *   w : packed weights [Cout][KH*KW][Cin] in the same 16-bit type as x (K-major)
  *   y : NHWC output, pixel stride ldy, dtype y_dtype; y = act(conv(x) + bias) ; then y = res + gamma * y if given
  * A Linear layer on [M, Cin] rows is B=1, H=1, W=M, KH=KW=1.  stride in {1,2}; pad < KH.
- * Cin % 8 == 0, Cout % 8 == 0 (pad the weight rows / output channels otherwise).  Outputs (and residuals) whose rows start on
- * 32-byte boundaries (ldy * sizeof % 32 == 0, y % 32 == 0) are written with one 256-bit store per 16 channels; other
- * layouts fall back to 128-bit stores.  Every launch is CUDA-graph capturable and uses programmatic dependent launch.
+ * Cin % 8 == 0, Cout % 8 == 0 (pad the weight rows / output channels otherwise).  The epilogue stores from the accumulator
+ * registers: each lane writes 32 bits (two 16-bit channels; 64 bits for fp32 y) per row and 8-channel chunk, and reads the
+ * residual the same way.  Every launch is CUDA-graph capturable and uses programmatic dependent launch.
  */
 typedef struct UcConv2d {
   const void* x;

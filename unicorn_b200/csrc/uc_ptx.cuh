@@ -57,17 +57,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (error surfaces as a CUDA launch failure) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (error surfaces as a CUDA launch failure) instead of hanging the GPU.  No printf here:
+// a function call (vprintf) between wgmma instructions makes ptxas serialize every wgmma of the kernel (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3FF) == 0 && (clock64() - t0) > 4000000000LL) {
-      printf("uc: mbarrier wait timeout block (%d,%d,%d) thread %d parity %u\n", blockIdx.x, blockIdx.y, blockIdx.z,
-             threadIdx.x, parity);
-      __trap();
-    }
+    if ((++spins & 0x3FF) == 0 && (clock64() - t0) > 4000000000LL) __trap();
   }
 }
 
