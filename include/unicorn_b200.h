@@ -14,6 +14,7 @@
  *                          backbone/convnext.py:41-54,82-87; network_blocks.py:50-51; unicorn.py:36-44;
  *                          unicorn_head.py:267-336; ops/modules/ms_deform_attn.py:94-113
  *   uc_stem_ln             backbone/convnext.py:77-80 (conv4x4s4 + channels_first LayerNorm)
+ *   uc_resnet_stem         backbone/resnet.py:148-152,209-212 (conv7x7s2 + BatchNorm + ReLU + maxpool3x3s2)
  *   uc_dwconv7_ln          backbone/convnext.py:43-45 (dwconv 7x7 + LayerNorm)
  *   uc_layernorm           backbone/convnext.py:176-184; deformable_transformer.py:113,121
  *   uc_groupnorm_*         GroupNorm(16,eps 1e-3) from exp/unicorn_track.py:450-470; unicorn.py:38
@@ -61,6 +62,7 @@ UC_API int uc_check_device(void);
  *   x : NHWC activations, 16-bit (bf16 or f16 per x_dtype), pixel stride ldx elements (ldx >= Cin, ldx % 8 == 0)
  *   w : packed weights [Cout][KH*KW][Cin] in the same 16-bit type as x (K-major)
  *   y : NHWC output, pixel stride ldy, dtype y_dtype; y = act(conv(x) + bias) ; then y = res + gamma * y if given
+ *       (act_after_res: y = relu(conv(x) + bias + res))
  * A Linear layer on [M, Cin] rows is B=1, H=1, W=M, KH=KW=1.  stride in {1,2}; pad < KH.
  * Cin % 8 == 0, Cout % 8 == 0 (pad the weight rows / output channels otherwise).  The epilogue stores from the accumulator
  * registers: each lane writes 32 bits (two 16-bit channels; 64 bits for fp32 y) per row and 8-channel chunk, and reads the
@@ -93,6 +95,10 @@ typedef struct UcConv2d {
   const void* row_stats;
   const float* col_s;
   float row_eps;
+  /* 1 = the activation comes after the residual: y = relu(conv(x) + bias + res) (ResNet Bottleneck, resnet.py:115-122: bn3 folded
+   * into w / bias, identity added, then ReLU).  Needs act = UC_ACT_RELU, res and bf16 x; rejected (UC_EINVAL) otherwise and with
+   * gamma, gn_stats or row_stats.  0 = as above. */
+  int act_after_res;
 } UcConv2d;
 UC_API int uc_conv2d(const UcConv2d* d, void* stream);
 
@@ -102,6 +108,16 @@ UC_API int uc_conv2d(const UcConv2d* d, void* stream);
  * w48 fp32 [48][C0] with k=(ci*4+kh)*4+kw; out NHWC bf16 [B,H/4,W/4,C0]. */
 UC_API int uc_stem_ln(const void* img, int img_is_u8_hwc, const float* w48, const float* bias, const float* lnw, const float* lnb,
                       void* out_bf16, int B, int H, int W, int C0, float eps, void* stream);
+
+/* ResNet-50 stem in ONE launch (backbone/resnet.py:148-152,209-212): conv 7x7 stride 2 pad 3 (3 -> 64) with the eval-mode
+ * BatchNorm folded into the weights and bias, ReLU, max-pool 3x3 stride 2 pad 1.  The H/2 x W/2 x 64 map before the pool stays in
+ * shared memory; only the pooled map is written.  The conv runs on tensor cores (mma.sync m16n8k16, fp16 operands, fp32 accumulate):
+ * the 0-255 integer pixels are exact in fp16, so the only roundings are those of the folded weights (fp16: 11-bit significand, 8x finer
+ * than bf16) and of the bf16 output.  img: fp32 NCHW [B,3,H,W] or, with img_is_u8_hwc = 1, the uint8 HWC BGR frame [B,H,W,3] (same
+ * forms as uc_stem_ln); w_f16 [64][160] fp16, k = ci*49 + kh*7 + kw, zero for k >= 147 (unicorn_b200.ops.pack_resnet_stem_weight);
+ * bias fp32 [64]; out NHWC bf16 [B,H/4,W/4,64], 16-byte aligned.  H % 4 == 0, W % 4 == 0. */
+UC_API int uc_resnet_stem(const void* img, int img_is_u8_hwc, const void* w_f16, const float* bias, void* out_bf16, int B, int H, int W,
+                          void* stream);
 
 /* ConvNeXt block front half in ONE launch: depthwise 7x7 (pad 3)+bias then LayerNorm over C (convnext.py:43-45); the
  * intermediate map stays in shared memory (C % 64 == 0; other C use a one-warp-row kernel).  Not in place.  The engine uses

@@ -1,0 +1,20 @@
+"""Dump the state_dict key->shape manifests of the ResNet-50 tracking models from the reference (build container only), like
+make_manifests.py does for the ConvNeXt configs.  They pin unicorn_b200.weights.param_shapes() for unicorn_track_r50{,_mask}."""
+import json
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(HERE)), "oracle"))
+sys.path.insert(0, HERE)
+import ref_import  # noqa: E402
+from make_golden_r50 import install_offline_resnet  # noqa: E402
+
+install_offline_resnet()
+for name in ("unicorn_track_r50", "unicorn_track_r50_mask"):
+    _, m = ref_import.get_model(name)
+    sd = m.state_dict()
+    man = {k: list(v.shape) for k, v in sd.items()}
+    with open(os.path.join(HERE, f"manifest_{name}.json"), "w") as f:
+        json.dump(man, f, indent=0, sort_keys=False)
+    print(name, len(man), sum(v.numel() for v in sd.values()) / 1e6, "M")

@@ -4,7 +4,10 @@
         (b) ByteTrack association on 100 synthetic objects per frame (random weights give few detections of their own).
   vos : configs[3] — ConvNeXt-L + CondInst mask head at 800x1280, n objects propagated from the first frame.
 Eager launches (no CUDA graph: the association step returns to the host every frame), wall clock around synchronised
-steps, synthetic video, seeded weights.  usage: bench_workloads.py mot|vos [frames]"""
+steps, synthetic video, seeded weights.
+  r50 : the SOT frame at 800x1280 of unicorn_track_r50 and, in the same process for comparison, of unicorn_track_large: CUDA graphs,
+        one frame and three frames in flight, three alternating rounds.
+usage: bench_workloads.py mot|vos|r50 [frames]"""
 import json, os, sys, time, types
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -75,6 +78,39 @@ if what == "mot":
     fps2, ms2, l2 = timed(lambda i: bt.update(dets100[i][0].numpy(), (H, W), (H, W)), n)
     print(json.dumps({"workload": "configs[2] ByteTrack update alone, 100 synthetic objects per frame (host Kalman + LAP, IoU on the GPU)",
                       "frames_per_s": round(fps2, 1), "ms_per_frame": round(ms2, 3), "kernels_per_frame": l2}))
+elif what == "r50":
+    import subprocess
+    from unicorn_b200.sot import UnicornSOTTrack
+    H, W = 800, 1280
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}))
+    frames, boxes = make_video(4, H, W, seed=0)
+    frames = [f[None].pin_memory() for f in frames]
+    trackers = {}
+    for cfg in ("unicorn_track_r50", "unicorn_track_large"):
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        for depth in (1, 3):
+            trk = UnicornSOTTrack(eng, (H, W), depth=depth)
+            trk.initialize_tensor(frames[0], boxes[0, 0])
+            trackers[cfg, depth] = trk
+
+    def in_flight(trk):
+        def step(i):
+            if trk.depth == 1:
+                trk.track_tensor(frames[1 + i % 3])
+                return
+            if trk._submitted - trk._collected == trk.depth:
+                trk.collect()
+            trk.submit(frames[1 + i % 3])
+        return step
+
+    for rnd in range(3):
+        for (cfg, depth), trk in trackers.items():
+            fps, ms, launches = timed(in_flight(trk), n, warm=6)
+            while trk._collected < trk._submitted:
+                trk.collect()
+            print(json.dumps({"workload": f"SOT 800x1280 {cfg}, CUDA graphs, {depth} frame(s) in flight", "round": rnd,
+                              "frames_per_s": round(fps, 2), "ms_per_frame": round(ms, 2), "kernels_per_frame": launches, "n_gpus": 1}))
 else:
     from unicorn_b200.vos import UnicornVOSTrack
     H, W = 800, 1280

@@ -75,7 +75,7 @@ if len(ck) != len(trace):
 else:
     agg, mism = {}, 0
     for e, t in zip(ck, trace):
-        bn, _, _, cl = [v.strip() for v in re.search(r"conv_gemm_kernel<([^>]*)>", e.name).group(1).split(",")]
+        bn, _, _, cl = [v.strip() for v in re.search(r"conv_gemm_kernel<([^>]*)>", e.name).group(1).split(",")][:4]
         code = int(bn) + (1000 if cl == "2" else 0)
         mism += bool(t["bn"]) and t["bn"] != code
         key = (t["M"], t["N"], t["K"], t["k"], t["s"], code, t["act"], t["gn"])

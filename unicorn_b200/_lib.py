@@ -25,6 +25,7 @@ class UcConv2d(ctypes.Structure):
         ("block_n", ctypes.c_int),
         ("gn_stats", ctypes.c_void_p), ("gn_groups", ctypes.c_int),
         ("row_stats", ctypes.c_void_p), ("col_s", ctypes.c_void_p), ("row_eps", ctypes.c_float),
+        ("act_after_res", ctypes.c_int),
     ]
 
 

@@ -64,7 +64,9 @@ struct alignas(64) ConvKernelParams {
 
 // Persistent kernel: grid = min(#tiles, SMs); every CTA (pair) walks work items item = blockIdx.x / CLUSTER + i * gridDim.x / CLUSTER
 // (N tile fastest, so CTAs running side by side share the activation tile in L2); item = (N tile, group of CLUSTER M tiles).
-template <int BLOCK_N, int STAGES, bool F16, int CLUSTER>
+// RELU_RES: y = relu(acc + bias + res) (ResNet Bottleneck; p.act is NONE).  A template parameter rather than a runtime flag: a branch
+// in the unrolled epilogue grows every instantiation's code and measurably slows layers that never use it.
+template <int BLOCK_N, int STAGES, bool F16, int CLUSTER, bool RELU_RES = false>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
   constexpr int B_BYTES = BLOCK_N * kBlockK * 2;
   constexpr int NACC = BLOCK_N / 2;  // accumulator registers per thread: m64 x BLOCK_N over 128 threads
@@ -262,6 +264,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             const uint32_t rw = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.res) + pix[h] * p.ldres + cbase));
             hv[h] = add2(hv[h], f16o ? pk2(bits16_to_float(rw & 0xffffu, UC_F16), bits16_to_float(rw >> 16, UC_F16)) : pk2(bf16lo(rw), bf16hi(rw)));
           }
+          if (RELU_RES) hv[h] = pk2(fmaxf(lo2(hv[h]), 0.f), fmaxf(hi2(hv[h]), 0.f));
           if (p.y_dtype == UC_F32) {
             *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + pix[h] * p.ldy + cbase) = hv[h];
           } else {
@@ -293,14 +296,17 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 
 // ------------------------------------------------------------------------------------------- host side
 
-template <int BLOCK_N, int STAGES, int CLUSTER>
+template <int BLOCK_N, int STAGES, int CLUSTER, bool RELU_RES>
 static int launch_conv(ConvKernelParams& p, bool f16, cudaStream_t stream) {
   constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2) + 1024 + 256 + kGnSmemBytes;
   static PerDeviceFlag attr_dev;
   bool& attr = attr_dev.get();
-  auto kern = f16 ? conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER> : conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>;
+  // the ReLU-after-residual variant exists for bf16 operands only (uc_conv2d rejects f16 x with act_after_res)
+  auto kern = RELU_RES ? conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER, true>
+                       : f16 ? conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER> : conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>;
   if (!attr) {
-    for (auto k : {conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER>, conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>}) {
+    for (auto k : {conv_gemm_kernel<BLOCK_N, STAGES, true, CLUSTER>, conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER>,
+                   conv_gemm_kernel<BLOCK_N, STAGES, false, CLUSTER, RELU_RES>}) {
       cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e != cudaSuccess) return set_error(static_cast<int>(e), "conv_gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
@@ -333,6 +339,28 @@ static int launch_conv(ConvKernelParams& p, bool f16, cudaStream_t stream) {
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
   if (e != cudaSuccess) return set_error(static_cast<int>(e), "conv_gemm<%d,%d,%d> launch: %s", BLOCK_N, STAGES, CLUSTER, cudaGetErrorString(e));
   return UC_OK;
+}
+
+template <bool RELU_RES>
+static int launch_block_n(ConvKernelParams& p, int bn, bool cluster2, bool f16, cudaStream_t stream) {
+  if (cluster2) {
+    switch (bn) {
+      case 256: return launch_conv<256, 4, 2, RELU_RES>(p, f16, stream);
+      case 192: return launch_conv<192, 5, 2, RELU_RES>(p, f16, stream);
+      case 128: return launch_conv<128, 6, 2, RELU_RES>(p, f16, stream);
+      default: return set_error(UC_EINVAL, "uc_conv2d: the cluster variant exists for block_n 128/192/256 only");
+    }
+  }
+  switch (bn) {  // stage rings of 144 - 200 KB (227 KB of shared memory per block)
+    case 256: return launch_conv<256, 4, 1, RELU_RES>(p, f16, stream);
+    case 192: return launch_conv<192, 5, 1, RELU_RES>(p, f16, stream);
+    case 128: return launch_conv<128, 6, 1, RELU_RES>(p, f16, stream);
+    case 96: return launch_conv<96, 6, 1, RELU_RES>(p, f16, stream);
+    case 64: return launch_conv<64, 8, 1, RELU_RES>(p, f16, stream);
+    case 32: return launch_conv<32, 8, 1, RELU_RES>(p, f16, stream);
+    case 16: return launch_conv<16, 8, 1, RELU_RES>(p, f16, stream);
+    default: return set_error(UC_EINVAL, "uc_conv2d: unsupported block_n %d", bn);
+  }
 }
 
 static int pick_block_n(int Cout, int m_tiles, int gn_gs) {
@@ -375,6 +403,8 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     return set_error(UC_EINVAL, "uc_conv2d: pointers must be 16-byte aligned");
   if (d->gn_stats && (d->gn_groups <= 0 || d->Cout % d->gn_groups))
     return set_error(UC_EINVAL, "uc_conv2d: bad GroupNorm grouping");
+  if (d->act_after_res && (d->act != UC_ACT_RELU || !d->res || d->x_dtype != UC_BF16 || d->gamma || d->gn_stats || d->row_stats))
+    return set_error(UC_EINVAL, "uc_conv2d: act_after_res needs act = ReLU, res and bf16 x, and excludes gamma, gn_stats and row_stats");
   int rc = ensure_driver();
   if (rc) return rc;
 
@@ -452,7 +482,7 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   }
   p.Cout = d->Cout;
   p.bias = d->bias; p.gamma = d->gamma; p.res = d->res; p.ldres = d->ldres;
-  p.y = d->y; p.ldy = d->ldy; p.y_dtype = d->y_dtype; p.act = d->act;
+  p.y = d->y; p.ldy = d->ldy; p.y_dtype = d->y_dtype; p.act = d->act_after_res ? UC_ACT_NONE : d->act;
   p.row_stats = static_cast<const long long*>(d->row_stats); p.col_s = d->col_s; p.row_inv = 1.f / (kGnFixedScale * static_cast<float>(d->Cin)); p.row_eps = d->row_eps;
   if (d->row_stats && (!d->col_s || d->KH != 1 || d->KW != 1 || d->stride != 1 || d->pad != 0))
     return set_error(UC_EINVAL, "uc_conv2d: row_stats (folded LayerNorm) needs a 1x1 stride-1 conv and col_s");
@@ -469,21 +499,6 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     uint32_t box[3] = {static_cast<uint32_t>(kBlockK), 1, static_cast<uint32_t>(bn / 2)};
     rc = encode_tmap(&p.tmBh, dt, 3, d->w, dims, strides, box);
     if (rc) return rc;
-    switch (bn) {
-      case 256: return launch_conv<256, 4, 2>(p, f16, stream);
-      case 192: return launch_conv<192, 5, 2>(p, f16, stream);
-      case 128: return launch_conv<128, 6, 2>(p, f16, stream);
-      default: return set_error(UC_EINVAL, "uc_conv2d: the cluster variant exists for block_n 128/192/256 only");
-    }
   }
-  switch (bn) {  // stage rings of 144 - 200 KB (227 KB of shared memory per block)
-    case 256: return launch_conv<256, 4, 1>(p, f16, stream);
-    case 192: return launch_conv<192, 5, 1>(p, f16, stream);
-    case 128: return launch_conv<128, 6, 1>(p, f16, stream);
-    case 96: return launch_conv<96, 6, 1>(p, f16, stream);
-    case 64: return launch_conv<64, 8, 1>(p, f16, stream);
-    case 32: return launch_conv<32, 8, 1>(p, f16, stream);
-    case 16: return launch_conv<16, 8, 1>(p, f16, stream);
-    default: return set_error(UC_EINVAL, "uc_conv2d: unsupported block_n %d", bn);
-  }
+  return d->act_after_res ? launch_block_n<true>(p, bn, cluster2, f16, stream) : launch_block_n<false>(p, bn, cluster2, f16, stream);
 }

@@ -19,7 +19,7 @@ import os
 import torch
 
 from . import ops
-from .weights import CONFIGS
+from .weights import CONFIGS, fold_bn
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = ops.ACT_NONE, ops.ACT_RELU, ops.ACT_GELU, ops.ACT_SILU
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
@@ -41,6 +41,7 @@ class UnicornEngine:
         self.cfg = CONFIGS[cfg_name]
         self.dev = torch.device(device)
         self.dims = self.cfg["dims"]
+        self.inc = self.cfg["in_channels"]  # channels of the s8 / s16 / s32 backbone outputs
         self.depths = self.cfg["depths"]
         self.ncls = self.cfg["num_classes"]
         self._bufs = {}
@@ -86,12 +87,6 @@ class UnicornEngine:
         pw = lambda k: ops.pack_conv_weight(sd[k].to(dev, F32))  # noqa: E731
         P = {}
         b = "backbone.backbone."
-        P["stem"] = (ops.pack_stem_weight(sd[b + "downsample_layers.0.0.weight"].to(dev)), f(b + "downsample_layers.0.0.bias"),
-                     f(b + "downsample_layers.0.1.weight"), f(b + "downsample_layers.0.1.bias"))
-        for i in range(1, 4):
-            P[f"down{i}"] = (f(b + f"downsample_layers.{i}.0.weight"), f(b + f"downsample_layers.{i}.0.bias"),
-                             pw(b + f"downsample_layers.{i}.1.weight"), f(b + f"downsample_layers.{i}.1.bias"))
-            P[f"outnorm{i}"] = (f(b + f"norm{i}.weight"), f(b + f"norm{i}.bias"))
 
         def block(p):
             d = dict(dw=ops.pack_dw_weight(sd[p + "dwconv.weight"].to(dev)), dwm=ops.pack_dw_weight_mma(sd[p + "dwconv.weight"].to(dev), sd[p + "dwconv.bias"].to(dev)), dwb=f(p + "dwconv.bias"), lnw=f(p + "norm.weight"),
@@ -105,7 +100,10 @@ class UnicornEngine:
                 d["c1"] = (w1 @ d["lnb"] + d["b1"]).contiguous()
             return d
 
-        P["stages"] = [[block(b + f"stages.{i}.{j}.") for j in range(self.depths[i])] for i in range(4)]
+        if self.cfg["backbone"] == "resnet50":
+            self._load_resnet(sd, P, b)
+        else:
+            self._load_convnext(sd, P, b, f, pw, block)
 
         def cgn(p, k, stride=1):
             return _ConvGN(pw(p + "conv.weight"), f(p + "bn.weight"), f(p + "bn.bias"), k, stride)
@@ -166,6 +164,39 @@ class UnicornEngine:
                              up2=(pw(mb + "up_mask_layer.2.weight"), f(mb + "up_mask_layer.2.bias")))
         self.P = P
 
+    def _load_convnext(self, sd, P, b, f, pw, block):
+        dev = self.dev
+        P["stem"] = (ops.pack_stem_weight(sd[b + "downsample_layers.0.0.weight"].to(dev)), f(b + "downsample_layers.0.0.bias"),
+                     f(b + "downsample_layers.0.1.weight"), f(b + "downsample_layers.0.1.bias"))
+        for i in range(1, 4):
+            P[f"down{i}"] = (f(b + f"downsample_layers.{i}.0.weight"), f(b + f"downsample_layers.{i}.0.bias"),
+                             pw(b + f"downsample_layers.{i}.1.weight"), f(b + f"downsample_layers.{i}.1.bias"))
+            P[f"outnorm{i}"] = (f(b + f"norm{i}.weight"), f(b + f"norm{i}.bias"))
+        P["stages"] = [[block(b + f"stages.{i}.{j}.") for j in range(self.depths[i])] for i in range(4)]
+
+    def _load_resnet(self, sd, P, b):
+        """ResNet-50 (backbone/resnet.py) with every eval-mode BatchNorm folded into its conv (fp32 fold, then one rounding to 16 bits)."""
+        dev = self.dev
+        sd = {k: v.to(dev) for k, v in sd.items() if k.startswith(b)}
+
+        def cb(conv, bn):
+            w, bias = fold_bn(sd[conv].to(F32), sd, bn)
+            return ops.pack_conv_weight(w), bias.contiguous()
+
+        w, bias = fold_bn(sd[b + "conv1.weight"].to(F32), sd, b + "bn1.")
+        P["rstem"] = (ops.pack_resnet_stem_weight(w), bias.contiguous())
+        P["layers"] = []
+        for i, n in enumerate(self.depths):
+            blocks = []
+            for j in range(n):
+                q = b + f"layer{i + 1}.{j}."
+                d = dict(c1=cb(q + "conv1.weight", q + "bn1."), c2=cb(q + "conv2.weight", q + "bn2."), c3=cb(q + "conv3.weight", q + "bn3."),
+                         stride=2 if i > 0 and j == 0 else 1)
+                if j == 0:
+                    d["ds"] = cb(q + "downsample.0.weight", q + "downsample.1.")
+                blocks.append(d)
+            P["layers"].append(blocks)
+
     # ------------------------------------------------------------------------------------------ buffers
     def buf(self, name, shape, dtype=BF16, zero=False):
         key = (name, tuple(shape), dtype)
@@ -182,7 +213,8 @@ class UnicornEngine:
         B, H, W, Cin = x.shape
         Cout = w.shape[0]
         gn = kw.get("gn_groups", 0)
-        key = (B, H, W, Cin, Cout, k, stride, pad, kw.get("act", 0), gn, kw.get("res") is not None, out.dtype) + (("lnfold",) if kw.get("row_stats") is not None else ())
+        res_key = "act_after_res" if kw.get("act_after_res") else kw.get("res") is not None  # residual field: none / res + act(y) / act(y + res)
+        key = (B, H, W, Cin, Cout, k, stride, pad, kw.get("act", 0), gn, res_key, out.dtype) + (("lnfold",) if kw.get("row_stats") is not None else ())
         key = "|".join(str(v) for v in key)
         bn = self._bn_cache.get(key)
         if bn is None:
@@ -397,9 +429,9 @@ class UnicornEngine:
         return fpn, seq, side_out
 
     def features(self, img, tag="cur"):
-        """img fp32 NCHW [1,3,H,W] -> (fpn_outs (p3,p4,p5) NHWC bf16, seq_dict{feat NHWC view, h, w}).
-        ConvNeXt.forward_features (convnext.py:141-154) + YOLOPAFPNNEW.forward (yolo_pafpn_new.py:137-155)."""
-        P, d = self.P, self.dims
+        """img fp32 NCHW [1,3,H,W] (or uint8 HWC BGR [1,H,W,3]) -> (backbone outputs (s8, s16, s32) NHWC bf16, seq_dict{feat NHWC view, h, w}).
+        The s8 / s16 outputs are written straight into their slots of the neck's concat buffers (yolo_pafpn_new.py:137-155)."""
+        inc = self.inc
         if img.dtype == torch.uint8:  # HWC BGR frame straight from the decoder / cv2.resize
             B, H, W, _ = img.shape
         else:
@@ -407,12 +439,23 @@ class UnicornEngine:
         assert B == 1 and H % 32 == 0 and W % 32 == 0
         h8, w8, h16, w16, h32, w32 = H // 8, W // 8, H // 16, W // 16, H // 32, W // 32
         # concat buffers of the neck (producers write into slices)
-        cat_p4 = self.buf(tag + ".cat_p4", (1, h16, w16, 2 * d[2]))
-        cat_p3 = self.buf(tag + ".cat_p3", (1, h8, w8, 2 * d[1]))
-        cat_n3 = self.buf(tag + ".cat_n3", (1, h16, w16, 2 * d[1]))
-        cat_n4 = self.buf(tag + ".cat_n4", (1, h32, w32, 2 * d[2]))
+        cat_p4 = self.buf(tag + ".cat_p4", (1, h16, w16, 2 * inc[1]))
+        cat_p3 = self.buf(tag + ".cat_p3", (1, h8, w8, 2 * inc[0]))
+        cat_n3 = self.buf(tag + ".cat_n3", (1, h16, w16, 2 * inc[0]))
+        cat_n4 = self.buf(tag + ".cat_n4", (1, h32, w32, 2 * inc[1]))
+        dst = (cat_p3[..., inc[0]:], cat_p4[..., inc[1]:], self.buf(tag + ".x0n", (1, h32, w32, inc[2])))
+        if self.cfg["backbone"] == "resnet50":
+            x = ops.resnet_stem(img, *self.P["rstem"], out=self.buf(tag + ".rstem", (1, H // 4, W // 4, 64)))
+            self._resnet_layers(x, dst, tag)
+        else:
+            self._convnext_features(img, dst, tag)
+        self._cat = dict(cat_p4=cat_p4, cat_p3=cat_p3, cat_n3=cat_n3, cat_n4=cat_n4)
+        return dst, {"feat": dst[1], "h": h16, "w": w16}
+
+    def _convnext_features(self, img, dst, tag):
+        """ConvNeXt.forward_features (convnext.py:141-154): stages 1-3 through their out-norms into dst."""
+        P, d = self.P, self.dims
         x = ops.stem_ln(img, *P["stem"])
-        feats = {}
         for i in range(4):
             if i > 0:
                 lw, lb, cw, cb = P[f"down{i}"]
@@ -424,16 +467,40 @@ class UnicornEngine:
             if i >= 1:
                 nw, nb = P[f"outnorm{i}"]
                 Bx, Hx, Wx, Cx = x.shape
-                dst = {1: cat_p3[..., d[1]:], 2: cat_p4[..., d[2]:], 3: self.buf(tag + ".x0n", (1, h32, w32, d[3]))}[i]
-                ops.layernorm(x.view(-1, Cx), nw, nb, 1e-6, out=_rows(dst))
-                feats[i] = dst
-        self._cat = dict(cat_p4=cat_p4, cat_p3=cat_p3, cat_n3=cat_n3, cat_n4=cat_n4)
-        return (feats[1], feats[2], feats[3]), {"feat": feats[2], "h": h16, "w": w16}
+                ops.layernorm(x.view(-1, Cx), nw, nb, 1e-6, out=_rows(dst[i - 1]))
+
+    def _resnet_layers(self, x, dst, tag):
+        """ResNet._forward_impl after the stem (backbone/resnet.py:214-224): layer1..4; the last Bottleneck of layer2/3/4 writes into
+        dst.  Within a layer the blocks update one buffer in place (the residual is read by the thread that overwrites it)."""
+        P = self.P
+        for i, blocks in enumerate(P["layers"]):
+            for j, bp in enumerate(blocks):
+                last = j == len(blocks) - 1
+                x = self.bottleneck(x, bp, dst[i - 1] if last and i > 0 else None, f"{tag}.l{i}")
+
+    def bottleneck(self, x, bp, out, tag):
+        """Bottleneck.forward (backbone/resnet.py:104-124) with folded BatchNorms: relu(conv1) -> relu(conv2, stride) -> conv3, + identity
+        (or the folded downsample conv), then ReLU in conv3's epilogue.  out=None: the layer's buffer (in place after block 0)."""
+        B, H, W, _ = x.shape
+        s = bp["stride"]
+        (w1, b1), (w2, b2), (w3, b3) = bp["c1"], bp["c2"], bp["c3"]
+        wd = w1.shape[0]
+        Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+        t1 = self.conv(x, w1, 1, bias=b1, act=ACT_RELU, out=self.buf(tag + ".t1", (B, H, W, wd)))
+        t2 = self.conv(t1, w2, 3, s, 1, bias=b2, act=ACT_RELU, out=self.buf(tag + ".t2", (B, Ho, Wo, wd)))
+        if "ds" in bp:
+            wds, bds = bp["ds"]
+            idt = self.conv(x, wds, 1, s, 0, bias=bds, out=self.buf(tag + ".x", (B, Ho, Wo, wds.shape[0])))
+        else:
+            idt = x
+        if out is None:
+            out = idt
+        return self.conv(t2, w3, 1, bias=b3, act=ACT_RELU, res=idt, act_after_res=True, out=out)
 
     def neck(self, feats, tag="cur"):
-        """YOLOPAFPNNEW.forward (yolo_pafpn_new.py:137-155) on the normed ConvNeXt outputs (already sitting in their
-        concat slots)."""
-        P, d = self.P, self.dims
+        """YOLOPAFPNNEW.forward (yolo_pafpn_new.py:137-155) on the backbone outputs (already sitting in their concat slots);
+        d[1..3] = in_channels."""
+        P, d = self.P, (None,) + tuple(self.inc)
         x2n, x1n, x0n = feats
         cat_p4, cat_p3, cat_n3, cat_n4 = (self._cat[k] for k in ("cat_p4", "cat_p3", "cat_n3", "cat_n4"))
         h8, w8 = x2n.shape[1:3]

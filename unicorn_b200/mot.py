@@ -62,7 +62,7 @@ class UnicornMOTTracker:
         self.collected = 0      # frames associated
         # pre_dict of the reference loop (mot_evaluator.py:1014-1020): the s16 feature of the last frame THAT HAD DETECTIONS, kept in
         # its own buffer and updated by a device-side conditional copy (no host decision inside the frame)
-        self._prev_feat = torch.zeros(1, H // 16, W // 16, engine.dims[2], dtype=torch.bfloat16, device=dev)
+        self._prev_feat = torch.zeros(1, H // 16, W // 16, engine.inc[1], dtype=torch.bfloat16, device=dev)
         self._has_prev = torch.zeros(1, dtype=torch.int32, device=dev)
         self._warned = False
         # two pinned result slots: at most one frame is in flight behind the one being associated

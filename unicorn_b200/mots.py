@@ -26,7 +26,7 @@ class UnicornMOTSTracker:
         self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=engine.dev)
         self.feats = torch.zeros(max_dets, 128, dtype=torch.float32, device=engine.dev)
         self.frame_id = 0
-        self._prev_feat = torch.zeros(1, H // 16, W // 16, engine.dims[2], dtype=torch.bfloat16, device=engine.dev)
+        self._prev_feat = torch.zeros(1, H // 16, W // 16, engine.inc[1], dtype=torch.bfloat16, device=engine.dev)
         self._has_prev = torch.zeros(1, dtype=torch.int32, device=engine.dev)
         self.last = {}
 

@@ -45,8 +45,9 @@ CONV_TRACE = None
 
 
 def conv2d(x, w_packed, KH, KW, stride=1, pad=0, bias=None, act=ACT_NONE, gamma=None, res=None, out=None,
-           out_dtype=None, block_n=0, gn_stats=None, gn_groups=0, row_stats=None, col_s=None, row_eps=1e-6):
-    """x: NHWC view (B,H,W,Cin) bf16/f16.  w_packed: [Cout, KH*KW, Cin].  Returns NHWC (B,Ho,Wo,Cout)."""
+           out_dtype=None, block_n=0, gn_stats=None, gn_groups=0, row_stats=None, col_s=None, row_eps=1e-6, act_after_res=False):
+    """x: NHWC view (B,H,W,Cin) bf16/f16.  w_packed: [Cout, KH*KW, Cin].  Returns NHWC (B,Ho,Wo,Cout).
+    act_after_res=True (with act=ACT_RELU and res): y = relu(conv + bias + res) instead of res + act(conv + bias)."""
     B, H, W, Cin = x.shape
     Cout = w_packed.shape[0]
     assert w_packed.shape[1] == KH * KW and w_packed.shape[2] == Cin and w_packed.is_contiguous()
@@ -73,6 +74,7 @@ def conv2d(x, w_packed, KH, KW, stride=1, pad=0, bias=None, act=ACT_NONE, gamma=
     d.block_n = block_n
     d.gn_stats, d.gn_groups = _p(gn_stats), gn_groups
     d.row_stats, d.col_s, d.row_eps = _p(row_stats), _p(col_s), row_eps
+    d.act_after_res = int(bool(act_after_res))
     if row_stats is not None:
         assert row_stats.dtype == torch.int64 and row_stats.numel() == B * H * W * 2 and col_s is not None and col_s.numel() >= Cout
     if CONV_TRACE is not None:  # tools/profile_frame.py: conv launches in issue order, to label an ncu launch list
@@ -171,6 +173,30 @@ def stem_ln(img, w48, bias, lnw, lnb, eps=1e-6):
     C0 = w48.shape[1]
     out = torch.empty(B, H // 4, W // 4, C0, dtype=torch.bfloat16, device=img.device)
     _lib.check(_L().uc_stem_ln(_p(img), int(u8), _p(w48), _p(bias), _p(lnw), _p(lnb), _p(out), B, H, W, C0, _f(eps), _S()), "uc_stem_ln")
+    return out
+
+
+def pack_resnet_stem_weight(w):
+    """[64,3,7,7] fp32 (BatchNorm already folded in) -> [64, 160] fp16, k = ci*49 + kh*7 + kw, zero for k >= 147."""
+    out = torch.zeros(w.shape[0], 160, dtype=torch.float16, device=w.device)
+    out[:, :147] = w.reshape(w.shape[0], 147).to(torch.float16)
+    return out
+
+
+def resnet_stem(img, w160, bias, out=None):
+    """conv7x7s2 + bias + ReLU + maxpool3x3s2 in one launch.  img: fp32 NCHW [B,3,H,W] or uint8 NHWC [B,H,W,3] (BGR).
+    Returns NHWC bf16 [B,H/4,W/4,64]."""
+    u8 = img.dtype == torch.uint8
+    if u8:
+        B, H, W, _ = img.shape
+    else:
+        B, _, H, W = img.shape
+        assert img.dtype == torch.float32
+    assert img.is_contiguous() and w160.dtype == torch.float16 and w160.shape == (64, 160) and bias.dtype == torch.float32
+    if out is None:
+        out = torch.empty(B, H // 4, W // 4, 64, dtype=torch.bfloat16, device=img.device)
+    assert out.shape == (B, H // 4, W // 4, 64) and out.is_contiguous() and out.dtype == torch.bfloat16
+    _lib.check(_L().uc_resnet_stem(_p(img), int(u8), _p(w160), _p(bias), _p(out), B, H, W, _S()), "uc_resnet_stem")
     return out
 
 

@@ -18,7 +18,11 @@ class Exp:
         cfg = CONFIGS[exp_name]
         self.exp_name = exp_name
         self.num_classes = cfg["num_classes"]       # unicorn_track.py:36 (8) / *_mot_challenge.py:18 (1)
-        self.backbone_name = "convnext_tiny" if "tiny" in exp_name else "convnext_large"
+        if cfg["backbone"] == "resnet50":
+            self.backbone_name = "resnet50"          # exps/default/unicorn_track_r50*.py
+        else:
+            self.backbone_name = "convnext_tiny" if "tiny" in exp_name else "convnext_large"
+        self.in_channels = list(cfg["in_channels"])  # unicorn_track.py:43, exps/default/unicorn_track_large.py:15, *_r50*.py
         self.normalize = False                      # unicorn_track.py:76
         self.test_size = (800, 1280)                # unicorn_track.py:104
         self.input_size = (800, 1280)

@@ -18,23 +18,69 @@ CONFIGS = {
     "unicorn_track_large_mot_challenge": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=1, mask=False),
     "unicorn_track_tiny_mask": dict(depths=(3, 3, 9, 3), dims=(96, 192, 384, 768), num_classes=8, mask=True),
     "unicorn_track_large_mask": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=8, mask=True),
+    # exps/default/unicorn_track_r50*.py: torchvision ResNet-50 (v1.5 Bottlenecks); dims = the stage output widths (4 x 64/128/256/512)
+    "unicorn_track_r50": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=False),
+    "unicorn_track_r50_mask": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=True),
 }
+for _c in CONFIGS.values():
+    _c.setdefault("backbone", "convnext")
+    _c["in_channels"] = tuple(_c["dims"][1:])  # channels of the s8 / s16 / s32 maps the neck, heads and interaction read
 
 
 def param_shapes(cfg_name):
     """OrderedDict name -> shape, in the reference's state_dict order."""
     cfg = CONFIGS[cfg_name]
     depths, dims, ncls = cfg["depths"], cfg["dims"], cfg["num_classes"]
-    inc = dims[1:]
+    inc = cfg["in_channels"]
     S = OrderedDict()
 
-    def block(p, d):
-        S[p + "gamma"] = (d,)
-        S[p + "dwconv.weight"] = (d, 1, 7, 7); S[p + "dwconv.bias"] = (d,)
-        S[p + "norm.weight"] = (d,); S[p + "norm.bias"] = (d,)
-        S[p + "pwconv1.weight"] = (4 * d, d); S[p + "pwconv1.bias"] = (4 * d,)
-        S[p + "pwconv2.weight"] = (d, 4 * d); S[p + "pwconv2.bias"] = (d,)
+    def bn(p, c):  # BatchNorm2d, kept as BN in the ResNet backbone (exp/unicorn_track.py:147-153)
+        S[p + "weight"] = (c,); S[p + "bias"] = (c,)
+        S[p + "running_mean"] = (c,); S[p + "running_var"] = (c,); S[p + "num_batches_tracked"] = ()
 
+    b = "backbone.backbone."
+    if cfg["backbone"] == "resnet50":  # backbone/resnet.py:127-204 (no fc: out_indices [1, 2, 3])
+        S[b + "conv1.weight"] = (64, 3, 7, 7)
+        bn(b + "bn1.", 64)
+        cin = 64
+        for i, n in enumerate(depths):
+            w = 64 << i
+            for j in range(n):
+                p = b + f"layer{i + 1}.{j}."
+                S[p + "conv1.weight"] = (w, cin, 1, 1); bn(p + "bn1.", w)
+                S[p + "conv2.weight"] = (w, w, 3, 3); bn(p + "bn2.", w)
+                S[p + "conv3.weight"] = (4 * w, w, 1, 1); bn(p + "bn3.", 4 * w)
+                if j == 0:
+                    S[p + "downsample.0.weight"] = (4 * w, cin, 1, 1); bn(p + "downsample.1.", 4 * w)
+                cin = 4 * w
+    else:
+        _convnext_shapes(S, b, depths, dims)
+    _neck_and_heads(S, inc, ncls, cfg["mask"])
+    return S
+
+
+def _convnext_block(S, p, d):
+    S[p + "gamma"] = (d,)
+    S[p + "dwconv.weight"] = (d, 1, 7, 7); S[p + "dwconv.bias"] = (d,)
+    S[p + "norm.weight"] = (d,); S[p + "norm.bias"] = (d,)
+    S[p + "pwconv1.weight"] = (4 * d, d); S[p + "pwconv1.bias"] = (4 * d,)
+    S[p + "pwconv2.weight"] = (d, 4 * d); S[p + "pwconv2.bias"] = (d,)
+
+
+def _convnext_shapes(S, b, depths, dims):
+    S[b + "downsample_layers.0.0.weight"] = (dims[0], 3, 4, 4); S[b + "downsample_layers.0.0.bias"] = (dims[0],)
+    S[b + "downsample_layers.0.1.weight"] = (dims[0],); S[b + "downsample_layers.0.1.bias"] = (dims[0],)
+    for i in range(1, 4):
+        S[b + f"downsample_layers.{i}.0.weight"] = (dims[i - 1],); S[b + f"downsample_layers.{i}.0.bias"] = (dims[i - 1],)
+        S[b + f"downsample_layers.{i}.1.weight"] = (dims[i], dims[i - 1], 2, 2); S[b + f"downsample_layers.{i}.1.bias"] = (dims[i],)
+    for i in range(4):
+        for j in range(depths[i]):
+            _convnext_block(S, b + f"stages.{i}.{j}.", dims[i])
+    for i in range(1, 4):
+        S[b + f"norm{i}.weight"] = (dims[i],); S[b + f"norm{i}.bias"] = (dims[i],)
+
+
+def _neck_and_heads(S, inc, ncls, mask):
     def baseconv(p, cin, cout, k):
         S[p + "conv.weight"] = (cout, cin, k, k)
         S[p + "bn.weight"] = (cout,); S[p + "bn.bias"] = (cout,)
@@ -48,17 +94,6 @@ def param_shapes(cfg_name):
             baseconv(p + f"m.{i}.conv1.", h, h, 1)
             baseconv(p + f"m.{i}.conv2.", h, h, 3)
 
-    b = "backbone.backbone."
-    S[b + "downsample_layers.0.0.weight"] = (dims[0], 3, 4, 4); S[b + "downsample_layers.0.0.bias"] = (dims[0],)
-    S[b + "downsample_layers.0.1.weight"] = (dims[0],); S[b + "downsample_layers.0.1.bias"] = (dims[0],)
-    for i in range(1, 4):
-        S[b + f"downsample_layers.{i}.0.weight"] = (dims[i - 1],); S[b + f"downsample_layers.{i}.0.bias"] = (dims[i - 1],)
-        S[b + f"downsample_layers.{i}.1.weight"] = (dims[i], dims[i - 1], 2, 2); S[b + f"downsample_layers.{i}.1.bias"] = (dims[i],)
-    for i in range(4):
-        for j in range(depths[i]):
-            block(b + f"stages.{i}.{j}.", dims[i])
-    for i in range(1, 4):
-        S[b + f"norm{i}.weight"] = (dims[i],); S[b + f"norm{i}.bias"] = (dims[i],)
     p = "backbone."
     baseconv(p + "lateral_conv0.", inc[2], inc[1], 1)
     csp(p + "C3_p4.", 2 * inc[1], inc[1])
@@ -81,7 +116,7 @@ def param_shapes(cfg_name):
                      ("reg_preds_sot", 4)):
         for k in range(3):
             S[h + f"{name}.{k}.weight"] = (co, 256, 1, 1); S[h + f"{name}.{k}.bias"] = (co,)
-    if cfg["mask"]:
+    if mask:
         S[h + "mask_head.sizes_of_interest"] = (5,)
         S[h + "mask_head._iter"] = (1,)
         for k in range(3):
@@ -99,7 +134,7 @@ def param_shapes(cfg_name):
         baseconv(h + f"stems.{k}.", inc[k], 256, 1)
     for k in range(3):
         for n in range(3):
-            block(h + f"att_layers.{k}.{n}.", 256)
+            _convnext_block(S, h + f"att_layers.{k}.{n}.", 256)
     S["bottleneck.0.weight"] = (256, inc[1], 1, 1); S["bottleneck.0.bias"] = (256,)
     S["bottleneck.1.weight"] = (256,); S["bottleneck.1.bias"] = (256,)
     S["upsample_layer.1.weight"] = (256, 64, 3, 3); S["upsample_layer.1.bias"] = (256,)
@@ -113,7 +148,6 @@ def param_shapes(cfg_name):
     S[t + "linear1.weight"] = (1024, 256); S[t + "linear1.bias"] = (1024,)
     S[t + "linear2.weight"] = (256, 1024); S[t + "linear2.bias"] = (256,)
     S[t + "norm2.weight"] = (256,); S[t + "norm2.bias"] = (256,)
-    return S
 
 
 def _gen(name, seed):
@@ -125,7 +159,8 @@ def make_state_dict(cfg_name, seed=0):
 
     Unlike the reference's init (zero attention/offset weights, -4.6 prediction biases, unit layer scales) every
     parameter is perturbed so that every kernel's output depends on its inputs and detections exist — the caveats
-    listed in SURVEY.md §8(c) — while activations stay O(1) through 36 residual blocks."""
+    listed in SURVEY.md §8(c) — while activations stay O(1) through 36 residual blocks.  BatchNorm buffers (ResNet-50) get positive
+    running variances and an int64 scalar num_batches_tracked, so the reference loads them with strict=True."""
     sd = OrderedDict()
     for name, shape in param_shapes(cfg_name).items():
         g = _gen(name, seed)
@@ -134,6 +169,15 @@ def make_state_dict(cfg_name, seed=0):
             t = torch.tensor([64.0, 128.0, 256.0, 512.0, 1024.0])  # dynamic_mask_head.py:106-107
         elif name.endswith("_iter"):
             t = torch.zeros(1)
+        elif name.endswith("num_batches_tracked"):
+            sd[name] = torch.tensor(0, dtype=torch.int64)
+            continue
+        elif name.endswith("running_mean"):
+            t = 0.1 * n(*shape)
+        elif name.endswith("running_var"):  # the stem conv sees 0-255 pixels: its BatchNorm statistics bring them to O(1)
+            t = (0.5 + torch.rand(*shape, generator=g)) * (2e4 if name == "backbone.backbone.bn1.running_var" else 1.0)
+        elif name.endswith("bn3.weight"):  # small residual-branch scale: activations stay O(1) through 16 un-normalised blocks
+            t = 0.3 * (1.0 + 0.2 * n(*shape))
         elif name.endswith("gamma"):
             t = 0.3 * (1.0 + 0.2 * n(*shape))
         elif "beta_" in name:
@@ -169,6 +213,14 @@ def make_state_dict(cfg_name, seed=0):
             t = n(*shape) / math.sqrt(fan_in)
         sd[name] = t.float().contiguous()
     return sd
+
+
+def fold_bn(w, sd, p, eps=1e-3):
+    """Eval-mode BatchNorm `p` (running statistics; eps 1e-3 as init_yolo sets it, exp/unicorn_track.py:118-122) folded into the
+    preceding bias-free conv weight w [Cout, ...]: s = gamma / sqrt(running_var + eps), W' = W s, b' = beta - running_mean s.
+    Computed in the dtype of w."""
+    s = sd[p + "weight"].to(w) / torch.sqrt(sd[p + "running_var"].to(w) + eps)
+    return w * s.view(-1, *([1] * (w.dim() - 1))), sd[p + "bias"].to(w) - sd[p + "running_mean"].to(w) * s
 
 
 def check_state_dict(state_dict, cfg_name, strict=True):
