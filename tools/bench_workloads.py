@@ -99,7 +99,7 @@ elif what == "r50":
             if trk.depth == 1:
                 trk.track_tensor(frames[1 + i % 3])
                 return
-            if trk._submitted - trk._collected == trk.depth:
+            if trk._ring.submitted - trk._ring.collected == trk.depth:
                 trk.collect()
             trk.submit(frames[1 + i % 3])
         return step
@@ -107,7 +107,7 @@ elif what == "r50":
     for rnd in range(3):
         for (cfg, depth), trk in trackers.items():
             fps, ms, launches = timed(in_flight(trk), n, warm=6)
-            while trk._collected < trk._submitted:
+            while trk._ring.collected < trk._ring.submitted:
                 trk.collect()
             print(json.dumps({"workload": f"SOT 800x1280 {cfg}, CUDA graphs, {depth} frame(s) in flight", "round": rnd,
                               "frames_per_s": round(fps, 2), "ms_per_frame": round(ms, 2), "kernels_per_frame": launches, "n_gpus": 1}))

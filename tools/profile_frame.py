@@ -52,11 +52,11 @@ c = trg._ctxs[0]
 dev_frame = frames[1:2].to(eng.dev)
 R = 20
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-trg._stage_input(dev_frame, c)
+c.stage(dev_frame)
 torch.cuda.synchronize()
 e0.record()
 for _ in range(R):
-    trg._stage_input(dev_frame, c)
+    c.stage(dev_frame)
     c.graph.replay()
 e1.record()
 torch.cuda.synchronize()

@@ -8,6 +8,8 @@ import torch.nn.functional as F
 
 from . import ops
 from .engine import UnicornEngine
+from .frames import anchor_count
+from .mot import QDEmbedding
 from .results import mots_frame_result
 from .tracker import QuasiDenseEmbedTracker
 
@@ -21,13 +23,10 @@ class UnicornMOTSTracker:
         self.mask_thres, self.d_rate, self.min_box_area = mask_thres, d_rate, min_box_area
         self.tracker = tracker or QuasiDenseEmbedTracker(device=engine.dev)
         H, W = self.input_size
-        A = (H // 8) * (W // 8) + (H // 16) * (W // 16) + (H // 32) * (W // 32)
-        self.ws = ops.PostWorkspace(A, engine.dev)
+        self.ws = ops.PostWorkspace(anchor_count(H, W), engine.dev)
         self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=engine.dev)
-        self.feats = torch.zeros(max_dets, 128, dtype=torch.float32, device=engine.dev)
+        self._qd = QDEmbedding(engine, H, W, max_dets, "mots.emb")
         self.frame_id = 0
-        self._prev_feat = torch.zeros(1, H // 16, W // 16, engine.inc[1], dtype=torch.bfloat16, device=engine.dev)
-        self._has_prev = torch.zeros(1, dtype=torch.int32, device=engine.dev)
         self.last = {}
 
     def step_tensor(self, frame, img_h, img_w):
@@ -44,14 +43,9 @@ class UnicornMOTSTracker:
         mf, um = e.mask_branch(fpn)
         hw = [(t.shape[1], t.shape[2]) for t in e.dyn_levels]
         masks = ops.dynamic_masks(mf, um, e.dyn_levels, hw, self.ws, self.max_dets, up_rate=8 // self.d_rate, d_rate=self.d_rate)
-        ops.copy_rows_if(self._has_prev, seq["feat"], self._prev_feat, invert=True)  # first frame with detections: pre_dict = cur_dict (:812-813)
-        _, f_cur = e.interaction(self._prev_feat, seq["feat"])
-        emb = e.upsample(f_cur, "mots.emb")
-        ops.sample_embed(emb, dets, self.max_dets, 8.0, count=cnt, out=self.feats)
-        ops.copy_rows_if(cnt, seq["feat"], self._prev_feat)  # pre_dict advances only on frames with detections (:803,818)
-        self._has_prev.bitwise_or_((cnt > 0).to(torch.int32))
+        self._qd(e, seq["feat"], dets, cnt)  # pre_dict as in the MOT driver (:803-818)
         n = min(int(cnt.item()), self.max_dets)
-        d, f = dets[:n].cpu(), self.feats[:n].cpu()
+        d, f = dets[:n].cpu(), self._qd.feats[:n].cpu()
         scale = min(H / float(img_h), W / float(img_w))
         # masks at the original image scale, thresholded (:804-805)
         m = F.interpolate(masks[:n, None], scale_factor=1 / scale, mode="bilinear", align_corners=False)[:, 0, :img_h, :img_w] > self.mask_thres

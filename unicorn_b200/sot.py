@@ -9,6 +9,7 @@ import torch
 
 from . import ops
 from .engine import UnicornEngine
+from .frames import FrameSlot, Ring, in_flight
 
 
 def get_label_map(box_xyxy, H, W, device):
@@ -36,23 +37,32 @@ def preprocess(img_rgb, input_size, out=None):
     return out, r
 
 
-class _Ctx:
-    """One frame in flight: an engine context (own activation buffers), static input buffers, NMS workspace, pinned result slot,
-    the captured CUDA graph and the stream it runs on."""
+def xyxy_resized(xywh, r):
+    """Reference-protocol box [x, y, w, h] in original-image pixels -> [x1, y1, x2, y2] in resized-image coordinates
+    (unicorn_sot.py:44-46, unicorn_vos.py:62-64)."""
+    b = torch.tensor(xywh, dtype=torch.float32).view(-1)
+    b[2:] += b[:2]
+    return b * r
 
-    def __init__(self, eng, H, W, max_inst, stream):
-        dev = eng.dev
-        self.eng, self.stream = eng, stream
-        self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=dev)
-        self.img_in_u8 = torch.empty(1, H, W, 3, dtype=torch.uint8, device=dev)
-        self.u8 = False
-        A = (H // 8) * (W // 8) + (H // 16) * (W // 16) + (H // 32) * (W // 32)
-        self.ws = ops.PostWorkspace(A, dev)
+
+def state_xywh(det, r, input_size):
+    """Detection row (corners in resized-image coordinates) -> the reference's state: corners clipped to the input, scaled back to
+    the original image, [x, y, w, h] as ints (unicorn_sot.py:64-75, unicorn_vos.py:132-143)."""
+    H, W = input_size
+    b = det[:4].clone()
+    b[0::2] = b[0::2].clamp(0, W)
+    b[1::2] = b[1::2].clamp(0, H)
+    b = (b / r).numpy()
+    return [int(b[0]), int(b[1]), int(b[2] - b[0]), int(b[3] - b[1])]
+
+
+class _Ctx(FrameSlot):
+    """A frame slot plus the pinned read-back of its detection count and top `max_inst` rows."""
+
+    def __init__(self, eng, H, W, stream, max_inst):
+        super().__init__(eng, H, W, stream)
         self.host_dets = torch.empty(max_inst, 7, dtype=torch.float32).pin_memory()
         self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self.graph = None
-        self.event = torch.cuda.Event()
-        self.last = {}
 
 
 class UnicornSOTTrack:
@@ -76,12 +86,11 @@ class UnicornSOTTrack:
         H, W = self.input_size
         assert depth >= 1
         self.depth = depth
-        self._ctxs = [_Ctx(engine if i == 0 else engine.fork(), H, W, max_inst,
-                           None if depth == 1 else torch.cuda.Stream(device=engine.dev)) for i in range(depth)]
-        self._submitted = self._collected = 0
+        self._ring = Ring(in_flight(engine, depth, lambda eng, stream: _Ctx(eng, H, W, stream, max_inst)))
+        self._ctxs = self._ring.slots  # bench.py reads pipe._ctxs[i]
         self.state = None
         self.frame_id = 0
-        self.launches_per_frame = 0
+        self.launches_per_frame = 0  # bench.py reads it
 
     # attributes of the single-context tracker (tests / bench read them): context 0
     img_in = property(lambda self: self._ctxs[0].img_in)
@@ -90,7 +99,7 @@ class UnicornSOTTrack:
     host_dets = property(lambda self: self._ctxs[0].host_dets)
     host_count = property(lambda self: self._ctxs[0].host_count)
     graph = property(lambda self: self._ctxs[0].graph)
-    last = property(lambda self: self._ctxs[(max(self._collected, 1) - 1) % self.depth].last)
+    last = property(lambda self: self._ctxs[(max(self._ring.collected, 1) - 1) % self.depth].last)
 
     # -------------------------------------------------------------------------------- device-side frame
     def _frame(self, c):
@@ -101,91 +110,53 @@ class UnicornSOTTrack:
             e_pre, e_cur = e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc")
             return f_pre, f_cur, e_pre, e_cur, e.propagate(e_pre, e_cur, self.lbs_pre)
 
-        fpn, seq, (f_pre, f_cur, e_pre, e_cur, priors) = e.backbone(c.img_in_u8 if c.u8 else c.img_in, tag="cur", side=correlate)
+        fpn, seq, (f_pre, f_cur, e_pre, e_cur, priors) = e.backbone(c.img, tag="cur", side=correlate)
         out = e.head(fpn, priors, "sot")
         ops.postprocess_device(out[0], 1, self.confthre, self.nmsthre, c.ws, max_keep=self.nms_keep)
         c.last = dict(fpn=fpn, feat=seq["feat"], inter_pre=f_pre, inter_cur=f_cur, embed_pre=e_pre, embed_cur=e_cur, priors=priors, head=out)
-
-    def _stage_input(self, frame, c=None):
-        """fp32 [1,3,H,W] (PreprocessorX format) or uint8 [1,H,W,3] (letterboxed BGR frame, 4x fewer H2D bytes)."""
-        c = c or self._ctxs[0]
-        u8 = frame.dtype == torch.uint8
-        if u8 != c.u8:
-            c.u8, c.graph = u8, None  # the captured graph reads one of the two static input buffers
-        (c.img_in_u8 if u8 else c.img_in).copy_(frame, non_blocking=True)
-        return c.img_in_u8 if u8 else c.img_in
 
     def initialize_tensor(self, ref_frame, init_box_xyxy):
         """ref_frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3] (host or device); init box in resized-image coordinates."""
         e = self.eng
         H, W = self.input_size
         torch.cuda.synchronize()
-        inp = self._stage_input(ref_frame)
+        inp = self._ctxs[0].stage(ref_frame)
         e.begin_frame()
         _, seq = e.backbone(inp, tag="ref")
         self.ref_feat = seq["feat"].clone()
         self.ref_proj = e.project_ref(self.ref_feat)  # this tracker's own copy (several trackers may share the engine)
         lab = get_label_map(init_box_xyxy, H, W, e.dev)
         self.lbs_pre = ops.bilinear(lab, H // 8, W // 8, 8.0, 8.0).reshape(1, -1).contiguous()
-        for c in self._ctxs:
-            c.graph = None
-        self.frame_id = self._submitted = self._collected = 0
+        self._ring.reset()
+        self.frame_id = 0
         torch.cuda.synchronize()
-
-    def _run(self, c, frame):
-        """Enqueue one frame on context c (current stream = c.stream when pipelined): input copy, graph replay (or eager launches),
-        asynchronous read-back of (count, top rows) into the context's pinned slot."""
-        self._stage_input(frame, c)
-        if not self.use_graph:
-            self._frame(c)
-        elif c.graph is None:
-            self._frame(c)  # warm-up: allocates every buffer, sets kernel attributes, plan-time autotuning
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            from . import _lib
-            l0 = _lib.LAUNCHES
-            with torch.cuda.graph(g, stream=c.stream):
-                self._frame(c)
-            self.launches_per_frame = _lib.LAUNCHES - l0  # kernels recorded in the graph (C-ABI launches only)
-            c.graph = g
-            c.graph.replay()
-        else:
-            c.graph.replay()
-        c.host_count.copy_(c.ws.count, non_blocking=True)
-        c.host_dets.copy_(c.ws.dets[:self.max_inst], non_blocking=True)
 
     def track_tensor(self, cur_frame):
         """cur_frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], ideally pinned host memory.  Returns (dets[:max_inst] cpu, count)."""
-        if self.depth > 1:
-            self.submit(cur_frame)
-            return self.collect()
-        self.frame_id += 1
-        self._submitted = self._collected = self.frame_id
-        c = self._ctxs[0]
-        self._run(c, cur_frame)
-        torch.cuda.current_stream().synchronize()
-        n = int(c.host_count.item())
-        return c.host_dets[:min(n, self.max_inst)].clone(), n
+        self.submit(cur_frame)
+        return self.collect()
 
     def submit(self, cur_frame):
-        """Pipelined protocol: enqueue a frame (returns immediately); at most `depth` frames may be uncollected."""
-        assert self._submitted - self._collected < self.depth, "collect() a frame first"
-        c = self._ctxs[self._submitted % self.depth]
-        self._submitted += 1
-        self.frame_id = self._submitted
-        if c.stream is None:
-            self._run(c, cur_frame)
-            c.event.record()
-            return
-        with torch.cuda.stream(c.stream):
-            self._run(c, cur_frame)
+        """Pipelined protocol: enqueue a frame (returns immediately); at most `depth` frames may be uncollected.  On the context's
+        stream: input copy, graph replay (or eager launches), asynchronous read-back of (count, top rows) into the context's pinned
+        slot.  A context's first graph frame is warm-up, capture and replay in one call, so the graph exists after one frame."""
+        c = self._ring.submit()
+        self.frame_id = self._ring.submitted
+        with torch.cuda.stream(c.stream):  # None: the current stream
+            c.stage(cur_frame)
+            if not self.use_graph:
+                self._frame(c)
+            elif c.graph is None:
+                c.graph, self.launches_per_frame = c.capture(lambda: self._frame(c), warmup=True)
+            else:
+                c.graph.replay()
+            c.host_count.copy_(c.ws.count, non_blocking=True)
+            c.host_dets.copy_(c.ws.dets[:self.max_inst], non_blocking=True)
             c.event.record()
 
     def collect(self):
         """Result of the oldest submitted frame: (dets[:max_inst] cpu, count)."""
-        assert self._collected < self._submitted, "nothing submitted"
-        c = self._ctxs[self._collected % self.depth]
-        self._collected += 1
+        c = self._ring.collect()
         c.event.synchronize()
         n = int(c.host_count.item())
         return c.host_dets[:min(n, self.max_inst)].clone(), n
@@ -205,18 +176,12 @@ class UnicornSOTTrack:
 
     def initialize(self, image, info: dict):
         ref, r = self._preprocess(image)
-        box = torch.tensor(info["init_bbox"], dtype=torch.float32).view(-1)
-        box[2:] += box[:2]
-        self.initialize_tensor(ref, box * r)
+        self.initialize_tensor(ref, xyxy_resized(info["init_bbox"], r))
         self.state = info["init_bbox"]
 
     def track(self, image, info: dict = None):
         cur, r = self._preprocess(image)
         dets, n = self.track_tensor(cur)
         if n > 0:
-            out = dets.numpy().copy()
-            out[:, 0:4:2] = out[:, 0:4:2].clip(0, self.input_size[1])
-            out[:, 1:4:2] = out[:, 1:4:2].clip(0, self.input_size[0])
-            b = out[0, :4] / r
-            self.state = [int(b[0]), int(b[1]), int(b[2] - b[0]), int(b[3] - b[1])]
+            self.state = state_xywh(dets[0], r, self.input_size)
         return {"target_bbox": self.state}

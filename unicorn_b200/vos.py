@@ -10,8 +10,8 @@ argmax run in one kernel on the device (uc_vos_aggregate); the only per-frame ho
 detection rows out.  With use_graph=True the steady-state frame is one CUDA-graph replay (re-captured when objects are added).
 
 depth > 1: like in SOT, a frame depends only on the reference frames of its objects, never on the previous frame's result, so
-`submit(frame)` / `collect()` keep `depth` steady-state frames in flight, each on its own stream and engine context (worker drivers
-on UnicornEngine.fork() that share the reference groups); frames that add objects go through track_tensor() with the pipeline drained.
+`submit(frame)` / `collect()` keep `depth` steady-state frames in flight, each in its own frame slot (engine fork, stream, buffers)
+sharing the reference groups; frames that add objects go through track_tensor() on slot 0 with the pipeline drained.
 """
 import ctypes
 
@@ -19,7 +19,8 @@ import torch
 
 from . import _lib, ops
 from .engine import UnicornEngine
-from .sot import get_label_map, preprocess
+from .frames import FrameSlot, Ring, in_flight
+from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
 
 
 class _Group:
@@ -27,6 +28,21 @@ class _Group:
 
     def __init__(self, ref_feat, ref_proj, obj_ids, lbs):
         self.ref_feat, self.ref_proj, self.obj_ids, self.lbs = ref_feat, ref_proj, list(obj_ids), lbs
+
+
+class _Slot(FrameSlot):
+    """One VOS frame in flight: a frame slot plus the per-object mask and detection buffers, the label map and soft masks at the
+    original resolution, the pinned detection rows and the group sizes its graph was captured for."""
+
+    def __init__(self, eng, H, W, stream):
+        super().__init__(eng, H, W, stream)
+        self.mask_bufs, self.det_bufs = [], []  # per object: fp32 [1,H,W] best-instance mask, fp32 [8] = det row + count
+        self.seg = self.soft = self.rows_host = self.graph_key = None
+        self.frames = 0  # since initialize_tensor: the first one runs eagerly
+
+    # bench.py reads vos._workers[i]._stream / ._graph
+    _stream = property(lambda self: self.stream)
+    _graph = property(lambda self: self.graph)
 
 
 class UnicornVOSTrack:
@@ -37,51 +53,31 @@ class UnicornVOSTrack:
         self.conf, self.nms, self.max_inst, self.d_rate = conf, nms, max_inst, d_rate
         self.num_classes = 1
         H, W = self.input_size
-        dev = engine.dev
-        A = (H // 8) * (W // 8) + (H // 16) * (W // 16) + (H // 32) * (W // 32)
-        self.ws = ops.PostWorkspace(A, dev)
-        self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=dev)
-        self.img_in_u8 = torch.empty(1, H, W, 3, dtype=torch.uint8, device=dev)
-        self._u8 = False
         self.use_graph = use_graph
-        self._graph, self._graph_key = None, None
-        self._mask_bufs, self._det_bufs = [], []   # per object slot: fp32 [1,H,W] best-instance mask, fp32 [8] = det row + count
-        self._seg = self._soft = None
         self.groups = []
         self.state_pre_dict = {}
-        self.frame_id = 0
-        self.launches_per_frame = 0
         self.debug = False  # tests: keep per-object copies of the head output and the controller maps
-        self.last = {}
-        self._rows_host, self._rows_ev, self._pending = None, torch.cuda.Event(), None
-        # frames in flight: worker 0 is this driver, the others are drivers on engine forks sharing groups / geometry
+        self.launches_per_frame = 0  # bench.py reads it
         self.depth = depth
-        self._stream = torch.cuda.Stream(device=dev) if depth > 1 else None
-        self._workers = [self] + [UnicornVOSTrack(engine.fork(), input_size, conf, nms, max_inst, d_rate, use_graph, depth=1) for _ in range(depth - 1)]
-        for w in self._workers[1:]:
-            w._stream = torch.cuda.Stream(device=dev)
-        self._submitted = self._collected = 0
+        self._ring = Ring(in_flight(engine, depth, lambda eng, stream: _Slot(eng, H, W, stream)))
+        self._workers = self._ring.slots  # bench.py reads vos._workers[i]
+
+    # slot 0 runs initialize_tensor() and track_tensor() (tests read these)
+    last = property(lambda self: self._workers[0].last)
+    _soft = property(lambda self: self._workers[0].soft)
 
     # ------------------------------------------------------------------------------------------ helpers
-    def _stage_input(self, frame):
-        u8 = frame.dtype == torch.uint8
-        if u8 != self._u8:
-            self._u8, self._graph = u8, None
-        buf = self.img_in_u8 if u8 else self.img_in
-        buf.copy_(frame, non_blocking=True)
-        return buf
-
     def _label_maps(self, boxes_xyxy):
         H, W = self.input_size
         maps = [ops.bilinear(get_label_map(b, H, W, self.eng.dev), H // 8, W // 8, 8.0, 8.0).reshape(1, -1) for b in boxes_xyxy]
         return torch.cat(maps, 0).contiguous()
 
-    def _slot(self, i):
+    def _obj_bufs(self, s, i):
         H, W = self.input_size
-        while len(self._mask_bufs) <= i:
-            self._mask_bufs.append(torch.zeros(1, H, W, dtype=torch.float32, device=self.eng.dev))
-            self._det_bufs.append(torch.zeros(8, dtype=torch.float32, device=self.eng.dev))
-        return self._mask_bufs[i], self._det_bufs[i]
+        while len(s.mask_bufs) <= i:
+            s.mask_bufs.append(torch.zeros(1, H, W, dtype=torch.float32, device=self.eng.dev))
+            s.det_bufs.append(torch.zeros(8, dtype=torch.float32, device=self.eng.dev))
+        return s.mask_bufs[i], s.det_bufs[i]
 
     @property
     def obj_ids(self):
@@ -93,7 +89,7 @@ class UnicornVOSTrack:
         (unicorn_vos.py:60-66); orig_size = (height, width) of the original frames (default: the network input size), r = resize
         ratio of the letterbox."""
         e = self.eng
-        inp = self._stage_input(ref_frame)
+        inp = self._workers[0].stage(ref_frame)
         e.begin_frame()
         _, seq = e.backbone(inp, tag="ref")
         ids = list(boxes_xyxy.keys())
@@ -101,20 +97,20 @@ class UnicornVOSTrack:
         self.groups = [_Group(ref_feat, e.project_ref(ref_feat), ids, self._label_maps([boxes_xyxy[o] for o in ids]))]
         self.orig_size = tuple(orig_size) if orig_size is not None else self.input_size
         self.r = float(r)
-        for w in self._workers:
-            w._graph, w.frame_id, w._pending = None, 0, None
-        self._submitted = self._collected = 0
+        self._ring.reset()
+        for s in self._workers:
+            s.frames = 0
         torch.cuda.synchronize()
 
-    def _device_frame(self):
-        """Every kernel of one steady-state frame (no host synchronisation; CUDA-graph capturable)."""
-        e = self.eng
+    def _device_frame(self, s):
+        """Every kernel of one steady-state frame in slot s (no host synchronisation; CUDA-graph capturable)."""
+        e = s.eng
         H, W = self.input_size
         hh, ww = H // 8, W // 8
         e.begin_frame()
-        fpn, seq = e.backbone(self.img_in_u8 if self._u8 else self.img_in, tag="cur")
+        fpn, seq = e.backbone(s.img, tag="cur")
         mf, um = e.mask_branch(fpn)  # identical for every object: computed once per frame
-        self.last = dict(mask_feats=mf, up_masks=um, per_obj={}, feat=seq["feat"], coarse={})
+        s.last = dict(mask_feats=mf, up_masks=um, per_obj={}, feat=seq["feat"], coarse={})
         slot = 0
         for gi, g in enumerate(self.groups):
             f_pre, f_cur = e.interaction(g.ref_feat, seq["feat"], ref_proj=g.ref_proj)
@@ -130,136 +126,114 @@ class UnicornVOSTrack:
                     pri = (c, ops.bilinear(c, hh // 2, ww // 2, 2.0, 2.0, out=e.buf("vos.p1", (1, hh // 2, ww // 2), torch.float32)),
                            ops.bilinear(c, hh // 4, ww // 4, 4.0, 4.0, out=e.buf("vos.p2", (1, hh // 4, ww // 4), torch.float32)))
                     head = e.head(fpn, pri, "sot", with_masks=True)
-                    ops.postprocess_device(head[0], 1, self.conf, self.nms, self.ws, max_keep=self.max_inst)
-                    mask, det = self._slot(slot)
+                    ops.postprocess_device(head[0], 1, self.conf, self.nms, s.ws, max_keep=self.max_inst)
+                    mask, det = self._obj_bufs(s, slot)
                     mask.zero_()  # an object without a detection contributes an all-zero mask (unicorn_vos.py:154-155)
                     hw = [(t.shape[1], t.shape[2]) for t in e.dyn_levels]
                     up = 8 // self.d_rate
-                    ops.dynamic_masks(mf, um, e.dyn_levels, hw, self.ws, 1, up_rate=up, d_rate=self.d_rate, out=mask,
+                    ops.dynamic_masks(mf, um, e.dyn_levels, hw, s.ws, 1, up_rate=up, d_rate=self.d_rate, out=mask,
                                       scratch=e.buf("vos.scratch", (hh * ww * (1 + up * up),), torch.float32))
-                    det[:7].copy_(self.ws.dets[0])
-                    det[7:8].copy_(self.ws.count.view(1).float())
+                    det[:7].copy_(s.ws.dets[0])
+                    det[7:8].copy_(s.ws.count.view(1).float())
                     keep = (lambda t: t.clone()) if self.debug else (lambda t: t)
-                    self.last["per_obj"][oid] = dict(head=keep(head), dyn=[keep(t) for t in e.dyn_levels], slot=slot)
-                    self.last["coarse"][oid] = c
+                    s.last["per_obj"][oid] = dict(head=keep(head), dyn=[keep(t) for t in e.dyn_levels], slot=slot)
+                    s.last["coarse"][oid] = c
                     slot += 1
         return seq
 
-    def _aggregate(self, new_ids=(), init_mask=None):
-        """unicorn_vos.py:100-127 on the device.  Returns (segmentation uint8 [H0,W0], soft masks fp32 [n,H0,W0])."""
+    def _aggregate(self, s, new_ids=(), init_mask=None):
+        """unicorn_vos.py:100-127 on the device, into s.seg (segmentation uint8 [H0,W0]) and s.soft (soft masks fp32 [n,H0,W0])."""
         H, W = self.input_size
         H0, W0 = self.orig_size
         ids = self.obj_ids + list(new_ids)
         n = len(ids)
-        if self._seg is None or self._seg.shape != (H0, W0) or self._soft.shape[0] < n:
-            self._seg = torch.zeros(H0, W0, dtype=torch.uint8, device=self.eng.dev)
-            self._soft = torch.zeros(max(n, 4), H0, W0, dtype=torch.float32, device=self.eng.dev)
+        if s.seg is None or s.seg.shape != (H0, W0) or s.soft.shape[0] < n:
+            s.seg = torch.zeros(H0, W0, dtype=torch.uint8, device=self.eng.dev)
+            s.soft = torch.zeros(max(n, 4), H0, W0, dtype=torch.float32, device=self.eng.dev)
         objs = (_lib.UcVosObject * n)()
         n_old = len(self.obj_ids)
         for k, oid in enumerate(ids):
             objs[k].id = int(oid)
             if k < n_old:
-                objs[k].mask = self._mask_bufs[k].data_ptr()
+                objs[k].mask = s.mask_bufs[k].data_ptr()
             else:
                 objs[k].init_mask = init_mask.data_ptr()
-        _lib.check(_lib.lib().uc_vos_aggregate(objs, n, H, W, H0, W0, ctypes.c_float(self.r), ctypes.c_void_p(self._soft.data_ptr()),
-                                               ctypes.c_void_p(self._seg.data_ptr()), _lib.stream_ptr()), "uc_vos_aggregate")
-        return self._seg, self._soft[:n]
+        _lib.check(_lib.lib().uc_vos_aggregate(objs, n, H, W, H0, W0, ctypes.c_float(self.r), ctypes.c_void_p(s.soft.data_ptr()),
+                                               ctypes.c_void_p(s.seg.data_ptr()), _lib.stream_ptr()), "uc_vos_aggregate")
 
-    def _enqueue(self, cur_frame, new_ids=(), new_boxes_xyxy=None, init_mask=None):
-        """Device half of a frame on the current stream + the asynchronous read of the detection rows; no host synchronisation
-        unless a graph has to be (re)captured."""
-        e = self.eng
-        self.frame_id += 1
-        self._stage_input(cur_frame)
+    def _enqueue(self, s, cur_frame, new_ids=(), new_boxes_xyxy=None, init_mask=None):
+        """Device half of a frame in slot s on the current stream + the asynchronous read of the detection rows; no host
+        synchronisation unless a graph has to be (re)captured."""
+        s.frames += 1
+        s.stage(cur_frame)
         key = tuple(len(g.obj_ids) for g in self.groups)
-        if self.use_graph and not new_ids and self.frame_id > 1:
-            if self._graph is None or self._graph_key != key:
-                self._device_frame()  # warm-up: buffers, kernel attributes, plan-time autotuning
-                self._aggregate()
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                l0 = _lib.LAUNCHES
-                with (torch.cuda.graph(g) if self._stream is None else torch.cuda.graph(g, stream=self._stream)):
-                    self._device_frame()
-                    self._aggregate()
-                self.launches_per_frame = _lib.LAUNCHES - l0
-                self._graph, self._graph_key, self._graph_last = g, key, self.last
-            self._graph.replay()
-            self.last = self._graph_last
-            seg, soft = self._seg, self._soft[:len(self.obj_ids)]
+        if self.use_graph and not new_ids and s.frames > 1:
+            if s.graph is None or s.graph_key != key:
+                s.graph, self.launches_per_frame = s.capture(lambda: (self._device_frame(s), self._aggregate(s)), warmup=True)
+                s.graph_key = key
+            else:
+                s.graph.replay()
         else:
-            seq = self._device_frame()
-            seg, soft = self._aggregate(new_ids, init_mask)
+            seq = self._device_frame(s)
+            self._aggregate(s, new_ids, init_mask)
             if new_ids:  # this frame becomes the reference of the new objects (unicorn_vos.py:87-88)
                 ref_feat = seq["feat"].clone()
-                self.groups.append(_Group(ref_feat, e.project_ref(ref_feat), new_ids, self._label_maps([new_boxes_xyxy[o] for o in new_ids])))
-                self._graph = None
-        n_old = len(self.last["per_obj"])
+                self.groups.append(_Group(ref_feat, self.eng.project_ref(ref_feat), new_ids, self._label_maps([new_boxes_xyxy[o] for o in new_ids])))
+                s.graph = None
+        n_old = len(s.last["per_obj"])
         if n_old:  # one D2H read: detection rows + counts, into pinned memory
-            if self._rows_host is None or self._rows_host.shape[0] < n_old:
-                self._rows_host = torch.zeros(max(n_old, 4), 8).pin_memory()
-            self._rows_host[:n_old].copy_(torch.stack(self._det_bufs[:n_old]), non_blocking=True)
-        self._rows_ev.record()
-        self._pending = (seg, soft, n_old, bool(new_ids))
+            if s.rows_host is None or s.rows_host.shape[0] < n_old:
+                s.rows_host = torch.zeros(max(n_old, 4), 8).pin_memory()
+            s.rows_host[:n_old].copy_(torch.stack(s.det_bufs[:n_old]), non_blocking=True)
+        s.event.record()
 
-    def _finish(self):
-        seg, soft, n_old, had_new = self._pending
-        self._pending = None
-        self._rows_ev.synchronize()
-        rows = self._rows_host[:n_old].clone() if n_old else torch.zeros(0, 8)
+    def _finish(self, s):
+        """Result of the frame enqueued in slot s (objects are only added with no frame in flight, so obj_ids are the frame's)."""
+        n_old = len(s.last["per_obj"])
+        s.event.synchronize()
+        rows = s.rows_host[:n_old].clone() if n_old else torch.zeros(0, 8)
         objects = {}
-        for oid, po in self.last["per_obj"].items():
+        for oid, po in s.last["per_obj"].items():
             row = rows[po["slot"]]
-            objects[oid] = (row[:7].clone(), self._mask_bufs[po["slot"]][0]) if row[7] > 0 else (None, None)
-        return dict(segmentation=seg, soft=soft, objects=objects, ids=self.obj_ids)
+            objects[oid] = (row[:7].clone(), s.mask_bufs[po["slot"]][0]) if row[7] > 0 else (None, None)
+        return dict(segmentation=s.seg, soft=s.soft[:len(self.obj_ids)], objects=objects, ids=self.obj_ids)
 
     def track_tensor(self, cur_frame, new_boxes_xyxy=None, init_mask=None):
         """cur_frame: preprocessed frame (fp32 NCHW or uint8 NHWC).  new_boxes_xyxy: dict obj_id -> box (resized-image coordinates)
         of objects that first appear in this frame, init_mask: their uint8 label map [H0,W0] (unicorn_vos.py:86-98).
         Returns dict(segmentation=uint8 [H0,W0] device tensor, soft=fp32 [n,H0,W0], objects={obj_id: (det_row [7] cpu | None,
         mask fp32 [H,W] device at network resolution | None)})."""
-        assert self._submitted == self._collected, "collect() the frames in flight first"
+        assert self._ring.submitted == self._ring.collected, "collect() the frames in flight first"
         new_ids = list(new_boxes_xyxy.keys()) if new_boxes_xyxy else []
         if new_ids:
             assert init_mask is not None and init_mask.dtype == torch.uint8 and tuple(init_mask.shape) == self.orig_size
             init_mask = init_mask.to(self.eng.dev).contiguous()
-        self._enqueue(cur_frame, new_ids, new_boxes_xyxy, init_mask)
-        return self._finish()
+        s = self._workers[0]
+        self._enqueue(s, cur_frame, new_ids, new_boxes_xyxy, init_mask)
+        return self._finish(s)
 
     # ------------------------------------------------------------------------------------------ frames in flight
     def submit(self, cur_frame):
-        """Enqueue a steady-state frame (no new objects) on the next worker's stream; at most `depth` frames may be uncollected.
-        The tensors of a collected result stay valid until that worker's next submit (`depth` submits later)."""
-        assert self._submitted - self._collected < self.depth, "collect() a frame first"
-        w = self._workers[self._submitted % self.depth]
-        self._submitted += 1
-        if w is not self:  # shared reference state and geometry
-            w.groups, w.orig_size, w.r = self.groups, self.orig_size, self.r
-        if w._stream is None:
-            return w._enqueue(cur_frame)
-        w._stream.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(w._stream):
-            w._enqueue(cur_frame)
+        """Enqueue a steady-state frame (no new objects) in the next slot, on its stream; at most `depth` frames may be uncollected.
+        The tensors of a collected result stay valid until that slot's next submit (`depth` submits later)."""
+        s = self._ring.submit()
+        if s.stream is not None:
+            s.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s.stream):
+            self._enqueue(s, cur_frame)
 
     def collect(self):
         """Result of the oldest submitted frame (same dict as track_tensor)."""
-        assert self._collected < self._submitted, "nothing submitted"
-        w = self._workers[self._collected % self.depth]
-        self._collected += 1
-        return w._finish()
+        return self._finish(self._ring.collect())
 
     # ------------------------------------------------------------------------------------------ reference protocol
     def initialize(self, image, info: dict):
         """image: RGB uint8 HWC; info: init_object_ids, init_bbox {id: [x,y,w,h]} (unicorn_vos.py:43-69)."""
         self.H, self.W = image.shape[:2]
         ref, r = preprocess(image, self.input_size)
-        boxes = {}
         for oid in info["init_object_ids"]:
             self.state_pre_dict[oid] = info["init_bbox"][oid]
-            b = torch.tensor(info["init_bbox"][oid], dtype=torch.float32).view(-1)
-            b[2:] += b[:2]
-            boxes[oid] = b * r
+        boxes = {oid: xyxy_resized(info["init_bbox"][oid], r) for oid in info["init_object_ids"]}
         self.initialize_tensor(ref, boxes, orig_size=(self.H, self.W), r=r)
 
     def track(self, image, info: dict = None):
@@ -268,20 +242,12 @@ class UnicornVOSTrack:
         cur, r = preprocess(image, self.input_size)
         new_boxes, init_mask = None, None
         if "init_object_ids" in info:
-            new_boxes = {}
             for oid in info["init_object_ids"]:
                 self.state_pre_dict[oid] = info["init_bbox"][oid]
-                b = torch.tensor(info["init_bbox"][oid], dtype=torch.float32).view(-1)
-                b[2:] += b[:2]
-                new_boxes[oid] = b * r
+            new_boxes = {oid: xyxy_resized(info["init_bbox"][oid], r) for oid in info["init_object_ids"]}
             init_mask = torch.as_tensor(info["init_mask"]).to(torch.uint8)
         out = self.track_tensor(cur, new_boxes, init_mask)
-        H, W = self.input_size
         for oid, (det, _) in out["objects"].items():  # unicorn_vos.py:137-149 (state of the best instance, xywh ints)
             if det is not None:
-                b = det[:4].clone()
-                b[0::2] = b[0::2].clamp(0, W)
-                b[1::2] = b[1::2].clamp(0, H)
-                b = (b / r).numpy()
-                self.state_pre_dict[oid] = [int(b[0]), int(b[1]), int(b[2] - b[0]), int(b[3] - b[1])]
+                self.state_pre_dict[oid] = state_xywh(det, r, self.input_size)
         return {"segmentation": out["segmentation"].cpu().numpy()}
