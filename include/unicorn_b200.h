@@ -64,9 +64,10 @@ UC_API int uc_check_device(void);
  *   y : NHWC output, pixel stride ldy, dtype y_dtype; y = act(conv(x) + bias) ; then y = res + gamma * y if given
  *       (act_after_res: y = relu(conv(x) + bias + res))
  * A Linear layer on [M, Cin] rows is B=1, H=1, W=M, KH=KW=1.  stride in {1,2}; pad < KH.
- * Cin % 8 == 0, Cout % 8 == 0 (pad the weight rows / output channels otherwise).  The epilogue stores from the accumulator
- * registers: each lane writes 32 bits (two 16-bit channels; 64 bits for fp32 y) per row and 8-channel chunk, and reads the
- * residual the same way.  Every launch is CUDA-graph capturable and uses programmatic dependent launch.
+ * Cin % 8 == 0, Cout % 8 == 0 (pad the weight rows / output channels otherwise).  x, w, y and res are 16-byte aligned.  A 16-bit
+ * y tile is staged in shared memory and written by TMA stores, and the residual is read by TMA into the same tile; fp32 y is stored
+ * straight from the accumulator registers (64 bits per lane, row and 8-channel chunk).  Every launch is CUDA-graph capturable and
+ * uses programmatic dependent launch.
  */
 typedef struct UcConv2d {
   const void* x;

@@ -11,12 +11,19 @@
 // optionally accumulate GroupNorm statistics, straight from the accumulator registers, while the producer is
 // already filling the ring with the next tile's boxes.
 //
+// 16-bit outputs leave through a shared-memory staging tile (128 rows x BLOCK_N, slabs of SLAB columns in the swizzled layout
+// of a TMA box {SLAB, tile_w, tile_h, 1}).  An epilogue DMA warp loads the tile's residual into it by TMA, and the tile's bias,
+// layer-scale and folded-LayerNorm column slices into small shared arrays, while the consumers still run the K loop; so the
+// epilogue waits on nothing global.  The consumers overwrite the residual with the output in place and the DMA warp stores the
+// tile by TMA (out-of-range rows and columns >= Cout are clipped by the hardware).  An in-place residual (res == y) is safe:
+// a tile's residual is read before that tile's store is issued, and tiles are disjoint.  fp32 outputs are stored directly.
+//
 // CLUSTER = 2 (block_n 1128 / 1192 / 1256): two CTAs of a thread-block cluster take consecutive M tiles of the same N tile.
 // Each loads its own activation box and HALF of the weight box, multicast by TMA into the same stage of both CTAs, so the
 // weights of a tile are read from L2 once per pair; a stage is refilled when the consumers of BOTH CTAs have released it
 // (remote mbarrier arrives).
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one warp), warpgroups 1-2 = MMA + epilogue.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0) and epilogue DMA (warp 1), warpgroups 1-2 = MMA + epilogue.
 // Reference call sites replaced: see include/unicorn_b200.h (uc_conv2d).
 #include <algorithm>
 #include <stdlib.h>
@@ -35,6 +42,14 @@ constexpr int kConvConsumers = 2;                       // warpgroups of 64 pixe
 constexpr int kConvThreads = (1 + kConvConsumers) * 128;
 constexpr int kGnMaxLocal = 64;                         // GroupNorm groups per N tile (tile width 256 / group size >= 4)
 constexpr int kGnSmemBytes = 2 * kGnMaxLocal * 2 * 8;   // two tile parities x {sum, sumsq} int64
+constexpr int kEpiBar = 2;                              // named barrier: consumers have staged a tile (id 1 is the GroupNorm one)
+
+// columns per staging slab: a 128-byte (64), 64-byte (32) or 32-byte (16) swizzled TMA box row that tiles BLOCK_N exactly
+constexpr int conv_slab(int block_n) { return block_n % 64 == 0 ? 64 : block_n % 32 == 0 ? 32 : 16; }
+// stage ring, 16-bit output staging tile, alignment slack, barriers, GroupNorm slots, bias / gamma / col_s slices
+constexpr int conv_smem_bytes(int block_n, int stages) {
+  return stages * (kABytes + block_n * kBlockK * 2) + kBlockM * block_n * 2 + 1024 + 256 + kGnSmemBytes + 3 * block_n * 4;
+}
 
 struct ConvTap {
   int16_t map, dw, dh, tap;
@@ -44,6 +59,7 @@ struct alignas(64) ConvKernelParams {
   CUtensorMap tmA[4];
   CUtensorMap tmB;
   CUtensorMap tmBh;  // half-height weight box of the cluster variant
+  CUtensorMap tmY, tmR;  // 16-bit output and residual {Cout, Wo, Ho, B}, box {SLAB, tile_w, tile_h, 1}
   ConvTap taps[kMaxTaps];
   int ntaps, kchunks;
   int n_tiles, m_tiles;
@@ -70,15 +86,21 @@ template <int BLOCK_N, int STAGES, bool F16, int CLUSTER, bool RELU_RES = false>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
   constexpr int B_BYTES = BLOCK_N * kBlockK * 2;
   constexpr int NACC = BLOCK_N / 2;  // accumulator registers per thread: m64 x BLOCK_N over 128 threads
+  constexpr int SLAB = conv_slab(BLOCK_N), SLAB_BYTES = kBlockM * SLAB * 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = sA + STAGES * kABytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
+  uint8_t* sY = sB + STAGES * B_BYTES;  // 16-bit output staging tile (1024-byte aligned, as the 128-byte swizzle needs)
+  uint64_t* full = reinterpret_cast<uint64_t*>(sY + kBlockM * BLOCK_N * 2);
   uint64_t* empty = full + STAGES;
+  uint64_t* epi_full = empty + STAGES;  // the tile's residual and column slices are in shared memory
   // per-CTA GroupNorm accumulators (fixed point): the epilogue adds into shared memory, ONE global atomic per group and tile
   // follows (the short-K GN convs are otherwise bound by global atomics on the few addresses of an image)
-  unsigned long long* gn_acc = reinterpret_cast<unsigned long long*>(smem + STAGES * (kABytes + B_BYTES) + 256);
+  unsigned long long* gn_acc = reinterpret_cast<unsigned long long*>(reinterpret_cast<uint8_t*>(full) + 256);
+  float* s_bias = reinterpret_cast<float*>(gn_acc + 2 * kGnMaxLocal * 2);
+  float* s_gamma = s_bias + BLOCK_N;
+  float* s_cols = s_gamma + BLOCK_N;
 
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kiters = p.ntaps * p.kchunks;
@@ -98,6 +120,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], kConvConsumers * CLUSTER);
     }
+    mbar_init(epi_full, 32);  // every lane of the DMA warp (their column-slice writes are released by their own arrive)
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < 2 * kGnMaxLocal * 2; i += kConvThreads) gn_acc[i] = 0ull;
@@ -137,6 +160,42 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         }
       }
     }
+  } else if (warp == 1) {
+    // ---------------- epilogue DMA: lane 0 issues (and so owns the bulk-store groups it waits on), every lane copies columns
+    const bool stage_y = p.y_dtype != UC_F32;
+    for (int item = item0; item < num_items; item += item_step) {
+      const int n0 = (item % p.n_tiles) * BLOCK_N;
+      const int mt = (item / p.n_tiles) * CLUSTER + crank;
+      const bool tile_ok = mt < p.m_tiles;
+      const int ow0 = (mt % p.tiles_w) * p.tile_w, oh0 = ((mt / p.tiles_w) % p.tiles_h) * p.tile_h;
+      const int b = mt / (p.tiles_w * p.tiles_h);
+      const int limit = min(BLOCK_N, p.Cout - n0);
+      const int nslabs = (limit + SLAB - 1) / SLAB;  // slabs holding valid columns
+      // the consumers are done with the previous tile's slices (kEpiBar below); no 16-byte alignment is guaranteed here
+      for (int i = lane; i < BLOCK_N; i += 32) {
+        const bool in = i < limit;
+        s_bias[i] = in && p.bias ? __ldg(p.bias + n0 + i) : 0.f;
+        s_gamma[i] = in && p.gamma ? __ldg(p.gamma + n0 + i) : 1.f;  // x * 1 is exact: no branch on gamma in the epilogue
+        if (p.row_stats) s_cols[i] = in ? __ldg(p.col_s + n0 + i) : 0.f;
+      }
+      if (lane == 0) {
+        tma_store_wait_read();  // the previous tile's store has read the staging tile
+        if (p.res && tile_ok) {
+          mbar_arrive_expect_tx(epi_full, nslabs * SLAB_BYTES);
+          for (int j = 0; j < nslabs; ++j) tma_load_4d(sY + j * SLAB_BYTES, &p.tmR, epi_full, n0 + j * SLAB, ow0, oh0, b);
+        } else {
+          mbar_arrive(epi_full);
+        }
+      } else {
+        mbar_arrive(epi_full);
+      }
+      named_sync(kEpiBar, kConvConsumers * 128 + 32);  // the consumers have staged this tile
+      if (stage_y && tile_ok && lane == 0) {
+        for (int j = 0; j < nslabs; ++j) tma_store_4d(&p.tmY, sY + j * SLAB_BYTES, n0 + j * SLAB, ow0, oh0, b);
+        tma_store_commit();
+      }
+    }
+    if (lane == 0) tma_store_wait_all();
   } else if (wg > 0) {
     regs_alloc<232>();
     // ---------------- consumers: warpgroup c = pixels 64c .. 64c+63 of the tile.  Accumulator fragment of thread (warp w of the
@@ -145,9 +204,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     const int c = wg - 1, ct = threadIdx.x - 128;
     const int g = lane >> 2, t = lane & 3;
     const int r0 = c * 64 + (warp & 3) * 16 + g;
-    const bool f16o = p.y_dtype == UC_F16;
+    const bool f16o = p.y_dtype == UC_F16, f32o = p.y_dtype == UC_F32, has_res = p.res != nullptr;
+    // this thread's two staging rows: byte offset inside a slab, and the swizzle (16-byte chunk XOR) of the row
+    uint32_t srow[2], sswz[2];
+  #pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      srow[h] = (r0 + 8 * h) * (SLAB * 2);
+      sswz[h] = ((srow[h] >> 7) & (SLAB / 8 - 1)) << 4;
+    }
     const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(sA + c * 64 * 128)), b_desc0 = wgmma_desc_sw128(smem_u32(sB));
-    int stage = 0, phase = 0, gpar = 0;
+    int stage = 0, phase = 0, gpar = 0, epar = 0;
     float acc[NACC];
     for (int item = item0; item < num_items; item += item_step) {
       const int n0 = (item % p.n_tiles) * BLOCK_N;
@@ -216,17 +282,21 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           gcur[j] = -1;
         }
       };
+      mbar_wait(epi_full, epar);  // residual (staged in place of the output) and column slices of this tile
+      epar ^= 1;
   #pragma unroll
       for (int i = 0; i < BLOCK_N / 8; ++i) {
         if (8 * i >= limit) break;  // warp-uniform
-        const int cbase = n0 + 8 * i + 2 * t;
-        const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + cbase)) : make_float2(0.f, 0.f);
+        const int cl = 8 * i + 2 * t, cbase = n0 + cl;
+        uint8_t* const slab = sY + (8 * i / SLAB) * SLAB_BYTES;
+        const uint32_t cbyte = (8 * i % SLAB + 2 * t) * 2;
+        const float2 bb = *reinterpret_cast<const float2*>(s_bias + cl);
         f32x2 hv[2];
   #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const f32x2 v = pk2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
           if (p.row_stats) {
-            const float2 cs = __ldg(reinterpret_cast<const float2*>(p.col_s + cbase));
+            const float2 cs = *reinterpret_cast<const float2*>(s_cols + cl);
             const f32x2 nm = pk2(-r_murstd[h], -r_murstd[h]);
             hv[h] = fma2(v, pk2(r_rstd[h], r_rstd[h]), fma2(nm, pk2(cs.x, cs.y), pk2(bb.x, bb.y)));
           } else {
@@ -252,26 +322,25 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             else hv[h] = pk2(apply_act(lo2(hv[h]), p.act), apply_act(hi2(hv[h]), p.act));
           }
         }
-        if (p.gamma) {
-          const float2 gm = __ldg(reinterpret_cast<const float2*>(p.gamma + cbase));
-  #pragma unroll
-          for (int h = 0; h < 2; ++h) hv[h] = mul2(hv[h], pk2(gm.x, gm.y));
-        }
+        const float2 gm = *reinterpret_cast<const float2*>(s_gamma + cl);
   #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (!valid[h]) continue;
-          if (p.res) {
-            const uint32_t rw = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.res) + pix[h] * p.ldres + cbase));
+          hv[h] = mul2(hv[h], pk2(gm.x, gm.y));
+          if (f32o) {  // no residual with fp32 y
+            if (valid[h]) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + pix[h] * p.ldy + cbase) = hv[h];
+            continue;
+          }
+          uint32_t* const sy = reinterpret_cast<uint32_t*>(slab + srow[h] + (cbyte ^ sswz[h]));
+          if (has_res) {
+            const uint32_t rw = *sy;
             hv[h] = add2(hv[h], f16o ? pk2(bits16_to_float(rw & 0xffffu, UC_F16), bits16_to_float(rw >> 16, UC_F16)) : pk2(bf16lo(rw), bf16hi(rw)));
           }
           if (RELU_RES) hv[h] = pk2(fmaxf(lo2(hv[h]), 0.f), fmaxf(hi2(hv[h]), 0.f));
-          if (p.y_dtype == UC_F32) {
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + pix[h] * p.ldy + cbase) = hv[h];
-          } else {
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.y) + pix[h] * p.ldy + cbase) = pack2_fast(lo2(hv[h]), hi2(hv[h]), f16o);
-          }
+          *sy = pack2_fast(lo2(hv[h]), hi2(hv[h]), f16o);
         }
       }
+      if (!f32o) fence_proxy_async();  // the TMA store (async proxy) reads what these generic-proxy writes staged
+      named_arrive(kEpiBar, kConvConsumers * 128 + 32);
       if (p.gn_stats) {
         gn_flush();
         // every consumer thread has added its partial sums of this tile: one global atomic per group, then the slots are cleared for
@@ -298,7 +367,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 
 template <int BLOCK_N, int STAGES, int CLUSTER, bool RELU_RES>
 static int launch_conv(ConvKernelParams& p, bool f16, cudaStream_t stream) {
-  constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2) + 1024 + 256 + kGnSmemBytes;
+  constexpr int smem = conv_smem_bytes(BLOCK_N, STAGES);
+  static_assert(smem <= 227 * 1024, "conv_gemm: shared memory over the 227 KB per-block limit");
   static PerDeviceFlag attr_dev;
   bool& attr = attr_dev.get();
   // the ReLU-after-residual variant exists for bf16 operands only (uc_conv2d rejects f16 x with act_after_res)
@@ -345,16 +415,16 @@ template <bool RELU_RES>
 static int launch_block_n(ConvKernelParams& p, int bn, bool cluster2, bool f16, cudaStream_t stream) {
   if (cluster2) {
     switch (bn) {
-      case 256: return launch_conv<256, 4, 2, RELU_RES>(p, f16, stream);
-      case 192: return launch_conv<192, 5, 2, RELU_RES>(p, f16, stream);
-      case 128: return launch_conv<128, 6, 2, RELU_RES>(p, f16, stream);
+      case 256: return launch_conv<256, 3, 2, RELU_RES>(p, f16, stream);
+      case 192: return launch_conv<192, 4, 2, RELU_RES>(p, f16, stream);
+      case 128: return launch_conv<128, 5, 2, RELU_RES>(p, f16, stream);
       default: return set_error(UC_EINVAL, "uc_conv2d: the cluster variant exists for block_n 128/192/256 only");
     }
   }
-  switch (bn) {  // stage rings of 144 - 200 KB (227 KB of shared memory per block)
-    case 256: return launch_conv<256, 4, 1, RELU_RES>(p, f16, stream);
-    case 192: return launch_conv<192, 5, 1, RELU_RES>(p, f16, stream);
-    case 128: return launch_conv<128, 6, 1, RELU_RES>(p, f16, stream);
+  switch (bn) {  // stage ring + output staging tile: 151 - 214 KB (227 KB of shared memory per block)
+    case 256: return launch_conv<256, 3, 1, RELU_RES>(p, f16, stream);
+    case 192: return launch_conv<192, 4, 1, RELU_RES>(p, f16, stream);
+    case 128: return launch_conv<128, 5, 1, RELU_RES>(p, f16, stream);
     case 96: return launch_conv<96, 6, 1, RELU_RES>(p, f16, stream);
     case 64: return launch_conv<64, 8, 1, RELU_RES>(p, f16, stream);
     case 32: return launch_conv<32, 8, 1, RELU_RES>(p, f16, stream);
@@ -399,7 +469,8 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   if (d->KH * d->KW > kMaxTaps || d->KH < 1 || d->KW < 1) return set_error(UC_EINVAL, "uc_conv2d: at most 9 taps");
   if (d->pad < 0 || d->pad >= d->KH + 1) return set_error(UC_EINVAL, "uc_conv2d: bad pad");
   if (d->res && (d->ldres % 8 || d->y_dtype == UC_F32)) return set_error(UC_EINVAL, "uc_conv2d: residual needs 16-bit y, ldres%%8==0");
-  if ((reinterpret_cast<uintptr_t>(d->x) | reinterpret_cast<uintptr_t>(d->w) | reinterpret_cast<uintptr_t>(d->y)) & 15)
+  if ((reinterpret_cast<uintptr_t>(d->x) | reinterpret_cast<uintptr_t>(d->w) | reinterpret_cast<uintptr_t>(d->y) |
+       reinterpret_cast<uintptr_t>(d->res)) & 15)
     return set_error(UC_EINVAL, "uc_conv2d: pointers must be 16-byte aligned");
   if (d->gn_stats && (d->gn_groups <= 0 || d->Cout % d->gn_groups))
     return set_error(UC_EINVAL, "uc_conv2d: bad GroupNorm grouping");
@@ -492,6 +563,19 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     return set_error(UC_EINVAL, "uc_conv2d: N tile %d incompatible with GroupNorm group size %d", bn, p.gn_gs);
   p.n_tiles = (d->Cout + bn - 1) / bn;
   p.m_tiles = m_tiles;
+  if (d->y_dtype != UC_F32) {  // 16-bit y (and the residual, same dtype and geometry) moves by TMA through the staging tile
+    const int slab = conv_slab(bn);
+    const CUtensorMapSwizzle swz = slab == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : slab == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+    const CUtensorMapDataType ydt = d->y_dtype == UC_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(p.Wo), static_cast<uint64_t>(p.Ho), static_cast<uint64_t>(B)};
+    uint32_t box[4] = {static_cast<uint32_t>(slab), static_cast<uint32_t>(p.tile_w), static_cast<uint32_t>(p.tile_h), 1};
+    for (int r = 0; r < (d->res ? 2 : 1); ++r) {
+      const uint64_t ld = static_cast<uint64_t>(r ? d->ldres : d->ldy) * es;
+      uint64_t strides[3] = {ld, ld * p.Wo, ld * p.Wo * p.Ho};
+      rc = encode_tmap(r ? &p.tmR : &p.tmY, ydt, 4, r ? d->res : d->y, dims, strides, box, swz);
+      if (rc) return rc;
+    }
+  }
   const bool f16 = d->x_dtype == UC_F16;
   if (cluster2) {
     uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(nt), static_cast<uint64_t>(d->Cout)};

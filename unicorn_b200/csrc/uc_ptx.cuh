@@ -133,6 +133,8 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed store of this thread has completed (its writes are performed)
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------- wgmma
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -152,6 +154,8 @@ template <int R>
 __device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // named barrier over `count` threads (ids 1.. ; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// arrive on a named barrier without waiting for it (the threads that need the result use named_sync on the same id and count)
+__device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // K-major operand tile in shared memory, rows of 128 bytes, 128B swizzle (what a TMA box with a 128-byte inner extent and
 // CU_TENSOR_MAP_SWIZZLE_128B writes; the tile starts on a 1024-byte boundary).  8-row groups are 1024 B apart (SBO); LBO

@@ -276,7 +276,7 @@ class UnicornEngine:
         return os.path.join(os.path.dirname(os.path.abspath(__file__)), "tuned", f"{self.cfg_name}.json")
 
     def load_tuning(self, path=None):
-        """Per-layer N-tile choices committed under unicorn_b200/tuned/ (measured on an H100 80GB HBM3 at a 400 W power limit;
+        """Per-layer N-tile choices committed under unicorn_b200/tuned/ (measured on an H100 80GB HBM3 at a 700 W power limit;
         plan-time autotuning fills in whatever is missing).
         Returns the number of entries loaded."""
         import glob
