@@ -1,0 +1,6 @@
+// conv_gemm instantiations (conv_gemm.cuh), one file per group of epilogue variants so that they compile in parallel.
+#include "conv_gemm.cuh"
+
+namespace uc {
+template int conv_launch<kEpiAny, false>(const ConvKernelParams&, int, bool, cudaStream_t);
+}  // namespace uc
