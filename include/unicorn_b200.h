@@ -129,6 +129,7 @@ UC_API int uc_dwconv7_ln(const void* x_bf16, const float* w49, const float* bias
 
 /* Depthwise 7x7 (pad 3) + bias of the ConvNeXt block (convnext.py:43), TMA staged (csrc/dwconv_tma.cu); follow with uc_layernorm,
  * or give ln_stats and fold the LayerNorm into pwconv1 (UcConv2d.row_stats).  x, y NHWC bf16 contiguous, not in place; w49 fp32 [49][C].
+ * C % 8 == 0; x, y and w49 16-byte aligned, bias 8-byte aligned (UC_EINVAL otherwise).
  * ln_stats (optional, may be NULL): [B*H*W][2] int64 fixed point (value * 2^22), zeroed by the caller; receives the per-pixel
  * {sum, sum of squares} over C of the stored outputs.  work_counter (optional, may be NULL): one device int, ZERO before the launch,
  * used to hand out the tiles dynamically (balanced SM loads on small maps); NULL = static round-robin. */

@@ -43,7 +43,7 @@ def test_no_cpu_fallback():
 
 
 def test_new_entry_points_validate_arguments_before_any_launch():
-    """uc_dwconv7_mma / uc_convnext_mlp reject bad arguments with UC_EINVAL and a message, without touching the device (so this runs on
+    """uc_dwconv7 / uc_dwconv7_mma / uc_convnext_mlp reject bad arguments with UC_EINVAL and a message, without touching the device (so this runs on
     the CPU box): null pointers, aliasing maps, unsupported channel counts, misaligned pointers."""
     from unicorn_b200 import _lib
     lib = _lib.lib()
@@ -54,6 +54,9 @@ def test_new_entry_points_validate_arguments_before_any_launch():
     assert lib.uc_dwconv7_mma(a, b, a, 1, 8, 8, 32, None, None) != 0 and b"in-place" in lib.uc_last_error()
     assert lib.uc_dwconv7_mma(a, b, c, 1, 8, 8, 36, None, None) != 0 and b"multiple of 8" in lib.uc_last_error()
     assert lib.uc_dwconv7_mma(P(0x10008), b, c, 1, 8, 8, 32, None, None) != 0 and b"aligned" in lib.uc_last_error()
+    assert lib.uc_dwconv7(a, b, c, c, 1, 8, 8, 36, None, None, None) != 0 and b"multiple of 8" in lib.uc_last_error()
+    assert lib.uc_dwconv7(P(0x10008), b, c, c, 1, 8, 8, 32, None, None, None) != 0 and b"aligned" in lib.uc_last_error()
+    assert lib.uc_dwconv7(a, b, P(0x30004), c, 1, 8, 8, 32, None, None, None) != 0 and b"aligned" in lib.uc_last_error()
     assert lib.uc_convnext_mlp_supported(192) == 1 and lib.uc_convnext_mlp_supported(768) == 0
     f = ctypes.c_float(1e-6)
     assert lib.uc_convnext_mlp(a, b, c, b, c, c, None, 128, 192, f, None) != 0

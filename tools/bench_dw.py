@@ -1,5 +1,5 @@
 """Micro-benchmark of the HBM/issue-bound kernels of a ConvNeXt block front half on the ConvNeXt-L@800x1280 shapes: uc_dwconv7
-(TMA kernel; UC_DW_TILED=1 selects the cp.async kernel), with and without LayerNorm statistics, and uc_layernorm — timed as
+(fp32-FMA TMA kernel) with and without LayerNorm statistics, uc_dwconv7_mma (tensor cores) and uc_layernorm — timed as
 back-to-back CUDA-graph kernel nodes (CUDA events around a replay), working set L2 resident like in the frame."""
 import os, sys
 import torch
@@ -46,4 +46,4 @@ for name, H, W, C in SHAPES:
     byt = 4.0 * H * W * C  # algorithmic bytes: read + write the bf16 map once
     fl = 98.0 * H * W * C
     print(f"{name:7s} {H:4d}x{W:<4d} C={C:5d}  dwconv {t_dw:7.1f} us ({byt/t_dw/1e3:7.1f} GB/s = {byt/t_dw/1e3/HBM*100:5.1f}% HBM, {fl/t_dw/1e6:5.1f} TFLOP/s fp32)"
-          f"  MMA {t_mma:7.1f} us ({byt/t_mma/1e3/HBM*100:5.1f}% HBM)  static-schedule {t_static:7.1f} us  +stats {t_st:7.1f} us  layernorm {t_ln:6.1f} us  tiled={os.environ.get('UC_DW_TILED', '0')}", flush=True)
+          f"  MMA {t_mma:7.1f} us ({byt/t_mma/1e3/HBM*100:5.1f}% HBM)  static-schedule {t_static:7.1f} us  +stats {t_st:7.1f} us  layernorm {t_ln:6.1f} us", flush=True)

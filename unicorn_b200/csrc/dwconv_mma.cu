@@ -30,7 +30,6 @@
 #include "uc_common.h"
 #include "../../include/unicorn_b200.h"
 #include <algorithm>
-#include <stdlib.h>
 
 namespace uc {
 
@@ -43,6 +42,7 @@ constexpr int kMmPlanarBytes = kMmCH * kMmPlaneBytes;                 // 33792
 constexpr int kMmPairBytes = kMmCH * 7 * 8 * 4;                       // 7168: tap pair table of one chunk ...
 constexpr int kMmQBytes = kMmPairBytes + kMmCH * 4;                   // ... + its 32 biases (fp32) = 7296
 constexpr int kMmSmem = kMmStageBytes + kMmPlanarBytes + kMmQBytes + 128 + 128;
+constexpr int kMmWarps = 4, kMmCtasPerSm = 3;
 
 struct alignas(64) DwMmaParams {
   CUtensorMap tmX;
@@ -66,10 +66,8 @@ struct DwFrag {
   uint32_t q[2];
 };
 
-// NW = warps per CTA: 4 (8 channels per warp, 3 CTAs / SM; the default) or 8 (4 channels per warp, 2 CTAs / SM; experiments only)
-template <int NW>
-__global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 2) dwconv7_mma_kernel(const __grid_constant__ DwMmaParams p) {
-  constexpr int CPW = kMmCH / NW;  // channels per warp
+__global__ void __launch_bounds__(kMmWarps * 32, kMmCtasPerSm) dwconv7_mma_kernel(const __grid_constant__ DwMmaParams p) {
+  constexpr int CPW = kMmCH / kMmWarps;  // 8 channels per warp
   extern __shared__ uint8_t dsm_raw[];
   uint8_t* stage = dsm_raw + ((128u - (smem_u32(dsm_raw) & 127u)) & 127u);
   uint8_t* planar = stage + kMmStageBytes;                                           // [32 planes][22][24] bf16
@@ -161,7 +159,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 2) dwconv7_mma_kernel(c
     {
       const uint4* st = reinterpret_cast<const uint4*>(stage);
 #pragma unroll 3
-      for (int pp = warp * 8 + (lane >> 2); pp < kMmHH * kMmHW / 2; pp += NW * 8) {
+      for (int pp = warp * 8 + (lane >> 2); pp < kMmHH * kMmHW / 2; pp += kMmWarps * 8) {
         const uint4 va = st[(2 * pp + tsw) * 4 + tq];
         const uint4 vb = st[(2 * pp + (tsw ^ 1)) * 4 + tq];
         const uint32_t wa[4] = {va.x, va.y, va.z, va.w}, wb[4] = {vb.x, vb.y, vb.z, vb.w};
@@ -214,15 +212,10 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 2) dwconv7_mma_kernel(c
         for (int e = 0; e < 4; ++e) {
           const int r = g + (e >> 1) * 8, cl = nb * 8 + 2 * t + (e & 1);
           if (oh0 + r < p.H && ow0 + cl < p.W) {
-            uint16_t* dst = yb + (static_cast<size_t>(r) * p.W + cl) * p.C;
-            if constexpr (CPW == 8) {
-              uint4 o;
-              o.x = pack_bf16(acc[0][nb][e], acc[1][nb][e]); o.y = pack_bf16(acc[2][nb][e], acc[3][nb][e]);
-              o.z = pack_bf16(acc[4][nb][e], acc[5][nb][e]); o.w = pack_bf16(acc[6][nb][e], acc[7][nb][e]);
-              *reinterpret_cast<uint4*>(dst) = o;
-            } else {
-              *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(acc[0][nb][e], acc[1][nb][e]), pack_bf16(acc[2][nb][e], acc[3][nb][e]));
-            }
+            uint4 o;
+            o.x = pack_bf16(acc[0][nb][e], acc[1][nb][e]); o.y = pack_bf16(acc[2][nb][e], acc[3][nb][e]);
+            o.z = pack_bf16(acc[4][nb][e], acc[5][nb][e]); o.w = pack_bf16(acc[6][nb][e], acc[7][nb][e]);
+            *reinterpret_cast<uint4*>(yb + (static_cast<size_t>(r) * p.W + cl) * p.C) = o;
           }
         }
     }
@@ -261,21 +254,15 @@ extern "C" int uc_dwconv7_mma(const void* x_bf16, const void* qtab, void* y_bf16
   const long items = static_cast<long>(p.tiles_w) * p.tiles_h * B * ((C + kMmCH - 1) / kMmCH);
   if (items > 0x7fffffffL) return set_error(UC_EINVAL, "uc_dwconv7_mma: too many tiles");
   p.n_items = static_cast<int>(items);
-  // 4 warps per item (3 CTAs per SM); the 8-warp variant (UC_DW_MMA_WARPS=8, 2 CTAs per SM) is kept for experiments
-  static int forced = -1;
-  if (forced < 0) { const char* e = getenv("UC_DW_MMA_WARPS"); forced = e ? atoi(e) : 0; }
-  const bool wide = forced == 8;
   static PerDeviceFlag attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dwconv7_mma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMmSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(dwconv7_mma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMmSmem);
+    cudaError_t e = cudaFuncSetAttribute(dwconv7_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMmSmem);
     if (e != cudaSuccess) return set_error(static_cast<int>(e), "uc_dwconv7_mma: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr = true;
   }
-  const int grid = static_cast<int>(std::min<long>(items, static_cast<long>(num_sms()) * (wide ? 2 : 3)));
-  cudaError_t e = wide ? launch_pdl(dwconv7_mma_kernel<8>, dim3(grid), dim3(256), kMmSmem, stream, p)
-                       : launch_pdl(dwconv7_mma_kernel<4>, dim3(grid), dim3(128), kMmSmem, stream, p);
+  const int grid = static_cast<int>(std::min<long>(items, static_cast<long>(num_sms()) * kMmCtasPerSm));
+  cudaError_t e = launch_pdl(dwconv7_mma_kernel, dim3(grid), dim3(kMmWarps * 32), kMmSmem, stream, p);
   if (e != cudaSuccess) return set_error(static_cast<int>(e), "uc_dwconv7_mma launch: %s", cudaGetErrorString(e));
   return check_launch("uc_dwconv7_mma");
 }

@@ -20,7 +20,6 @@
 #include "uc_common.h"
 #include "../../include/unicorn_b200.h"
 #include <algorithm>
-#include <stdlib.h>
 
 namespace uc {
 
@@ -197,28 +196,19 @@ __global__ void __launch_bounds__(kDwThreads, kDwCtasPerSm) dwconv7_tma_kernel(c
   }
 }
 
-static bool dw_use_tiled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("UC_DW_TILED"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v != 0;
-}
-
 }  // namespace uc
 
 using namespace uc;
-
-extern "C" int uc_dwconv7_tiled(const void* x_bf16, const float* w49, const float* bias, void* y_bf16, int B, int H, int W, int C,
-                                void* ln_stats, void* stream_v);
 
 extern "C" int uc_dwconv7(const void* x_bf16, const float* w49, const float* bias, void* y_bf16, int B, int H, int W, int C,
                           void* ln_stats, int* work_counter, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (!x_bf16 || !w49 || !bias || !y_bf16) return set_error(UC_EINVAL, "uc_dwconv7: null pointer");
   if (x_bf16 == y_bf16) return set_error(UC_EINVAL, "uc_dwconv7: not an in-place operation");
-  if (B < 1 || H < 1 || W < 1 || C < 8) return set_error(UC_EINVAL, "uc_dwconv7: bad sizes");
-  if (dw_use_tiled() || C % 8 || (reinterpret_cast<uintptr_t>(x_bf16) & 15) || (reinterpret_cast<uintptr_t>(w49) & 15) ||
+  if (B < 1 || H < 1 || W < 1 || C < 8 || C % 8) return set_error(UC_EINVAL, "uc_dwconv7: C must be a multiple of 8");
+  if (((reinterpret_cast<uintptr_t>(x_bf16) | reinterpret_cast<uintptr_t>(y_bf16) | reinterpret_cast<uintptr_t>(w49)) & 15) ||
       (reinterpret_cast<uintptr_t>(bias) & 7))
-    return uc_dwconv7_tiled(x_bf16, w49, bias, y_bf16, B, H, W, C, ln_stats, stream_v);  // cp.async kernel (no TMA alignment needs)
+    return set_error(UC_EINVAL, "uc_dwconv7: 16-byte aligned maps and taps, 8-byte aligned bias");
   int rc = ensure_driver();
   if (rc) return rc;
   DwParams p;

@@ -182,108 +182,6 @@ __global__ void __launch_bounds__(768) dwconv7_ln_kernel(const uint32_t* __restr
   }
 }
 
-// ------------------------------------------------------------------------------------------------ dwconv7 (tiled)
-// Depthwise 7x7 (pad 3) + bias on a channel chunk of CCH channels and a TH x 16 output tile staged (with its 3-pixel
-// halo) in shared memory by cp.async; out-of-map halo pixels are zero-filled.  The LayerNorm that follows in the
-// ConvNeXt block runs as uc_layernorm on the (L2-resident) result.  x, y NHWC bf16 [B,H,W,C]; w [49][C] fp32.
-template <int CCH>
-__global__ void __launch_bounds__(512, 2) dwconv7_tiled_kernel(const uint16_t* __restrict__ x, const float* __restrict__ w,
-                                                                const float* __restrict__ bias, uint16_t* __restrict__ y, int H,
-                                                                int W, int C, int tiles_w, long long* __restrict__ ln_stats) {
-  pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
-  pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
-  // 512 threads = (CCH/2 channel pairs) x (TH rows) x (2 half rows of 8 pixels): 16 accumulators + 14 staged inputs per
-  // thread stay in registers (a 16-pixel strip per thread made the compiler re-read shared memory for every tap).
-  constexpr int TW = 16, PX = 8, PAIRS = CCH / 2, TH = 512 / (PAIRS * 2), HW_ = TW + 6, HH_ = TH + 6;
-  constexpr int PIX_BYTES = CCH * 2, CHUNKS = PIX_BYTES / 16;
-  extern __shared__ __align__(16) uint8_t dsm[];
-  uint8_t* tile = dsm;                                             // [HH_][HW_][CCH] bf16
-  float* sw = reinterpret_cast<float*>(dsm + HH_ * HW_ * PIX_BYTES);  // [49][CCH]
-  const int b = blockIdx.z;
-  const int c0 = blockIdx.y * CCH;
-  const int ow0 = (blockIdx.x % tiles_w) * TW, oh0 = (blockIdx.x / tiles_w) * TH;
-  const uint16_t* xb = x + static_cast<long>(b) * H * W * C;
-  for (int i = threadIdx.x; i < HH_ * HW_ * CHUNKS; i += 512) {
-    const int ch = i % CHUNKS, px = i / CHUNKS;
-    const int hx = px % HW_, hy = px / HW_;
-    const int ih = oh0 + hy - 3, iw = ow0 + hx - 3;
-    uint8_t* dst = tile + px * PIX_BYTES + ch * 16;
-    if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
-      const uint16_t* src = xb + (static_cast<long>(ih) * W + iw) * C + c0 + ch * 8;
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(dst))), "l"(src) : "memory");
-    } else {
-      *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
-  for (int i = threadIdx.x; i < 49 * CCH; i += 512) sw[i] = __ldg(w + static_cast<long>(i / CCH) * C + c0 + (i % CCH));
-  asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-  __syncthreads();
-  const int cp = threadIdx.x % PAIRS;
-  const int hx = (threadIdx.x / PAIRS) & 1, r = threadIdx.x / (PAIRS * 2);
-  // accumulators and operands are (channel 2cp, channel 2cp+1) pairs: one fma_pair per tap
-  // and pixel instead of two scalar FMAs — the kernel is instruction-issue bound.
-  unsigned long long acc[PX];
-  {
-    const float b0 = __ldg(bias + c0 + 2 * cp), b1 = __ldg(bias + c0 + 2 * cp + 1);
-    const unsigned long long bb = (static_cast<unsigned long long>(__float_as_uint(b1)) << 32) | __float_as_uint(b0);
-#pragma unroll
-    for (int p = 0; p < PX; ++p) acc[p] = bb;
-  }
-#pragma unroll 1
-  for (int kh = 0; kh < 7; ++kh) {
-    const uint32_t* rowp = reinterpret_cast<const uint32_t*>(tile + ((r + kh) * HW_ + hx * PX) * PIX_BYTES) + cp;
-    unsigned long long v[PX + 6];
-#pragma unroll
-    for (int j = 0; j < PX + 6; ++j) {
-      const uint32_t u = rowp[j * (PIX_BYTES / 4)];
-      v[j] = (static_cast<unsigned long long>(u & 0xffff0000u) << 32) | (u << 16);  // (lo -> .x, hi -> .y) as fp32 bits
-    }
-#pragma unroll
-    for (int kw = 0; kw < 7; ++kw) {
-      const unsigned long long wv = *reinterpret_cast<const unsigned long long*>(sw + (kh * 7 + kw) * CCH + 2 * cp);
-#pragma unroll
-      for (int p = 0; p < PX; ++p) fma_pair(acc[p], v[p + kw], wv);
-    }
-  }
-  float a0[PX], a1[PX];
-#pragma unroll
-  for (int p = 0; p < PX; ++p) {
-    a0[p] = __uint_as_float(static_cast<uint32_t>(acc[p] & 0xffffffffull));
-    a1[p] = __uint_as_float(static_cast<uint32_t>(acc[p] >> 32));
-  }
-  const int oh = oh0 + r;
-  if (ln_stats) {
-    // Per-pixel LayerNorm statistics of the STORED (bf16-rounded) values, summed over this CTA's CCH channels and added to
-    // [pixel]{sum, sumsq} in fixed point (order independent): the following pwconv1 applies the normalisation in its
-    // epilogue (LayerNorm folded into the GEMM), so the separate LayerNorm pass disappears.
-#pragma unroll
-    for (int p = 0; p < PX; ++p) {
-      const uint32_t pk = pack_bf16(a0[p], a1[p]);
-      const float r0 = bf16lo(pk), r1 = bf16hi(pk);
-      float s1 = r0 + r1, s2 = fmaf(r0, r0, r1 * r1);
-#pragma unroll
-      for (int o = PAIRS / 2; o > 0; o >>= 1) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-      }
-      const int ow = ow0 + hx * PX + p;
-      if (cp == 0 && oh < H && ow < W) {
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(ln_stats) + ((static_cast<long>(b) * H + oh) * W + ow) * 2;
-        atomicAdd(dst, static_cast<unsigned long long>(__float2ll_rn(s1 * kGnFixedScale)));
-        atomicAdd(dst + 1, static_cast<unsigned long long>(__float2ll_rn(s2 * kGnFixedScale)));
-      }
-    }
-  }
-  if (oh < H) {
-    uint32_t* yr = reinterpret_cast<uint32_t*>(y + (static_cast<long>(b) * H + oh) * W * C + c0) + cp;
-#pragma unroll
-    for (int p = 0; p < PX; ++p) {
-      const int ow = ow0 + hx * PX + p;
-      if (ow < W) yr[static_cast<long>(ow) * (C / 2)] = pack_bf16(a0[p], a1[p]);
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ dwconv7 + LayerNorm (fused)
 // ConvNeXt block head (convnext.py:43-45, 48): y = LN_C(dwconv7x7(x) + bias).  One CTA owns a TW x TH pixel tile and ALL C
 // channels of it: it walks the channels in chunks of 64, staging each chunk's (TW+6) x (TH+6) halo tile and its 49 x 64
@@ -681,29 +579,6 @@ extern "C" int uc_dwconv7_ln(const void* x_bf16, const float* w49, const float* 
       static_cast<const uint32_t*>(x_bf16), reinterpret_cast<const float2*>(w49), reinterpret_cast<const float2*>(bias),
       reinterpret_cast<const float2*>(lnw), reinterpret_cast<const float2*>(lnb), static_cast<uint32_t*>(y_bf16), B, H, W, C2, eps);
   return check_launch("uc_dwconv7_ln");
-}
-
-// cp.async-staged depthwise kernel: the fallback of uc_dwconv7 (csrc/dwconv_tma.cu) for maps the TMA path cannot describe
-// (C % 8 != 0 / unaligned pointers) and the A/B reference for it (UC_DW_TILED=1).  Not part of the public C ABI.
-extern "C" int uc_dwconv7_tiled(const void* x_bf16, const float* w49, const float* bias, void* y_bf16, int B, int H, int W, int C,
-                                void* ln_stats, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!x_bf16 || !w49 || !bias || !y_bf16) return set_error(UC_EINVAL, "uc_dwconv7: null pointer");
-  if (C % 32) return set_error(UC_EINVAL, "uc_dwconv7: C must be a multiple of 32");
-  const int tiles_w = (W + 15) / 16;
-  if (C % 64 == 0) {
-    constexpr int smem = (8 + 6) * 22 * 128 + 49 * 64 * 4;
-    static PerDeviceFlag attr_dev;
-    bool& attr = attr_dev.get();
-    if (!attr) { cudaFuncSetAttribute(dwconv7_tiled_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr = true; }
-    dim3 grid(tiles_w * ((H + 7) / 8), C / 64, B);
-    launch_pdl(dwconv7_tiled_kernel<64>, grid, 512, smem, stream, static_cast<const uint16_t*>(x_bf16), w49, bias, static_cast<uint16_t*>(y_bf16), H, W, C, tiles_w, static_cast<long long*>(ln_stats));
-  } else {
-    constexpr int smem = (16 + 6) * 22 * 64 + 49 * 32 * 4;
-    dim3 grid(tiles_w * ((H + 15) / 16), C / 32, B);
-    launch_pdl(dwconv7_tiled_kernel<32>, grid, 512, smem, stream, static_cast<const uint16_t*>(x_bf16), w49, bias, static_cast<uint16_t*>(y_bf16), H, W, C, tiles_w, static_cast<long long*>(ln_stats));
-  }
-  return check_launch("uc_dwconv7");
 }
 
 extern "C" int uc_layernorm(const void* x, int ldx, const void* res, int ldres, const float* w, const float* b, void* y,

@@ -35,7 +35,7 @@ class _ConvGN:
 
 
 class UnicornEngine:
-    def __init__(self, state_dict, cfg_name, device="cuda", autotune=True, ln_fold=None):
+    def __init__(self, state_dict, cfg_name, device="cuda", autotune=True, ln_fold=False):
         ops._lib.check(ops._lib.lib().uc_check_device(), "uc_check_device")  # fail loudly without an sm_90 GPU
         self.cfg_name = cfg_name
         self.cfg = CONFIGS[cfg_name]
@@ -53,14 +53,9 @@ class UnicornEngine:
         self._with_masks = False
         self._bn_cache = {}
         self._bn_dirty = False
-        # ln_fold: the ConvNeXt blocks' LayerNorm is folded into pwconv1 (statistics from the depthwise kernel, normalisation in
-        # the GEMM epilogue) — UNTESTED on a GPU (round-2 item, DESIGN.md 9.2); off unless asked for / UC_LN_FOLD=1
-        self.ln_fold = bool(int(os.environ.get("UC_LN_FOLD", "0"))) if ln_fold is None else bool(ln_fold)
-        # depthwise 7x7 on tensor cores (csrc/dwconv_mma.cu; taps rounded to bf16) instead of the fp32-FMA kernel (csrc/dwconv_tma.cu)
-        self.dw_mma = bool(int(os.environ.get("UC_DW_MMA", "1")))
-        # LayerNorm -> pwconv1 -> GELU -> pwconv2 -> layer scale -> residual of the blocks with C = 96 / 192 / 256 / 384 in one launch (csrc/mlp_fused.cu)
-        self.mlp_fused = bool(int(os.environ.get("UC_MLP_FUSED", "1")))
-        self.mlp_min_rows = int(os.environ.get("UC_MLP_MIN_ROWS", "0"))  # head (C = 256) blocks: fused on maps with at least this many pixels (see convnext_block)
+        # ln_fold: the LayerNorm of the ConvNeXt blocks without a fused MLP is folded into pwconv1 (statistics from the fp32-FMA
+        # depthwise kernel, normalisation in the GEMM epilogue; tests/test_lnfold_gpu.py); off by default
+        self.ln_fold = bool(ln_fold)
         self._row_arena, self._row_used = None, 0
         self._ctr_arena, self._ctr_used = None, 0  # work counters of the dynamically scheduled kernels (zeroed by begin_frame)
         self.autotune = autotune
@@ -92,7 +87,8 @@ class UnicornEngine:
             d = dict(dw=ops.pack_dw_weight(sd[p + "dwconv.weight"].to(dev)), dwm=ops.pack_dw_weight_mma(sd[p + "dwconv.weight"].to(dev), sd[p + "dwconv.bias"].to(dev)), dwb=f(p + "dwconv.bias"), lnw=f(p + "norm.weight"),
                      lnb=f(p + "norm.bias"), w1=pw(p + "pwconv1.weight"), b1=f(p + "pwconv1.bias"), w2=pw(p + "pwconv2.weight"),
                      b2=f(p + "pwconv2.bias"), gamma=f(p + "gamma"))
-            d["fused"] = self.mlp_fused and ops.convnext_mlp_supported(d["lnw"].numel())
+            # LayerNorm -> pwconv1 -> GELU -> pwconv2 -> layer scale -> residual in one launch for C = 96 / 192 / 256 / 384 (csrc/mlp_fused.cu)
+            d["fused"] = ops.convnext_mlp_supported(d["lnw"].numel())
             if self.ln_fold or d["fused"]:  # W' = W diag(g) (16-bit), colsum(W') of the ROUNDED weights, c = W beta + b
                 w1 = sd[p + "pwconv1.weight"].to(dev, F32).reshape(d["b1"].numel(), -1)
                 d["w1f"] = ops.pack_conv_weight((w1 * d["lnw"][None, :])[:, :, None, None])
@@ -356,46 +352,27 @@ class UnicornEngine:
     def convnext_block(self, x, bp, tag):
         """In place on x (NHWC contiguous) — convnext.py:41-54."""
         B, H, W, C = x.shape
-        # two launches: the channel-chunked tiled depthwise kernel + a row LayerNorm on the L2-resident result (the fused
-        # one-CTA-per-pixel-tile kernel ops.dwconv7_ln needs 2.3x the instructions per output).
-        # The 4C hidden map of the first stages is larger than what stays in L2 next to everything else (64000 x 768 x 2 B = 98 MB in
-        # stage 1): pwconv1 -> pwconv2 pays an HBM round trip for it.  Running the pair per band of rows with ONE band-sized hidden
-        # buffer (rewritten by every band, so it stays in L2) quadruples the launches on a quarter of the rows each, so it is off by
-        # default (UC_MLP_BAND_MB = band size limit in MB enables it).
-        band_mb = float(os.environ.get("UC_MLP_BAND_MB", "0"))
-        nb = 1
-        if band_mb > 0 and B == 1:
-            nb = max(1, -(-(H * W * 4 * C * 2) // int(band_mb * 2 ** 20)))
-            while H % nb:
-                nb += 1
-        hb = H // nb
         # fused back half (csrc/mlp_fused.cu): one CTA per 128 rows.  On the head's small levels (32 and 8 row tiles at 800x1280) the launch
-        # occupies few SMs but the levels run on parallel streams next to other frames in flight, so there is no size gate by default
-        if bp.get("fused") and (C != 256 or B * H * W >= self.mlp_min_rows):
-            if self.dw_mma:
-                t = ops.dwconv7_mma(x, bp["dwm"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
-            else:
-                t = ops.dwconv7(x, bp["dw"], bp["dwb"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
+        # occupies few SMs but the levels run on parallel streams next to other frames in flight, so there is no size gate
+        if bp["fused"]:
+            t = ops.dwconv7_mma(x, bp["dwm"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
             ops.convnext_mlp(t.view(-1, C), bp["w1f"], bp["c1"], bp["w2"], bp["b2"], bp["gamma"], x.view(-1, C), 1e-6)
             return x
-        hid = self.buf(tag + ".h", (B, hb, W, 4 * C))
+        # The 4C hidden map can be larger than what stays in L2 next to everything else: pwconv1 -> pwconv2 then pays an HBM round trip
+        # for it.  Running the pair per band of rows with one band-sized hidden buffer quadruples the launches on a quarter of the rows
+        # each, so the whole map goes through at once.
+        hid = self.buf(tag + ".h", (B, H, W, 4 * C))
         if self.ln_fold and C % 32 == 0:
             rs = self._row_stats(B * H * W)
             t = ops.dwconv7(x, bp["dw"], bp["dwb"], out=self.buf(tag + ".t", x.shape), ln_stats=rs, work_counter=self._ctr())
-            for i in range(nb):
-                xs, ts = x[:, i * hb:(i + 1) * hb], t[:, i * hb:(i + 1) * hb]
-                self.conv(ts, bp["w1f"], 1, bias=bp["c1"], act=ACT_GELU, out=hid, row_stats=rs[i * hb * W:(i + 1) * hb * W], col_s=bp["s1"], row_eps=1e-6)
-                self.conv(hid, bp["w2"], 1, bias=bp["b2"], gamma=bp["gamma"], res=xs, out=xs)
-            return x
-        if self.dw_mma and C % 8 == 0:
-            t = ops.dwconv7_mma(x, bp["dwm"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
+            self.conv(t, bp["w1f"], 1, bias=bp["c1"], act=ACT_GELU, out=hid, row_stats=rs, col_s=bp["s1"], row_eps=1e-6)
         else:
-            t = ops.dwconv7(x, bp["dw"], bp["dwb"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
-        ops.layernorm(t.view(-1, C), bp["lnw"], bp["lnb"], 1e-6, out=t.view(-1, C))
-        for i in range(nb):
-            xs, ts = x[:, i * hb:(i + 1) * hb], t[:, i * hb:(i + 1) * hb]
-            self.conv(ts, bp["w1"], 1, bias=bp["b1"], act=ACT_GELU, out=hid)
-            self.conv(hid, bp["w2"], 1, bias=bp["b2"], gamma=bp["gamma"], res=xs, out=xs)
+            # two launches: the depthwise kernel + a row LayerNorm on the L2-resident result (the fused one-CTA-per-pixel-tile kernel
+            # ops.dwconv7_ln needs 2.3x the instructions per output)
+            t = ops.dwconv7_mma(x, bp["dwm"], out=self.buf(tag + ".t", x.shape), work_counter=self._ctr())
+            ops.layernorm(t.view(-1, C), bp["lnw"], bp["lnb"], 1e-6, out=t.view(-1, C))
+            self.conv(t, bp["w1"], 1, bias=bp["b1"], act=ACT_GELU, out=hid)
+        self.conv(hid, bp["w2"], 1, bias=bp["b2"], gamma=bp["gamma"], res=x, out=x)
         return x
 
     def csp(self, x, cp, out, tag):
