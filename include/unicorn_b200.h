@@ -266,6 +266,21 @@ typedef struct UcVosObject {
 UC_API int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win, int H, int W, float r, float* soft_out,
                             uint8_t* seg_out, void* stream);
 
+/* MOTS result encoding on the device (unicorn/evaluators/mot_evaluator.py:804-805, :858-866, :884-888): for the k instances of
+ * one frame, masks f32 [n_max,Hin,Win] (the uc_dynamic_masks output) are resized to the original H x W frame as in uc_vos_aggregate
+ * (only the hm x wm corner F.interpolate produces, hm = min(H, floor(Hin/r)), is encoded), thresholded (> thr), made overlap free
+ * (instance j keeps the pixels no instance before it in `order` had in its thresholded mask) and written as COCO compressed RLE
+ * strings (column-major runs from the zero run, unicorn_b200.results.rle_encode).  order: device int32 [k], the mask rows in
+ * ascending track id; emit: device uint8 [k], 0 = the instance still hides pixels from the later ones but gets an empty string.
+ * r is the letterbox ratio in double precision (the output size floor(Hin/r) depends on its last bits).  offsets: device int64
+ * [k+1], string j is chars[offsets[j] .. offsets[j+1]), offsets[k] = the chars needed; chars: device buffer of `capacity` bytes,
+ * nothing at or past capacity is written (re-run with a larger buffer: the call is idempotent).  workspace: device, 16-byte
+ * aligned, uc_mots_encode_workspace_bytes(k, H, W) bytes.  Three launches for k > 0, one for k = 0. */
+UC_API long uc_mots_encode_workspace_bytes(int k_max, int H, int W);
+UC_API int uc_mots_encode(const float* masks, int n_max, int Hin, int Win, const int* order, const uint8_t* emit, int k, float thr,
+                          double r, int H, int W, void* workspace, long workspace_bytes, char* chars, long capacity,
+                          long long* offsets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,10 @@ Eager launches (no CUDA graph: the association step returns to the host every fr
 steps, synthetic video, seeded weights.
   r50 : the SOT frame at 800x1280 of unicorn_track_r50 and, in the same process for comparison, of unicorn_track_large: CUDA graphs,
         one frame and three frames in flight, three alternating rounds.
-usage: bench_workloads.py mot|vos|r50 [frames]"""
+  mots: the MOTS frame of unicorn_track_large_mot_challenge_mask at 800x1280 from 1080x1920 originals, sequential eager and pipelined
+        with CUDA graphs, the host half it replaced on the same masks, and the mask encoding alone on 20 and 50 synthetic instances
+        (uc_mots_encode against results.mots_frame_result).
+usage: bench_workloads.py mot|vos|r50|mots [frames]"""
 import json, os, sys, time, types
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -111,6 +114,68 @@ elif what == "r50":
                 trk.collect()
             print(json.dumps({"workload": f"SOT 800x1280 {cfg}, CUDA graphs, {depth} frame(s) in flight", "round": rnd,
                               "frames_per_s": round(fps, 2), "ms_per_frame": round(ms, 2), "kernels_per_frame": launches, "n_gpus": 1}))
+elif what == "mots":
+    import subprocess
+    import torch.nn.functional as F
+    from unicorn_b200 import results as R
+    from unicorn_b200.mots import MaskEncoder, UnicornMOTSTracker
+    H, W, h0, w0 = 800, 1280, 1080, 1920
+    scale = min(H / float(h0), W / float(w0))
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}))
+    cfg = "unicorn_track_large_mot_challenge_mask"
+    eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+    frames, _ = make_video(4, H, W, seed=1, n_obj=6)
+    frames = [f[None].to(dev) for f in frames]
+    trk = UnicornMOTSTracker(eng, (H, W))
+    tracked = []
+    fps, ms, launches = timed(lambda i: tracked.append(len(trk.step_tensor(frames[i % 4], h0, w0)[1])), n)
+    print(json.dumps({"workload": f"MOTS 800x1280 {cfg} from 1080x1920 frames: detector + masks + QDTrack + device RLE, sequential eager",
+                      "frames_per_s": round(fps, 2), "ms_per_frame": round(ms, 2), "kernels_per_frame": launches,
+                      "tracks_per_frame": tracked[-n:], "n_gpus": 1}))
+
+    def host_half(i):
+        """the host half this driver replaced, on the driver's own masks: resize at the original size, read back, overlap, RLE"""
+        last = trk.last
+        m = torch.zeros(0, h0, w0, dtype=torch.bool)
+        if last["rows"].numel():
+            m = F.interpolate(last["masks"][last["rows"]][:, None], scale_factor=1 / scale, mode="bilinear",
+                              align_corners=False)[:, 0, :h0, :w0] > trk.mask_thres
+        R.mots_frame_result(i, last["boxes"], last["ids"], m.cpu(), h0, w0, trk.min_box_area)
+    trk.step_tensor(frames[0], h0, w0)
+    fps, ms, _ = timed(host_half, n)
+    print(json.dumps({"workload": "MOTS old host half on the same frame's masks (F.interpolate + .cpu() + results.mots_frame_result)",
+                      "tracks": int(trk.last["rows"].numel()), "ms_per_frame": round(ms, 3)}))
+    trk = UnicornMOTSTracker(eng, (H, W), use_graph=True)
+    trk.submit(frames[0], h0, w0)
+
+    def step(i):
+        trk.submit(frames[(i + 1) % 4], h0, w0)
+        trk.collect()
+    fps, ms, launches = timed(step, n, warm=5)
+    trk.collect()
+    print(json.dumps({"workload": "MOTS same, device half as CUDA graphs, host half of frame t overlapped with frame t+1",
+                      "frames_per_s": round(fps, 2), "ms_per_frame": round(ms, 2), "kernels_per_frame": launches, "n_gpus": 1}))
+    # seeded weights give few detections: the encode alone on synthetic elliptical instances at the original 1080x1920
+    yy, xx = torch.meshgrid(torch.arange(H, device=dev, dtype=torch.float32), torch.arange(W, device=dev, dtype=torch.float32), indexing="ij")
+    g = torch.Generator().manual_seed(0)
+    for k in (20, 50):
+        p = torch.rand(k, 4, generator=g).tolist()
+        masks = torch.stack([(((yy - a * H) / (40 + b * H / 4)) ** 2 + ((xx - c * W) / (40 + d * W / 4)) ** 2 < 1).float()
+                             for a, b, c, d in p]).contiguous()
+        boxes = torch.tensor([[0.0, 0.0, 100.0, 100.0, 1.0]] * k)
+        ids = torch.arange(k)
+        enc = MaskEncoder(k, dev)
+        dev_ms = timed(lambda i: enc(masks, list(range(k)), [True] * k, 0.3, scale, h0, w0), 2 * n)[1]
+        got = enc(masks, list(range(k)), [True] * k, 0.3, scale, h0, w0)
+
+        def host(i):
+            m = F.interpolate(masks[:, None], scale_factor=1 / scale, mode="bilinear", align_corners=False)[:, 0, :h0, :w0] > 0.3
+            return R.mots_frame_result(i, boxes, ids, m.cpu(), h0, w0, 0)
+        host_ms = timed(host, 3, warm=1)[1]
+        same = host(0)[5] == got
+        print(json.dumps({"workload": f"MOTS encode alone, {k} instances, 1080x1920", "uc_mots_encode_ms": round(dev_ms, 3),
+                          "host_mots_frame_result_ms": round(host_ms, 1), "identical_strings": same}))
 else:
     from unicorn_b200.vos import UnicornVOSTrack
     H, W = 800, 1280

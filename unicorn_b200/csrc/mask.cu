@@ -160,6 +160,31 @@ __global__ void __launch_bounds__(256) mask_final_up_kernel(const float* __restr
 }
 
 
+// ------------------------------------------------------------------------------------------------ resize to the original frame
+// F.interpolate(m, scale_factor=1/r, mode="bilinear", align_corners=False)[..., :H, :W] of an Hin x Win map, as the VOS and MOTS
+// evaluators resize network-resolution masks to the original frame.  PyTorch's output size is floor(in * (1/r)) in double
+// precision and its source scale is 1 / (1/r) rounded to float, so the result can be SHORTER than H x W (an 800-row input and a
+// 402-row frame give 401 rows): only the hm x wm corner is covered.
+struct FrameResize {
+  int hm, wm;
+  float scale;
+};
+static FrameResize frame_resize(int Hin, int Win, int H, int W, double r) {
+  const double sf = 1.0 / r;
+  return FrameResize{std::min(H, static_cast<int>(std::floor(Hin * sf))), std::min(W, static_cast<int>(std::floor(Win * sf))),
+                     static_cast<float>(1.0 / sf)};
+}
+// PyTorch's source index rule (see bilinear_kernel in misc_kernels.cu) for output index i of a source of n samples
+__device__ __forceinline__ void resize_src(int i, float scale, int n, int& i0, int& i1, float& l) {
+  const float f = fmaxf((i + 0.5f) * scale - 0.5f, 0.f);
+  i0 = min(static_cast<int>(f), n - 1);
+  i1 = min(i0 + 1, n - 1);
+  l = f - i0;
+}
+__device__ __forceinline__ float resize_sample(const float* s, int ld, int y0, int y1, int x0, int x1, float ly, float lx) {
+  return (1.f - ly) * ((1.f - lx) * s[y0 * ld + x0] + lx * s[y0 * ld + x1]) + ly * ((1.f - lx) * s[y1 * ld + x0] + lx * s[y1 * ld + x1]);
+}
+
 // ------------------------------------------------------------------------------------------------ VOS soft aggregation
 // external/lib/test/tracker/unicorn_vos.py:129-155 (resize of every object's best mask to the original frame:
 // F.interpolate(scale_factor=1/r, bilinear, align_corners=False)[:H, :W] into a zero map) and :105-121 (soft aggregation:
@@ -185,11 +210,9 @@ __global__ void __launch_bounds__(256) vos_aggregate_kernel(VosObjs o, int Hin, 
     const bool inside = y < hm && x < wm;
     int y0 = 0, y1 = 0, x0 = 0, x1 = 0;
     float ly = 0.f, lx = 0.f;
-    if (inside) {  // PyTorch's source index rule (see bilinear_kernel in misc_kernels.cu)
-      const float fy = fmaxf((y + 0.5f) * scale - 0.5f, 0.f), fx = fmaxf((x + 0.5f) * scale - 0.5f, 0.f);
-      y0 = min(static_cast<int>(fy), Hin - 1); x0 = min(static_cast<int>(fx), Win - 1);
-      y1 = min(y0 + 1, Hin - 1); x1 = min(x0 + 1, Win - 1);
-      ly = fy - y0; lx = fx - x0;
+    if (inside) {
+      resize_src(y, scale, Hin, y0, y1, ly);
+      resize_src(x, scale, Win, x0, x1, lx);
     }
     float bg = 1.f;
 #pragma unroll 1
@@ -198,8 +221,7 @@ __global__ void __launch_bounds__(256) vos_aggregate_kernel(VosObjs o, int Hin, 
       if (o.init_mask[k]) {
         v = o.init_mask[k][i] == static_cast<uint8_t>(o.id[k]) ? 1.f : 0.f;
       } else if (o.mask[k] && inside) {
-        const float* s = o.mask[k];
-        v = (1.f - ly) * ((1.f - lx) * s[y0 * Win + x0] + lx * s[y0 * Win + x1]) + ly * ((1.f - lx) * s[y1 * Win + x0] + lx * s[y1 * Win + x1]);
+        v = resize_sample(o.mask[k], Win, y0, y1, x0, x1, ly, lx);
       }
       m[k] = v;
       if (soft) soft[static_cast<long>(k) * total + i] = v;
@@ -214,6 +236,203 @@ __global__ void __launch_bounds__(256) vos_aggregate_kernel(VosObjs o, int Hin, 
     }
     seg[i] = static_cast<uint8_t>(label);
   }
+}
+
+// ------------------------------------------------------------------------------------------------ MOTS mask encoding
+// unicorn/evaluators/mot_evaluator.py:804-805 (resize + threshold), :858-866 (overlap free in ascending track id order against the
+// ORIGINAL masks of the earlier instances), :884-888 (COCO compressed RLE of the Fortran-ordered mask, results.rle_encode).
+// A mask is a column-major bit sequence of P = hm * wm pixels, stored as 32-bit words that never straddle a column: word
+// (x, wy) holds rows 32 wy .. 32 wy + 31 of column x.  The runs start with the zero run, so a run ends at every pixel whose bit
+// differs from the previous one (pixel -1 counts as 0) and at P; pass 1 stores exactly those boundary bits.
+constexpr int kMotsThreads = 1024;
+
+struct MotsWs {
+  uint32_t* diff;      // [k][words] run boundaries of the emitted instances
+  int4* state;         // [k][kMotsThreads] run state before each thread's chunk of words
+  int* char_off;       // [k][kMotsThreads] chars before each thread's chunk, within the instance
+  long long* nchars;   // [k] chars of each instance (0 when not emitted)
+};
+static inline long align16(long b) { return (b + 15) & ~15L; }
+static long mots_workspace_bytes(int k, long words) {
+  return align16(4L * k * words) + align16(16L * k * kMotsThreads) + align16(4L * k * kMotsThreads) + align16(8L * k);
+}
+static MotsWs mots_ws(void* base, int k, long words) {
+  char* p = static_cast<char*>(base);
+  MotsWs w;
+  w.diff = reinterpret_cast<uint32_t*>(p);
+  p += align16(4L * k * words);
+  w.state = reinterpret_cast<int4*>(p);
+  p += align16(16L * k * kMotsThreads);
+  w.char_off = reinterpret_cast<int*>(p);
+  p += align16(4L * k * kMotsThreads);
+  w.nchars = reinterpret_cast<long long*>(p);
+  return w;
+}
+
+// Pass 1: one thread per word, looping over the instances in `order`; the 32 lanes of a warp take 32 neighbouring columns of the
+// same rows, so their bilinear taps share source rows.  The pixel before the word is resampled too, so the boundary bits of the
+// word need no neighbour.
+__global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restrict__ masks, int n_max, int Hin, int Win,
+                                                          const int* __restrict__ order, const uint8_t* __restrict__ emit, int k, float thr,
+                                                          int hm, int wm, float scale, MotsWs ws) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int x = blockIdx.x * 32 + threadIdx.x, wy = blockIdx.y * 8 + threadIdx.y, hw32 = (hm + 31) / 32;
+  if (x >= wm || wy >= hw32) return;
+  const long words = static_cast<long>(wm) * hw32;
+  int x0, x1;
+  float lx;
+  resize_src(x, scale, Win, x0, x1, lx);
+  const bool has_prev = wy > 0 || x > 0;  // the pixel before this word in column-major order
+  int py0 = 0, py1 = 0, px0 = 0, px1 = 0;
+  float ply = 0.f, plx = 0.f;
+  if (has_prev) {
+    resize_src(wy > 0 ? 32 * wy - 1 : hm - 1, scale, Hin, py0, py1, ply);
+    resize_src(wy > 0 ? x : x - 1, scale, Win, px0, px1, plx);
+  }
+  const int ybase = 32 * wy, nrows = min(32, hm - ybase);
+  const uint32_t valid = nrows == 32 ? ~0u : (1u << nrows) - 1u;
+  uint32_t acc = 0, accp = 0;  // pixels claimed by the original masks of the earlier instances
+#pragma unroll 1
+  for (int j = 0; j < k; ++j) {
+    const int row = order[j];
+    uint32_t raw = 0, rawp = 0;
+    if (row >= 0 && row < n_max) {  // a row outside the mask buffer reads as an empty mask
+      const float* s = masks + static_cast<long>(row) * Hin * Win;
+#pragma unroll 4
+      for (int r = 0; r < nrows; ++r) {
+        int y0, y1;
+        float ly;
+        resize_src(ybase + r, scale, Hin, y0, y1, ly);
+        raw |= static_cast<uint32_t>(resize_sample(s, Win, y0, y1, x0, x1, ly, lx) > thr) << r;
+      }
+      if (has_prev) rawp = resize_sample(s, Win, py0, py1, px0, px1, ply, plx) > thr;
+    }
+    const uint32_t fr = raw & ~acc, frp = rawp & ~accp;
+    acc |= raw;
+    accp |= rawp;
+    if (emit[j]) ws.diff[j * words + static_cast<long>(x) * hw32 + wy] = (fr ^ ((fr << 1) | frp)) & valid;
+  }
+}
+
+// Run state after a prefix of the boundaries: their number and the last three boundary positions (-1: none).
+__device__ __forceinline__ int4 run_push(int4 s, int pos) { return make_int4(s.x + 1, pos, s.y, s.z); }
+__device__ __forceinline__ int4 run_cat(int4 a, int4 b) {
+  if (b.x >= 3) return make_int4(a.x + b.x, b.y, b.z, b.w);
+  if (b.x == 2) return make_int4(a.x + 2, b.y, b.z, a.y);
+  if (b.x == 1) return make_int4(a.x + 1, b.y, a.y, a.z);
+  return a;
+}
+// The COCO count that ends at `pos`, minus the count two before it (rleToString: "if (i > 2) x -= cnts[i - 2]").
+__device__ __forceinline__ int run_delta(int4 s, int pos) {
+  const int c = pos - (s.x >= 1 ? s.y : 0);
+  return s.x > 2 ? c - (s.z - s.w) : c;  // count i - 2 spans boundaries i - 3 .. i - 2
+}
+// 5 data bits per char with a continuation bit, +48; writes the chars below `cap` when out != nullptr, returns their number.
+__device__ __forceinline__ int rle_chars(int x, char* out, long long off, long cap) {
+  int n = 0;
+  bool more = true;
+  while (more) {
+    int c = x & 0x1f;
+    x >>= 5;
+    more = (c & 0x10) ? x != -1 : x != 0;
+    if (more) c |= 0x20;
+    if (out && off + n < cap) out[off + n] = static_cast<char>(c + 48);
+    ++n;
+  }
+  return n;
+}
+
+template <typename T, typename Op>
+__device__ T block_exclusive_scan(T v, T identity, Op op, T* sh, T& total) {
+  const int t = threadIdx.x, n = blockDim.x;
+  sh[t] = v;
+  __syncthreads();
+  for (int o = 1; o < n; o <<= 1) {
+    const T a = t >= o ? sh[t - o] : identity;
+    __syncthreads();
+    if (t >= o) sh[t] = op(a, sh[t]);
+    __syncthreads();
+  }
+  const T excl = t > 0 ? sh[t - 1] : identity;
+  total = sh[n - 1];
+  __syncthreads();
+  return excl;
+}
+
+// Walks the boundaries of words [w0, w1) of one instance from run state s; f(pos, s) sees the state before each boundary.
+template <typename F>
+__device__ __forceinline__ int4 mots_walk(const uint32_t* __restrict__ d, long w0, long w1, int hm, int hw32, int4 s, F f) {
+  for (long w = w0; w < w1; ++w) {
+    uint32_t bits = d[w];
+    if (!bits) continue;
+    const int x = static_cast<int>(w / hw32), wy = static_cast<int>(w - static_cast<long>(x) * hw32);
+    const int base = x * hm + 32 * wy;
+    while (bits) {
+      const int pos = base + __ffs(bits) - 1;
+      bits &= bits - 1;
+      f(pos, s);
+      s = run_push(s, pos);
+    }
+  }
+  return s;
+}
+
+// Pass 2: one block per instance; each thread owns a contiguous chunk of words.  Scan of the run states over the chunks, then the
+// number of chars of every count, scanned into each chunk's char offset.
+__global__ void __launch_bounds__(kMotsThreads) mots_runs_kernel(const uint8_t* __restrict__ emit, int k, int hm, int wm, MotsWs ws) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ int4 sh_state[kMotsThreads];
+  __shared__ long long sh_chars[kMotsThreads];
+  const int j = blockIdx.x, t = threadIdx.x;
+  if (!emit[j]) {
+    if (t == 0) ws.nchars[j] = 0;
+    return;
+  }
+  const int hw32 = (hm + 31) / 32;
+  const long words = static_cast<long>(wm) * hw32, chunk = (words + kMotsThreads - 1) / kMotsThreads;
+  const long w0 = std::min(words, t * chunk), w1 = std::min(words, w0 + chunk);
+  const uint32_t* d = ws.diff + j * words;
+  const int4 none = make_int4(0, -1, -1, -1);
+  const int4 mine = mots_walk(d, w0, w1, hm, hw32, none, [](int, int4) {});
+  int4 all;
+  const int4 pre = block_exclusive_scan(mine, none, [](int4 a, int4 b) { return run_cat(a, b); }, sh_state, all);
+  ws.state[j * kMotsThreads + t] = pre;
+  long long n = 0;
+  mots_walk(d, w0, w1, hm, hw32, pre, [&](int pos, int4 s) { n += rle_chars(run_delta(s, pos), nullptr, 0, 0); });
+  if (t == kMotsThreads - 1) n += rle_chars(run_delta(all, hm * wm), nullptr, 0, 0);  // the last run ends at P
+  long long total;
+  const long long off = block_exclusive_scan(n, 0LL, [](long long a, long long b) { return a + b; }, sh_chars, total);
+  ws.char_off[j * kMotsThreads + t] = static_cast<int>(off);
+  if (t == 0) ws.nchars[j] = total;
+}
+
+// Pass 3: the offsets of the k strings (block 0) and the chars of every emitted instance (block j), clipped at the capacity.
+__global__ void __launch_bounds__(kMotsThreads) mots_chars_kernel(const uint8_t* __restrict__ emit, int k, int hm, int wm, MotsWs ws,
+                                                                  char* __restrict__ chars, long capacity, long long* __restrict__ offsets) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ long long base;
+  const int j = blockIdx.x, t = threadIdx.x;
+  if (t == 0) {
+    long long b = 0;
+    for (int i = 0; i < k; ++i) {
+      if (j == 0) offsets[i] = b;
+      if (i == j) base = b;
+      b += ws.nchars[i];
+    }
+    if (j == 0) offsets[k] = b;
+  }
+  __syncthreads();
+  if (j >= k || !emit[j]) return;
+  const int hw32 = (hm + 31) / 32;
+  const long words = static_cast<long>(wm) * hw32, chunk = (words + kMotsThreads - 1) / kMotsThreads;
+  const long w0 = std::min(words, t * chunk), w1 = std::min(words, w0 + chunk);
+  long long off = base + ws.char_off[j * kMotsThreads + t];
+  const int4 end = mots_walk(ws.diff + j * words, w0, w1, hm, hw32, ws.state[j * kMotsThreads + t],
+                             [&](int pos, int4 s) { off += rle_chars(run_delta(s, pos), chars, off, capacity); });
+  if (t == kMotsThreads - 1) rle_chars(run_delta(end, hm * wm), chars, off, capacity);
 }
 
 }  // namespace uc
@@ -270,11 +489,42 @@ extern "C" int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win
     o.mask[k] = objs[k].mask; o.init_mask[k] = objs[k].init_mask; o.id[k] = objs[k].id; o.by_id[k] = k;
   }
   std::stable_sort(o.by_id, o.by_id + n, [&](int a, int b) { return o.id[a] < o.id[b]; });
-  // F.interpolate(scale_factor = 1/r): output size floor(in * (1/r)) in double precision, source scale 1 / (1/r) as a float
-  const double sf = 1.0 / static_cast<double>(r);
-  const int hm = std::min(H, static_cast<int>(std::floor(Hin * sf))), wm = std::min(W, static_cast<int>(std::floor(Win * sf)));
+  const FrameResize rs = frame_resize(Hin, Win, H, W, r);
   const long total = static_cast<long>(H) * W;
   const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, static_cast<long>(num_sms()) * 16)));
-  launch_pdl(vos_aggregate_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream_v), o, Hin, Win, H, W, hm, wm, static_cast<float>(1.0 / sf), soft_out, seg_out);
+  launch_pdl(vos_aggregate_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream_v), o, Hin, Win, H, W, rs.hm, rs.wm, rs.scale, soft_out, seg_out);
   return check_launch("uc_vos_aggregate");
+}
+
+extern "C" long uc_mots_encode_workspace_bytes(int k_max, int H, int W) {
+  if (k_max < 0 || H < 1 || W < 1) return -1;
+  return mots_workspace_bytes(k_max, W * ((H + 31) / 32));
+}
+
+extern "C" int uc_mots_encode(const float* masks, int n_max, int Hin, int Win, const int* order, const uint8_t* emit, int k, float thr,
+                              double r, int H, int W, void* workspace, long workspace_bytes, char* chars, long capacity,
+                              long long* offsets, void* stream_v) {
+  if (!masks || !order || !emit || !offsets || (k > 0 && !workspace) || (capacity > 0 && !chars))
+    return set_error(UC_EINVAL, "uc_mots_encode: null pointer");
+  if (n_max < 1 || Hin < 1 || Win < 1 || H < 1 || W < 1 || !(r > 0.0)) return set_error(UC_EINVAL, "uc_mots_encode: bad sizes");
+  if (k < 0 || k > n_max) return set_error(UC_EINVAL, "uc_mots_encode: k = %d must be in 0..n_max (%d)", k, n_max);
+  if (capacity < 0) return set_error(UC_EINVAL, "uc_mots_encode: negative capacity");
+  if ((reinterpret_cast<uintptr_t>(masks) | reinterpret_cast<uintptr_t>(order)) % 4 || reinterpret_cast<uintptr_t>(offsets) % 8 ||
+      reinterpret_cast<uintptr_t>(workspace) % 16)
+    return set_error(UC_EINVAL, "uc_mots_encode: masks / order must be 4-byte, offsets 8-byte, workspace 16-byte aligned");
+  const FrameResize rs = frame_resize(Hin, Win, H, W, r);
+  if (rs.hm < 1 || rs.wm < 1) return set_error(UC_EINVAL, "uc_mots_encode: the resized mask is empty (r too large)");
+  const int hw32 = (rs.hm + 31) / 32;
+  const long words = static_cast<long>(rs.wm) * hw32;
+  if (words > (1L << 31) / 32) return set_error(UC_EINVAL, "uc_mots_encode: frame too large");
+  if (workspace_bytes < mots_workspace_bytes(k, words)) return set_error(UC_EINVAL, "uc_mots_encode: workspace too small");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  MotsWs ws = mots_ws(workspace, k, words);
+  if (k > 0) {
+    launch_pdl(mots_planes_kernel, dim3((rs.wm + 31) / 32, (hw32 + 7) / 8), dim3(32, 8), 0, stream, masks, n_max, Hin, Win, order, emit, k, thr,
+               rs.hm, rs.wm, rs.scale, ws);
+    launch_pdl(mots_runs_kernel, k, kMotsThreads, 0, stream, emit, k, rs.hm, rs.wm, ws);
+  }
+  launch_pdl(mots_chars_kernel, std::max(k, 1), kMotsThreads, 0, stream, emit, k, rs.hm, rs.wm, ws, chars, capacity, offsets);
+  return check_launch("uc_mots_encode");
 }

@@ -1,62 +1,187 @@
-"""MOTS per-frame driver (UNTESTED ON A GPU — written after the round-1 GPU budget was spent; see tests/test_mots_gpu.py):
-the per-frame body of MOTEvaluator.evaluate_omni_mots (unicorn/evaluators/mot_evaluator.py:776-897) on the H100 engine:
-whole-mode detector with the CondInst controllers -> NMS -> dynamic-conv masks of the kept detections -> embedding
-sampling -> QuasiDenseEmbedTracker.match(return_index=True) -> masks of the tracked boxes in ascending-id order,
-overlap free, area filter, RLE (results.mots_frame_result)."""
+"""MOTS per-frame driver on the H100 engine — the per-frame body of MOTEvaluator.evaluate_omni_mots
+(unicorn/evaluators/mot_evaluator.py:776-897): whole-mode detector with the CondInst controllers -> NMS -> dynamic-conv masks of the
+kept detections -> embedding sampling -> QuasiDenseEmbedTracker.match(return_index=True) -> masks of the tracked boxes in
+ascending-id order, resized to the original frame, overlap free, area filter, COCO RLE.
+
+Like the QD arm of the MOT driver (mot.py) the frame is split in a device half and a host half:
+
+  submit(frame, img_h, img_w)  enqueues every kernel of the frame (with use_graph, one CUDA-graph replay from the second frame of
+                               a slot on), the masks into the slot's own buffer, and asynchronous copies of (count, detections,
+                               sampled embeddings) into pinned slot memory;
+  collect()                    waits for the oldest slot, runs the association on the host, and encodes the tracked masks on the
+                               device (uc_mots_encode on the association stream, so it does not queue behind the next frame).
+
+Two slots: submit(t+1) may precede collect(t).  The host reads back only detections, embeddings and the RLE strings; the masks
+never leave the device.  results.mots_frame_result is the host restatement the tests compare against."""
 import torch
-import torch.nn.functional as F
 
 from . import ops
 from .engine import UnicornEngine
-from .frames import anchor_count
+from .frames import FrameSlot, Ring
 from .mot import QDEmbedding
-from .results import mots_frame_result
 from .tracker import QuasiDenseEmbedTracker
+from .tracker._stream import assoc_stream
+
+
+class MaskEncoder:
+    """uc_mots_encode for one frame at a time, with the buffers it needs: the order / emit rows are uploaded from pinned memory and
+    the strings are read back into a pinned buffer.  When a frame needs more chars than the buffers hold, they grow and the
+    (idempotent) encode runs again."""
+
+    def __init__(self, k_max, device, capacity=1 << 16):
+        self.dev, self.k_max = torch.device(device), k_max
+        self.h_order = torch.zeros(k_max, dtype=torch.int32).pin_memory()
+        self.h_emit = torch.zeros(k_max, dtype=torch.uint8).pin_memory()
+        self.d_order = torch.zeros(k_max, dtype=torch.int32, device=device)
+        self.d_emit = torch.zeros(k_max, dtype=torch.uint8, device=device)
+        self.d_offsets = torch.zeros(k_max + 1, dtype=torch.int64, device=device)
+        self.h_offsets = torch.zeros(k_max + 1, dtype=torch.int64).pin_memory()
+        self.ws, self.ws_hw = None, (0, 0)
+        self._alloc(capacity)
+
+    def _alloc(self, capacity):
+        self.d_chars = torch.empty(capacity, dtype=torch.uint8, device=self.dev)
+        self.h_chars = torch.empty(capacity, dtype=torch.uint8).pin_memory()
+
+    def __call__(self, masks, order, emit, thr, r, img_h, img_w):
+        """masks fp32 [n_max,Hin,Win] (device); order: mask rows in ascending track id, emit: bools (host sequences).  Runs on the
+        current stream and waits for its result.  Returns the k strings ("" where emit is false)."""
+        k = len(order)
+        assert k <= self.k_max
+        if k == 0:
+            return []
+        if self.ws is None or img_h > self.ws_hw[0] or img_w > self.ws_hw[1]:
+            self.ws_hw = (max(img_h, self.ws_hw[0]), max(img_w, self.ws_hw[1]))
+            self.ws = ops.mots_encode_workspace(self.k_max, *self.ws_hw, self.dev)
+        self.h_order[:k] = torch.as_tensor(order, dtype=torch.int32)
+        self.h_emit[:k] = torch.as_tensor(emit, dtype=torch.uint8)
+        self.d_order[:k].copy_(self.h_order[:k], non_blocking=True)
+        self.d_emit[:k].copy_(self.h_emit[:k], non_blocking=True)
+        stream = torch.cuda.current_stream()
+        while True:
+            ops.mots_encode(masks, self.d_order[:k], self.d_emit[:k], thr, r, img_h, img_w, self.ws, self.d_chars, self.d_offsets)
+            self.h_offsets[:k + 1].copy_(self.d_offsets[:k + 1], non_blocking=True)
+            stream.synchronize()
+            total = int(self.h_offsets[k])
+            if total <= self.d_chars.numel():
+                break
+            self._alloc(max(total, 2 * self.d_chars.numel()))
+        self.h_chars[:total].copy_(self.d_chars[:total], non_blocking=True)
+        stream.synchronize()
+        s = self.h_chars[:total].numpy().tobytes().decode("ascii")
+        off = self.h_offsets[:k + 1].tolist()
+        return [s[off[i]:off[i + 1]] for i in range(k)]
+
+
+class _Slot(FrameSlot):
+    """One MOTS frame in flight: a frame slot plus its engine buffer tag, its mask buffer and its pinned results."""
+
+    def __init__(self, eng, H, W, tag, max_dets):
+        super().__init__(eng, H, W)
+        self.tag = tag
+        self.masks = torch.zeros(max_dets, H, W, dtype=torch.float32, device=eng.dev)  # uc_dynamic_masks output of the slot's frame
+        self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self.host_dets = torch.zeros(max_dets, 7).pin_memory()
+        self.host_feats = torch.zeros(max_dets, 128).pin_memory()
+        self.frame_id, self.img_hw = 0, (0, 0)
+        self.warm_u8 = None  # input dtype the slot last ran eagerly with: its next frame with it is captured
 
 
 class UnicornMOTSTracker:
     def __init__(self, engine: UnicornEngine, input_size, conf=0.01, nms=0.7, score_thr=0.1, max_dets=64, mask_thres=0.3, d_rate=2,
-                 min_box_area=100, tracker=None):
+                 min_box_area=100, tracker=None, use_graph=False):
         assert engine.cfg["mask"], "MOTS needs a *_mask model"
         self.eng, self.input_size = engine, tuple(input_size)
         self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets
         self.mask_thres, self.d_rate, self.min_box_area = mask_thres, d_rate, min_box_area
         self.tracker = tracker or QuasiDenseEmbedTracker(device=engine.dev)
+        self.use_graph = use_graph
         H, W = self.input_size
-        self.ws = ops.PostWorkspace(anchor_count(H, W), engine.dev)
-        self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=engine.dev)
         self._qd = QDEmbedding(engine, H, W, max_dets, "mots.emb")
-        self.frame_id = 0
+        up = 8 // d_rate
+        self._scratch = torch.empty(max_dets * (H // 8) * (W // 8) * (1 + up * up), dtype=torch.float32, device=engine.dev)
+        # two slots on this engine and the current stream, so that submit(t+1) may precede collect(t); they share the input buffers
+        # and the NMS workspace, each has its own backbone buffers (tag) and mask buffer
+        slots = [_Slot(engine, H, W, "mots%d" % i, max_dets) for i in range(2)]
+        slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
+        self._ring = Ring(slots)
+        self._slots = slots
+        self._enc = MaskEncoder(max_dets, engine.dev)
+        self.frame_id = 0  # frames submitted
         self.last = {}
 
-    def step_tensor(self, frame, img_h, img_w):
-        """frame: preprocessed fp32 [1,3,H,W]; (img_h, img_w): original image size.  Returns the tuple write_results_mots()
-        consumes for this frame: (frame_id, ids (1-based), cat_id, img_h, img_w, rles)."""
-        e = self.eng
-        H, W = self.input_size
-        self.frame_id += 1
-        self.img_in.copy_(frame, non_blocking=True)
+    # ------------------------------------------------------------------------------------------ device half
+    def _frame(self, c):
+        e = c.eng
         e.begin_frame()
-        fpn, seq = e.backbone(self.img_in, tag="mots%d" % (self.frame_id & 1))
+        fpn, seq = e.backbone(c.img, tag=c.tag)
         out = e.head(fpn, None, "mot", with_masks=True)
-        dets, cnt = ops.postprocess_device(out[0], e.ncls, self.conf, self.nms, self.ws)
+        dets, cnt = ops.postprocess_device(out[0], e.ncls, self.conf, self.nms, c.ws)
         mf, um = e.mask_branch(fpn)
         hw = [(t.shape[1], t.shape[2]) for t in e.dyn_levels]
-        masks = ops.dynamic_masks(mf, um, e.dyn_levels, hw, self.ws, self.max_dets, up_rate=8 // self.d_rate, d_rate=self.d_rate)
+        ops.dynamic_masks(mf, um, e.dyn_levels, hw, c.ws, self.max_dets, up_rate=8 // self.d_rate, d_rate=self.d_rate, out=c.masks,
+                          scratch=self._scratch)
         self._qd(e, seq["feat"], dets, cnt)  # pre_dict as in the MOT driver (:803-818)
-        n = min(int(cnt.item()), self.max_dets)
-        d, f = dets[:n].cpu(), self._qd.feats[:n].cpu()
+        c.last = dict(head=out, mask_feats=mf, up_masks=um, dyn=list(e.dyn_levels))
+
+    def submit(self, frame, img_h, img_w):
+        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; (img_h, img_w): original image size.  Enqueues
+        the frame; returns immediately."""
+        c = self._ring.submit()
+        self.frame_id = self._ring.submitted
+        c.stage(frame)
+        if c.graph is not None:
+            c.graph.replay()
+        elif self.use_graph and c.warm_u8 == c.u8:
+            # the slot's first frame ran eagerly (plan-time autotuning, buffer allocation); the second is captured without a
+            # warm-up run: a QD frame advances pre_dict, so it must not run twice
+            c.graph, _ = c.capture(lambda: self._frame(c))
+        else:
+            self._frame(c)
+            c.warm_u8 = c.u8
+        c.host_count.copy_(c.ws.count, non_blocking=True)
+        c.host_dets.copy_(c.ws.dets[:self.max_dets], non_blocking=True)
+        c.host_feats.copy_(self._qd.feats, non_blocking=True)
+        c.frame_id, c.img_hw = self.frame_id, (img_h, img_w)
+        c.event.record()
+        self.last = c.last
+
+    # ------------------------------------------------------------------------------------------ host half
+    def collect(self):
+        """Association and mask encoding of the oldest submitted frame.  Returns the tuple write_results_mots() consumes:
+        (frame_id, ids (1-based), cat_id, img_h, img_w, rles)."""
+        c = self._ring.collect()
+        c.event.synchronize()
+        img_h, img_w = c.img_hw
+        H, W = self.input_size
+        n = min(int(c.host_count[0]), self.max_dets)
+        d, f = c.host_dets[:n].clone(), c.host_feats[:n].clone()
         scale = min(H / float(img_h), W / float(img_w))
-        # masks at the original image scale, thresholded (:804-805)
-        m = F.interpolate(masks[:n, None], scale_factor=1 / scale, mode="bilinear", align_corners=False)[:, 0, :img_h, :img_w] > self.mask_thres
         scores = d[:, 4] * d[:, 5]
         keep = scores > self.score_thr
         boxes = torch.cat([d[keep, :4] / scale, scores[keep, None]], 1)
-        m, f = m[keep.to(m.device)], f[keep]
-        self.last = dict(dets=d, masks=masks[:n], head=out, mask_feats=mf, up_masks=um, dyn=[t for t in e.dyn_levels])
+        # the tracked boxes, their ids and mask rows (ascending id), what the frame's strings encode
+        c.last.update(dets=d, masks=c.masks[:n], boxes=torch.zeros(0, 5), ids=torch.zeros(0, dtype=torch.long),
+                      rows=torch.zeros(0, dtype=torch.long))
+        self.last = c.last
         if n == 0:  # outputs[0] is None: no tracking for this frame (mot_evaluator.py:803)
-            return self.frame_id, [], 2, img_h, img_w, []
-        ob, _, oid, idx = self.tracker.match(boxes, torch.ones(boxes.size(0)), f, self.frame_id, return_index=True)
-        m = m[idx.to(m.device)]
+            return c.frame_id, [], 2, img_h, img_w, []
+        ob, _, oid, idx = self.tracker.match(boxes, torch.ones(boxes.size(0)), f[keep], c.frame_id, return_index=True)
+        rows = torch.nonzero(keep).flatten()[idx]  # the mask row of every matched box (masks[keep][indexs], :838-840)
         valid = oid > -1
-        return mots_frame_result(self.frame_id, ob[valid], oid[valid], m[valid.to(m.device)].cpu(), img_h, img_w, self.min_box_area)
+        ob, oid, rows = ob[valid], oid[valid], rows[valid]
+        srt = oid.sort()[1]  # ascending track id (:842-846)
+        ob, oid, rows = ob[srt], oid[srt], rows[srt]
+        emit = [(x2 - x1) * (y2 - y1) > self.min_box_area for x1, y1, x2, y2 in ob[:, :4].tolist()]
+        c.last.update(boxes=ob, ids=oid, rows=rows)
+        stream = assoc_stream(self.eng.dev)
+        with torch.cuda.stream(stream):  # not behind the next frame's kernels on the main stream
+            stream.wait_event(c.event)
+            rles = self._enc(c.masks, rows.tolist(), emit, self.mask_thres, scale, img_h, img_w)
+        ids = [int(t) + 1 for t, e in zip(oid.tolist(), emit) if e]  # 1-based ids for the MOTS files
+        return c.frame_id, ids, 2, img_h, img_w, [s for s, e in zip(rles, emit) if e]
+
+    def step_tensor(self, frame, img_h, img_w):
+        """Sequential protocol of the reference: one frame in, its write_results_mots() tuple out."""
+        self.submit(frame, img_h, img_w)
+        return self.collect()

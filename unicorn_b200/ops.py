@@ -453,3 +453,23 @@ def dynamic_masks(mask_feats, up_masks, dyn_levels, level_hw, ws, n_max, up_rate
     _lib.check(_L().uc_dynamic_masks(_p(mask_feats), _p(up_masks), h, w, up_rate, d_rate, dl, dyn_levels[0].shape[-1], hw, st, so,
                                      _p(ws.anchors), _p(ws.count), n_max, _p(scratch), _p(out), _S()), "uc_dynamic_masks", 3)
     return out
+
+
+def mots_encode_workspace(k_max, H, W, device):
+    """Device workspace of uc_mots_encode for up to k_max instances on an H x W original frame."""
+    fn = _L().uc_mots_encode_workspace_bytes
+    fn.restype = ctypes.c_long
+    return torch.empty(fn(int(k_max), int(H), int(W)), dtype=torch.uint8, device=device)
+
+
+def mots_encode(masks, order, emit, thr, r, H, W, ws, chars, offsets):
+    """COCO RLE strings of the resized, thresholded, overlap-free masks of one MOTS frame (uc_mots_encode).  masks fp32
+    [n_max,Hin,Win]; order int32 [k] / emit uint8 [k] device; chars uint8 device buffer (its size is the capacity); offsets int64
+    device [>= k+1].  Launches only: offsets[k] is the number of chars needed, chars past the capacity are not written."""
+    n_max, Hin, Win = masks.shape
+    k = order.numel()
+    assert masks.dtype == torch.float32 and masks.is_contiguous() and order.dtype == torch.int32 and emit.dtype == torch.uint8
+    assert emit.numel() == k and chars.dtype == torch.uint8 and offsets.dtype == torch.int64 and offsets.numel() >= k + 1
+    _lib.check(_L().uc_mots_encode(_p(masks), n_max, Hin, Win, _p(order), _p(emit), k, _f(thr), ctypes.c_double(r), int(H), int(W),
+                                   _p(ws), _l(ws.numel()), _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_mots_encode", 3 if k else 1)
+    return offsets

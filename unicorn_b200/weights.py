@@ -18,6 +18,8 @@ CONFIGS = {
     "unicorn_track_large_mot_challenge": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=1, mask=False),
     "unicorn_track_tiny_mask": dict(depths=(3, 3, 9, 3), dims=(96, 192, 384, 768), num_classes=8, mask=True),
     "unicorn_track_large_mask": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=8, mask=True),
+    # the released MOTS20 model: the 1-class head of *_mot_challenge with the mask head of *_mask
+    "unicorn_track_large_mot_challenge_mask": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=1, mask=True),
     # exps/default/unicorn_track_r50*.py: torchvision ResNet-50 (v1.5 Bottlenecks); dims = the stage output widths (4 x 64/128/256/512)
     "unicorn_track_r50": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=False),
     "unicorn_track_r50_mask": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=True),
