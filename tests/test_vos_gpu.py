@@ -18,8 +18,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 def test_vos_aggregate_kernel_matches_definition():
     """unicorn_vos.py:139-155 (F.interpolate(scale_factor=1/r)[:H,:W] into a zero map) + :105-121 (float32 background product in
     list order, argmax with the lower channel winning ties) on random soft masks, one object given by its initial label map."""
-    import ctypes
-    from unicorn_b200 import _lib
+    from unicorn_b200 import ops
     g = torch.Generator().manual_seed(3)
     Hin, Win, H0, W0 = 96, 160, 113, 187
     r = min(Hin / H0, Win / W0)
@@ -41,15 +40,7 @@ def test_vos_aggregate_kernel_matches_definition():
     md, ld = masks.cuda().contiguous(), lab.cuda()
     soft = torch.zeros(4, H0, W0, device="cuda")
     seg = torch.zeros(H0, W0, dtype=torch.uint8, device="cuda")
-    objs = (_lib.UcVosObject * 4)()
-    for k, i in enumerate(ids):
-        objs[k].id = i
-        if k < 3:
-            objs[k].mask = md[k].data_ptr()
-        else:
-            objs[k].init_mask = ld.data_ptr()
-    _lib.check(_lib.lib().uc_vos_aggregate(objs, 4, Hin, Win, H0, W0, ctypes.c_float(r), ctypes.c_void_p(soft.data_ptr()),
-                                           ctypes.c_void_p(seg.data_ptr()), _lib.stream_ptr()), "uc_vos_aggregate")
+    ops.vos_aggregate([md[k] for k in range(3)], ld, ids, Hin, Win, r, soft, seg)
     assert np.abs(soft.cpu().numpy() - soft_ref).max() < 2e-6
     agree = (seg.cpu().numpy() == seg_ref).mean()
     assert agree > 0.9995, agree  # exact up to last-ulp differences of the bilinear weights at near ties

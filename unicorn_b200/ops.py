@@ -455,6 +455,28 @@ def dynamic_masks(mask_feats, up_masks, dyn_levels, level_hw, ws, n_max, up_rate
     return out
 
 
+def vos_aggregate(masks, init_mask, ids, Hin, Win, r, soft, seg):
+    """Result assembly of a VOS frame (uc_vos_aggregate): the soft masks of `ids` resized by 1/r to the original frame into soft fp32
+    [>= n, H0, W0], and the label map seg uint8 [H0, W0] (argmax over the background product and the objects, in list order).
+    masks: fp32 [1, Hin, Win] network-resolution masks of the first len(masks) ids; the remaining ids take (init_mask == id) of
+    init_mask, a uint8 [H0, W0] label map."""
+    n = len(ids)
+    H0, W0 = seg.shape
+    assert soft.dtype == torch.float32 and soft.is_contiguous() and soft.shape[0] >= n and tuple(soft.shape[1:]) == (H0, W0)
+    assert seg.dtype == torch.uint8 and seg.is_contiguous() and len(masks) <= n
+    objs = (_lib.UcVosObject * n)()
+    for k, oid in enumerate(ids):
+        objs[k].id = int(oid)
+        if k < len(masks):
+            assert masks[k].dtype == torch.float32 and masks[k].is_contiguous() and tuple(masks[k].shape[-2:]) == (Hin, Win)
+            objs[k].mask = masks[k].data_ptr()
+        else:
+            assert init_mask is not None and init_mask.dtype == torch.uint8 and tuple(init_mask.shape) == (H0, W0)
+            objs[k].init_mask = init_mask.data_ptr()
+    _lib.check(_L().uc_vos_aggregate(objs, n, Hin, Win, H0, W0, _f(r), _p(soft), _p(seg), _S()), "uc_vos_aggregate")
+    return seg
+
+
 def mots_encode_workspace(k_max, H, W, device):
     """Device workspace of uc_mots_encode for up to k_max instances on an H x W original frame."""
     fn = _L().uc_mots_encode_workspace_bytes

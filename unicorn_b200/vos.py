@@ -13,11 +13,9 @@ depth > 1: like in SOT, a frame depends only on the reference frames of its obje
 `submit(frame)` / `collect()` keep `depth` steady-state frames in flight, each in its own frame slot (engine fork, stream, buffers)
 sharing the reference groups; frames that add objects go through track_tensor() on slot 0 with the pipeline drained.
 """
-import ctypes
-
 import torch
 
-from . import _lib, ops
+from . import ops
 from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, in_flight
 from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
@@ -150,16 +148,7 @@ class UnicornVOSTrack:
         if s.seg is None or s.seg.shape != (H0, W0) or s.soft.shape[0] < n:
             s.seg = torch.zeros(H0, W0, dtype=torch.uint8, device=self.eng.dev)
             s.soft = torch.zeros(max(n, 4), H0, W0, dtype=torch.float32, device=self.eng.dev)
-        objs = (_lib.UcVosObject * n)()
-        n_old = len(self.obj_ids)
-        for k, oid in enumerate(ids):
-            objs[k].id = int(oid)
-            if k < n_old:
-                objs[k].mask = s.mask_bufs[k].data_ptr()
-            else:
-                objs[k].init_mask = init_mask.data_ptr()
-        _lib.check(_lib.lib().uc_vos_aggregate(objs, n, H, W, H0, W0, ctypes.c_float(self.r), ctypes.c_void_p(s.soft.data_ptr()),
-                                               ctypes.c_void_p(s.seg.data_ptr()), _lib.stream_ptr()), "uc_vos_aggregate")
+        ops.vos_aggregate(s.mask_bufs[:len(self.obj_ids)], init_mask, ids, H, W, self.r, s.soft, s.seg)
 
     def _enqueue(self, s, cur_frame, new_ids=(), new_boxes_xyxy=None, init_mask=None):
         """Device half of a frame in slot s on the current stream + the asynchronous read of the detection rows; no host
