@@ -191,11 +191,16 @@ UC_API int uc_nhwc_to_nchw_f32(const void* src, int lds, float* dst, int B, int 
 UC_API int uc_msda_forward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
                                const float* sampling_loc, const float* attn_weight, int B, int S, int M, int D, int L,
                                int Lq, int P, float* out, void* stream);
-/* Fused form used by the H100 path (B=1, head dim 32): value bf16 [S, M*32]; offlog f32 [Lq, ld] = raw
+/* Fused form used by the H100 path (head dim 32): value bf16 [S, M*32]; offlog f32 [Lq, ld] = raw
  * sampling_offsets (M*L*P*2) followed by attention logits (M*L*P); queries = concatenated level grids;
  * level_hw host int[2L] (h,w).  out bf16 [Lq, M*32]. */
 UC_API int uc_msda_fused_bf16(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw,
                               int L, int M, int P, void* stream);
+/* The same for B >= 1 images in one launch.  Rows of value / offlog / out are level-major with the images inside each level:
+ * level l of image b starts at row B * (h_0*w_0 + ... + h_{l-1}*w_{l-1}) + b * h_l*w_l (B = 1 is uc_msda_fused_bf16's layout).
+ * Every image samples only its own value rows.  B < 1: UC_EINVAL. */
+UC_API int uc_msda_fused_bf16_batched(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw,
+                                      int L, int M, int P, int B, void* stream);
 
 /* Fused correlation + softmax over reference positions + label propagation
  * (external/lib/test/tracker/unicorn_sot.py:95-100; unicorn_vos.py:171-181):
@@ -203,12 +208,23 @@ UC_API int uc_msda_fused_bf16(const void* value, const float* offlog, int ld_off
  * embed_* [n, C=128] 16-bit rows (NHWC embedding maps), values f32 [n_obj, ldv], out f32 [n_obj, ldo]; n_obj <= 8. */
 UC_API int uc_corr_propagate(const void* embed_ref, int ld_ref, int n_ref, const void* embed_cur, int ld_cur, int n_cur,
                              int C, int dtype, const float* values, int ldv, int n_obj, float* out, int ldo, void* stream);
+/* B >= 1 independent (embed_ref, embed_cur, values) -> out problems in one launch (grid: current-position tiles x sequences).
+ * bs_* are the element strides from one sequence to the next: bs_ref, bs_cur multiples of 8 and >= ld * n; bs_values >= ldv * n_obj;
+ * bs_out >= ldo * n_obj (UC_EINVAL otherwise; ignored when B = 1).  Each sequence's output equals its own uc_corr_propagate. */
+UC_API int uc_corr_propagate_batched(const void* embed_ref, int ld_ref, long bs_ref, int n_ref, const void* embed_cur, int ld_cur,
+                                     long bs_cur, int n_cur, int C, int dtype, const float* values, int ldv, long bs_values, int n_obj,
+                                     float* out, int ldo, long bs_out, int B, void* stream);
 
 /* Head decode (unicorn_head.py:332-334,467-482): per level regobj f32 [HW, ld_ro] = reg(4), obj logit;
  * cls f32 [HW, ld_cls] = class logits.  regobj/cls/hw/strides are HOST arrays of 3 device pointers / ints.
  * out f32 [sum HW, 5+ncls] = cx,cy,w,h,sigmoid(obj),sigmoid(cls..). */
 UC_API int uc_head_decode(const float* const* regobj, const float* const* cls, const int* hw, const int* strides,
                           int ld_ro, int ld_cls, int ncls, float* out, void* stream);
+/* B >= 1 images: image b of level k starts at regobj[k] + b * bs_ro[k] / cls[k] + b * bs_cls[k] (HOST arrays of 3 element
+ * strides, each >= h_k*w_k*ld; ignored when B = 1); out f32 [B, sum HW, 5+ncls]. */
+UC_API int uc_head_decode_batched(const float* const* regobj, const float* const* cls, const int* hw, const int* strides,
+                                  int ld_ro, int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float* out,
+                                  void* stream);
 
 /* postprocess (utils/boxes.py:33-77) on the device: out_dets f32 [<=A, 7] rows (x1,y1,x2,y2,obj,cls_conf,cls_id)
  * in descending score order, *out_count (device int) = number of rows.  max_keep > 0 stops the greedy scan once that
@@ -219,6 +235,12 @@ UC_API int uc_head_decode(const float* const* regobj, const float* const* cls, c
 UC_API long uc_postprocess_workspace_bytes(int max_anchors);
 UC_API int uc_postprocess(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, void* workspace,
                           long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream);
+/* The same for B >= 1 images in one launch sequence (one CTA per image in each of the four kernels): pred f32 [B, A, 5+ncls],
+ * out_dets [B, A, 7], out_count [B], out_anchor [B, A] (or NULL); max_keep applies per image.  The workspace holds B per-image
+ * slices: uc_postprocess_workspace_bytes_batched(A, B) bytes (0 for B < 1).  B < 1 or a smaller workspace: UC_EINVAL. */
+UC_API long uc_postprocess_workspace_bytes_batched(int max_anchors, int B);
+UC_API int uc_postprocess_batched(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
+                                  void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream);
 
 /* Instance-embedding sampling at box centres (unicorn/evaluators/mot_evaluator.py:1024-1034): embed NHWC 16-bit
  * [h,w,C] (pixel stride ld), boxes f32 [n,ldb] xyxy in network-input pixels, stride = 8; grid_sample(bilinear,

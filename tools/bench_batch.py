@@ -1,0 +1,105 @@
+"""Several SOT sequences per GPU: one batched frame (UnicornSOTBatch, n_seq sequences in lock step) against frames in flight of one
+sequence (UnicornSOTTrack, depth 1 and 3), on the 800x1280 SOT frame with CUDA graphs.
+
+    python tools/bench_batch.py [--steps 60] [--rounds 3] [--configs unicorn_track_large unicorn_track_r50] [--n-seq 1 2 4 8]
+
+Device-resident timing like bench.py's `value`: the frames are already in HBM, each step is an input copy and a graph replay, timed
+with CUDA events.  Every driver of a config is built first (plan-time autotuning of the batched layer shapes, graph capture); the
+timed rounds then alternate over the drivers so that clock and neighbour drift spread over all of them.  Printed per driver: aggregate
+frames/s (sequences x steps / s), ms per step, and the device memory the driver added on top of what was already allocated (the
+engine's weights and the drivers built before it): the peak torch allocation while it was built and warmed up, minus the allocation
+before.  One JSON line per result."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--configs", nargs="+", default=["unicorn_track_large", "unicorn_track_r50"])
+    ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
+    ap.add_argument("--n-seq", type=int, nargs="+", default=[1, 2, 4, 8])
+    ap.add_argument("--depths", type=int, nargs="+", default=[1, 3])
+    ap.add_argument("--steps", type=int, default=60)
+    ap.add_argument("--rounds", type=int, default=3)
+    args = ap.parse_args()
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.sot import UnicornSOTBatch, UnicornSOTTrack
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.weights import make_state_dict
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
+    H, W = args.size
+    N = max(args.n_seq)
+    to_u8 = lambda f: f.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()  # noqa: E731
+    main_stream = torch.cuda.current_stream()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        videos = [make_video(5, H, W, seed=s) for s in range(N)]
+        refs = [(to_u8(fr[0:1]), bx[0, 0]) for fr, bx in videos]
+        steps_u8 = [torch.stack([to_u8(fr[1 + t:2 + t])[0] for fr, _ in videos]).cuda() for t in range(4)]  # [N,H,W,3] per step
+        drivers = {}
+        for n in args.n_seq:
+            m0 = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            sb = UnicornSOTBatch(eng, (H, W), n)
+            for i in range(n):
+                sb.initialize_tensor(i, *refs[i])
+            for t in range(3):
+                sb.track_tensor(steps_u8[t][:n])
+
+            def batch_step(t, sb=sb, n=n):
+                sb.slot.img_in_u8.copy_(steps_u8[t % 4][:n], non_blocking=True)
+                sb.slot.graph.replay()
+            drivers[f"batch{n}"] = (batch_step, n, [], torch.cuda.max_memory_allocated() - m0)
+        for d in args.depths:
+            m0 = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            trk = UnicornSOTTrack(eng, (H, W), depth=d)
+            trk.initialize_tensor(*refs[0])
+            for t in range(2 * d + 1):
+                trk.track_tensor(steps_u8[t % 4][0:1])
+
+            def pipe_step(t, trk=trk, d=d):
+                c = trk._ctxs[t % d]
+                with torch.cuda.stream(c.stream):
+                    c.img_in_u8.copy_(steps_u8[t % 4][0:1], non_blocking=True)
+                    c.graph.replay()
+            drivers[f"depth{d}"] = (pipe_step, 1, [c.stream for c in trk._ctxs if c.stream is not None], torch.cuda.max_memory_allocated() - m0)
+        times = {k: [] for k in drivers}
+        for _ in range(args.rounds):
+            for k, (step, n, streams, _) in drivers.items():
+                torch.cuda.synchronize()
+                e0.record()
+                for st in streams:  # frames in flight: fork from the timed region's start, join before its end
+                    st.wait_stream(main_stream)
+                for t in range(args.steps):
+                    step(t)
+                for st in streams:
+                    main_stream.wait_stream(st)
+                e1.record()
+                torch.cuda.synchronize()
+                times[k].append(e0.elapsed_time(e1) / 1e3)
+        for k, (step, n, streams, mem) in drivers.items():
+            ts = times[k]
+            fps = [n * args.steps / t for t in ts]
+            print(json.dumps({"config": cfg, "size": [H, W], "driver": "UnicornSOTBatch" if k.startswith("batch") else "UnicornSOTTrack",
+                              "n_seq": n, "depth": max(1, len(streams)), "frames_per_s": round(statistics.median(fps), 1),
+                              "frames_per_s_min_max": [round(min(fps), 1), round(max(fps), 1)],
+                              "ms_per_step": round(1e3 * statistics.median(ts) / args.steps, 2),
+                              "added_peak_alloc_gib": round(mem / 2 ** 30, 2), "steps": args.steps, "rounds": args.rounds}), flush=True)
+        del drivers, eng, sb, trk, batch_step, pipe_step
+        torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()

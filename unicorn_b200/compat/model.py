@@ -53,14 +53,18 @@ class _Head:
         self.mask_head = _MaskHeadHandle() if model.cfg["mask"] else None
 
     def __call__(self, fpn_outs, prior_ms=None, mode="sot"):
-        """fpn_outs: 3 NCHW fp32 maps; prior_ms: 3 fp32 maps (1,1,h,w).  -> (1, A, 5+ncls), or UnicornHeadMask's tuple
-        (outputs, locations (A,2), dynamic_params (1,A,169), fpn_levels (1,A), mask_feats (1,8,h,w), up_masks (1,144,h,w))."""
+        """fpn_outs: 3 NCHW fp32 maps (B,C,h,w); prior_ms: 3 fp32 maps (B,1,h,w).  -> (B, A, 5+ncls), or (B = 1 only)
+        UnicornHeadMask's tuple (outputs, locations (A,2), dynamic_params (1,A,169), fpn_levels (1,A), mask_feats (1,8,h,w),
+        up_masks (1,144,h,w))."""
         e = self._m._engine()
+        B = fpn_outs[0].shape[0]
+        if self._m.cfg["mask"] and B != 1:
+            raise ValueError(f"UnicornB200Model.head: the mask head runs one image per call (got a batch of {B})")
         fpn = [_nhwc(t) for t in fpn_outs]
         pri = None
         if prior_ms is not None:
             if mode == "sot":
-                pri = [p.float().reshape(1, p.shape[-2], p.shape[-1]).contiguous() for p in prior_ms]
+                pri = [p.float().reshape(B, p.shape[-2], p.shape[-1]).contiguous() for p in prior_ms]
             else:  # the reference adds x + m * beta in "mot" mode too; its only caller passes zeros (unicorn.py:136-139)
                 assert all(float(p.abs().max()) == 0.0 for p in prior_ms), "non-zero priors with mode='mot' are not supported"
         e.begin_frame()
@@ -150,7 +154,7 @@ class UnicornB200Model:
 
     def _backbone(self, imgs):
         e = self._engine()
-        assert imgs.is_cuda and imgs.dim() == 4 and imgs.shape[0] == 1, "one frame per call (the reference's tracking drivers use batch 1)"
+        assert imgs.is_cuda and imgs.dim() == 4 and imgs.shape[0] >= 1, "CUDA NCHW frames [B,3,H,W]"
         e.begin_frame()
         fpn, seq = e.backbone(imgs.float().contiguous(), tag="compat")
         h, w = seq["h"], seq["w"]
@@ -169,6 +173,8 @@ class UnicornB200Model:
         if mode == "upsample":
             return ops.nhwc_to_nchw(e.upsample(_nhwc(feat), "compat"))
         if mode == "whole":  # backbone + head with zero priors, MOT prediction set (unicorn.py:133-139)
+            if self.cfg["mask"] and imgs.shape[0] != 1:
+                raise ValueError(f"UnicornB200Model(mode='whole'): the mask head runs one image per call (got a batch of {imgs.shape[0]})")
             fpn, seq_dict = self._backbone(imgs)
             if not self.cfg["mask"]:
                 return e.head(fpn, None, "mot").clone(), seq_dict
@@ -187,16 +193,15 @@ def _to_corners_(prediction):
 
 
 def postprocess(prediction, num_classes, conf_thre=0.7, nms_thre=0.45):
-    """unicorn.utils.postprocess (utils/boxes.py:33-77): list with one (M,7) tensor of rows
-    (x1,y1,x2,y2,obj_conf,class_conf,class_pred), descending score, or None when nothing passes — on the GPU.
-    Like the reference, the boxes of `prediction` are converted to corner form in place."""
-    out = []
-    for i in range(prediction.shape[0]):
-        p = prediction[i].float().contiguous()
-        ws = ops.PostWorkspace(p.shape[0], p.device)
-        dets, cnt = ops.postprocess_device(p, num_classes, conf_thre, nms_thre, ws)
-        n = int(cnt.item())
-        out.append(dets[:n].clone() if n > 0 else None)
+    """unicorn.utils.postprocess (utils/boxes.py:33-77): list with one (M,7) tensor of rows per image
+    (x1,y1,x2,y2,obj_conf,class_conf,class_pred), descending score, or None when nothing passes — on the GPU, every image of the
+    batch in one launch sequence.  Like the reference, the boxes of `prediction` are converted to corner form in place."""
+    p = prediction.float().contiguous()
+    B, A = p.shape[:2]
+    ws = ops.PostWorkspace(A, p.device, B)
+    dets, cnt = ops.postprocess_device(p, num_classes, conf_thre, nms_thre, ws)
+    dets = dets.view(B, A, 7)
+    out = [dets[i, :n].clone() if n > 0 else None for i, n in enumerate(cnt.tolist())]
     _to_corners_(prediction)
     return out
 

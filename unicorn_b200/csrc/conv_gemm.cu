@@ -60,7 +60,9 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   const CUtensorMapDataType dt = d->x_dtype == UC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool flat = (d->KH == 1 && d->KW == 1 && s == 1 && d->pad == 0);
   int B = d->B, Hm = d->H, Wm = d->W;  // map geometry
-  if (flat) { Wm = d->B * d->H * d->W; Hm = 1; B = 1; }
+  // a flat conv is one row of H*W pixels per image; the batch stays the 4th map dimension, so no tile spans two images and each
+  // tile's GroupNorm sums go to its own image's slot
+  if (flat) { Wm = d->H * d->W; Hm = 1; }
   p.Wo = flat ? Wm : Wo;
   p.Ho = flat ? 1 : Ho;
   p.B = B;

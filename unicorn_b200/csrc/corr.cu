@@ -27,9 +27,10 @@ constexpr int kCorrConsumers = 2;
 constexpr int kCorrThreads = (1 + kCorrConsumers) * 128;
 
 struct alignas(64) CorrParams {
-  CUtensorMap tmQ, tmK;
-  const float* V;  // [n_obj, ldv]
-  float* out;      // [n_obj, ldo]
+  CUtensorMap tmQ, tmK;  // [B][n][C]
+  const float* V;  // [B][n_obj, ldv], sequence stride bsv
+  float* out;      // [B][n_obj, ldo], sequence stride bso
+  long bsv, bso;
   int ldv, ldo, n_cur, n_ref, n_obj;
 };
 
@@ -65,6 +66,8 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
 
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int j0 = blockIdx.x * kCorrTile;
+  const int seq = blockIdx.y;  // one (reference, current, values) triple per grid row
+  const float* const V = p.V + seq * p.bsv;
   const int nchunks = (p.n_ref + kCorrChunk - 1) / kCorrChunk;
 
   if (threadIdx.x == 0) {
@@ -85,8 +88,8 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
     // same stage.  The producer runs up to kCorrStages chunks ahead, so the L2 latency of these loads is off the softmax's path.
     if (elect_one()) {
       mbar_arrive_expect_tx(q_full, kCorrQBytes);
-      tma_load_2d(sQ, &p.tmQ, q_full, 0, j0);
-      tma_load_2d(sQ + kCorrQBytes / 2, &p.tmQ, q_full, 64, j0);
+      tma_load_3d(sQ, &p.tmQ, q_full, 0, j0, seq);
+      tma_load_3d(sQ + kCorrQBytes / 2, &p.tmQ, q_full, 64, j0, seq);
     }
     __syncwarp();
     int stage = 0, phase = 0;
@@ -96,8 +99,8 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
       if (elect_one()) {
         mbar_arrive_expect_tx(&k_full[stage], kCorrKBytes);
         uint8_t* dst = sK + stage * kCorrKBytes;
-        tma_load_2d(dst, &p.tmK, &k_full[stage], 0, i0);
-        tma_load_2d(dst + kCorrKBytes / 2, &p.tmK, &k_full[stage], 64, i0);
+        tma_load_3d(dst, &p.tmK, &k_full[stage], 0, i0, seq);
+        tma_load_3d(dst + kCorrKBytes / 2, &p.tmK, &k_full[stage], 64, i0, seq);
       }
       float* vb = sV + stage * NOBJ * kCorrChunk;
 #pragma unroll
@@ -105,7 +108,7 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
 #pragma unroll
         for (int t = 0; t < kCorrChunk / 32; ++t) {
           const int i = i0 + t * 32 + lane;
-          vb[o * kCorrChunk + t * 32 + lane] = (o < p.n_obj && i < p.n_ref) ? __ldg(p.V + static_cast<long>(o) * p.ldv + i) : 0.f;
+          vb[o * kCorrChunk + t * 32 + lane] = (o < p.n_obj && i < p.n_ref) ? __ldg(V + static_cast<long>(o) * p.ldv + i) : 0.f;
         }
       }
       __syncwarp();
@@ -210,13 +213,13 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_kernel(const __grid_cons
       const float inv = 1.f / L;
 #pragma unroll
       for (int o = 0; o < NOBJ; ++o)
-        if (o < p.n_obj) p.out[static_cast<long>(o) * p.ldo + j] = A[o] * inv;
+        if (o < p.n_obj) p.out[seq * p.bso + static_cast<long>(o) * p.ldo + j] = A[o] * inv;
     }
   }
 }
 
 template <int NOBJ>
-static int launch_corr(const CorrParams& p, bool f16, int grid, cudaStream_t stream) {
+static int launch_corr(const CorrParams& p, bool f16, dim3 grid, const char* what, cudaStream_t stream) {
   constexpr int smem = kCorrQBytes + kCorrStages * kCorrKBytes + kCorrStages * NOBJ * kCorrChunk * 4 + 256 + 1024;
   static PerDeviceFlag attr_dev;
   bool& attr_set = attr_dev.get();
@@ -228,7 +231,54 @@ static int launch_corr(const CorrParams& p, bool f16, int grid, cudaStream_t str
     attr_set = true;
   }
   launch_pdl(f16 ? corr_kernel<NOBJ, true> : corr_kernel<NOBJ, false>, grid, kCorrThreads, smem, stream, p);
-  return check_launch("uc_corr_propagate");
+  return check_launch(what);
+}
+
+// B (reference, current, values) triples; the strides bs_* between sequences are in elements.  B = 1 ignores them.
+static int corr_propagate(const char* what, const void* embed_ref, int ld_ref, long bs_ref, int n_ref, const void* embed_cur, int ld_cur,
+                          long bs_cur, int n_cur, int C, int dtype, const float* values, int ldv, long bs_v, int n_obj, float* out,
+                          int ldo, long bs_out, int B, void* stream_v) {
+  if (!embed_ref || !embed_cur || !values || !out) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (C != kCorrC) return set_error(UC_EINVAL, "%s: embedding dim must be %d (got %d)", what, kCorrC, C);
+  if (dtype != UC_BF16 && dtype != UC_F16) return set_error(UC_EINVAL, "%s: embeddings must be bf16/f16", what);
+  if (n_obj < 1 || n_obj > 8) return set_error(UC_EINVAL, "%s: 1 <= n_obj <= 8 (got %d)", what, n_obj);
+  if (ld_ref % 8 || ld_cur % 8 || n_ref < 1 || n_cur < 1 || ldv < n_ref || ldo < n_cur) return set_error(UC_EINVAL, "%s: bad sizes/strides", what);
+  if (B == 1) {
+    bs_ref = static_cast<long>(ld_ref) * n_ref; bs_cur = static_cast<long>(ld_cur) * n_cur;
+    bs_v = static_cast<long>(ldv) * n_obj; bs_out = static_cast<long>(ldo) * n_obj;
+  } else if (bs_ref % 8 || bs_cur % 8 || bs_ref < static_cast<long>(ld_ref) * n_ref || bs_cur < static_cast<long>(ld_cur) * n_cur ||
+             bs_v < static_cast<long>(ldv) * n_obj || bs_out < static_cast<long>(ldo) * n_obj) {
+    return set_error(UC_EINVAL, "%s: bad per-sequence strides (embeddings: multiple of 8 and >= ld*n; values / out: >= ld*n_obj)", what);
+  }
+  int rc = ensure_driver();
+  if (rc) return rc;
+  CorrParams p;
+  memset(&p, 0, sizeof(p));
+  const CUtensorMapDataType dt = dtype == UC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  {
+    uint64_t dims[3] = {static_cast<uint64_t>(C), static_cast<uint64_t>(n_cur), static_cast<uint64_t>(B)};
+    uint64_t strides[2] = {static_cast<uint64_t>(ld_cur) * 2, static_cast<uint64_t>(bs_cur) * 2};
+    uint32_t box[3] = {64, kCorrTile, 1};
+    rc = encode_tmap(&p.tmQ, dt, 3, embed_cur, dims, strides, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[3] = {static_cast<uint64_t>(C), static_cast<uint64_t>(n_ref), static_cast<uint64_t>(B)};
+    uint64_t strides[2] = {static_cast<uint64_t>(ld_ref) * 2, static_cast<uint64_t>(bs_ref) * 2};
+    uint32_t box[3] = {64, kCorrChunk, 1};
+    rc = encode_tmap(&p.tmK, dt, 3, embed_ref, dims, strides, box);
+    if (rc) return rc;
+  }
+  p.V = values; p.out = out; p.bsv = bs_v; p.bso = bs_out;
+  p.ldv = ldv; p.ldo = ldo; p.n_cur = n_cur; p.n_ref = n_ref; p.n_obj = n_obj;
+  const bool f16 = dtype == UC_F16;
+  const dim3 grid((n_cur + kCorrTile - 1) / kCorrTile, B);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (n_obj == 1) return launch_corr<1>(p, f16, grid, what, stream);
+  if (n_obj == 2) return launch_corr<2>(p, f16, grid, what, stream);
+  if (n_obj <= 4) return launch_corr<4>(p, f16, grid, what, stream);
+  return launch_corr<8>(p, f16, grid, what, stream);
 }
 
 }  // namespace uc
@@ -238,36 +288,13 @@ using namespace uc;
 extern "C" int uc_corr_propagate(const void* embed_ref, int ld_ref, int n_ref, const void* embed_cur, int ld_cur, int n_cur,
                                  int C, int dtype, const float* values, int ldv, int n_obj, float* out, int ldo,
                                  void* stream_v) {
-  if (!embed_ref || !embed_cur || !values || !out) return set_error(UC_EINVAL, "uc_corr_propagate: null pointer");
-  if (C != kCorrC) return set_error(UC_EINVAL, "uc_corr_propagate: embedding dim must be %d (got %d)", kCorrC, C);
-  if (dtype != UC_BF16 && dtype != UC_F16) return set_error(UC_EINVAL, "uc_corr_propagate: embeddings must be bf16/f16");
-  if (n_obj < 1 || n_obj > 8) return set_error(UC_EINVAL, "uc_corr_propagate: 1 <= n_obj <= 8 (got %d)", n_obj);
-  if (ld_ref % 8 || ld_cur % 8 || n_ref < 1 || n_cur < 1 || ldv < n_ref || ldo < n_cur) return set_error(UC_EINVAL, "uc_corr_propagate: bad sizes/strides");
-  int rc = ensure_driver();
-  if (rc) return rc;
-  CorrParams p;
-  memset(&p, 0, sizeof(p));
-  const CUtensorMapDataType dt = dtype == UC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(n_cur)};
-    uint64_t strides[1] = {static_cast<uint64_t>(ld_cur) * 2};
-    uint32_t box[2] = {64, kCorrTile};
-    rc = encode_tmap(&p.tmQ, dt, 2, embed_cur, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(n_ref)};
-    uint64_t strides[1] = {static_cast<uint64_t>(ld_ref) * 2};
-    uint32_t box[2] = {64, kCorrChunk};
-    rc = encode_tmap(&p.tmK, dt, 2, embed_ref, dims, strides, box);
-    if (rc) return rc;
-  }
-  p.V = values; p.out = out; p.ldv = ldv; p.ldo = ldo; p.n_cur = n_cur; p.n_ref = n_ref; p.n_obj = n_obj;
-  const bool f16 = dtype == UC_F16;
-  const int grid = (n_cur + kCorrTile - 1) / kCorrTile;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (n_obj == 1) return launch_corr<1>(p, f16, grid, stream);
-  if (n_obj == 2) return launch_corr<2>(p, f16, grid, stream);
-  if (n_obj <= 4) return launch_corr<4>(p, f16, grid, stream);
-  return launch_corr<8>(p, f16, grid, stream);
+  return corr_propagate("uc_corr_propagate", embed_ref, ld_ref, 0, n_ref, embed_cur, ld_cur, 0, n_cur, C, dtype, values, ldv, 0, n_obj,
+                        out, ldo, 0, 1, stream_v);
+}
+
+extern "C" int uc_corr_propagate_batched(const void* embed_ref, int ld_ref, long bs_ref, int n_ref, const void* embed_cur, int ld_cur,
+                                         long bs_cur, int n_cur, int C, int dtype, const float* values, int ldv, long bs_values,
+                                         int n_obj, float* out, int ldo, long bs_out, int B, void* stream_v) {
+  return corr_propagate("uc_corr_propagate_batched", embed_ref, ld_ref, bs_ref, n_ref, embed_cur, ld_cur, bs_cur, n_cur, C, dtype, values,
+                        ldv, bs_values, n_obj, out, ldo, bs_out, B, stream_v);
 }

@@ -58,25 +58,29 @@ struct MsdaLevels {
   int H[4], W[4], start[4];
 };
 
-// 8 lanes per (query, head); each lane owns 4 of the head's 32 channels.  value bf16 [S, M*32]; offlog fp32
-// [Lq, M*L*P*2 + M*L*P]; queries are the concatenation of the levels' pixel grids (query q lives on level ql with
-// pixel (qy,qx)) and its reference point (qx+0.5)/Wq, (qy+0.5)/Hq is shared by all levels.
+// 8 lanes per (image, query, head); each lane owns 4 of the head's 32 channels.  Rows (value, offlog, out) are level-major,
+// images within a level: level l of image b starts at row B * start[l] + b * H[l] * W[l] (for B = 1 the concatenation of the
+// levels).  value bf16 rows of M*32; offlog fp32 rows of M*L*P*2 + M*L*P; an image's queries are its levels' pixel grids (query
+// qi of level ql at pixel (qy,qx)), and the reference point (qx+0.5)/Wq, (qy+0.5)/Hq is shared by all levels of that image.
 __global__ void __launch_bounds__(256) msda_fused_kernel(const uint2* __restrict__ value, const float* __restrict__ offlog,
                                                           uint2* __restrict__ out, MsdaLevels lv, int M, int L, int P, int Lq,
-                                                          int ld_offlog) {
+                                                          int ld_offlog, int B) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
-  const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 3;  // (q, m)
+  const long g = (static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 3;  // (b, q, m)
   const int sub = threadIdx.x & 7;
-  if (g >= Lq * M) return;
-  const int q = g / M, m = g % M;
+  if (g >= static_cast<long>(B) * Lq * M) return;
+  const int b = static_cast<int>(g / (static_cast<long>(Lq) * M));
+  const int qm = static_cast<int>(g - static_cast<long>(b) * Lq * M);
+  const int qq = qm / M, m = qm % M;
   int ql = 0;
-  while (ql + 1 < L && q >= lv.start[ql + 1]) ++ql;
-  const int qi = q - lv.start[ql];
+  while (ql + 1 < L && qq >= lv.start[ql + 1]) ++ql;
+  const int qi = qq - lv.start[ql];
+  const long q = static_cast<long>(B) * lv.start[ql] + static_cast<long>(b) * lv.H[ql] * lv.W[ql] + qi;  // row of this query
   const float rx = ((qi % lv.W[ql]) + 0.5f) / lv.W[ql], ry = ((qi / lv.W[ql]) + 0.5f) / lv.H[ql];
   const int LP = L * P;
-  const float* off = offlog + static_cast<long>(q) * ld_offlog + m * LP * 2;
-  const float* lg = offlog + static_cast<long>(q) * ld_offlog + M * LP * 2 + m * LP;
+  const float* off = offlog + q * ld_offlog + m * LP * 2;
+  const float* lg = offlog + q * ld_offlog + M * LP * 2 + m * LP;
   float mx = -INFINITY;
   for (int i = 0; i < LP; ++i) mx = fmaxf(mx, __ldg(lg + i));
   float den = 0.f;
@@ -86,7 +90,7 @@ __global__ void __launch_bounds__(256) msda_fused_kernel(const uint2* __restrict
   const int rs = M * 8;  // row stride in uint2 (4 bf16)
   for (int l = 0; l < L; ++l) {
     const int H = lv.H[l], W = lv.W[l];
-    const uint2* vb = value + static_cast<long>(lv.start[l]) * rs + m * 8 + sub;
+    const uint2* vb = value + (static_cast<long>(B) * lv.start[l] + static_cast<long>(b) * H * W) * rs + m * 8 + sub;
     for (int p = 0; p < P; ++p) {
       const float a = __expf(__ldg(lg + l * P + p) - mx) * inv;
       const float lx = rx + __ldg(off + (l * P + p) * 2) / W, ly = ry + __ldg(off + (l * P + p) * 2 + 1) / H;
@@ -107,7 +111,7 @@ __global__ void __launch_bounds__(256) msda_fused_kernel(const uint2* __restrict
       }
     }
   }
-  out[static_cast<long>(q) * rs + m * 8 + sub] = make_uint2(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]));
+  out[q * rs + m * 8 + sub] = make_uint2(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]));
 }
 
 }  // namespace uc
@@ -127,10 +131,11 @@ extern "C" int uc_msda_forward_f32(const float* value, const int64_t* spatial_sh
   return check_launch("uc_msda_forward_f32");
 }
 
-extern "C" int uc_msda_fused_bf16(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw, int L,
-                                  int M, int P, void* stream_v) {
-  if (!value || !offlog || !out || !level_hw) return set_error(UC_EINVAL, "uc_msda_fused_bf16: null pointer");
-  if (L < 1 || L > 4 || L * P > 16 || M < 1) return set_error(UC_EINVAL, "uc_msda_fused_bf16: L<=4, L*P<=16 (head dim fixed at 32)");
+static int msda_fused(const char* what, const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw, int L,
+                      int M, int P, int B, void* stream_v) {
+  if (!value || !offlog || !out || !level_hw) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (L < 1 || L > 4 || L * P > 16 || M < 1) return set_error(UC_EINVAL, "%s: L<=4, L*P<=16 (head dim fixed at 32)", what);
   MsdaLevels lv;
   int start = 0;
   for (int l = 0; l < 4; ++l) {
@@ -140,8 +145,18 @@ extern "C" int uc_msda_fused_bf16(const void* value, const float* offlog, int ld
     if (l < L) start += lv.H[l] * lv.W[l];
   }
   const int Lq = start;
-  const long threads = static_cast<long>(Lq) * M * 8;
-  launch_pdl(msda_fused_kernel, static_cast<unsigned>((threads + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream_v), 
-      static_cast<const uint2*>(value), offlog, static_cast<uint2*>(out), lv, M, L, P, Lq, ld_offlog);
-  return check_launch("uc_msda_fused_bf16");
+  const long threads = static_cast<long>(B) * Lq * M * 8;
+  launch_pdl(msda_fused_kernel, static_cast<unsigned>((threads + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream_v),
+      static_cast<const uint2*>(value), offlog, static_cast<uint2*>(out), lv, M, L, P, Lq, ld_offlog, B);
+  return check_launch(what);
+}
+
+extern "C" int uc_msda_fused_bf16(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw, int L,
+                                  int M, int P, void* stream_v) {
+  return msda_fused("uc_msda_fused_bf16", value, offlog, ld_offlog, out, level_hw, L, M, P, 1, stream_v);
+}
+
+extern "C" int uc_msda_fused_bf16_batched(const void* value, const float* offlog, int ld_offlog, void* out, const int* level_hw, int L,
+                                          int M, int P, int B, void* stream_v) {
+  return msda_fused("uc_msda_fused_bf16_batched", value, offlog, ld_offlog, out, level_hw, L, M, P, B, stream_v);
 }

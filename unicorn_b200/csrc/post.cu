@@ -12,8 +12,9 @@
 namespace uc {
 
 struct DecodeLevels {
-  const float* regobj[3];  // [HW, ld_ro]: reg(4), obj logit
-  const float* cls[3];     // [HW, ld_cls]: class logits
+  const float* regobj[3];  // [B][HW, ld_ro]: reg(4), obj logit
+  const float* cls[3];     // [B][HW, ld_cls]: class logits
+  long bs_ro[3], bs_cls[3];  // per-level image strides (elements)
   int h[3], w[3], stride[3], start[3];
   int ld_ro, ld_cls, ncls, total;
 };
@@ -22,6 +23,7 @@ __global__ void __launch_bounds__(256) head_decode_kernel(DecodeLevels lv, float
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = blockIdx.y;  // image
   if (i >= lv.total) return;
   int k = 0;
   if (i >= lv.start[1]) k = 1;
@@ -29,9 +31,9 @@ __global__ void __launch_bounds__(256) head_decode_kernel(DecodeLevels lv, float
   const int a = i - lv.start[k];
   const int x = a % lv.w[k], y = a / lv.w[k];
   const float s = static_cast<float>(lv.stride[k]);
-  const float* ro = lv.regobj[k] + static_cast<long>(a) * lv.ld_ro;
-  const float* cl = lv.cls[k] + static_cast<long>(a) * lv.ld_cls;
-  float* o = out + static_cast<long>(i) * (5 + lv.ncls);
+  const float* ro = lv.regobj[k] + b * lv.bs_ro[k] + static_cast<long>(a) * lv.ld_ro;
+  const float* cl = lv.cls[k] + b * lv.bs_cls[k] + static_cast<long>(a) * lv.ld_cls;
+  float* o = out + (static_cast<long>(b) * lv.total + i) * (5 + lv.ncls);
   o[0] = (ro[0] + x) * s;
   o[1] = (ro[1] + y) * s;
   o[2] = expf(ro[2]) * s;
@@ -40,13 +42,34 @@ __global__ void __launch_bounds__(256) head_decode_kernel(DecodeLevels lv, float
   for (int c = 0; c < lv.ncls; ++c) o[5 + c] = 1.f / (1.f + expf(-cl[c]));
 }
 
+// Per-image slices of the postprocess workspace: image b owns bytes [b * per_image, (b + 1) * per_image), laid out as
+// count (256 bytes), det [A][7], sorted [A][7] (fp32), keys [a2] (u64), det_anchor [A], sorted_anchor [A] (int).
+struct PostSlices {
+  uint8_t* ws;
+  long per_image, a2;
+  int A;
+  __device__ __forceinline__ uint8_t* base(int b) const { return ws + b * per_image; }
+  __device__ __forceinline__ int* count(int b) const { return reinterpret_cast<int*>(base(b)); }
+  __device__ __forceinline__ float* det(int b) const { return reinterpret_cast<float*>(base(b) + 256); }
+  __device__ __forceinline__ float* sorted(int b) const { return det(b) + static_cast<long>(A) * 7; }
+  __device__ __forceinline__ unsigned long long* keys(int b) const {
+    return reinterpret_cast<unsigned long long*>(sorted(b) + static_cast<long>(A) * 7);
+  }
+  __device__ __forceinline__ int* det_anchor(int b) const { return reinterpret_cast<int*>(keys(b) + a2); }
+  __device__ __forceinline__ int* sorted_anchor(int b) const { return det_anchor(b) + A; }
+};
+
 // ---- filter: deterministic compaction (anchor order) of candidates with obj*class_conf >= conf.
 // det rows: x1,y1,x2,y2,obj,class_conf,class_pred ; key = (score bits << 32) | (0xffffffff - candidate index)
-__global__ void __launch_bounds__(1024) det_filter_kernel(const float* __restrict__ pred, int A, int ncls, float conf,
-                                                           float* __restrict__ det, unsigned long long* __restrict__ keys,
-                                                           int* __restrict__ count, int cap, int* __restrict__ det_anchor) {
+__global__ void __launch_bounds__(1024) det_filter_kernel(const float* __restrict__ pred, int A, int ncls, float conf, PostSlices sl) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
+  const int cap = A;
+  pred += static_cast<long>(blockIdx.x) * A * (5 + ncls);
+  float* const det = sl.det(blockIdx.x);
+  unsigned long long* const keys = sl.keys(blockIdx.x);
+  int* const count = sl.count(blockIdx.x);
+  int* const det_anchor = sl.det_anchor(blockIdx.x);
   __shared__ int warp_cnt[32];
   __shared__ int warp_excl[32];
   __shared__ int base, round_total;
@@ -102,10 +125,13 @@ __global__ void __launch_bounds__(1024) det_filter_kernel(const float* __restric
   if (threadIdx.x == 0) *count = min(base, cap);
 }
 
-// ---- sort keys descending (bitonic, one CTA, n2 = power of two >= count; pads with 0 keys)
-__global__ void __launch_bounds__(1024) sort_desc_kernel(unsigned long long* __restrict__ keys, const int* __restrict__ count, int cap2) {
+// ---- sort keys descending (bitonic, one CTA per image, n2 = power of two >= count; pads with 0 keys)
+__global__ void __launch_bounds__(1024) sort_desc_kernel(PostSlices sl) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
+  unsigned long long* const keys = sl.keys(blockIdx.x);
+  const int* const count = sl.count(blockIdx.x);
+  const int cap2 = static_cast<int>(sl.a2);
   const int n = *count;
   int n2 = 1;
   while (n2 < n) n2 <<= 1;
@@ -127,11 +153,16 @@ __global__ void __launch_bounds__(1024) sort_desc_kernel(unsigned long long* __r
 }
 
 // ---- gather rows in sorted order
-__global__ void __launch_bounds__(256) det_gather_kernel(const float* __restrict__ det, const unsigned long long* __restrict__ keys,
-                                                          const int* __restrict__ count, float* __restrict__ sorted,
-                                                          const int* __restrict__ det_anchor, int* __restrict__ sorted_anchor) {
+__global__ void __launch_bounds__(256) det_gather_kernel(PostSlices sl) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
+  const int img = blockIdx.y;
+  const float* const det = sl.det(img);
+  const unsigned long long* const keys = sl.keys(img);
+  const int* const count = sl.count(img);
+  float* const sorted = sl.sorted(img);
+  const int* const det_anchor = sl.det_anchor(img);
+  int* const sorted_anchor = sl.sorted_anchor(img);
   const int n = *count;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const unsigned idx = 0xffffffffu - static_cast<unsigned>(keys[i] & 0xffffffffull);
@@ -160,11 +191,17 @@ __device__ __forceinline__ bool nms_hit(const float4 a, const float4 b, float th
   return inter / (sa + sb - inter) > thr;
 }
 
-__global__ void __launch_bounds__(1024) nms_greedy_kernel(const float* __restrict__ sorted, const int* __restrict__ count, float thr,
-                                                           float* __restrict__ out, int* __restrict__ out_count, int max_keep,
-                                                           const int* __restrict__ sorted_anchor, int* __restrict__ out_anchor) {
+__global__ void __launch_bounds__(1024) nms_greedy_kernel(PostSlices sl, float thr, float* __restrict__ out, int* __restrict__ out_count,
+                                                           int max_keep, int* __restrict__ out_anchor) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
+  const int img = blockIdx.x;
+  const float* const sorted = sl.sorted(img);
+  const int* const count = sl.count(img);
+  const int* const sorted_anchor = sl.sorted_anchor(img);
+  out += static_cast<long>(img) * sl.A * 7;
+  out_count += img;
+  if (out_anchor) out_anchor += static_cast<long>(img) * sl.A;
   extern __shared__ float4 kept_box[];                       // [kNmsKeepSmem]
   float* kept_cls = reinterpret_cast<float*>(kept_box + kNmsKeepSmem);  // [kNmsKeepSmem]
   __shared__ float4 cbox[kNmsChunk];
@@ -266,19 +303,36 @@ __global__ void __launch_bounds__(1024) nms_greedy_kernel(const float* __restric
 
 using namespace uc;
 
-extern "C" int uc_head_decode(const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
-                              int ld_cls, int ncls, float* out, void* stream_v) {
-  if (!regobj || !cls || !hw || !strides || !out || ncls < 1 || ncls > ld_cls || ld_ro < 5) return set_error(UC_EINVAL, "uc_head_decode: bad arguments");
+static int head_decode(const char* what, const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                       int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float* out, void* stream_v) {
+  if (!regobj || !cls || !hw || !strides || !out || ncls < 1 || ncls > ld_cls || ld_ro < 5) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
   DecodeLevels lv;
   int start = 0;
   for (int k = 0; k < 3; ++k) {
     lv.regobj[k] = regobj[k]; lv.cls[k] = cls[k];
     lv.h[k] = hw[2 * k]; lv.w[k] = hw[2 * k + 1]; lv.stride[k] = strides[k]; lv.start[k] = start;
+    const long hwk = static_cast<long>(lv.h[k]) * lv.w[k];
+    lv.bs_ro[k] = B > 1 ? bs_ro[k] : hwk * ld_ro;
+    lv.bs_cls[k] = B > 1 ? bs_cls[k] : hwk * ld_cls;
+    if (lv.bs_ro[k] < hwk * ld_ro || lv.bs_cls[k] < hwk * ld_cls)
+      return set_error(UC_EINVAL, "%s: bad per-image strides of level %d (need >= h*w*ld)", what, k);
     start += lv.h[k] * lv.w[k];
   }
   lv.ld_ro = ld_ro; lv.ld_cls = ld_cls; lv.ncls = ncls; lv.total = start;
-  launch_pdl(head_decode_kernel, (start + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream_v), lv, out);
-  return check_launch("uc_head_decode");
+  launch_pdl(head_decode_kernel, dim3((start + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream_v), lv, out);
+  return check_launch(what);
+}
+
+extern "C" int uc_head_decode(const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                              int ld_cls, int ncls, float* out, void* stream_v) {
+  return head_decode("uc_head_decode", regobj, cls, hw, strides, ld_ro, ld_cls, nullptr, nullptr, ncls, 1, out, stream_v);
+}
+
+extern "C" int uc_head_decode_batched(const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                                      int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float* out, void* stream_v) {
+  if (B > 1 && (!bs_ro || !bs_cls)) return set_error(UC_EINVAL, "uc_head_decode_batched: null per-image strides");
+  return head_decode("uc_head_decode_batched", regobj, cls, hw, strides, ld_ro, ld_cls, bs_ro, bs_cls, ncls, B, out, stream_v);
 }
 
 extern "C" long uc_postprocess_workspace_bytes(int max_anchors) {
@@ -288,23 +342,28 @@ extern "C" long uc_postprocess_workspace_bytes(int max_anchors) {
   return A * 7 * 4 * 2 + a2 * 8 + A * 4 * 2 + 256;
 }
 
-extern "C" int uc_postprocess(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, void* workspace,
-                              long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
+extern "C" long uc_postprocess_workspace_bytes_batched(int max_anchors, int B) {
+  return B < 1 ? 0 : B * uc_postprocess_workspace_bytes(max_anchors);
+}
+
+static int postprocess(const char* what, const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
+                       void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!pred || !workspace || !out_dets || !out_count || A < 1 || ncls < 1) return set_error(UC_EINVAL, "uc_postprocess: bad arguments");
-  if (workspace_bytes < uc_postprocess_workspace_bytes(A)) return set_error(UC_EINVAL, "uc_postprocess: workspace too small");
+  if (!pred || !workspace || !out_dets || !out_count || A < 1 || ncls < 1) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (workspace_bytes < B * uc_postprocess_workspace_bytes(A))
+    return set_error(UC_EINVAL, "%s: workspace too small (%ld bytes for %d images of %d anchors, need %ld)", what, workspace_bytes, B, A,
+                     B * uc_postprocess_workspace_bytes(A));
   long a2 = 1;
   while (a2 < A) a2 <<= 1;
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  int* count = reinterpret_cast<int*>(ws);
-  float* det = reinterpret_cast<float*>(ws + 256);
-  float* sorted = det + static_cast<long>(A) * 7;
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(sorted + static_cast<long>(A) * 7);
-  int* det_anchor = reinterpret_cast<int*>(keys + a2);
-  int* sorted_anchor = det_anchor + A;
-  launch_pdl(det_filter_kernel, 1, 1024, 0, stream, pred, A, ncls, conf_thre, det, keys, count, A, det_anchor);
-  launch_pdl(sort_desc_kernel, 1, 1024, 0, stream, keys, count, static_cast<int>(a2));
-  launch_pdl(det_gather_kernel, std::min(num_sms() * 4, (A + 255) / 256), 256, 0, stream, det, keys, count, sorted, det_anchor, sorted_anchor);
+  PostSlices sl;
+  sl.ws = static_cast<uint8_t*>(workspace);
+  sl.per_image = uc_postprocess_workspace_bytes(A);
+  sl.a2 = a2;
+  sl.A = A;
+  launch_pdl(det_filter_kernel, B, 1024, 0, stream, pred, A, ncls, conf_thre, sl);
+  launch_pdl(sort_desc_kernel, B, 1024, 0, stream, sl);
+  launch_pdl(det_gather_kernel, dim3(std::min(num_sms() * 4, (A + 255) / 256), B), 256, 0, stream, sl);
   constexpr int smem = kNmsKeepSmem * (16 + 4);
   static PerDeviceFlag attr_dev;
   bool& attr = attr_dev.get();
@@ -312,7 +371,19 @@ extern "C" int uc_postprocess(const float* pred, int A, int ncls, float conf_thr
     cudaFuncSetAttribute(nms_greedy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     attr = true;
   }
-  launch_pdl(nms_greedy_kernel, 1, 1024, smem, stream, sorted, count, nms_thre, out_dets, out_count, max_keep > 0 ? max_keep : 0x7fffffff,
-                                               sorted_anchor, out_anchor);
-  return check_launch("uc_postprocess");
+  launch_pdl(nms_greedy_kernel, B, 1024, smem, stream, sl, nms_thre, out_dets, out_count, max_keep > 0 ? max_keep : 0x7fffffff, out_anchor);
+  return check_launch(what);
+}
+
+extern "C" int uc_postprocess(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, void* workspace,
+                              long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
+  return postprocess("uc_postprocess", pred, A, ncls, conf_thre, nms_thre, max_keep, 1, workspace, workspace_bytes, out_dets, out_count,
+                     out_anchor, stream_v);
+}
+
+extern "C" int uc_postprocess_batched(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
+                                      void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor,
+                                      void* stream_v) {
+  return postprocess("uc_postprocess_batched", pred, A, ncls, conf_thre, nms_thre, max_keep, B, workspace, workspace_bytes, out_dets,
+                     out_count, out_anchor, stream_v);
 }

@@ -47,6 +47,7 @@ class UnicornEngine:
         self._bufs = {}
         self._stats_arena = None
         self._stats_used = 0
+        self._retired = []
         self._pos_cache = {}
         self._side_streams = None
         self._fork_stream = None
@@ -69,7 +70,7 @@ class UnicornEngine:
         import copy
         ctx = copy.copy(self)
         ctx._bufs = {}
-        ctx._stats_arena, ctx._stats_used = None, 0
+        ctx._stats_arena, ctx._stats_used, ctx._retired = None, 0, []
         ctx._row_arena, ctx._row_used = None, 0
         ctx._ctr_arena, ctx._ctr_used = None, 0
         ctx._side_streams, ctx._fork_stream = None, None
@@ -335,16 +336,26 @@ class UnicornEngine:
         assert self._ctr_used <= self._ctr_arena.shape[0]
         return c
 
-    def _stats(self, groups):
-        s = self._stats_arena[self._stats_used]
-        self._stats_used += 1
-        assert self._stats_used <= self._stats_arena.shape[0]
-        return s[:groups]
+    def _stats(self, groups, B=1):
+        """GroupNorm statistics of one conv: [G, 2] (B = 1) or [B, G, 2] int64, B consecutive slots of the per-frame arena."""
+        if B == 1:
+            s = self._stats_arena[self._stats_used]
+            self._stats_used += 1
+            assert self._stats_used <= self._stats_arena.shape[0]
+            return s[:groups]
+        need = self._stats_used + B
+        if need > self._stats_arena.shape[0]:  # a batched frame needs B slots per conv
+            assert not torch.cuda.is_current_stream_capturing(), "statistics arena must be sized by an eager frame first"
+            self._retired.append(self._stats_arena)  # graphs captured earlier read and zero the old arena: it stays allocated
+            self._stats_arena = torch.zeros(max(need, 2 * self._stats_arena.shape[0]), 32, 2, dtype=torch.int64, device=self.dev)
+        s = self._stats_arena[self._stats_used:need]
+        self._stats_used = need
+        return s.view(-1)[:B * groups * 2].view(B, groups, 2)
 
     # ------------------------------------------------------------------------------------------ building blocks
     def conv_gn(self, x, c, out, act=ACT_SILU, prior=None, beta=None, add2=None, out2=None):
         """x NHWC view -> out NHWC view (may be a channel slice)."""
-        st = self._stats(c.groups)
+        st = self._stats(c.groups, x.shape[0])
         self.conv(x, c.w, c.k, c.stride, (c.k - 1) // 2, bias=c.bias, out=out, gn_stats=st, gn_groups=c.groups)
         ops.groupnorm_apply(out, st, c.gw, c.gb, c.groups, c.eps, act, prior=prior, beta=beta, add2=add2, out2=out2)
         return out
@@ -406,23 +417,23 @@ class UnicornEngine:
         return fpn, seq, side_out
 
     def features(self, img, tag="cur"):
-        """img fp32 NCHW [1,3,H,W] (or uint8 HWC BGR [1,H,W,3]) -> (backbone outputs (s8, s16, s32) NHWC bf16, seq_dict{feat NHWC view, h, w}).
+        """img fp32 NCHW [B,3,H,W] (or uint8 HWC BGR [B,H,W,3]) -> (backbone outputs (s8, s16, s32) NHWC bf16, seq_dict{feat NHWC view, h, w}).
         The s8 / s16 outputs are written straight into their slots of the neck's concat buffers (yolo_pafpn_new.py:137-155)."""
         inc = self.inc
         if img.dtype == torch.uint8:  # HWC BGR frame straight from the decoder / cv2.resize
             B, H, W, _ = img.shape
         else:
             B, _, H, W = img.shape
-        assert B == 1 and H % 32 == 0 and W % 32 == 0
+        assert B >= 1 and H % 32 == 0 and W % 32 == 0
         h8, w8, h16, w16, h32, w32 = H // 8, W // 8, H // 16, W // 16, H // 32, W // 32
         # concat buffers of the neck (producers write into slices)
-        cat_p4 = self.buf(tag + ".cat_p4", (1, h16, w16, 2 * inc[1]))
-        cat_p3 = self.buf(tag + ".cat_p3", (1, h8, w8, 2 * inc[0]))
-        cat_n3 = self.buf(tag + ".cat_n3", (1, h16, w16, 2 * inc[0]))
-        cat_n4 = self.buf(tag + ".cat_n4", (1, h32, w32, 2 * inc[1]))
-        dst = (cat_p3[..., inc[0]:], cat_p4[..., inc[1]:], self.buf(tag + ".x0n", (1, h32, w32, inc[2])))
+        cat_p4 = self.buf(tag + ".cat_p4", (B, h16, w16, 2 * inc[1]))
+        cat_p3 = self.buf(tag + ".cat_p3", (B, h8, w8, 2 * inc[0]))
+        cat_n3 = self.buf(tag + ".cat_n3", (B, h16, w16, 2 * inc[0]))
+        cat_n4 = self.buf(tag + ".cat_n4", (B, h32, w32, 2 * inc[1]))
+        dst = (cat_p3[..., inc[0]:], cat_p4[..., inc[1]:], self.buf(tag + ".x0n", (B, h32, w32, inc[2])))
         if self.cfg["backbone"] == "resnet50":
-            x = ops.resnet_stem(img, *self.P["rstem"], out=self.buf(tag + ".rstem", (1, H // 4, W // 4, 64)))
+            x = ops.resnet_stem(img, *self.P["rstem"], out=self.buf(tag + ".rstem", (B, H // 4, W // 4, 64)))
             self._resnet_layers(x, dst, tag)
         else:
             self._convnext_features(img, dst, tag)
@@ -437,8 +448,8 @@ class UnicornEngine:
             if i > 0:
                 lw, lb, cw, cb = P[f"down{i}"]
                 Bx, Hx, Wx, Cx = x.shape
-                t = ops.layernorm(x.view(-1, Cx), lw, lb, 1e-6, out=self.buf(f"{tag}.dn{i}", (Hx * Wx, Cx))).view(1, Hx, Wx, Cx)
-                x = self.conv(t, cw, 2, 2, 0, bias=cb, out=self.buf(f"{tag}.x{i}", (1, Hx // 2, Wx // 2, d[i])))
+                t = ops.layernorm(x.view(-1, Cx), lw, lb, 1e-6, out=self.buf(f"{tag}.dn{i}", (Bx * Hx * Wx, Cx))).view(Bx, Hx, Wx, Cx)
+                x = self.conv(t, cw, 2, 2, 0, bias=cb, out=self.buf(f"{tag}.x{i}", (Bx, Hx // 2, Wx // 2, d[i])))
             for j, bp in enumerate(P["stages"][i]):
                 self.convnext_block(x, bp, f"{tag}.s{i}")
             if i >= 1:
@@ -486,15 +497,16 @@ class UnicornEngine:
         # top-down
         fpn_out0 = self.conv_gn(x0n, P["lateral_conv0"], cat_n4[..., d[2]:])
         ops.copy_upsample(fpn_out0, cat_p4[..., :d[2]], 2)
-        f_out0 = self.csp(cat_p4, P["C3_p4"], self.buf(tag + ".f_out0", (1, h16, w16, d[2])), tag + ".C3_p4")
+        B = x0n.shape[0]
+        f_out0 = self.csp(cat_p4, P["C3_p4"], self.buf(tag + ".f_out0", (B, h16, w16, d[2])), tag + ".C3_p4")
         fpn_out1 = self.conv_gn(f_out0, P["reduce_conv1"], cat_n3[..., d[1]:])
         ops.copy_upsample(fpn_out1, cat_p3[..., :d[1]], 2)
-        pan_out2 = self.csp(cat_p3, P["C3_p3"], self.buf(tag + ".pan_out2", (1, h8, w8, d[1])), tag + ".C3_p3")
+        pan_out2 = self.csp(cat_p3, P["C3_p3"], self.buf(tag + ".pan_out2", (B, h8, w8, d[1])), tag + ".C3_p3")
         # bottom-up
         self.conv_gn(pan_out2, P["bu_conv2"], cat_n3[..., :d[1]])
-        pan_out1 = self.csp(cat_n3, P["C3_n3"], self.buf(tag + ".pan_out1", (1, h16, w16, d[2])), tag + ".C3_n3")
+        pan_out1 = self.csp(cat_n3, P["C3_n3"], self.buf(tag + ".pan_out1", (B, h16, w16, d[2])), tag + ".C3_n3")
         self.conv_gn(pan_out1, P["bu_conv1"], cat_n4[..., :d[2]])
-        pan_out0 = self.csp(cat_n4, P["C3_n4"], self.buf(tag + ".pan_out0", (1, h32, w32, d[3])), tag + ".C3_n4")
+        pan_out0 = self.csp(cat_n4, P["C3_n4"], self.buf(tag + ".pan_out0", (B, h32, w32, d[3])), tag + ".C3_n4")
         self.dbg = dict(x2n=x2n, x1n=x1n, x0n=x0n, fpn_out0=fpn_out0, f_out0=f_out0, fpn_out1=fpn_out1, pan_out2=pan_out2,
                         pan_out1=pan_out1, pan_out0=pan_out0)
         return (pan_out2, pan_out1, pan_out0)
@@ -513,28 +525,38 @@ class UnicornEngine:
             self._pos_cache[key] = (toks.to(BF16).contiguous(), pos)
         return self._pos_cache[key]
 
+    def _pos_batch(self, h, w, B):
+        """pos_tokens(h, w)[0] repeated for B images: [2, B*h*w, 256] bf16 (the GroupNorm epilogue adds it per pixel of every image)."""
+        if B == 1:
+            return self.pos_tokens(h, w)[0]
+        key = (h, w, B)
+        if key not in self._pos_cache:
+            self._pos_cache[key] = self.pos_tokens(h, w)[0].repeat(1, B, 1).contiguous()
+        return self._pos_cache[key]
+
     def project_tokens(self, feat, lvl, src_rows, q_rows):
-        """bottleneck conv1x1+bias -> GN32 (unicorn.py:36-38,265); writes `src_rows` [h*w, 256] and
+        """bottleneck conv1x1+bias -> GN32 (unicorn.py:36-38,265) of feat [B,h,w,C]; writes `src_rows` [B*h*w, 256] and
         `q_rows = src + pos + level_embed[lvl]`."""
-        h, w = feat.shape[1:3]
-        pos_lvl = self.pos_tokens(h, w)[0]
-        self.conv_gn(feat, self.P["bottleneck"], src_rows.view(1, h, w, 256), act=ACT_NONE, add2=pos_lvl[lvl].view(1, h, w, 256),
-                     out2=q_rows.view(1, h, w, 256))
+        B, h, w = feat.shape[:3]
+        pos_lvl = self._pos_batch(h, w, B)
+        self.conv_gn(feat, self.P["bottleneck"], src_rows.view(B, h, w, 256), act=ACT_NONE, add2=pos_lvl[lvl].view(B, h, w, 256),
+                     out2=q_rows.view(B, h, w, 256))
 
     def project_ref(self, feat):
         """Projection of a fixed reference frame (level 0 of the encoder input), computed once and OWNED BY THE CALLER: several
         trackers may share one engine, each keeps its own reference (the reference repo keeps `out_dict_pre` per tracker,
-        unicorn_sot.py:47).  Pass the result to interaction(ref_proj=...)."""
-        h, w = feat.shape[1:3]
-        src = torch.empty(h * w, 256, dtype=BF16, device=self.dev)
-        q = torch.empty(h * w, 256, dtype=BF16, device=self.dev)
+        unicorn_sot.py:47).  Pass the result to interaction(ref_proj=...).  feat [B,h,w,C] -> (src, q) [B*h*w, 256] each."""
+        B, h, w = feat.shape[:3]
+        src = torch.empty(B * h * w, 256, dtype=BF16, device=self.dev)
+        q = torch.empty(B * h * w, 256, dtype=BF16, device=self.dev)
         self.begin_frame()
         self.project_tokens(feat, 0, src, q)
         return src, q
 
     def encoder(self, src, q, h, w):
         """One deformable encoder layer over the two frames as two levels (deformable_transformer.py:122-131,
-        ops/modules/ms_deform_attn.py:94-115).  src, q: [2hw, 256] bf16.  Returns [2hw, 256] bf16 (new buffer)."""
+        ops/modules/ms_deform_attn.py:94-115).  src, q: [2Bhw, 256] bf16, all images' reference rows, then all their current rows.
+        Returns [2Bhw, 256] bf16 (new buffer)."""
         P = self.P
         S = src.shape[0]
         value = ops.linear(src, P["value_proj"][0], bias=P["value_proj"][1], out=self.buf("enc.value", (S, 256)))
@@ -548,10 +570,12 @@ class UnicornEngine:
         return y
 
     def interaction(self, feat0, feat1, ref_proj=None):
-        """Unicorn.forward_deform_interact (unicorn.py:260-276): -> (new_feat0, new_feat1) NHWC bf16 [1,h,w,256].
-        ref_proj = project_ref(feat0) of a fixed reference frame: its rows are copied in instead of being recomputed."""
-        h, w = feat1.shape[1:3]
-        n = h * w
+        """Unicorn.forward_deform_interact (unicorn.py:260-276) of B frame pairs: feat [B,h,w,C] -> (new_feat0, new_feat1) NHWC bf16
+        [B,h,w,256].  ref_proj = project_ref(feat0) of fixed reference frames ([B*h*w, 256] each): its rows are copied in instead
+        of being recomputed.  Token rows are [2][B][h*w] (all reference rows, then all current rows): every projection is one
+        batched conv, and the deformable attention samples each image's own rows."""
+        B, h, w = feat1.shape[:3]
+        n = B * h * w
         src, q = self.buf("enc.src", (2 * n, 256)), self.buf("enc.q", (2 * n, 256))
         if ref_proj is None:
             self.project_tokens(feat0, 0, src[:n], q[:n])
@@ -560,24 +584,32 @@ class UnicornEngine:
             q[:n].copy_(ref_proj[1])
         self.project_tokens(feat1, 1, src[n:], q[n:])
         y = self.encoder(src, q, h, w)
-        return y[:n].view(1, h, w, 256), y[n:].view(1, h, w, 256)
+        return y[:n].view(B, h, w, 256), y[n:].view(B, h, w, 256)
 
     def upsample(self, feat, tag):
-        """Unicorn.forward_upsample (unicorn.py:41-44,311-313): [1,h,w,256] -> embedding [1,2h,2w,128] fp16."""
-        _, h, w, _ = feat.shape
-        ps = ops.pixel_shuffle2(feat, out=self.buf(tag + ".ps", (1, 2 * h, 2 * w, 64)))
-        t = self.conv(ps, self.P["up1"][0], 3, 1, 1, bias=self.P["up1"][1], act=ACT_RELU, out=self.buf(tag + ".u1", (1, 2 * h, 2 * w, 256)))
-        return self.conv(t, self.P["up3"][0], 3, 1, 1, bias=self.P["up3"][1], out=self.buf(tag + ".emb", (1, 2 * h, 2 * w, 128), F16))
+        """Unicorn.forward_upsample (unicorn.py:41-44,311-313): [B,h,w,256] -> embedding [B,2h,2w,128] fp16."""
+        B, h, w, _ = feat.shape
+        ps = ops.pixel_shuffle2(feat, out=self.buf(tag + ".ps", (B, 2 * h, 2 * w, 64)))
+        t = self.conv(ps, self.P["up1"][0], 3, 1, 1, bias=self.P["up1"][1], act=ACT_RELU, out=self.buf(tag + ".u1", (B, 2 * h, 2 * w, 256)))
+        return self.conv(t, self.P["up3"][0], 3, 1, 1, bias=self.P["up3"][1], out=self.buf(tag + ".emb", (B, 2 * h, 2 * w, 128), F16))
 
     # ------------------------------------------------------------------------------------------ correlation
     def propagate(self, embed_ref, embed_cur, values):
-        """unicorn_sot.py:88-105: label propagation + prior pyramid.  values fp32 [K, h8*w8] -> 3 fp32 maps [K,h,w]."""
-        _, hh, ww, C = embed_cur.shape
-        K = values.shape[0]
-        coarse = ops.corr_propagate(embed_ref.view(-1, C), embed_cur.view(-1, C), values, out=self.buf("corr.out", (K, hh * ww), F32))
-        c0 = coarse.view(K, hh, ww)
-        c1 = ops.bilinear(c0, hh // 2, ww // 2, 2.0, 2.0, out=self.buf("corr.p1", (K, hh // 2, ww // 2), F32))
-        c2 = ops.bilinear(c0, hh // 4, ww // 4, 4.0, 4.0, out=self.buf("corr.p2", (K, hh // 4, ww // 4), F32))
+        """unicorn_sot.py:88-105: label propagation + prior pyramid.  B = 1: values fp32 [K, h8*w8] -> 3 fp32 maps [K,h,w].
+        B > 1 (embeddings [B,h,w,C]): values [B, K, h8*w8] -> 3 maps [B,K,h,w], every sequence against its own reference."""
+        B, hh, ww, C = embed_cur.shape
+        if B == 1:
+            K = values.shape[0]
+            coarse = ops.corr_propagate(embed_ref.view(-1, C), embed_cur.view(-1, C), values, out=self.buf("corr.out", (K, hh * ww), F32))
+            lead = (K,)
+        else:
+            K = values.shape[1]
+            coarse = ops.corr_propagate(embed_ref.view(B, -1, C), embed_cur.view(B, -1, C), values,
+                                        out=self.buf("corr.out", (B, K, hh * ww), F32))
+            lead = (B, K)
+        c0 = coarse.view(*lead, hh, ww)
+        c1 = ops.bilinear(c0, hh // 2, ww // 2, 2.0, 2.0, out=self.buf("corr.p1", (*lead, hh // 2, ww // 2), F32))
+        c2 = ops.bilinear(c0, hh // 4, ww // 4, 4.0, 4.0, out=self.buf("corr.p2", (*lead, hh // 4, ww // 4), F32))
         return (c0, c1, c2)
 
     # ------------------------------------------------------------------------------------------ head
@@ -585,7 +617,9 @@ class UnicornEngine:
         """MaskBranch.forward with use_raft (condinst/mask_branch.py:77-96,158-162): -> (mask_feats fp32 [1,h8,w8,8],
         up_masks fp32 [1,h8,w8,144])."""
         M = self.P["mask"]
-        _, h, w, _ = fpn[0].shape
+        B, h, w, _ = fpn[0].shape
+        if B != 1:
+            raise ValueError(f"UnicornEngine.mask_branch runs one image (got a batch of {B}); the mask path is not batched")
         x = self.conv_gn(fpn[0], M["refine"][0], self.buf("mask.x", (1, h, w, 128)), act=ACT_RELU)
         for i in (1, 2):
             _, hi, wi, _ = fpn[i].shape
@@ -600,10 +634,13 @@ class UnicornEngine:
         return mf, um
 
     def head(self, fpn, priors, mode, with_masks=False):
-        """UnicornHead.forward eval branch (unicorn_head.py:267-336) + decode_outputs (:467-482).
-        fpn: 3 NHWC bf16 maps; priors: 3 fp32 [1,h,w] maps or None (MOT: zero prior == no fusion term).
-        Returns fp32 [1, A, 5+ncls_mode].  with_masks=True (UnicornHeadMask, unicorn_head_mask.py:333-343) also runs the
+        """UnicornHead.forward eval branch (unicorn_head.py:267-336) + decode_outputs (:467-482) of B images.
+        fpn: 3 NHWC bf16 maps [B,h,w,C]; priors: 3 fp32 maps with B*h*w elements each ([B,h,w], or [B,1,h,w] from propagate) or None
+        (MOT: zero prior == no fusion term).  Returns fp32 [B, A, 5+ncls_mode].  with_masks=True (UnicornHeadMask, unicorn_head_mask.py:333-343) also runs the
         controller convs; their outputs are left in self.dyn_levels (3 x fp32 [1,h,w,176]) for ops.dynamic_masks."""
+        B = fpn[0].shape[0]
+        if with_masks and B != 1:
+            raise ValueError(f"UnicornEngine.head(with_masks=True) runs one image (got a batch of {B}); the mask path is not batched")
         self._with_masks = with_masks
         self.dyn_levels = [None] * 3
         sfx = "_sot" if mode == "sot" else ""
@@ -623,13 +660,13 @@ class UnicornEngine:
         for s_ in self._side_streams:  # join
             main.wait_stream(s_)
         A = sum(h * w for h, w in hw)
-        return ops.head_decode(ro_outs, cls_outs, hw, STRIDES, ncls, out=self.buf(f"head.out{ncls}", (1, A, 5 + ncls), F32))
+        return ops.head_decode(ro_outs, cls_outs, hw, STRIDES, ncls, out=self.buf(f"head.out{ncls}", (B, A, 5 + ncls), F32))
 
     def _head_level(self, k, fpn, priors, sfx, ro_outs, cls_outs, hw):
         if True:
             L = self.P["head"][k]
-            _, h, w, _ = fpn[k].shape
-            x = self.buf(f"head{k}.x", (1, h, w, 256))
+            B, h, w, _ = fpn[k].shape
+            x = self.buf(f"head{k}.x", (B, h, w, 256))
             pr = priors[k].reshape(-1) if priors is not None else None
             self.conv_gn(fpn[k], L["stem"], x, prior=pr, beta=L["beta"] if pr is not None else None)
             for i in range(3):
@@ -638,11 +675,11 @@ class UnicornEngine:
             for name in ("cls", "reg"):
                 cur = x
                 for i, c in enumerate(L[name]):
-                    cur = self.conv_gn(cur, c, self.buf(f"head{k}.{name}{i % 2}", (1, h, w, 256)))
+                    cur = self.conv_gn(cur, c, self.buf(f"head{k}.{name}{i % 2}", (B, h, w, 256)))
                 feats.append(cur)
             row, rob, cw, cb, _ = L["pred" + sfx]
-            cls_outs[k] = ops.conv2d(feats[0], cw, 1, 1, bias=cb, out=self.buf(f"head{k}.clso", (1, h, w, 8), F32))
-            ro_outs[k] = ops.conv2d(feats[1], row, 1, 1, bias=rob, out=self.buf(f"head{k}.roo", (1, h, w, 8), F32))
+            cls_outs[k] = ops.conv2d(feats[0], cw, 1, 1, bias=cb, out=self.buf(f"head{k}.clso", (B, h, w, 8), F32))
+            ro_outs[k] = ops.conv2d(feats[1], row, 1, 1, bias=rob, out=self.buf(f"head{k}.roo", (B, h, w, 8), F32))
             hw[k] = (h, w)
             if self._with_masks:
                 cw_, cb_ = L["ctrl"]
@@ -650,6 +687,6 @@ class UnicornEngine:
 
 
 def _rows(t):
-    """[1,H,W,C] channel-slice view -> [H*W, C] strided rows view."""
-    _, H, W, C = t.shape
-    return t.as_strided((H * W, C), (t.stride(2), 1), t.storage_offset())
+    """[B,H,W,C] channel-slice view -> [B*H*W, C] strided rows view."""
+    B, H, W, C = t.shape
+    return t.as_strided((B * H * W, C), (t.stride(2), 1), t.storage_offset())

@@ -13,15 +13,15 @@ def anchor_count(H, W):
 class FrameSlot:
     """One frame in flight: the engine or engine fork (own activation buffers) it runs on, its stream (None: the current one), the
     two static input buffers a captured graph reads, the NMS workspace, the graph, a completion event and the frame's
-    intermediate tensors (`last`)."""
+    intermediate tensors (`last`).  batch > 1: the inputs hold that many frames and the workspace that many images."""
 
-    def __init__(self, eng, H, W, stream=None):
+    def __init__(self, eng, H, W, stream=None, batch=1):
         dev = eng.dev
         self.eng, self.stream = eng, stream
-        self.img_in = torch.empty(1, 3, H, W, dtype=torch.float32, device=dev)   # PreprocessorX format
-        self.img_in_u8 = torch.empty(1, H, W, 3, dtype=torch.uint8, device=dev)  # letterboxed BGR frame: 4x fewer H2D bytes
+        self.img_in = torch.empty(batch, 3, H, W, dtype=torch.float32, device=dev)   # PreprocessorX format
+        self.img_in_u8 = torch.empty(batch, H, W, 3, dtype=torch.uint8, device=dev)  # letterboxed BGR frame: 4x fewer H2D bytes
         self.u8 = False
-        self.ws = ops.PostWorkspace(anchor_count(H, W), dev)
+        self.ws = ops.PostWorkspace(anchor_count(H, W), dev, batch)
         self.graph = None
         self.event = torch.cuda.Event()
         self.last = {}
@@ -31,12 +31,15 @@ class FrameSlot:
         """The input buffer the frame reads."""
         return self.img_in_u8 if self.u8 else self.img_in
 
-    def stage(self, frame):
-        """Copy fp32 [1,3,H,W] or uint8 [1,H,W,3] `frame` (host or device) into the matching static buffer; returns the buffer."""
-        u8 = frame.dtype == torch.uint8
+    def use_u8(self, u8):
+        """Select the input buffer the frame reads (dropping a graph captured on the other one); returns it."""
         if u8 != self.u8:
             self.u8, self.graph = u8, None  # the captured graph reads the other buffer
-        self.img.copy_(frame, non_blocking=True)
+        return self.img
+
+    def stage(self, frame):
+        """Copy fp32 [B,3,H,W] or uint8 [B,H,W,3] `frame` (host or device) into the matching static buffer; returns the buffer."""
+        self.use_u8(frame.dtype == torch.uint8).copy_(frame, non_blocking=True)
         return self.img
 
     def capture(self, frame_fn, warmup=False):

@@ -330,62 +330,107 @@ def msda_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_we
 
 
 def msda_fused(value, offlog, level_hw, M=8, P=4, out=None):
+    """value bf16 [B*Lq, M*32] with Lq = sum h*w over the levels: B images whose rows are level-major, the images inside each level
+    (level l of image b at row B*start_l + b*h_l*w_l; B = 1 is the plain concatenation of the levels).  offlog and out: same rows."""
     L = len(level_hw)
     Lq = sum(h * w for h, w in level_hw)
-    assert value.shape == (Lq, M * 32) and value.dtype == torch.bfloat16 and value.is_contiguous()
-    assert offlog.dtype == torch.float32 and offlog.shape[0] == Lq and offlog.shape[1] >= M * L * P * 3
+    B = value.shape[0] // Lq
+    assert value.shape == (B * Lq, M * 32) and B >= 1 and value.dtype == torch.bfloat16 and value.is_contiguous()
+    assert offlog.dtype == torch.float32 and offlog.shape[0] == B * Lq and offlog.shape[1] >= M * L * P * 3
     if out is None:
-        out = torch.empty(Lq, M * 32, dtype=torch.bfloat16, device=value.device)
+        out = torch.empty(B * Lq, M * 32, dtype=torch.bfloat16, device=value.device)
     hw = (ctypes.c_int * (2 * L))(*[v for pair in level_hw for v in pair])
-    _lib.check(_L().uc_msda_fused_bf16(_p(value), _p(offlog), offlog.stride(0), _p(out), hw, L, M, P, _S()), "uc_msda_fused_bf16")
+    if B == 1:
+        _lib.check(_L().uc_msda_fused_bf16(_p(value), _p(offlog), offlog.stride(0), _p(out), hw, L, M, P, _S()), "uc_msda_fused_bf16")
+    else:
+        _lib.check(_L().uc_msda_fused_bf16_batched(_p(value), _p(offlog), offlog.stride(0), _p(out), hw, L, M, P, B, _S()),
+                   "uc_msda_fused_bf16_batched")
     return out
 
 
 def corr_propagate(embed_ref, embed_cur, values, out=None):
-    """embed_* [n, 128] 16-bit rows; values fp32 [n_obj, n_ref] -> fp32 [n_obj, n_cur]."""
-    n_ref, C = embed_ref.shape
-    n_cur = embed_cur.shape[0]
-    n_obj = values.shape[0]
-    assert values.dtype == torch.float32 and values.stride(1) == 1 and values.shape[1] == n_ref
+    """embed_* [n, 128] 16-bit rows; values fp32 [n_obj, n_ref] -> fp32 [n_obj, n_cur].  With a leading batch dimension (embed_*
+    [B, n, 128], values [B, n_obj, n_ref], out [B, n_obj, n_cur]) the B sequences run in one launch, each as its own 2-D call."""
+    if embed_ref.dim() == 2:
+        n_ref, C = embed_ref.shape
+        n_cur = embed_cur.shape[0]
+        n_obj = values.shape[0]
+        assert values.dtype == torch.float32 and values.stride(1) == 1 and values.shape[1] == n_ref
+        if out is None:
+            out = torch.empty(n_obj, n_cur, dtype=torch.float32, device=values.device)
+        _lib.check(_L().uc_corr_propagate(_p(embed_ref), embed_ref.stride(0), n_ref, _p(embed_cur), embed_cur.stride(0), n_cur, C,
+                                          _DT[embed_ref.dtype], _p(values), values.stride(0), n_obj, _p(out), out.stride(0), _S()),
+                   "uc_corr_propagate")
+        return out
+    B, n_ref, C = embed_ref.shape
+    n_cur = embed_cur.shape[1]
+    n_obj = values.shape[1]
+    assert embed_cur.shape[0] == B and values.shape[0] == B and values.shape[2] == n_ref
+    assert values.dtype == torch.float32 and values.stride(2) == 1 and embed_ref.stride(2) == 1 and embed_cur.stride(2) == 1
     if out is None:
-        out = torch.empty(n_obj, n_cur, dtype=torch.float32, device=values.device)
-    _lib.check(_L().uc_corr_propagate(_p(embed_ref), embed_ref.stride(0), n_ref, _p(embed_cur), embed_cur.stride(0), n_cur, C,
-                                      _DT[embed_ref.dtype], _p(values), values.stride(0), n_obj, _p(out), out.stride(0), _S()),
-               "uc_corr_propagate")
+        out = torch.empty(B, n_obj, n_cur, dtype=torch.float32, device=values.device)
+    assert out.shape == (B, n_obj, n_cur) and out.stride(2) == 1
+    _lib.check(_L().uc_corr_propagate_batched(_p(embed_ref), embed_ref.stride(1), _l(embed_ref.stride(0)), n_ref, _p(embed_cur),
+                                              embed_cur.stride(1), _l(embed_cur.stride(0)), n_cur, C, _DT[embed_ref.dtype], _p(values),
+                                              values.stride(1), _l(values.stride(0)), n_obj, _p(out), out.stride(1), _l(out.stride(0)), B,
+                                              _S()), "uc_corr_propagate_batched")
     return out
 
 
 def head_decode(regobj, cls, hw, strides, ncls, out=None):
+    """regobj / cls: 3 fp32 maps per level, rows [h*w, ld] of one image or NHWC [B,h,w,ld] of B images (image stride stride(0)).
+    Returns fp32 [B, A, 5+ncls]."""
     A = sum(h * w for h, w in hw)
+    B = regobj[0].shape[0] if regobj[0].dim() == 4 else 1
     if out is None:
-        out = torch.empty(1, A, 5 + ncls, dtype=torch.float32, device=regobj[0].device)
+        out = torch.empty(B, A, 5 + ncls, dtype=torch.float32, device=regobj[0].device)
     ro = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in regobj])
     cl = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in cls])
     hwa = (ctypes.c_int * 6)(*[v for pair in hw for v in pair])
     st = (ctypes.c_int * 3)(*strides)
-    _lib.check(_L().uc_head_decode(ro, cl, hwa, st, regobj[0].shape[-1], cls[0].shape[-1], ncls, _p(out), _S()), "uc_head_decode")
+    if B == 1:
+        _lib.check(_L().uc_head_decode(ro, cl, hwa, st, regobj[0].shape[-1], cls[0].shape[-1], ncls, _p(out), _S()), "uc_head_decode")
+        return out
+    assert all(t.dim() == 4 and t.shape[0] == B for t in list(regobj) + list(cls)) and out.shape == (B, A, 5 + ncls) and out.is_contiguous()
+    bs_ro = (ctypes.c_long * 3)(*[t.stride(0) for t in regobj])
+    bs_cl = (ctypes.c_long * 3)(*[t.stride(0) for t in cls])
+    _lib.check(_L().uc_head_decode_batched(ro, cl, hwa, st, regobj[0].shape[-1], cls[0].shape[-1], bs_ro, bs_cl, ncls, B, _p(out), _S()),
+               "uc_head_decode_batched")
     return out
 
 
 class PostWorkspace:
-    def __init__(self, max_anchors, device):
-        fn = _L().uc_postprocess_workspace_bytes
+    """Device workspace and outputs of postprocess_device.  batch = 1: dets [A, 7], count [1], anchors [A]; batch = B > 1: one
+    slice per image, dets [B, A, 7], count [B], anchors [B, A]."""
+
+    def __init__(self, max_anchors, device, batch=1):
+        fn = _L().uc_postprocess_workspace_bytes_batched
         fn.restype = ctypes.c_long
-        self.nbytes = fn(max_anchors)
+        self.nbytes = fn(max_anchors, batch)
+        assert self.nbytes > 0, "PostWorkspace: batch must be >= 1"
+        lead = (batch,) if batch > 1 else ()
         self.buf = torch.empty(self.nbytes, dtype=torch.uint8, device=device)
-        self.dets = torch.empty(max_anchors, 7, dtype=torch.float32, device=device)
-        self.count = torch.zeros(1, dtype=torch.int32, device=device)
-        self.anchors = torch.zeros(max_anchors, dtype=torch.int32, device=device)
-        self.max_anchors = max_anchors
+        self.dets = torch.empty(*lead, max_anchors, 7, dtype=torch.float32, device=device)
+        self.count = torch.zeros(batch, dtype=torch.int32, device=device)
+        self.anchors = torch.zeros(*lead, max_anchors, dtype=torch.int32, device=device)
+        self.max_anchors, self.batch = max_anchors, batch
 
 
 def postprocess_device(pred, ncls, conf, nms, ws, max_keep=0):
-    """pred fp32 [A, 5+ncls] (decoded).  Launches only; ws.dets / ws.count hold the result.
-    max_keep > 0 returns exactly the first max_keep rows of the full NMS result."""
-    A = pred.shape[0]
-    assert pred.is_contiguous() and pred.dtype == torch.float32 and A <= ws.max_anchors
-    _lib.check(_L().uc_postprocess(_p(pred), A, ncls, _f(conf), _f(nms), int(max_keep), _p(ws.buf), _l(ws.nbytes), _p(ws.dets), _p(ws.count), _p(ws.anchors), _S()),
-               "uc_postprocess", 4)
+    """pred fp32 [A, 5+ncls] (decoded), or [B, A, 5+ncls] with a workspace of batch B.  Launches only; ws.dets / ws.count hold the
+    result.  max_keep > 0 returns exactly the first max_keep rows of the full NMS result (per image)."""
+    assert pred.is_contiguous() and pred.dtype == torch.float32 and pred.shape[-2] <= ws.max_anchors
+    if pred.dim() == 3 and pred.shape[0] == 1:
+        pred = pred[0]
+    if pred.dim() == 2:
+        A = pred.shape[0]
+        _lib.check(_L().uc_postprocess(_p(pred), A, ncls, _f(conf), _f(nms), int(max_keep), _p(ws.buf), _l(ws.nbytes), _p(ws.dets), _p(ws.count), _p(ws.anchors), _S()),
+                   "uc_postprocess", 4)
+        return ws.dets, ws.count
+    B, A = pred.shape[:2]
+    assert B == ws.batch and A == ws.max_anchors, "postprocess_device: a batch of B images needs a PostWorkspace(A, device, batch=B)"
+    _lib.check(_L().uc_postprocess_batched(_p(pred), A, ncls, _f(conf), _f(nms), int(max_keep), B, _p(ws.buf), _l(ws.nbytes), _p(ws.dets),
+                                           _p(ws.count), _p(ws.anchors), _S()), "uc_postprocess_batched", 4)
     return ws.dets, ws.count
 
 

@@ -185,3 +185,134 @@ class UnicornSOTTrack:
         if n > 0:
             self.state = state_xywh(dets[0], r, self.input_size)
         return {"target_bbox": self.state}
+
+
+class UnicornSOTBatch:
+    """`n_seq` SOT sequences in lock step: one batched frame (backbone -> interaction -> upsample -> correlation -> head -> NMS over
+    all sequences) per step, captured as one CUDA graph.  Each sequence's results equal those of its own UnicornSOTTrack: every
+    kernel of the batched frame computes each image as its B = 1 launch does.
+
+    initialize(i, ...) sets sequence slot i at any time: its reference frame runs at B = 1 and its reference projection and label
+    values are written in place into the static batched buffers the graph reads, so the graph stays valid and the other slots are
+    unaffected.  A slot that has not been initialised, or gets None in track(), computes on whatever its input buffer holds and its
+    result is discarded."""
+
+    def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.001, nms=0.65, max_inst=3, use_graph=True, device_preproc=False):
+        assert n_seq >= 1
+        self.eng, self.input_size, self.n_seq = engine, tuple(input_size), n_seq
+        self.confthre, self.nmsthre, self.max_inst = conf, nms, max_inst
+        self.use_graph, self.device_preproc = use_graph, device_preproc
+        H, W = self.input_size
+        dev = engine.dev
+        self.slot = FrameSlot(engine, H, W, batch=n_seq)
+        self._ref_slot = FrameSlot(engine, H, W)  # B = 1 input of initialize
+        n16 = (H // 16) * (W // 16)
+        self.ref_proj = (torch.zeros(n_seq * n16, 256, dtype=torch.bfloat16, device=dev), torch.zeros(n_seq * n16, 256, dtype=torch.bfloat16, device=dev))
+        self.lbs_pre = torch.zeros(n_seq, 1, (H // 8) * (W // 8), dtype=torch.float32, device=dev)
+        self.host_dets = torch.empty(n_seq, max_inst, 7, dtype=torch.float32).pin_memory()
+        self.host_count = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
+        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()  # host-letterboxed frames (track())
+        self._raw = [None] * n_seq
+        self.ready = [False] * n_seq
+        self.states = [None] * n_seq
+        self.launches_per_frame = 0
+
+    # -------------------------------------------------------------------------------- device-side frame
+    def _frame(self):
+        e, n = self.eng, self.n_seq
+        e.begin_frame()
+        values = self.lbs_pre if n > 1 else self.lbs_pre[0]
+
+        def correlate(seq):
+            f_pre, f_cur = e.interaction(None, seq["feat"], ref_proj=self.ref_proj)
+            e_pre, e_cur = e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc")
+            return e.propagate(e_pre, e_cur, values)
+
+        fpn, seq, priors = e.backbone(self.slot.img, tag="cur", side=correlate)
+        out = e.head(fpn, priors, "sot")
+        ops.postprocess_device(out, 1, self.confthre, self.nmsthre, self.slot.ws, max_keep=self.max_inst)
+        self.slot.last = dict(fpn=fpn, feat=seq["feat"], priors=priors, head=out)
+
+    def _run(self):
+        s = self.slot
+        if not self.use_graph:
+            self._frame()
+        elif s.graph is None:
+            s.graph, self.launches_per_frame = s.capture(self._frame, warmup=True)
+        else:
+            s.graph.replay()
+        dets = s.ws.dets.view(self.n_seq, -1, 7)
+        self.host_count.copy_(s.ws.count, non_blocking=True)
+        self.host_dets.copy_(dets[:, :self.max_inst], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+
+    def initialize_tensor(self, i, ref_frame, init_box_xyxy):
+        """Slot i: ref_frame preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3] (host or device); init box in resized-image coordinates."""
+        assert 0 <= i < self.n_seq
+        e = self.eng
+        H, W = self.input_size
+        n16 = (H // 16) * (W // 16)
+        torch.cuda.synchronize()
+        inp = self._ref_slot.stage(ref_frame)
+        e.begin_frame()
+        _, seq = e.backbone(inp, tag="ref")
+        src, q = e.project_ref(seq["feat"])
+        self.ref_proj[0][i * n16:(i + 1) * n16].copy_(src)
+        self.ref_proj[1][i * n16:(i + 1) * n16].copy_(q)
+        lab = get_label_map(init_box_xyxy, H, W, e.dev)
+        self.lbs_pre[i].copy_(ops.bilinear(lab, H // 8, W // 8, 8.0, 8.0).reshape(1, -1))
+        self.ready[i] = True
+        torch.cuda.synchronize()
+
+    def track_tensor(self, frames):
+        """frames: [n_seq,H,W,3] uint8 or [n_seq,3,H,W] fp32 preprocessed (ideally pinned host memory).  Returns (dets
+        [n_seq, max_inst, 7], counts [n_seq]) on the host; rows past a sequence's count are stale."""
+        self.slot.stage(frames)
+        self._run()
+        return self.host_dets.clone(), self.host_count.clone()
+
+    # -------------------------------------------------------------------------------- reference protocol
+    def initialize(self, i, image, info: dict):
+        if self.device_preproc:
+            ref, r = self._device_letterbox(i, image, None)
+        else:
+            ref, r = preprocess(image, self.input_size)
+        self.initialize_tensor(i, ref, xyxy_resized(info["init_bbox"], r))
+        self.states[i] = info["init_bbox"]
+
+    def _device_letterbox(self, i, image, out):
+        src = torch.from_numpy(image) if not torch.is_tensor(image) else image
+        assert src.dtype == torch.uint8 and src.dim() == 3 and src.shape[2] == 3
+        if self._raw[i] is None or self._raw[i][0].shape != src.shape:
+            self._raw[i] = (torch.empty(src.shape, dtype=torch.uint8, device=self.eng.dev), torch.empty(src.shape, dtype=torch.uint8).pin_memory())
+        dev_raw, host_raw = self._raw[i]
+        host_raw.copy_(src)
+        dev_raw.copy_(host_raw, non_blocking=True)
+        return ops.letterbox_u8(dev_raw, self.input_size, swap_rb=True, out=out)
+
+    def track(self, images):
+        """images: n_seq RGB frames (HWC uint8), None for an idle slot.  Returns n_seq results {"target_bbox": [x, y, w, h]}, None for
+        idle or uninitialised slots."""
+        assert len(images) == self.n_seq
+        ratios = [None] * self.n_seq
+        if self.device_preproc:
+            buf = self.slot.use_u8(True)
+            for i, im in enumerate(images):
+                if im is not None:
+                    ratios[i] = self._device_letterbox(i, im, buf[i:i + 1])[1]
+            self._run()
+        else:
+            for i, im in enumerate(images):
+                if im is not None:
+                    ratios[i] = preprocess(im, self.input_size, out=self._host_in[i:i + 1])[1]
+            self.slot.stage(self._host_in)
+            self._run()
+        res = [None] * self.n_seq
+        for i, r in enumerate(ratios):
+            if r is None or not self.ready[i]:
+                continue
+            n = int(self.host_count[i])
+            if n > 0:
+                self.states[i] = state_xywh(self.host_dets[i, 0], r, self.input_size)
+            res[i] = {"target_bbox": self.states[i]}
+        return res
