@@ -265,6 +265,10 @@ UC_API int uc_box_iou(const float* a, int lda, int N, const float* b, int ldb, i
 
 /* dst += aligned_bilinear(src, factor) on NHWC bf16 maps (condinst/comm.py:5-27; mask_branch.py:81-96). */
 UC_API int uc_aligned_bilinear_add(const void* src, int lds, int hs, int ws, void* dst, int ldd, int C, int factor, void* stream);
+/* The same for B >= 1 images in one launch: image b reads src + b * bs_src and updates dst + b * bs_dst (element strides, even,
+ * bs_src >= hs*ws*lds, bs_dst >= hs*f*ws*f*ldd).  B < 1, null pointers or smaller strides: UC_EINVAL. */
+UC_API int uc_aligned_bilinear_add_batched(const void* src, int lds, long bs_src, int hs, int ws, void* dst, int ldd, long bs_dst, int C,
+                                           int factor, int B, void* stream);
 /* Per-instance CondInst masks (condinst/dynamic_mask_head.py:61-87,159-225,284; utils/boxes.py:138-145) for the first
  * min(*count_dev, n_max) rows of the NMS output: mask_feats f32 [h,w,8], up_masks f32 [h,w,9*up_rate^2],
  * dyn_levels = HOST array of 3 device pointers to the controller outputs [h_k*w_k, ld_dyn] (169 used), level_hw /
@@ -274,6 +278,18 @@ UC_API int uc_dynamic_masks(const float* mask_feats, const float* up_masks, int 
                             const float* const* dyn_levels, int ld_dyn, const int* level_hw, const int* level_strides,
                             const float* level_soi, const int* anchors_dev, const int* count_dev, int n_max, float* scratch,
                             float* out_masks, void* stream);
+/* The same for B >= 1 head images in one launch sequence (grid: pixels x instances x images).  Head image b has its controller
+ * outputs at dyn_levels[k] + b * bs_dyn[k] (HOST array of 3 element strides, each >= h_k*w_k*ld_dyn), its NMS result at
+ * anchors_dev + b * bs_anchors (bs_anchors >= the anchor count sum h_k*w_k) and count_dev[b] (the [B, A] / [B] layout of
+ * uc_postprocess_batched), and reads mask-branch image image_of[b] (device int32 [B]) of the S images mask_feats f32 [S,h,w,8] /
+ * up_masks f32 [S,h,w,9*up_rate^2]; an image_of entry outside [0, S) skips head image b (nothing is read or written for it).
+ * scratch >= B*n_max*h*w*(1+up^2) floats; out_masks f32 [B, n_max, h*up*d, w*up*d].  Each image's masks equal its own
+ * uc_dynamic_masks call.  B < 1, S < 1, null pointers (image_of and bs_dyn included) or smaller strides: UC_EINVAL. */
+UC_API int uc_dynamic_masks_batched(const float* mask_feats, const float* up_masks, int S, int h, int w, int up_rate, int d_rate,
+                                    const float* const* dyn_levels, int ld_dyn, const long* bs_dyn, const int* level_hw,
+                                    const int* level_strides, const float* level_soi, const int* anchors_dev, long bs_anchors,
+                                    const int* count_dev, const int* image_of, int B, int n_max, float* scratch, float* out_masks,
+                                    void* stream);
 
 /* VOS result assembly on the device (external/lib/test/tracker/unicorn_vos.py:129-155 mask resize to the original frame,
  * :105-121 soft aggregation + argmax): for every object either `mask` (f32 [Hin,Win] soft mask at network resolution, resized

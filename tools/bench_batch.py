@@ -3,6 +3,10 @@ sequence (UnicornSOTTrack, depth 1 and 3), on the 800x1280 SOT frame with CUDA g
 
     python tools/bench_batch.py [--steps 60] [--rounds 3] [--configs unicorn_track_large unicorn_track_r50] [--n-seq 1 2 4 8]
 
+--workload vos: the same for VOS with 1 and 3 objects per sequence (--objects): UnicornVOSBatch at n_seq 1 / 2 / 4 against
+UnicornVOSTrack at depth 1 and 3, unicorn_track_large_mask by default.  A VOS step is timed end to end (host clock around steps that
+end in a device synchronise): input copy, graph replay, the read-back of the detection rows and the per-sequence result assembly.
+
 Device-resident timing like bench.py's `value`: the frames are already in HBM, each step is an input copy and a graph replay, timed
 with CUDA events.  Every driver of a config is built first (plan-time autotuning of the batched layer shapes, graph capture); the
 timed rounds then alternate over the drivers so that clock and neighbour drift spread over all of them.  Printed per driver: aggregate
@@ -23,13 +27,21 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--configs", nargs="+", default=["unicorn_track_large", "unicorn_track_r50"])
+    ap.add_argument("--workload", choices=["sot", "vos"], default="sot")
+    ap.add_argument("--configs", nargs="+", default=None)
     ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
-    ap.add_argument("--n-seq", type=int, nargs="+", default=[1, 2, 4, 8])
+    ap.add_argument("--n-seq", type=int, nargs="+", default=None)
+    ap.add_argument("--objects", type=int, nargs="+", default=[1, 3])
     ap.add_argument("--depths", type=int, nargs="+", default=[1, 3])
     ap.add_argument("--steps", type=int, default=60)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
+    if args.workload == "vos":
+        args.configs = args.configs or ["unicorn_track_large_mask"]
+        args.n_seq = args.n_seq or [1, 2, 4]
+        return main_vos(args)
+    args.configs = args.configs or ["unicorn_track_large", "unicorn_track_r50"]
+    args.n_seq = args.n_seq or [1, 2, 4, 8]
     from unicorn_b200.engine import UnicornEngine
     from unicorn_b200.sot import UnicornSOTBatch, UnicornSOTTrack
     from unicorn_b200.synthetic import make_video
@@ -99,6 +111,74 @@ def main():
                               "added_peak_alloc_gib": round(mem / 2 ** 30, 2), "steps": args.steps, "rounds": args.rounds}), flush=True)
         del drivers, eng, sb, trk, batch_step, pipe_step
         torch.cuda.empty_cache()
+
+
+def main_vos(args):
+    import time
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.vos import UnicornVOSBatch, UnicornVOSTrack
+    from unicorn_b200.weights import make_state_dict
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
+    H, W = args.size
+    N = max(args.n_seq)
+    to_u8 = lambda f: f.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()  # noqa: E731
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        for k in args.objects:
+            videos = [make_video(5, H, W, seed=s, n_obj=k) for s in range(N)]
+            refs = [(to_u8(fr[0:1]).cuda(), {o + 1: bx[0, o] for o in range(k)}) for fr, bx in videos]
+            steps_u8 = [torch.stack([to_u8(fr[1 + t:2 + t])[0] for fr, _ in videos]).cuda() for t in range(4)]  # [N,H,W,3] per step
+            drivers = {}
+            for n in args.n_seq:
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                vb = UnicornVOSBatch(eng, (H, W), n, max_objects=n * k, max_groups=n * -(-k // 8))
+                for i in range(n):
+                    vb.initialize_tensor(i, *refs[i])
+                for t in range(3):
+                    vb.track_tensor(steps_u8[t][:n])
+
+                def batch_round(steps, vb=vb, n=n):
+                    for t in range(steps):
+                        vb.track_tensor(steps_u8[t % 4][:n])
+                drivers[f"batch{n}"] = ("UnicornVOSBatch", batch_round, n, 1, torch.cuda.max_memory_allocated() - m0, vb)
+            for d in args.depths:
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                trk = UnicornVOSTrack(eng, (H, W), use_graph=True, depth=d)
+                trk.initialize_tensor(*refs[0])
+                for t in range(2 * d + 1):
+                    trk.track_tensor(steps_u8[t % 4][0:1])
+
+                def pipe_round(steps, trk=trk, d=d):
+                    sub = 0
+                    for c in range(steps):
+                        while sub < steps and sub - c < d:
+                            trk.submit(steps_u8[sub % 4][0:1])
+                            sub += 1
+                        trk.collect()
+                drivers[f"depth{d}"] = ("UnicornVOSTrack", pipe_round, 1, d, torch.cuda.max_memory_allocated() - m0, trk)
+            times = {key: [] for key in drivers}
+            for _ in range(args.rounds):
+                for key, (_, run, _, _, _, _) in drivers.items():
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    run(args.steps)
+                    torch.cuda.synchronize()
+                    times[key].append(time.perf_counter() - t0)
+            for key, (name, _, n, d, mem, drv) in drivers.items():
+                ts = times[key]
+                fps = [n * args.steps / t for t in ts]
+                print(json.dumps({"workload": "vos", "config": cfg, "size": [H, W], "objects_per_seq": k, "driver": name, "n_seq": n, "depth": d,
+                                  "frames_per_s": round(statistics.median(fps), 1), "frames_per_s_min_max": [round(min(fps), 1), round(max(fps), 1)],
+                                  "ms_per_step": round(1e3 * statistics.median(ts) / args.steps, 2),
+                                  "launches_per_step": drv.launches_per_frame,
+                                  "added_peak_alloc_gib": round(mem / 2 ** 30, 2), "steps": args.steps, "rounds": args.rounds}), flush=True)
+            del drivers, vb, trk, drv, batch_round, pipe_round
+            torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":

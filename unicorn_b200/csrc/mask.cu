@@ -21,10 +21,13 @@ __device__ __forceinline__ void ab_coord(int i, int f, int n, int& i0, int& i1, 
   i0 = min(i0, n - 1);
 }
 
-__global__ void __launch_bounds__(256) aligned_bilinear_add_kernel(const uint16_t* __restrict__ src, int lds, int hs, int ws,
-                                                                    uint16_t* __restrict__ dst, int ldd, int C, int f) {
+// blockIdx.y = image: image b reads src + b * bs_src and updates dst + b * bs_dst
+__global__ void __launch_bounds__(256) aligned_bilinear_add_kernel(const uint16_t* __restrict__ src, int lds, long bs_src, int hs, int ws,
+                                                                    uint16_t* __restrict__ dst, int ldd, long bs_dst, int C, int f) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
+  src += blockIdx.y * bs_src;
+  dst += blockIdx.y * bs_dst;
   const int C2 = C >> 1, hd = hs * f, wd = ws * f;
   const long total = static_cast<long>(hd) * wd * C2;
   for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
@@ -49,20 +52,33 @@ __global__ void __launch_bounds__(256) aligned_bilinear_add_kernel(const uint16_
 }
 
 struct MaskLevels {
-  const float* dyn[3];  // per level [h*w, ld_dyn] controller outputs
+  const float* dyn[3];  // per level [h*w, ld_dyn] controller outputs of image 0
+  long bs[3];           // per level: elements from one image's controller outputs to the next
   int h[3], w[3], stride[3], start[3];
   float soi[3];
 };
 
+// Head image b (blockIdx.z) of a batch: its NMS slice is count[b] / anchors + b * bs_anchors, and it reads the mask-branch image
+// image_of[b] (image 0 when image_of is null).  Returns -1 when that index is outside [0, S): the image is skipped.
+__device__ __forceinline__ int mask_image(const int* __restrict__ image_of, int S) {
+  const int img = image_of ? image_of[blockIdx.z] : 0;
+  return img >= 0 && img < S ? img : -1;
+}
+
 // logits[n, y, x] for instance n (anchor index from the NMS output) — one thread per (instance, pixel)
 __global__ void __launch_bounds__(256) mask_logits_kernel(const float* __restrict__ mask_feats, int h, int w, MaskLevels lv, int ld_dyn,
-                                                           const int* __restrict__ anchors, const int* __restrict__ count, int n_max,
-                                                           float* __restrict__ logits) {
+                                                           const int* __restrict__ anchors, long bs_anchors, const int* __restrict__ count,
+                                                           const int* __restrict__ image_of, int S, int n_max, float* __restrict__ logits) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
   __shared__ float prm[169];
   __shared__ float inst[3];
-  const int n = min(*count, n_max);
+  const int b = blockIdx.z, img = mask_image(image_of, S);
+  if (img < 0) return;
+  mask_feats += static_cast<long>(img) * h * w * 8;
+  anchors += b * bs_anchors;
+  logits += static_cast<long>(b) * n_max * h * w;
+  const int n = min(count[b], n_max);
   const int ins = blockIdx.y;
   if (ins >= n) return;
   if (threadIdx.x < 169 || threadIdx.x == 255) {
@@ -71,7 +87,7 @@ __global__ void __launch_bounds__(256) mask_logits_kernel(const float* __restric
     if (a >= lv.start[1]) k = 1;
     if (a >= lv.start[2]) k = 2;
     const int ai = a - lv.start[k];
-    if (threadIdx.x < 169) prm[threadIdx.x] = lv.dyn[k][static_cast<long>(ai) * ld_dyn + threadIdx.x];
+    if (threadIdx.x < 169) prm[threadIdx.x] = lv.dyn[k][b * lv.bs[k] + static_cast<long>(ai) * ld_dyn + threadIdx.x];
     else {
       inst[0] = ((ai % lv.w[k]) + 0.5f) * lv.stride[k];  // locations = (grid + 0.5) * stride (unicorn_head_mask.py:518)
       inst[1] = ((ai / lv.w[k]) + 0.5f) * lv.stride[k];
@@ -110,14 +126,19 @@ __global__ void __launch_bounds__(256) mask_logits_kernel(const float* __restric
 
 // convex upsampling x up (softmax over the 9 neighbours, weights from up_masks [h,w,9*up*up]) + sigmoid
 __global__ void __launch_bounds__(256) mask_convex_up_kernel(const float* __restrict__ logits, const float* __restrict__ up_masks, int h,
-                                                              int w, int up, const int* __restrict__ count, int n_max,
-                                                              float* __restrict__ out) {
+                                                              int w, int up, const int* __restrict__ count, const int* __restrict__ image_of,
+                                                              int S, int n_max, float* __restrict__ out) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
-  const int n = min(*count, n_max);
+  const int b = blockIdx.z, img = mask_image(image_of, S);
+  if (img < 0) return;
+  const int n = min(count[b], n_max);
   const int ins = blockIdx.y;
   if (ins >= n) return;
   const int H = h * up, W = w * up;
+  up_masks += static_cast<long>(img) * h * w * (9 * up * up);
+  logits += static_cast<long>(b) * n_max * h * w;
+  out += static_cast<long>(b) * n_max * H * W;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= H * W) return;
   const int X = t % W, Y = t / W;
@@ -141,13 +162,18 @@ __global__ void __launch_bounds__(256) mask_convex_up_kernel(const float* __rest
 }
 
 __global__ void __launch_bounds__(256) mask_final_up_kernel(const float* __restrict__ src, int hs, int ws, int f,
-                                                             const int* __restrict__ count, int n_max, float* __restrict__ out) {
+                                                             const int* __restrict__ count, const int* __restrict__ image_of, int S,
+                                                             int n_max, float* __restrict__ out) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
-  const int n = min(*count, n_max);
+  const int b = blockIdx.z;
+  if (mask_image(image_of, S) < 0) return;
+  const int n = min(count[b], n_max);
   const int ins = blockIdx.y;
   if (ins >= n) return;
   const int hd = hs * f, wd = ws * f;
+  src += static_cast<long>(b) * n_max * hs * ws;
+  out += static_cast<long>(b) * n_max * hd * wd;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= hd * wd) return;
   int y0, y1, x0, x1;
@@ -435,46 +461,95 @@ __global__ void __launch_bounds__(kMotsThreads) mots_chars_kernel(const uint8_t*
   if (t == kMotsThreads - 1) rle_chars(run_delta(end, hm * wm), chars, off, capacity);
 }
 
+// B images; the batched entry points validate every argument before any CUDA call, with errors prefixed by `what`.
+static int aligned_bilinear_add(const char* what, const void* src, int lds, long bs_src, int hs, int ws, void* dst, int ldd, long bs_dst, int C,
+                                int factor, int B, cudaStream_t stream) {
+  if (!src || !dst) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (C % 2 || lds % 2 || ldd % 2 || factor < 1 || hs < 1 || ws < 1 || lds < C || ldd < C) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  const long src_img = static_cast<long>(hs) * ws * lds, dst_img = static_cast<long>(hs) * factor * ws * factor * ldd;
+  if (bs_src % 2 || bs_dst % 2 || bs_src < src_img || bs_dst < dst_img)
+    return set_error(UC_EINVAL, "%s: bad per-image strides (even, src >= hs*ws*lds = %ld, dst >= (hs*f)*(ws*f)*ldd = %ld)", what, src_img, dst_img);
+  const long total = static_cast<long>(hs) * factor * ws * factor * (C / 2);
+  const long cap = std::max<long>(1, static_cast<long>(num_sms()) * 16 / B);  // the whole batch keeps the B = 1 launch's CTA budget
+  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, cap)));
+  launch_pdl(aligned_bilinear_add_kernel, dim3(grid, B), 256, 0, stream, static_cast<const uint16_t*>(src), lds, bs_src, hs, ws,
+             static_cast<uint16_t*>(dst), ldd, bs_dst, C, factor);
+  return check_launch(what);
+}
+
+static int dynamic_masks(const char* what, const float* mask_feats, const float* up_masks, int S, int h, int w, int up_rate, int d_rate,
+                         const float* const* dyn_levels, int ld_dyn, const long* bs_dyn, const int* level_hw, const int* level_strides,
+                         const float* level_soi, const int* anchors_dev, long bs_anchors, const int* count_dev, const int* image_of, int B,
+                         int n_max, float* scratch, float* out_masks, cudaStream_t stream) {
+  if (!mask_feats || !up_masks || !dyn_levels || !level_hw || !level_strides || !level_soi || !anchors_dev || !count_dev || !scratch || !out_masks)
+    return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (S < 1) return set_error(UC_EINVAL, "%s: S (mask-branch images) must be >= 1 (got %d)", what, S);
+  if (n_max < 1 || ld_dyn < 169 || up_rate < 1 || d_rate < 1 || h < 1 || w < 1) return set_error(UC_EINVAL, "%s: bad sizes", what);
+  if (B > 65535 || n_max > 65535) return set_error(UC_EINVAL, "%s: B and n_max must be <= 65535", what);
+  MaskLevels lv;
+  int start = 0;
+  for (int k = 0; k < 3; ++k) {
+    if (!dyn_levels[k]) return set_error(UC_EINVAL, "%s: null pointer", what);
+    lv.dyn[k] = dyn_levels[k];
+    lv.h[k] = level_hw[2 * k]; lv.w[k] = level_hw[2 * k + 1]; lv.stride[k] = level_strides[k]; lv.soi[k] = level_soi[k];
+    lv.bs[k] = bs_dyn ? bs_dyn[k] : 0;
+    lv.start[k] = start;
+    start += lv.h[k] * lv.w[k];
+    if (bs_dyn && lv.bs[k] < static_cast<long>(lv.h[k]) * lv.w[k] * ld_dyn)
+      return set_error(UC_EINVAL, "%s: bad per-image strides of level %d (controller outputs: >= h*w*ld_dyn = %ld)", what, k,
+                       static_cast<long>(lv.h[k]) * lv.w[k] * ld_dyn);
+  }
+  if (bs_dyn && bs_anchors < start) return set_error(UC_EINVAL, "%s: bad per-image anchor stride %ld (>= %d anchors)", what, bs_anchors, start);
+  float* logits = scratch;                                       // [B, n_max, h, w]
+  float* mid = scratch + static_cast<long>(B) * n_max * h * w;    // [B, n_max, h*up, w*up]
+  launch_pdl(mask_logits_kernel, dim3((h * w + 255) / 256, n_max, B), 256, 0, stream, mask_feats, h, w, lv, ld_dyn, anchors_dev, bs_anchors,
+             count_dev, image_of, S, n_max, logits);
+  const int H1 = h * up_rate, W1 = w * up_rate;
+  launch_pdl(mask_convex_up_kernel, dim3((H1 * W1 + 255) / 256, n_max, B), 256, 0, stream, logits, up_masks, h, w, up_rate, count_dev, image_of,
+             S, n_max, d_rate == 1 ? out_masks : mid);
+  if (d_rate != 1) {
+    const int H2 = H1 * d_rate, W2 = W1 * d_rate;
+    launch_pdl(mask_final_up_kernel, dim3((H2 * W2 + 255) / 256, n_max, B), 256, 0, stream, mid, H1, W1, d_rate, count_dev, image_of, S, n_max,
+               out_masks);
+  }
+  return check_launch(what);
+}
+
 }  // namespace uc
 
 using namespace uc;
 
 extern "C" int uc_aligned_bilinear_add(const void* src, int lds, int hs, int ws, void* dst, int ldd, int C, int factor, void* stream_v) {
   if (!src || !dst || C % 2 || lds % 2 || ldd % 2 || factor < 1) return set_error(UC_EINVAL, "uc_aligned_bilinear_add: bad arguments");
-  const long total = static_cast<long>(hs) * factor * ws * factor * (C / 2);
-  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, static_cast<long>(num_sms()) * 16)));
-  launch_pdl(aligned_bilinear_add_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream_v), static_cast<const uint16_t*>(src), lds, hs, ws,
-                                                                                     static_cast<uint16_t*>(dst), ldd, C, factor);
-  return check_launch("uc_aligned_bilinear_add");
+  return aligned_bilinear_add("uc_aligned_bilinear_add", src, lds, static_cast<long>(hs) * ws * lds, hs, ws, dst, ldd,
+                              static_cast<long>(hs) * factor * ws * factor * ldd, C, factor, 1, static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_aligned_bilinear_add_batched(const void* src, int lds, long bs_src, int hs, int ws, void* dst, int ldd, long bs_dst, int C,
+                                               int factor, int B, void* stream_v) {
+  return aligned_bilinear_add("uc_aligned_bilinear_add_batched", src, lds, bs_src, hs, ws, dst, ldd, bs_dst, C, factor, B,
+                              static_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int uc_dynamic_masks(const float* mask_feats, const float* up_masks, int h, int w, int up_rate, int d_rate,
                                 const float* const* dyn_levels, int ld_dyn, const int* level_hw, const int* level_strides,
                                 const float* level_soi, const int* anchors_dev, const int* count_dev, int n_max, float* scratch,
                                 float* out_masks, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!mask_feats || !up_masks || !dyn_levels || !level_hw || !level_strides || !level_soi || !anchors_dev || !count_dev || !scratch || !out_masks)
-    return set_error(UC_EINVAL, "uc_dynamic_masks: null pointer");
-  if (n_max < 1 || ld_dyn < 169 || up_rate < 1 || d_rate < 1) return set_error(UC_EINVAL, "uc_dynamic_masks: bad sizes");
-  MaskLevels lv;
-  int start = 0;
-  for (int k = 0; k < 3; ++k) {
-    lv.dyn[k] = dyn_levels[k];
-    lv.h[k] = level_hw[2 * k]; lv.w[k] = level_hw[2 * k + 1]; lv.stride[k] = level_strides[k]; lv.soi[k] = level_soi[k];
-    lv.start[k] = start;
-    start += lv.h[k] * lv.w[k];
-  }
-  float* logits = scratch;                                   // [n_max, h, w]
-  float* mid = scratch + static_cast<long>(n_max) * h * w;    // [n_max, h*up, w*up]
-  launch_pdl(mask_logits_kernel, dim3((h * w + 255) / 256, n_max), 256, 0, stream, mask_feats, h, w, lv, ld_dyn, anchors_dev, count_dev, n_max, logits);
-  const int H1 = h * up_rate, W1 = w * up_rate;
-  launch_pdl(mask_convex_up_kernel, dim3((H1 * W1 + 255) / 256, n_max), 256, 0, stream, logits, up_masks, h, w, up_rate, count_dev, n_max,
-                                                                                d_rate == 1 ? out_masks : mid);
-  if (d_rate != 1) {
-    const int H2 = H1 * d_rate, W2 = W1 * d_rate;
-    launch_pdl(mask_final_up_kernel, dim3((H2 * W2 + 255) / 256, n_max), 256, 0, stream, mid, H1, W1, d_rate, count_dev, n_max, out_masks);
-  }
-  return check_launch("uc_dynamic_masks");
+  return dynamic_masks("uc_dynamic_masks", mask_feats, up_masks, 1, h, w, up_rate, d_rate, dyn_levels, ld_dyn, nullptr, level_hw, level_strides,
+                       level_soi, anchors_dev, 0, count_dev, nullptr, 1, n_max, scratch, out_masks, static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_dynamic_masks_batched(const float* mask_feats, const float* up_masks, int S, int h, int w, int up_rate, int d_rate,
+                                        const float* const* dyn_levels, int ld_dyn, const long* bs_dyn, const int* level_hw,
+                                        const int* level_strides, const float* level_soi, const int* anchors_dev, long bs_anchors,
+                                        const int* count_dev, const int* image_of, int B, int n_max, float* scratch, float* out_masks,
+                                        void* stream_v) {
+  if (!bs_dyn || !image_of) return set_error(UC_EINVAL, "uc_dynamic_masks_batched: null pointer (bs_dyn and image_of are required)");
+  return dynamic_masks("uc_dynamic_masks_batched", mask_feats, up_masks, S, h, w, up_rate, d_rate, dyn_levels, ld_dyn, bs_dyn, level_hw,
+                       level_strides, level_soi, anchors_dev, bs_anchors, count_dev, image_of, B, n_max, scratch, out_masks,
+                       static_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win, int H, int W, float r, float* soft_out, uint8_t* seg_out,

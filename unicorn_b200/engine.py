@@ -614,33 +614,29 @@ class UnicornEngine:
 
     # ------------------------------------------------------------------------------------------ head
     def mask_branch(self, fpn):
-        """MaskBranch.forward with use_raft (condinst/mask_branch.py:77-96,158-162): -> (mask_feats fp32 [1,h8,w8,8],
-        up_masks fp32 [1,h8,w8,144])."""
+        """MaskBranch.forward with use_raft (condinst/mask_branch.py:77-96,158-162) of B images: -> (mask_feats fp32 [B,h8,w8,8],
+        up_masks fp32 [B,h8,w8,144])."""
         M = self.P["mask"]
         B, h, w, _ = fpn[0].shape
-        if B != 1:
-            raise ValueError(f"UnicornEngine.mask_branch runs one image (got a batch of {B}); the mask path is not batched")
-        x = self.conv_gn(fpn[0], M["refine"][0], self.buf("mask.x", (1, h, w, 128)), act=ACT_RELU)
+        x = self.conv_gn(fpn[0], M["refine"][0], self.buf("mask.x", (B, h, w, 128)), act=ACT_RELU)
         for i in (1, 2):
             _, hi, wi, _ = fpn[i].shape
-            xp = self.conv_gn(fpn[i], M["refine"][i], self.buf(f"mask.r{i}", (1, hi, wi, 128)), act=ACT_RELU)
+            xp = self.conv_gn(fpn[i], M["refine"][i], self.buf(f"mask.r{i}", (B, hi, wi, 128)), act=ACT_RELU)
             ops.aligned_bilinear_add(xp, x, h // hi)
         t = x
         for i in range(4):
-            t = self.conv_gn(t, M["tower"][i], self.buf(f"mask.t{i % 2}", (1, h, w, 128)), act=ACT_RELU)
-        mf = self.conv(t, M["out"][0], 1, bias=M["out"][1], out=self.buf("mask.feats", (1, h, w, 8), F32))
-        u = self.conv(x, M["up0"][0], 3, 1, 1, bias=M["up0"][1], act=ACT_RELU, out=self.buf("mask.u0", (1, h, w, 128)))
-        um = self.conv(u, M["up2"][0], 1, bias=M["up2"][1], out=self.buf("mask.up", (1, h, w, 144), F32))
+            t = self.conv_gn(t, M["tower"][i], self.buf(f"mask.t{i % 2}", (B, h, w, 128)), act=ACT_RELU)
+        mf = self.conv(t, M["out"][0], 1, bias=M["out"][1], out=self.buf("mask.feats", (B, h, w, 8), F32))
+        u = self.conv(x, M["up0"][0], 3, 1, 1, bias=M["up0"][1], act=ACT_RELU, out=self.buf("mask.u0", (B, h, w, 128)))
+        um = self.conv(u, M["up2"][0], 1, bias=M["up2"][1], out=self.buf("mask.up", (B, h, w, 144), F32))
         return mf, um
 
     def head(self, fpn, priors, mode, with_masks=False):
         """UnicornHead.forward eval branch (unicorn_head.py:267-336) + decode_outputs (:467-482) of B images.
         fpn: 3 NHWC bf16 maps [B,h,w,C]; priors: 3 fp32 maps with B*h*w elements each ([B,h,w], or [B,1,h,w] from propagate) or None
         (MOT: zero prior == no fusion term).  Returns fp32 [B, A, 5+ncls_mode].  with_masks=True (UnicornHeadMask, unicorn_head_mask.py:333-343) also runs the
-        controller convs; their outputs are left in self.dyn_levels (3 x fp32 [1,h,w,176]) for ops.dynamic_masks."""
+        controller convs; their outputs are left in self.dyn_levels (3 x fp32 [B,h,w,176]) for ops.dynamic_masks."""
         B = fpn[0].shape[0]
-        if with_masks and B != 1:
-            raise ValueError(f"UnicornEngine.head(with_masks=True) runs one image (got a batch of {B}); the mask path is not batched")
         self._with_masks = with_masks
         self.dyn_levels = [None] * 3
         sfx = "_sot" if mode == "sot" else ""
@@ -683,7 +679,7 @@ class UnicornEngine:
             hw[k] = (h, w)
             if self._with_masks:
                 cw_, cb_ = L["ctrl"]
-                self.dyn_levels[k] = self.conv(feats[1], cw_, 3, 1, 1, bias=cb_, out=self.buf(f"head{k}.dyn", (1, h, w, 176), F32))
+                self.dyn_levels[k] = self.conv(feats[1], cw_, 3, 1, 1, bias=cb_, out=self.buf(f"head{k}.dyn", (B, h, w, 176), F32))
 
 
 def _rows(t):

@@ -475,28 +475,53 @@ def box_iou(a, b, plus_one=False):
 
 
 def aligned_bilinear_add(src, dst, factor):
-    _, hs, ws, C = src.shape
-    assert dst.shape == (1, hs * factor, ws * factor, C)
-    _lib.check(_L().uc_aligned_bilinear_add(_p(src), _nhwc_ld(src), hs, ws, _p(dst), _nhwc_ld(dst), C, factor, _S()), "uc_aligned_bilinear_add")
+    """dst += aligned_bilinear(src, factor) on NHWC bf16 maps [B,hs,ws,C] -> [B,hs*f,ws*f,C]; B > 1 images run in one launch."""
+    B, hs, ws, C = src.shape
+    assert dst.shape == (B, hs * factor, ws * factor, C)
+    if B == 1:
+        _lib.check(_L().uc_aligned_bilinear_add(_p(src), _nhwc_ld(src), hs, ws, _p(dst), _nhwc_ld(dst), C, factor, _S()), "uc_aligned_bilinear_add")
+        return dst
+    _lib.check(_L().uc_aligned_bilinear_add_batched(_p(src), _nhwc_ld(src), _l(src.stride(0)), hs, ws, _p(dst), _nhwc_ld(dst), _l(dst.stride(0)), C,
+                                                    factor, B, _S()), "uc_aligned_bilinear_add_batched")
     return dst
 
 
 def dynamic_masks(mask_feats, up_masks, dyn_levels, level_hw, ws, n_max, up_rate=4, d_rate=2, strides=(8, 16, 32), soi=(64.0, 128.0, 256.0),
-                  out=None, scratch=None):
+                  out=None, scratch=None, image_of=None):
     """mask_feats fp32 [1,h,w,8]; up_masks fp32 [1,h,w,9*up^2]; dyn_levels: 3 fp32 [1,hk,wk,ld] controller outputs;
-    ws: PostWorkspace after postprocess_device.  Returns fp32 [n_max, h*up*d, w*up*d]."""
-    _, h, w, _ = mask_feats.shape
+    ws: PostWorkspace after postprocess_device.  Returns fp32 [n_max, h*up*d, w*up*d].
+    Batched: dyn_levels of B head images [B,hk,wk,ld], ws a PostWorkspace of batch B, and S mask-branch images (mask_feats
+    [S,h,w,8], up_masks [S,h,w,9*up^2]); head image b reads mask-branch image image_of[b] (device int32 [B]; default b, with S = B)
+    and an entry outside [0, S) skips it.  Returns fp32 [B, n_max, h*up*d, w*up*d]."""
+    S, h, w, _ = mask_feats.shape
+    B = dyn_levels[0].shape[0]
     H, W = h * up_rate * d_rate, w * up_rate * d_rate
-    if out is None:
-        out = torch.zeros(n_max, H, W, dtype=torch.float32, device=mask_feats.device)
-    if scratch is None:
-        scratch = torch.empty(n_max * h * w * (1 + up_rate * up_rate), dtype=torch.float32, device=mask_feats.device)
     dl = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in dyn_levels])
     hw = (ctypes.c_int * 6)(*[v for pair in level_hw for v in pair])
     st = (ctypes.c_int * 3)(*strides)
     so = (ctypes.c_float * 3)(*soi)
-    _lib.check(_L().uc_dynamic_masks(_p(mask_feats), _p(up_masks), h, w, up_rate, d_rate, dl, dyn_levels[0].shape[-1], hw, st, so,
-                                     _p(ws.anchors), _p(ws.count), n_max, _p(scratch), _p(out), _S()), "uc_dynamic_masks", 3)
+    if scratch is None:
+        scratch = torch.empty(B * n_max * h * w * (1 + up_rate * up_rate), dtype=torch.float32, device=mask_feats.device)
+    if B == 1 and image_of is None:
+        if out is None:
+            out = torch.zeros(n_max, H, W, dtype=torch.float32, device=mask_feats.device)
+        _lib.check(_L().uc_dynamic_masks(_p(mask_feats), _p(up_masks), h, w, up_rate, d_rate, dl, dyn_levels[0].shape[-1], hw, st, so,
+                                         _p(ws.anchors), _p(ws.count), n_max, _p(scratch), _p(out), _S()), "uc_dynamic_masks", 3)
+        return out
+    assert ws.batch == B and all(t.shape[0] == B and t.stride(-1) == 1 for t in dyn_levels), "dynamic_masks: B head images need a PostWorkspace of batch B"
+    assert mask_feats.is_contiguous() and up_masks.is_contiguous() and up_masks.shape[0] == S
+    assert scratch.numel() >= B * n_max * h * w * (1 + up_rate * up_rate)
+    if image_of is None:
+        assert S == B, "dynamic_masks: image_of is needed when the mask-branch images are not the head images"
+        image_of = torch.arange(B, dtype=torch.int32, device=mask_feats.device)
+    assert image_of.dtype == torch.int32 and image_of.numel() == B and image_of.is_contiguous()
+    if out is None:
+        out = torch.zeros(B, n_max, H, W, dtype=torch.float32, device=mask_feats.device)
+    assert out.shape == (B, n_max, H, W) and out.is_contiguous()
+    bs = (ctypes.c_long * 3)(*[t.stride(0) for t in dyn_levels])
+    _lib.check(_L().uc_dynamic_masks_batched(_p(mask_feats), _p(up_masks), S, h, w, up_rate, d_rate, dl, dyn_levels[0].shape[-1], bs, hw, st, so,
+                                             _p(ws.anchors), _l(ws.max_anchors), _p(ws.count), _p(image_of), B, n_max, _p(scratch), _p(out),
+                                             _S()), "uc_dynamic_masks_batched", 3)
     return out
 
 
