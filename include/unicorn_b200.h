@@ -182,6 +182,12 @@ UC_API int uc_add(const void* a, int lda, const void* b, int ldb, void* y, int l
  * frame needs no host decision (CUDA-graph replay).  16-byte aligned rows / strides. */
 UC_API int uc_copy_rows_if(const int* flag_dev, int invert, const void* src, long src_ld_bytes, void* dst, long dst_ld_bytes, long rows,
                            int row_bytes, void* stream);
+/* The same for B >= 1 images in one launch: image b copies its rows (src + b * src_bs_bytes -> dst + b * dst_bs_bytes) when
+ * (gate_dev == NULL || gate_dev[b] != 0) && ((flag_dev[b] != 0) != invert); flag_dev / gate_dev device int32 [B].  The multi-sequence
+ * MOT driver gates with the step's active-slot table so that an idle slot keeps its pre_dict.  Rows and strides as uc_copy_rows_if
+ * (16-byte aligned), per-image strides multiples of 16 and >= rows * ld.  B < 1, null pointers or smaller strides: UC_EINVAL. */
+UC_API int uc_copy_rows_if_batched(const int* flag_dev, const int* gate_dev, int invert, const void* src, long src_ld_bytes, long src_bs_bytes,
+                                   void* dst, long dst_ld_bytes, long dst_bs_bytes, long rows, int row_bytes, int B, void* stream);
 UC_API int uc_nchw_f32_to_nhwc(const float* src, void* dst, int ldd, int B, int C, long HW, int dtype, void* stream);
 UC_API int uc_nhwc_to_nchw_f32(const void* src, int lds, float* dst, int B, int C, long HW, int dtype, void* stream);
 
@@ -248,6 +254,13 @@ UC_API int uc_postprocess_batched(const float* pred, int A, int ncls, float conf
  * (count_dev may be NULL).  out f32 [n_max, C]. */
 UC_API int uc_sample_embed(const void* embed, int ld, int h, int w, int C, int dtype, const float* boxes, int ldb,
                            const int* count_dev, int n_max, float stride, float* out, void* stream);
+/* The same for B >= 1 images in one launch (grid: boxes x images): image b samples embed + b * bs_embed at the boxes
+ * boxes + b * bs_boxes (the [B, A, 7] NMS output of uc_postprocess_batched) for its first min(count_dev[b], n_max) rows and writes
+ * out + b * bs_out; rows at or past that count are not written.  Element strides bs_embed >= h*w*ld, bs_boxes >= n_max*ldb,
+ * bs_out >= n_max*C.  B < 1, null pointers (count_dev included) or smaller strides: UC_EINVAL.  Each image's rows equal its own
+ * uc_sample_embed call. */
+UC_API int uc_sample_embed_batched(const void* embed, int ld, long bs_embed, int h, int w, int C, int dtype, const float* boxes, int ldb,
+                                   long bs_boxes, const int* count_dev, int n_max, float stride, float* out, long bs_out, int B, void* stream);
 /* Quasi-dense association score (unicorn/tracker/quasi_dense_embed_tracker.py:166-175): scores = (softmax_rows(F) +
  * softmax_cols(F)) / 2 with F = E M^T, zeroed where labels differ (labels may be NULL).  workspace >= N*M+2N+2M floats. */
 UC_API int uc_bisoftmax(const float* det_embeds, const float* memo_embeds, int N, int M, int C, const float* det_labels,

@@ -1,0 +1,300 @@
+"""Several MOT sequences in one batched frame: the batched kernels against their per-image launches, and UnicornMOTBatch against one
+UnicornMOTTracker per sequence, bit for bit (torch.equal) in every case: boxes, ids, NMS rows and sampled embeddings (QD arm), the
+rows handed to each BYTETracker (ByteTrack arm)."""
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+SIZE = (320, 320)
+STEPS = 8
+
+
+# ------------------------------------------------------------------------------------------------ kernels
+def test_sample_embed_batched_matches_per_image():
+    from unicorn_b200 import ops
+    g = torch.Generator().manual_seed(3)
+    B, h, w, C, n_max = 4, 20, 36, 128, 50
+    wide = torch.randn(B, h, w, C + 32, generator=g).half().cuda()
+    emb = wide[..., :C]  # pixel stride 160: a channel slice of a wider buffer
+    boxes = torch.rand(B, 64, 7, generator=g) * torch.tensor([288.0, 160.0, 288.0, 160.0, 1, 1, 1])
+    boxes[..., 2:4] += boxes[..., :2]
+    boxes[1, 0, :4] = torch.tensor([-50.0, -20.0, 4.0, 6.0])  # centre clamps to the border
+    boxes = boxes.cuda()
+    count = torch.tensor([0, 17, n_max, 80], dtype=torch.int32, device="cuda")  # empty, in range, at and above n_max
+    got = torch.full((B, n_max, C), -7.0, device="cuda")
+    ref = got.clone()
+    ops.sample_embed(emb, boxes, n_max, 8.0, count=count, out=got)
+    for b in range(B):
+        ops.sample_embed(emb[b:b + 1], boxes[b], n_max, 8.0, count=count[b:b + 1], out=ref[b])
+    torch.cuda.synchronize()
+    assert torch.equal(got, ref)
+    assert (got[0] == -7.0).all() and (got[1, 17:] == -7.0).all() and not (got[1, :17] == -7.0).any()
+
+
+@pytest.mark.parametrize("with_gate", [False, True])
+@pytest.mark.parametrize("invert", [False, True])
+def test_copy_rows_if_batched_matches_per_image(invert, with_gate):
+    from unicorn_b200 import ops
+    g = torch.Generator().manual_seed(5)
+    B, h, w, C = 4, 10, 12, 256
+    src = torch.randn(B, h, w, C, generator=g).bfloat16().cuda()
+    dst_wide = torch.randn(B, h, w, C + 64, generator=g).bfloat16().cuda()  # the channels past C must not change
+    ref_wide = dst_wide.clone()
+    flag = torch.tensor([0, 1, 0, 1], dtype=torch.int32, device="cuda")
+    gate = torch.tensor([0, 0, 1, 1], dtype=torch.int32, device="cuda") if with_gate else None
+    ops.copy_rows_if(flag, src, dst_wide[..., :C], invert=invert, gate=gate)
+    for b in range(B):
+        if gate is None or int(gate[b]):
+            ops.copy_rows_if(flag[b:b + 1], src[b:b + 1], ref_wide[b:b + 1, ..., :C], invert=invert)
+    torch.cuda.synchronize()
+    assert torch.equal(dst_wide, ref_wide)
+    copied = [(gate is None or int(gate[b])) and (int(flag[b]) != 0) != invert for b in range(B)]
+    assert any(copied) and not all(copied)
+
+
+# ------------------------------------------------------------------------------------------------ QD driver
+@pytest.fixture(scope="module")
+def tiny():
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.weights import make_state_dict
+    name = "unicorn_track_tiny"
+    eng = UnicornEngine(make_state_dict(name, 0), name)
+    videos = [make_video(STEPS, *SIZE, seed=20 + s, n_obj=3)[0] for s in range(4)]
+    return eng, videos
+
+
+def qd_tracker():
+    from unicorn_b200.tracker import QuasiDenseEmbedTracker
+    # seeded random weights give low scores: lower the tracker's score gates so that tracklets are created (as test_tracker_gpu.py)
+    return QuasiDenseEmbedTracker(init_score_thr=0.05, obj_score_thr=0.03)
+
+
+KW = dict(conf=0.01, nms=0.7, score_thr=0.02)
+
+
+def reference(eng, frames, kw=KW):
+    """One UnicornMOTTracker fed `frames` in order: per frame (boxes, ids, NMS rows, sampled embeddings)."""
+    from unicorn_b200.mot import UnicornMOTTracker
+    trk = UnicornMOTTracker(eng, SIZE, tracker=qd_tracker(), **kw)
+    out = []
+    for f in frames:
+        b, i = trk.step_tensor(f[None])
+        out.append((b.clone(), i.clone(), trk.last["dets"].clone(), trk.last["feats"].clone()))
+    return out
+
+
+def run_batch(eng, n_seq, steps, use_graph, pipelined, kw=KW):
+    """steps: per step a dict {"start": [slots started before the step], "frames": n_seq frames [3,H,W] or None (idle)}.  Returns per
+    step the n_seq results as (boxes, ids, NMS rows, embeddings) or None."""
+    from unicorn_b200.mot import UnicornMOTBatch
+    mb = UnicornMOTBatch(eng, SIZE, n_seq, use_graph=use_graph, **kw)
+    filler = torch.zeros(3, *SIZE)
+    results, graphs = [], []
+
+    def submit(t):
+        for i in steps[t].get("start", []):
+            if use_graph and t >= 4:
+                graphs.append([c.graph for c in mb._ctxs])
+            mb.start(i, qd_tracker())
+        fr = steps[t]["frames"]
+        mb.submit(torch.stack([f if f is not None else filler for f in fr]), active=[f is not None for f in fr])
+
+    def collect():
+        res = mb.collect()
+        assert all((r is None) == (mb.last_dets[i] is None) == (mb.last_feats[i] is None) for i, r in enumerate(res))
+        results.append([None if r is None else (r[0].clone(), r[1].clone(), mb.last_dets[i].clone(), mb.last_feats[i].clone())
+                        for i, r in enumerate(res)])
+
+    if pipelined:
+        submit(0)
+        for t in range(len(steps)):
+            if t + 1 < len(steps):
+                submit(t + 1)
+            collect()
+    else:
+        for t in range(len(steps)):
+            submit(t)
+            collect()
+    if use_graph:
+        assert len(mb._graphs) == 2
+        for gs in graphs:  # start() after the captures: the graphs were not re-captured
+            assert all(a is b for a, b in zip(gs, [c.graph for c in mb._ctxs]))
+    return mb, results
+
+
+def assert_same(got, ref, what):
+    assert got is not None, what
+    for k, name in enumerate(("boxes", "ids", "NMS rows", "embeddings")):
+        assert torch.equal(got[k], ref[k]), f"{what}: {name} differ"
+
+
+@pytest.mark.parametrize("pipelined", [False, True], ids=["sequential", "pipelined"])
+@pytest.mark.parametrize("use_graph", [False, True], ids=["eager", "graph"])
+def test_qd_batch_matches_separate_trackers(tiny, use_graph, pipelined):
+    """Slot 0 runs throughout; slot 1 sits out step 3 (against a tracker that skipped that frame); slot 2 is restarted with another
+    video at step 5 (against a fresh tracker)."""
+    eng, (va, vb, vc, vd) = tiny
+    restart = 5
+    steps = []
+    for t in range(STEPS):
+        steps.append({"start": [0, 1, 2] if t == 0 else [2] if t == restart else [],
+                      "frames": [va[t], None if t == 3 else vb[t], vc[t] if t < restart else vd[t - restart]]})
+    ref0 = reference(eng, list(va))
+    ref1 = reference(eng, [vb[t] for t in range(STEPS) if t != 3])
+    ref2a, ref2b = reference(eng, list(vc[:restart])), reference(eng, list(vd[:STEPS - restart]))
+    _, got = run_batch(eng, 3, steps, use_graph, pipelined)
+    assert sum(r[1].numel() for r in ref0) > 0 and any(r[2].shape[0] > 0 for r in ref1), "no detections or tracks: a vacuous test"
+    k1 = 0
+    for t in range(STEPS):
+        assert_same(got[t][0], ref0[t], f"step {t} slot 0")
+        if t == 3:
+            assert got[t][1] is None
+        else:
+            assert_same(got[t][1], ref1[k1], f"step {t} slot 1")
+            k1 += 1
+        assert_same(got[t][2], ref2a[t] if t < restart else ref2b[t - restart], f"step {t} slot 2")
+
+
+def test_qd_batch_unstarted_slot_and_first_frame_without_detections(tiny):
+    """Slot 1 is never started: its result is None and the others are unaffected.  Slot 2's first frame has no detections (a black
+    frame), so its pre_dict is taken from its second frame, as a separate tracker does."""
+    eng, (va, vb, vc, _) = tiny
+    # with the seeded weights a black frame scores at most 0.0503 and every frame of these two videos more than 0.0529
+    kw = dict(KW, conf=0.052)
+    blank = torch.zeros(3, *SIZE)
+    ref0, ref2 = reference(eng, list(va[:5]), kw), reference(eng, [blank] + list(vc[:4]), kw)
+    assert ref2[0][2].shape[0] == 0 and all(r[2].shape[0] > 0 for r in ref2[1:] + ref0), "the black frame alone was meant to have no detections"
+    steps = [{"start": [0, 2] if t == 0 else [], "frames": [va[t], vb[t], blank if t == 0 else vc[t - 1]]} for t in range(5)]
+    _, got = run_batch(eng, 3, steps, use_graph=True, pipelined=True, kw=kw)
+    for t in range(5):
+        assert got[t][1] is None
+        assert_same(got[t][0], ref0[t], f"step {t} slot 0")
+        assert_same(got[t][2], ref2[t], f"step {t} slot 2")
+
+
+def test_launches_per_frame_do_not_depend_on_n_seq(tiny):
+    from unicorn_b200.mot import UnicornMOTBatch
+    eng, (va, vb, vc, _) = tiny
+    counts = []
+    for n in (1, 3):
+        mb = UnicornMOTBatch(eng, SIZE, n, **KW)
+        for i in range(n):
+            mb.start(i, qd_tracker())
+        mb.step_tensor(torch.stack([va[0], vb[0], vc[0]][:n]))
+        counts.append(mb.launches_per_frame)
+    assert counts[0] == counts[1] > 0, counts
+
+
+def test_validation_leaves_state_unchanged(tiny):
+    from unicorn_b200.mot import UnicornMOTBatch
+    eng, (va, vb, vc, _) = tiny
+    mb = UnicornMOTBatch(eng, SIZE, 3, **KW)
+    for i in range(3):
+        mb.start(i, qd_tracker())
+    mb.step_tensor(torch.stack([va[0], vb[0], vc[0]]))
+    torch.cuda.synchronize()
+    before = (list(mb.frame_ids), mb._ring.submitted, mb.has_prev.clone(), mb.prev_feat.clone())
+    good = torch.stack([va[1], vb[1], vc[1]])
+    for kw in (dict(frames=good[:2]), dict(frames=good[:, :, :160]), dict(frames=good.double()), dict(frames=good, active=[1, 1]),
+               dict(frames=good, scales=[1.0])):
+        with pytest.raises(ValueError):
+            mb.submit(**kw)
+    with pytest.raises(ValueError):
+        mb.start(3)
+    torch.cuda.synchronize()
+    assert mb.frame_ids == before[0] and mb._ring.submitted == before[1]
+    assert torch.equal(mb.has_prev, before[2]) and torch.equal(mb.prev_feat, before[3])
+
+
+def test_failed_input_copy_leaves_state_unchanged(tiny, monkeypatch):
+    """A frame copy that fails (here forced) leaves the frame counters, the ring and the slot's staged step as they were; the next
+    step runs normally."""
+    from unicorn_b200.frames import FrameSlot
+    from unicorn_b200.mot import UnicornMOTBatch
+    eng, (va, vb, vc, _) = tiny
+    mb = UnicornMOTBatch(eng, SIZE, 3, **KW)
+    for i in range(3):
+        mb.start(i, qd_tracker())
+    mb.step_tensor(torch.stack([va[0], vb[0], vc[0]]))
+    nxt = mb._ctxs[mb._ring.submitted % 2]
+    before = (list(mb.frame_ids), mb._ring.submitted, list(nxt.mask), nxt.u8, nxt.graph)
+
+    def fail(self, frames):
+        raise RuntimeError("copy failed")
+    with monkeypatch.context() as m:
+        m.setattr(FrameSlot, "stage", fail)
+        with pytest.raises(RuntimeError):
+            mb.submit(torch.stack([va[1], vb[1], vc[1]]), active=[True, False, True])
+    assert (list(mb.frame_ids), mb._ring.submitted, list(nxt.mask), nxt.u8, nxt.graph) == before
+    res = mb.step_tensor(torch.stack([va[1], vb[1], vc[1]]))
+    assert all(r is not None for r in res) and mb.frame_ids == [2, 2, 2]
+
+
+# ------------------------------------------------------------------------------------------------ ByteTrack arm
+class Recorder:  # stands in for BYTETracker: update(dets [n,7] numpy, img_info, img_size)
+    def __init__(self):
+        self.rows = []
+
+    def update(self, dets, img_info, img_size):
+        self.rows.append(torch.from_numpy(dets).clone())
+        return []
+
+
+def test_byte_batch_matches_one_stream(tiny):
+    from unicorn_b200.mot import UnicornMOTBatch, UnicornMOTTracker
+    eng, videos = tiny
+    u8 = [v.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous() for v in videos[:3]]
+    refs = []
+    for v in u8:
+        rec = Recorder()
+        trk = UnicornMOTTracker(eng, SIZE, conf=0.01, nms=0.7, assoc="byte", tracker=rec)
+        for t in range(6):
+            trk.step_tensor(v[t:t + 1], img_info=SIZE)
+        refs.append(rec)
+    got = [Recorder() for _ in range(3)]
+    mb = UnicornMOTBatch(eng, SIZE, 3, conf=0.01, nms=0.7, assoc="byte", use_graph=True)
+    for i in range(3):
+        mb.start(i, got[i])
+    step = lambda t: torch.stack([v[t] for v in u8]).pin_memory()  # noqa: E731
+    mb.submit(step(0))
+    for t in range(6):
+        if t + 1 < 6:
+            mb.submit(step(t + 1))
+        assert mb.collect([SIZE] * 3) == [[], [], []]
+    assert len(mb._graphs) == 2
+    for i in range(3):
+        assert len(got[i].rows) == len(refs[i].rows) == 6 and sum(r.shape[0] for r in refs[i].rows) > 6
+        for t, (r, g) in enumerate(zip(refs[i].rows, got[i].rows)):
+            assert r.shape == g.shape and torch.equal(r, g), f"slot {i} frame {t}"
+
+
+# ------------------------------------------------------------------------------------------------ full size
+def test_qd_batch_full_size_matches_separate_trackers():
+    """ConvNeXt-L at 800x1280, two sequences: the batched layer shapes get their own plan-time tiles."""
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mot import UnicornMOTBatch, UnicornMOTTracker
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.weights import make_state_dict
+    name, size = "unicorn_track_large", (800, 1280)
+    eng = UnicornEngine(make_state_dict(name, 0), name)
+    videos = [make_video(3, *size, seed=30 + s, n_obj=3)[0] for s in range(2)]
+    refs = []
+    for v in videos:
+        trk = UnicornMOTTracker(eng, size, tracker=qd_tracker(), **KW)
+        refs.append([])
+        for t in range(3):
+            b, i = trk.step_tensor(v[t:t + 1])
+            refs[-1].append((b.clone(), i.clone(), trk.last["dets"].clone(), trk.last["feats"].clone()))
+    mb = UnicornMOTBatch(eng, size, 2, use_graph=True, **KW)
+    for i in range(2):
+        mb.start(i, qd_tracker())
+    assert any(r[2].shape[0] > 0 for rs in refs for r in rs), "no detections: a vacuous test"
+    mb.submit(torch.stack([v[0] for v in videos]))
+    for t in range(3):
+        if t + 1 < 3:
+            mb.submit(torch.stack([v[t + 1] for v in videos]))
+        res = mb.collect()
+        for i in range(2):
+            assert_same((res[i][0], res[i][1], mb.last_dets[i], mb.last_feats[i]), refs[i][t], f"frame {t} sequence {i}")

@@ -7,6 +7,12 @@ sequence (UnicornSOTTrack, depth 1 and 3), on the 800x1280 SOT frame with CUDA g
 UnicornVOSTrack at depth 1 and 3, unicorn_track_large_mask by default.  A VOS step is timed end to end (host clock around steps that
 end in a device synchronise): input copy, graph replay, the read-back of the detection rows and the per-sequence result assembly.
 
+--workload mot: UnicornMOTBatch at n_seq 1 / 2 / 4 against UnicornMOTTracker(use_graph=True) driven with pipelined submit / collect, QD
+arm, unicorn_track_large; --assoc byte: the ByteTrack arm, against UnicornMOTTracker(assoc="byte") at depth 1 and 3.  A step is timed
+end to end (host clock around steps that end in a device synchronise, the association included).  Also printed: the device-only step
+(CUDA events around graph replays of the step), the mean host association per step (collect() of a step whose device work is done),
+the mean detections handed to the trackers per frame and the kernels launched per step.
+
 Device-resident timing like bench.py's `value`: the frames are already in HBM, each step is an input copy and a graph replay, timed
 with CUDA events.  Every driver of a config is built first (plan-time autotuning of the batched layer shapes, graph capture); the
 timed rounds then alternate over the drivers so that clock and neighbour drift spread over all of them.  Printed per driver: aggregate
@@ -27,7 +33,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["sot", "vos"], default="sot")
+    ap.add_argument("--workload", choices=["sot", "vos", "mot"], default="sot")
+    ap.add_argument("--assoc", choices=["qd", "byte"], default="qd")
+    ap.add_argument("--n-obj", type=int, default=6)
     ap.add_argument("--configs", nargs="+", default=None)
     ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
     ap.add_argument("--n-seq", type=int, nargs="+", default=None)
@@ -40,6 +48,10 @@ def main():
         args.configs = args.configs or ["unicorn_track_large_mask"]
         args.n_seq = args.n_seq or [1, 2, 4]
         return main_vos(args)
+    if args.workload == "mot":
+        args.configs = args.configs or ["unicorn_track_large"]
+        args.n_seq = args.n_seq or [1, 2, 4]
+        return main_mot(args)
     args.configs = args.configs or ["unicorn_track_large", "unicorn_track_r50"]
     args.n_seq = args.n_seq or [1, 2, 4, 8]
     from unicorn_b200.engine import UnicornEngine
@@ -179,6 +191,155 @@ def main_vos(args):
                                   "added_peak_alloc_gib": round(mem / 2 ** 30, 2), "steps": args.steps, "rounds": args.rounds}), flush=True)
             del drivers, vb, trk, drv, batch_round, pipe_round
             torch.cuda.empty_cache()
+
+
+class _Counting:
+    """Forwards to a tracker and counts the detections handed to it (QD: the boxes passed to match, ByteTrack: the rows passed to
+    update)."""
+
+    def __init__(self, trk):
+        self.trk, self.dets, self.calls = trk, 0, 0
+
+    def match(self, boxes, *a, **kw):
+        self.dets, self.calls = self.dets + boxes.shape[0], self.calls + 1
+        return self.trk.match(boxes, *a, **kw)
+
+    def update(self, dets, *a, **kw):
+        self.dets, self.calls = self.dets + dets.shape[0], self.calls + 1
+        return self.trk.update(dets, *a, **kw)
+
+    def __getattr__(self, name):
+        return getattr(self.trk, name)
+
+
+def main_mot(args):
+    import time
+    import types
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mot import UnicornMOTBatch, UnicornMOTTracker
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.tracker import QuasiDenseEmbedTracker
+    from unicorn_b200.tracker.byte_tracker import BYTETracker
+    from unicorn_b200.weights import make_state_dict
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
+    H, W = args.size
+    N = max(args.n_seq)
+    to_u8 = lambda f: f.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()  # noqa: E731
+    bargs = types.SimpleNamespace(track_thresh=0.5, track_buffer=30, match_thresh=0.8, mot20=False)
+    new_tracker = lambda: _Counting(QuasiDenseEmbedTracker() if args.assoc == "qd" else BYTETracker(bargs))  # noqa: E731
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        videos = [make_video(4, H, W, seed=s, n_obj=args.n_obj)[0] for s in range(N)]
+        steps_u8 = [torch.stack([to_u8(v[t:t + 1])[0] for v in videos]).cuda() for t in range(4)]  # [N,H,W,3] per step
+        drivers = {}
+        for n in args.n_seq:
+            m0 = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            mb = UnicornMOTBatch(eng, (H, W), n, assoc=args.assoc, use_graph=True)
+            trackers = [new_tracker() for _ in range(n)]
+            for i in range(n):
+                mb.start(i, trackers[i])
+
+            def batch_round(steps, mb=mb, n=n):  # submit(t+1) before collect(t)
+                mb.submit(steps_u8[0][:n])
+                for t in range(steps):
+                    if t + 1 < steps:
+                        mb.submit(steps_u8[(t + 1) % 4][:n])
+                    mb.collect()
+
+            def batch_assoc(t, mb=mb, n=n):
+                mb.submit(steps_u8[t % 4][:n])
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                mb.collect()
+                return time.perf_counter() - t0
+
+            def batch_replay(t, mb=mb, n=n):
+                c = mb._ctxs[t % 2]
+                c.img_in_u8.copy_(steps_u8[t % 4][:n], non_blocking=True)
+                c.graph.replay()
+            batch_round(4)
+            drivers[f"batch{n}"] = ("UnicornMOTBatch", batch_round, batch_assoc, batch_replay, n, 1, mb, mb.launches_per_frame, trackers,
+                                    torch.cuda.max_memory_allocated() - m0)
+        for d in ([1] if args.assoc == "qd" else args.depths):
+            m0 = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            trk = UnicornMOTTracker(eng, (H, W), assoc=args.assoc, tracker=new_tracker(), use_graph=True, depth=d)
+            trk.step_tensor(steps_u8[0][0:1], img_info=(H, W))
+            l0 = _launches()
+            trk.submit(steps_u8[1][0:1])  # a slot's first frame runs eagerly: its launches are every frame's device half
+            launches = _launches() - l0
+            trk.collect((H, W))
+            inflight = max(2, d)  # depth 1: the two parity slots let submit(t+1) precede collect(t)
+
+            def pipe_round(steps, trk=trk, k=inflight):
+                sub = 0
+                for c in range(steps):
+                    while sub < steps and sub - c < k:
+                        trk.submit(steps_u8[sub % 4][0:1])
+                        sub += 1
+                    trk.collect((H, W))
+
+            def pipe_assoc(t, trk=trk):
+                trk.submit(steps_u8[t % 4][0:1])
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                trk.collect((H, W))
+                return time.perf_counter() - t0
+
+            def pipe_replay(t, trk=trk):
+                c = trk._ctxs[t % len(trk._ctxs)]
+                with torch.cuda.stream(c.stream):
+                    c.img_in_u8.copy_(steps_u8[t % 4][0:1], non_blocking=True)
+                    c.graph.replay()
+            pipe_round(4 + 2 * d)
+            drivers[f"depth{d}"] = ("UnicornMOTTracker", pipe_round, pipe_assoc, pipe_replay, 1, d, trk, launches, [trk.tracker],
+                                    torch.cuda.max_memory_allocated() - m0)
+        times = {key: [] for key in drivers}
+        for _ in range(args.rounds):
+            for key, (_, run, *_rest) in drivers.items():
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                run(args.steps)
+                torch.cuda.synchronize()
+                times[key].append(time.perf_counter() - t0)
+        main_stream = torch.cuda.current_stream()
+        for key, (name, _, assoc, replay, n, d, drv, launches, trackers, mem) in drivers.items():
+            for t in trackers:
+                t.dets = t.calls = 0
+            a = [assoc(t) for t in range(10)]
+            frames = sum(t.calls for t in trackers)
+            streams = [c.stream for c in drv._ctxs if c.stream is not None]
+            torch.cuda.synchronize()
+            e0.record()
+            for st in streams:
+                st.wait_stream(main_stream)
+            for t in range(args.steps):
+                replay(t)
+            for st in streams:
+                main_stream.wait_stream(st)
+            e1.record()
+            torch.cuda.synchronize()
+            ts = times[key]
+            fps = [n * args.steps / t for t in ts]
+            print(json.dumps({"workload": "mot", "assoc": args.assoc, "config": cfg, "size": [H, W], "driver": name, "n_seq": n, "depth": d,
+                              "frames_per_s": round(statistics.median(fps), 1), "frames_per_s_min_max": [round(min(fps), 1), round(max(fps), 1)],
+                              "ms_per_step": round(1e3 * statistics.median(ts) / args.steps, 2),
+                              "device_ms_per_step": round(e0.elapsed_time(e1) / args.steps, 2),
+                              "assoc_ms_per_step": round(1e3 * statistics.mean(a), 2),
+                              "dets_per_frame": round(sum(t.dets for t in trackers) / max(frames, 1), 1),
+                              "launches_per_step": launches,
+                              "added_peak_alloc_gib": round(mem / 2 ** 30, 2), "steps": args.steps, "rounds": args.rounds}), flush=True)
+        del drivers, drv, trackers, eng
+        torch.cuda.empty_cache()
+
+
+def _launches():
+    from unicorn_b200 import _lib
+    return _lib.LAUNCHES
 
 
 if __name__ == "__main__":

@@ -1,5 +1,6 @@
 // Instance-embedding sampling and association scoring for the MOT path.
-//   uc_sample_embed   unicorn/evaluators/mot_evaluator.py:1024-1034 (one F.grid_sample per box in the reference)
+//   uc_sample_embed   unicorn/evaluators/mot_evaluator.py:1024-1034 (one F.grid_sample per box in the reference); the
+//                     _batched entry point samples B images (B sequences' frames) in one launch
 //   uc_bisoftmax      unicorn/tracker/quasi_dense_embed_tracker.py:166-175 (feats = E M^T, bi-softmax, class gate)
 //   uc_box_iou        torchvision.ops.box_iou as used at quasi_dense_embed_tracker.py:80,146
 // All three are tiny (N, M <= a few hundred): one launch each, fp32 arithmetic in the reference's operation order.
@@ -8,17 +9,22 @@
 
 namespace uc {
 
-// one warp per box, lane owns channels lane, lane+32, ...  embed NHWC 16-bit [h,w,C]
-__global__ void __launch_bounds__(256) sample_embed_kernel(const uint16_t* __restrict__ embed, int ld, int h, int w, int C, int dtype,
-                                                            const float* __restrict__ boxes, int ldb, const int* __restrict__ count,
-                                                            int n_max, float stride, float* __restrict__ out) {
+// one warp per box, lane owns channels lane, lane+32, ...  embed NHWC 16-bit [h,w,C]; blockIdx.y = image: image b reads
+// embed + b * bs_embed, boxes + b * bs_boxes and count[b], and writes out + b * bs_out
+__global__ void __launch_bounds__(256) sample_embed_kernel(const uint16_t* __restrict__ embed, int ld, long bs_embed, int h, int w, int C,
+                                                            int dtype, const float* __restrict__ boxes, int ldb, long bs_boxes,
+                                                            const int* __restrict__ count, int n_max, float stride, float* __restrict__ out,
+                                                            long bs_out) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
-  const int n = count ? min(*count, n_max) : n_max;
+  const int b = blockIdx.y;
+  const int n = count ? min(count[b], n_max) : n_max;
   const int i = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (i >= n) return;
-  const float* bx = boxes + static_cast<long>(i) * ldb;
+  embed += b * bs_embed;
+  out += b * bs_out;
+  const float* bx = boxes + b * bs_boxes + static_cast<long>(i) * ldb;
   // centre in embedding-map pixels, clamped, normalised to [-1,1] exactly as the reference does ...
   float cx = (bx[0] + bx[2]) / 2 / stride - 0.5f, cy = (bx[1] + bx[3]) / 2 / stride - 0.5f;
   cx = (fminf(fmaxf(cx, 0.f), static_cast<float>(w - 1)) / (w - 1) - 0.5f) * 2.0f;
@@ -156,13 +162,32 @@ __global__ void __launch_bounds__(256) qd_assign_kernel(const float* __restrict_
 
 using namespace uc;
 
+static int sample_embed(const char* name, const void* embed, int ld, long bs_embed, int h, int w, int C, int dtype, const float* boxes,
+                        int ldb, long bs_boxes, const int* count_dev, int n_max, float stride, float* out, long bs_out, int B,
+                        cudaStream_t stream) {
+  if (n_max == 0) return UC_OK;
+  launch_pdl(sample_embed_kernel, dim3((n_max + 7) / 8, B), 256, 0, stream, static_cast<const uint16_t*>(embed), ld, bs_embed, h, w, C, dtype,
+             boxes, ldb, bs_boxes, count_dev, n_max, stride, out, bs_out);
+  return check_launch(name);
+}
+
 extern "C" int uc_sample_embed(const void* embed, int ld, int h, int w, int C, int dtype, const float* boxes, int ldb,
                                const int* count_dev, int n_max, float stride, float* out, void* stream_v) {
   if (!embed || !boxes || !out || n_max < 0 || h < 2 || w < 2 || ldb < 4) return set_error(UC_EINVAL, "uc_sample_embed: bad arguments");
-  if (n_max == 0) return UC_OK;
-  launch_pdl(sample_embed_kernel, (n_max + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream_v), static_cast<const uint16_t*>(embed), ld, h, w, C, dtype,
-                                                                                        boxes, ldb, count_dev, n_max, stride, out);
-  return check_launch("uc_sample_embed");
+  return sample_embed("uc_sample_embed", embed, ld, 0, h, w, C, dtype, boxes, ldb, 0, count_dev, n_max, stride, out, 0, 1,
+                      static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_sample_embed_batched(const void* embed, int ld, long bs_embed, int h, int w, int C, int dtype, const float* boxes, int ldb,
+                                       long bs_boxes, const int* count_dev, int n_max, float stride, float* out, long bs_out, int B,
+                                       void* stream_v) {
+  if (B < 1) return set_error(UC_EINVAL, "uc_sample_embed_batched: B must be >= 1");
+  if (!embed || !boxes || !count_dev || !out) return set_error(UC_EINVAL, "uc_sample_embed_batched: null pointer");
+  if (n_max < 0 || h < 2 || w < 2 || C < 1 || ld < C || ldb < 4) return set_error(UC_EINVAL, "uc_sample_embed_batched: bad arguments");
+  if (bs_embed < static_cast<long>(h) * w * ld || bs_boxes < static_cast<long>(n_max) * ldb || bs_out < static_cast<long>(n_max) * C)
+    return set_error(UC_EINVAL, "uc_sample_embed_batched: bad per-image strides (each must cover one image)");
+  return sample_embed("uc_sample_embed_batched", embed, ld, bs_embed, h, w, C, dtype, boxes, ldb, bs_boxes, count_dev, n_max, stride, out,
+                      bs_out, B, static_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int uc_bisoftmax(const float* det_embeds, const float* memo_embeds, int N, int M, int C, const float* det_labels,

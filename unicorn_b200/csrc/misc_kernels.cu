@@ -192,11 +192,17 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_kernel(const uint16_t* __res
 // ------------------------------------------------------------------------------------------------ conditional row copy
 // dst rows <- src rows when (*flag != 0) != invert, else nothing: device-side "pre_dict = cur_dict only if this frame had
 // detections" (unicorn/evaluators/mot_evaluator.py:1005,1014-1020) without a host round trip, so the MOT frame stays one CUDA graph.
-__global__ void __launch_bounds__(256) copy_rows_if_kernel(const int* __restrict__ flag, int invert, const uint8_t* __restrict__ src, long src_ld,
-                                                            uint8_t* __restrict__ dst, long dst_ld, long rows, int row_chunks) {
+// blockIdx.y = image: image b copies src + b * src_bs to dst + b * dst_bs when (gate == NULL || gate[b] != 0) and
+// (flag[b] != 0) != invert (a sequence slot that sits out a step keeps its pre_dict through the gate).
+__global__ void __launch_bounds__(256) copy_rows_if_kernel(const int* __restrict__ flag, const int* __restrict__ gate, int invert,
+                                                            const uint8_t* __restrict__ src, long src_ld, long src_bs, uint8_t* __restrict__ dst,
+                                                            long dst_ld, long dst_bs, long rows, int row_chunks) {
   pdl_wait();
   pdl_launch_dependents();
-  if ((*flag != 0) == (invert != 0)) return;
+  const int b = blockIdx.y;
+  if ((gate && gate[b] == 0) || (flag[b] != 0) == (invert != 0)) return;
+  src += b * src_bs;
+  dst += b * dst_bs;
   const long total = rows * row_chunks;
   for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const long r = i / row_chunks;
@@ -272,12 +278,36 @@ extern "C" int uc_nhwc_to_nchw_f32(const void* src, int lds, float* dst, int B, 
   return check_launch("uc_nhwc_to_nchw_f32");
 }
 
+static int copy_rows_if(const char* name, const int* flag_dev, const int* gate_dev, int invert, const void* src, long src_ld_bytes,
+                        long src_bs_bytes, void* dst, long dst_ld_bytes, long dst_bs_bytes, long rows, int row_bytes, int B, cudaStream_t stream) {
+  launch_pdl(copy_rows_if_kernel, dim3(grid_for(rows * (row_bytes / 16)), B), 256, 0, stream, flag_dev, gate_dev, invert,
+             static_cast<const uint8_t*>(src), src_ld_bytes, src_bs_bytes, static_cast<uint8_t*>(dst), dst_ld_bytes, dst_bs_bytes, rows,
+             row_bytes / 16);
+  return check_launch(name);
+}
+
+static bool aligned_rows(const void* src, long src_ld_bytes, const void* dst, long dst_ld_bytes, long rows, int row_bytes) {
+  return rows >= 1 && row_bytes >= 16 && row_bytes % 16 == 0 && src_ld_bytes % 16 == 0 && dst_ld_bytes % 16 == 0 &&
+         ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+}
+
 extern "C" int uc_copy_rows_if(const int* flag_dev, int invert, const void* src, long src_ld_bytes, void* dst, long dst_ld_bytes, long rows,
                                int row_bytes, void* stream_v) {
-  if (!flag_dev || !src || !dst || rows < 1 || row_bytes < 16 || row_bytes % 16 || src_ld_bytes % 16 || dst_ld_bytes % 16 ||
-      ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15))
+  if (!flag_dev || !src || !dst || !aligned_rows(src, src_ld_bytes, dst, dst_ld_bytes, rows, row_bytes))
     return set_error(UC_EINVAL, "uc_copy_rows_if: 16-byte aligned rows only");
-  launch_pdl(copy_rows_if_kernel, grid_for(rows * (row_bytes / 16)), 256, 0, static_cast<cudaStream_t>(stream_v), flag_dev, invert,
-             static_cast<const uint8_t*>(src), src_ld_bytes, static_cast<uint8_t*>(dst), dst_ld_bytes, rows, row_bytes / 16);
-  return check_launch("uc_copy_rows_if");
+  return copy_rows_if("uc_copy_rows_if", flag_dev, nullptr, invert, src, src_ld_bytes, 0, dst, dst_ld_bytes, 0, rows, row_bytes, 1,
+                      static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_copy_rows_if_batched(const int* flag_dev, const int* gate_dev, int invert, const void* src, long src_ld_bytes,
+                                       long src_bs_bytes, void* dst, long dst_ld_bytes, long dst_bs_bytes, long rows, int row_bytes, int B,
+                                       void* stream_v) {
+  if (B < 1) return set_error(UC_EINVAL, "uc_copy_rows_if_batched: B must be >= 1");
+  if (!flag_dev || !src || !dst) return set_error(UC_EINVAL, "uc_copy_rows_if_batched: null pointer");
+  if (!aligned_rows(src, src_ld_bytes, dst, dst_ld_bytes, rows, row_bytes) || src_bs_bytes % 16 || dst_bs_bytes % 16)
+    return set_error(UC_EINVAL, "uc_copy_rows_if_batched: 16-byte aligned rows only");
+  if (src_bs_bytes < rows * src_ld_bytes || dst_bs_bytes < rows * dst_ld_bytes)
+    return set_error(UC_EINVAL, "uc_copy_rows_if_batched: bad per-image strides (each must cover one image)");
+  return copy_rows_if("uc_copy_rows_if_batched", flag_dev, gate_dev, invert, src, src_ld_bytes, src_bs_bytes, dst, dst_ld_bytes, dst_bs_bytes,
+                      rows, row_bytes, B, static_cast<cudaStream_t>(stream_v));
 }

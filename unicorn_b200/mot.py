@@ -17,13 +17,35 @@ the sequential `step_tensor`, throughput max(device, host) instead of their sum.
 
 With `assoc="byte"` the frames do not even share the s16 feature: `depth` > 1 keeps that many frames in flight ON THE DEVICE, each on
 its own stream and engine context (UnicornEngine.fork(): same weights, own activations) like UnicornSOTTrack(depth=...); the detections
-are identical to the one-stream driver's (tests/test_tracker_gpu.py), collect() still returns them in frame order."""
+are identical to the one-stream driver's (tests/test_tracker_gpu.py), collect() still returns them in frame order.
+
+UnicornMOTBatch runs several MOT sequences in lock step: one batched frame per step (every kernel computes each image as its B = 1 launch
+does), one host association per sequence."""
+import warnings
+
 import torch
 
-from . import ops
+from . import _lib, ops
 from .engine import UnicornEngine
-from .frames import FrameSlot, Ring, in_flight
+from .frames import FrameSlot, Ring, anchor_count, in_flight
 from .tracker import QuasiDenseEmbedTracker
+
+
+def _qd_match(tracker, d, f, scale, score_thr, frame_id):
+    """The host half of a QD frame: score filter and QuasiDenseEmbedTracker.match on the NMS rows d [n,7] and their embeddings f [n,128]
+    -> (bboxes [n,5] in original-image coordinates, ids [n]) ordered by id."""
+    scores = d[:, 4] * d[:, 5]
+    keep = scores > score_thr  # :1008-1012
+    boxes = torch.cat([d[keep, :4] / scale, scores[keep, None]], 1)
+    labels = torch.ones(boxes.size(0))  # :1013 (all labels = 1)
+    if d.shape[0] == 0:  # outputs[0] is None: the reference skips tracking for this frame altogether (:1005)
+        return torch.zeros(0, 5), torch.zeros(0, dtype=torch.long)
+    # detections exist but none may pass the score filter: match() still runs (tracklets age, backdrops are replaced)
+    ob, _, oid = tracker.match(boxes, labels, f[keep], frame_id)
+    valid = oid > -1  # :1047-1053
+    ob, oid = ob[valid], oid[valid]
+    order = oid.sort()[1]
+    return ob[order], oid[order]
 
 
 class QDEmbedding:
@@ -141,7 +163,6 @@ class UnicornMOTTracker:
         c.event.synchronize()
         total = int(c.host_count[0])
         if total > self.max_dets and not self._warned:
-            import warnings
             warnings.warn(f"UnicornMOTTracker: {total} detections after NMS, only the {self.max_dets} best are associated "
                           "(raise max_dets; the reference has no cap)")
             self._warned = True
@@ -152,21 +173,192 @@ class UnicornMOTTracker:
             info = img_info if img_info is not None else (H / c.scale, W / c.scale)
             return self.tracker.update(d.numpy(), info, (H, W))
         f = c.host_feats[:n].clone()
-        scores = d[:, 4] * d[:, 5]
-        keep = scores > self.score_thr  # :1008-1012
-        boxes = torch.cat([d[keep, :4] / c.scale, scores[keep, None]], 1)
-        labels = torch.ones(boxes.size(0))  # :1013 (all labels = 1)
         self.last.update(dets=d, feats=f)
-        if n == 0:  # outputs[0] is None: the reference skips tracking for this frame altogether (:1005)
-            return torch.zeros(0, 5), torch.zeros(0, dtype=torch.long)
-        # detections exist but none may pass the score filter: match() still runs (tracklets age, backdrops are replaced)
-        ob, _, oid = self.tracker.match(boxes, labels, f[keep], c.frame_id)
-        valid = oid > -1  # :1047-1053
-        ob, oid = ob[valid], oid[valid]
-        order = oid.sort()[1]
-        return ob[order], oid[order]
+        return _qd_match(self.tracker, d, f, c.scale, self.score_thr, c.frame_id)
 
     def step_tensor(self, frame, scale=1.0, img_info=None):
         """Sequential protocol of the reference: one frame in, its tracks out."""
         self.submit(frame, scale)
         return self.collect(img_info)
+
+
+class _BatchSlot(FrameSlot):
+    """One batched MOT step in flight: a frame slot of n_seq images, its engine buffer tag, its pinned results and the step's inputs
+    (which slots are active, their scales, frame numbers and trackers), staged per slot so that a step in flight never reads the
+    next step's values."""
+
+    def __init__(self, eng, H, W, n_seq, tag, n_keep, feats):
+        super().__init__(eng, H, W, batch=n_seq)
+        self.tag = tag
+        self.host_count = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
+        self.host_dets = torch.zeros(n_seq, n_keep, 7).pin_memory()
+        self.host_feats = torch.zeros(n_seq, n_keep, 128).pin_memory() if feats else None
+        self.host_active = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
+        self.active = torch.zeros(n_seq, dtype=torch.int32, device=eng.dev)  # the step's active table, read by the captured graph
+        self.mask, self.scales, self.frame_ids, self.trackers = [False] * n_seq, [1.0] * n_seq, [0] * n_seq, [None] * n_seq
+        self.warm_u8 = None
+
+
+class UnicornMOTBatch:
+    """`n_seq` MOT sequences in lock step: one batched frame per step (whole-mode backbone and head, NMS, and for the QD arm the
+    conditional pre_dict update, interaction with the previous features, upsample and embedding sampling, all at B = n_seq), optionally
+    captured as one CUDA graph; then each sequence's own tracker on the host.  Each sequence's results equal those of its own
+    UnicornMOTTracker (conf, nms, score_thr, max_dets, assoc and use_graph mean what they mean there).
+
+    start(i, tracker=None) begins a sequence in slot i at any time (a fresh QuasiDenseEmbedTracker for the QD arm unless one is given;
+    the ByteTrack arm needs a BYTETracker); it writes only slot i's state and keeps the graphs.  A slot never started, or inactive in a
+    step, runs on whatever its input holds: its pre_dict, first-frame flag, tracker and frame counter are left as they were and its
+    result is None, as if its own tracker had not been stepped.
+
+    Protocol as UnicornMOTTracker: submit(frames, scales, active) enqueues a step, collect(img_infos) associates the oldest one;
+    two parity slots let submit(t+1) precede collect(t), so the host association of step t overlaps the device work of step t+1."""
+
+    def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, assoc="qd",
+                 use_graph=False):
+        if n_seq < 1 or assoc not in ("qd", "byte"):
+            raise ValueError(f"UnicornMOTBatch: n_seq >= 1 and assoc 'qd' or 'byte' (got {n_seq}, {assoc!r})")
+        self.eng, self.input_size, self.n_seq = engine, tuple(input_size), n_seq
+        self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets
+        self.assoc, self.use_graph = assoc, use_graph
+        H, W = self.input_size
+        dev = engine.dev
+        self.n_keep = min(max_dets, anchor_count(H, W))  # rows a sequence can have after NMS and that are read back
+        qd = assoc == "qd"
+        if qd:  # QDEmbedding's state, one row per sequence
+            self.prev_feat = torch.zeros(n_seq, H // 16, W // 16, engine.inc[1], dtype=torch.bfloat16, device=dev)
+            self.has_prev = torch.zeros(n_seq, dtype=torch.int32, device=dev)
+            self.feats = torch.zeros(n_seq, self.n_keep, 128, dtype=torch.float32, device=dev)
+        # two parity slots on the current stream: one input buffer and one NMS workspace, own backbone buffers (tag) and graph each
+        slots = [_BatchSlot(engine, H, W, n_seq, "motb%d" % i, self.n_keep, qd) for i in range(2)]
+        slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
+        self._ring = Ring(slots)
+        self._ctxs = slots
+        self.trackers = [None] * n_seq
+        self.frame_ids = [0] * n_seq  # frames each sequence has run since its start()
+        self.launches_per_frame = 0
+        self.last, self.last_dets, self.last_feats = {}, [None] * n_seq, [None] * n_seq
+        self._warned = False
+
+    img_in_u8 = property(lambda self: self._ctxs[0].img_in_u8)
+    _graphs = property(lambda self: [(c.graph, c.last) for c in self._ctxs if c.graph is not None])
+    ws = property(lambda self: self._ctxs[0].ws)
+
+    def start(self, i, tracker=None):
+        """Begin a new sequence in slot i: its first-frame flag and frame counter are reset and `tracker` (default: a fresh
+        QuasiDenseEmbedTracker, as the reference creates one at frame_id == 1) is installed.  Steps already submitted finish with the
+        slot's previous tracker."""
+        if not 0 <= i < self.n_seq:
+            raise ValueError(f"UnicornMOTBatch.start: slot {i} outside [0, {self.n_seq})")
+        if tracker is None:
+            if self.assoc == "byte":
+                raise ValueError("UnicornMOTBatch.start: assoc='byte' needs a BYTETracker instance")
+            tracker = QuasiDenseEmbedTracker(device=self.eng.dev)
+        if self.assoc == "qd":
+            self.has_prev[i].zero_()  # stream-ordered after the steps in flight
+        self.trackers[i], self.frame_ids[i] = tracker, 0
+
+    # ------------------------------------------------------------------------------------------ device half
+    def _frame(self, c):
+        e, n = c.eng, self.n_seq
+        e.begin_frame()
+        fpn, seq = e.backbone(c.img, tag=c.tag)
+        out = e.head(fpn, None, "mot")  # [n, A, 5+ncls]
+        dets, cnt = ops.postprocess_device(out, e.ncls, self.conf, self.nms, c.ws)
+        embed = None
+        if self.assoc == "qd":
+            # QDEmbedding per slot: pre_dict = cur_dict on a slot's first frame with detections, afterwards only on frames with
+            # detections; the gate keeps an idle slot's pre_dict and first-frame flag
+            feat = seq["feat"]
+            ops.copy_rows_if(self.has_prev, feat, self.prev_feat, invert=True, gate=c.active)
+            _, f_cur = e.interaction(self.prev_feat, feat)
+            embed = e.upsample(f_cur, "motb.emb")
+            ops.sample_embed(embed, dets.view(n, -1, 7), self.n_keep, 8.0, count=cnt, out=self.feats)
+            ops.copy_rows_if(cnt, feat, self.prev_feat, gate=c.active)
+            self.has_prev.bitwise_or_(((cnt > 0) & (c.active != 0)).to(torch.int32))
+        c.last = dict(embed=embed, head=out)
+
+    def _check(self, frames, scales, active):
+        n, (H, W) = self.n_seq, self.input_size
+        ok = torch.is_tensor(frames) and ((frames.dtype == torch.uint8 and tuple(frames.shape) == (n, H, W, 3)) or
+                                          (frames.dtype == torch.float32 and tuple(frames.shape) == (n, 3, H, W)))
+        if not ok:
+            got = (tuple(frames.shape), frames.dtype) if torch.is_tensor(frames) else type(frames)
+            raise ValueError(f"UnicornMOTBatch: frames must be uint8 [{n},{H},{W},3] or float32 [{n},3,{H},{W}], got {got}")
+        if scales is not None and len(scales) != n:
+            raise ValueError(f"UnicornMOTBatch: {len(scales)} scales for {n} sequences")
+        if active is not None and len(active) != n:
+            raise ValueError(f"UnicornMOTBatch: active has {len(active)} entries for {n} sequences")
+
+    def submit(self, frames, scales=None, active=None):
+        """frames: preprocessed fp32 [n_seq,3,H,W] or uint8 [n_seq,H,W,3], host or device; scales: n_seq letterbox ratios (default
+        1); active: n_seq flags (default: every started slot).  Enqueues the step; returns immediately."""
+        self._check(frames, scales, active)
+        n = self.n_seq
+        c = self._ring.submit()
+        u8, graph = c.u8, c.graph
+        try:
+            c.stage(frames)  # the last step that can fail (e.g. frames on another device): nothing has changed before it
+        except BaseException:
+            self._ring.submitted -= 1
+            c.u8, c.graph = u8, graph
+            raise
+        c.mask = [self.trackers[i] is not None and (active is None or bool(active[i])) for i in range(n)]
+        for i in range(n):
+            self.frame_ids[i] += c.mask[i]
+        c.scales = [1.0] * n if scales is None else [float(s) for s in scales]
+        c.frame_ids, c.trackers = list(self.frame_ids), list(self.trackers)
+        # the slot's previous step was collected, so its pinned staging buffer is free again
+        c.host_active.copy_(torch.tensor(c.mask, dtype=torch.int32))
+        c.active.copy_(c.host_active, non_blocking=True)
+        if c.graph is not None:
+            c.graph.replay()
+        elif self.use_graph and c.warm_u8 == c.u8:
+            # first step of a slot eager, second captured without a warm-up: a QD step advances pre_dict, so it must not run twice
+            c.graph, self.launches_per_frame = c.capture(lambda: self._frame(c))
+        else:
+            l0 = _lib.LAUNCHES
+            self._frame(c)
+            self.launches_per_frame = _lib.LAUNCHES - l0
+            c.warm_u8 = c.u8
+        c.host_count.copy_(c.ws.count, non_blocking=True)
+        c.host_dets.copy_(c.ws.dets.view(n, -1, 7)[:, :self.n_keep], non_blocking=True)
+        if self.assoc == "qd":
+            c.host_feats.copy_(self.feats, non_blocking=True)
+        c.event.record()
+        self.last = c.last
+
+    # ------------------------------------------------------------------------------------------ host half
+    def collect(self, img_infos=None):
+        """Association of the oldest submitted step: a list of n_seq results, None for an idle slot.  QDTrack: (bboxes [n,5] in
+        original-image coordinates, ids [n]); ByteTrack: the active STracks (img_infos[i] = (height, width) of slot i's original image).
+        last_dets[i] / last_feats[i] then hold the NMS rows / embeddings slot i's tracker was given in this step, None for an idle slot
+        (and last_feats for the ByteTrack arm)."""
+        c = self._ring.collect()
+        c.event.synchronize()
+        H, W = self.input_size
+        res = [None] * self.n_seq
+        self.last_dets, self.last_feats = [None] * self.n_seq, [None] * self.n_seq
+        for i in range(self.n_seq):
+            if not c.mask[i]:
+                continue
+            total = int(c.host_count[i])
+            if total > self.max_dets and not self._warned:
+                warnings.warn(f"UnicornMOTBatch: {total} detections after NMS in slot {i}, only the {self.max_dets} best are associated "
+                              "(raise max_dets; the reference has no cap)")
+                self._warned = True
+            k = min(total, self.n_keep)
+            d = c.host_dets[i, :k].clone()
+            self.last_dets[i] = d
+            if self.assoc == "byte":
+                info = img_infos[i] if img_infos is not None and img_infos[i] is not None else (H / c.scales[i], W / c.scales[i])
+                res[i] = c.trackers[i].update(d.numpy(), info, (H, W))
+                continue
+            f = c.host_feats[i, :k].clone()
+            self.last_feats[i] = f
+            res[i] = _qd_match(c.trackers[i], d, f, c.scales[i], self.score_thr, c.frame_ids[i])
+        return res
+
+    def step_tensor(self, frames, scales=None, active=None, img_infos=None):
+        """Sequential protocol: one step in, its n_seq results out."""
+        self.submit(frames, scales, active)
+        return self.collect(img_infos)

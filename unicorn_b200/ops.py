@@ -278,14 +278,23 @@ def add(a2d, b2d, out=None):
     return out
 
 
-def copy_rows_if(flag, src, dst, invert=False):
-    """dst <- src (NHWC views of equal shape, channel-contiguous) when (flag[0] != 0) != invert — decided on the device."""
+def copy_rows_if(flag, src, dst, invert=False, gate=None):
+    """dst <- src (NHWC views of equal shape, channel-contiguous) when (flag[0] != 0) != invert — decided on the device.
+    With B > 1 images ([B,h,w,C] maps, flag int32 [B]) or a gate (int32 [B]), image b is copied when (gate is None or gate[b] != 0)
+    and (flag[b] != 0) != invert, all images in one launch."""
     assert src.shape == dst.shape and src.dtype == dst.dtype and flag.dtype == torch.int32
-    C = src.shape[-1]
-    rows = src.numel() // C
+    B, C = src.shape[0], src.shape[-1]
     es = src.element_size()
-    _lib.check(_L().uc_copy_rows_if(_p(flag), int(bool(invert)), _p(src), _l(_nhwc_ld(src) * es), _p(dst), _l(_nhwc_ld(dst) * es), _l(rows), C * es, _S()),
-               "uc_copy_rows_if")
+    if B == 1 and gate is None:
+        rows = src.numel() // C
+        _lib.check(_L().uc_copy_rows_if(_p(flag), int(bool(invert)), _p(src), _l(_nhwc_ld(src) * es), _p(dst), _l(_nhwc_ld(dst) * es), _l(rows), C * es, _S()),
+                   "uc_copy_rows_if")
+        return dst
+    assert src.dim() == 4 and flag.numel() == B and (gate is None or (gate.dtype == torch.int32 and gate.numel() == B))
+    rows = src.numel() // (B * C)
+    lds, ldd = _nhwc_ld(src), _nhwc_ld(dst)
+    _lib.check(_L().uc_copy_rows_if_batched(_p(flag), _p(gate), int(bool(invert)), _p(src), _l(lds * es), _l(rows * lds * es), _p(dst), _l(ldd * es),
+                                            _l(rows * ldd * es), _l(rows), C * es, B, _S()), "uc_copy_rows_if_batched")
     return dst
 
 
@@ -435,12 +444,27 @@ def postprocess_device(pred, ncls, conf, nms, ws, max_keep=0):
 
 
 def sample_embed(embed, boxes, n_max, stride=8.0, count=None, out=None):
-    """embed NHWC 16-bit [1,h,w,C]; boxes fp32 [>=n_max, >=4] (device); returns fp32 [n_max, C]."""
-    _, h, w, C = embed.shape
+    """embed NHWC 16-bit [1,h,w,C]; boxes fp32 [>=n_max, >=4] (device); returns fp32 [n_max, C].
+    B images: embed [B,h,w,C], boxes [B, >=n_max, >=4] (a batched PostWorkspace's dets), count int32 [B]; returns fp32 [B, n_max, C],
+    image b sampling its own map at its own first min(count[b], n_max) boxes in one launch (the rows past that count are not written)."""
+    B, h, w, C = embed.shape
+    if boxes.dim() == 2:
+        if out is None:
+            out = torch.zeros(n_max, C, dtype=torch.float32, device=embed.device)
+        _lib.check(_L().uc_sample_embed(_p(embed), _nhwc_ld(embed), h, w, C, _DT[embed.dtype], _p(boxes), boxes.stride(0), _p(count), n_max,
+                                        _f(stride), _p(out), _S()), "uc_sample_embed")
+        return out
+    assert boxes.shape[0] == B and boxes.shape[1] >= n_max and boxes.stride(2) == 1 and count is not None and count.numel() == B
     if out is None:
-        out = torch.zeros(n_max, C, dtype=torch.float32, device=embed.device)
-    _lib.check(_L().uc_sample_embed(_p(embed), _nhwc_ld(embed), h, w, C, _DT[embed.dtype], _p(boxes), boxes.stride(0), _p(count), n_max,
-                                    _f(stride), _p(out), _S()), "uc_sample_embed")
+        out = torch.zeros(B, n_max, C, dtype=torch.float32, device=embed.device)
+    assert out.shape == (B, n_max, C) and out.dtype == torch.float32 and out.stride(2) == 1 and out.stride(1) == C
+    if B == 1:
+        _lib.check(_L().uc_sample_embed(_p(embed), _nhwc_ld(embed), h, w, C, _DT[embed.dtype], _p(boxes), boxes.stride(1), _p(count), n_max,
+                                        _f(stride), _p(out), _S()), "uc_sample_embed")
+        return out
+    _lib.check(_L().uc_sample_embed_batched(_p(embed), _nhwc_ld(embed), _l(embed.stride(0)), h, w, C, _DT[embed.dtype], _p(boxes), boxes.stride(1),
+                                            _l(boxes.stride(0)), _p(count), n_max, _f(stride), _p(out), _l(out.stride(0)), B, _S()),
+               "uc_sample_embed_batched")
     return out
 
 
