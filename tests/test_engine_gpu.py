@@ -162,8 +162,9 @@ def test_reference_api_facade(setup):
 
 def test_pipelined_tracker_matches_sequential(setup):
     """depth=2: two frames in flight on two streams / engine contexts (sot.py submit / collect).  The frames of a sequence are
-    independent, so every result must equal the sequential tracker's, bit for bit, in order."""
-    from unicorn_b200.sot import UnicornSOTTrack
+    independent, so every result must equal the sequential tracker's, bit for bit, in order.  Then the same for two sequences per
+    step (n_seq = 2)."""
+    from unicorn_b200.sot import UnicornSOTBatch, UnicornSOTTrack
     from unicorn_b200.synthetic import make_video
     trk = setup["trk"]
     frames, boxes = make_video(8, 320, 320, seed=6)
@@ -184,3 +185,24 @@ def test_pipelined_tracker_matches_sequential(setup):
     # the synchronous call of a pipelined tracker is submit + collect
     d, n = pipe.track_tensor(host[3])
     assert n == ref[2][1] and torch.equal(d, ref[2][0])
+    # n_seq = 2: the second sequence is another video, its frames fed in reverse order
+    frames2, boxes2 = make_video(8, 320, 320, seed=7)
+    steps = [torch.stack([frames[i], frames2[8 - i]]).pin_memory() for i in range(1, 8)]
+    seq2 = UnicornSOTBatch(trk.eng, (320, 320), 2, use_graph=True)
+    pipe2 = UnicornSOTBatch(trk.eng, (320, 320), 2, use_graph=True, depth=2)
+    for b in (seq2, pipe2):
+        b.initialize_tensor(0, host[0], boxes[0, 0])
+        b.initialize_tensor(1, frames2[0:1], boxes2[0, 0])
+    ref2 = [seq2.track_tensor(s) for s in steps]
+    pipe2.submit(steps[0])
+    got2 = []
+    for s in steps[1:]:
+        pipe2.submit(s)
+        got2.append(pipe2.collect())
+    got2.append(pipe2.collect())
+    assert all(c.graph is not None for c in pipe2._ctxs)
+    for t, ((d0, n0), (d1, n1)) in enumerate(zip(ref2, got2)):
+        assert torch.equal(n0, n1), f"step {t}"
+        for i in range(2):
+            k = min(int(n0[i]), 3)
+            assert torch.equal(d0[i, :k], d1[i, :k]), f"step {t} sequence {i}"

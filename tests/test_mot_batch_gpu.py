@@ -157,6 +157,22 @@ def test_qd_batch_matches_separate_trackers(tiny, use_graph, pipelined):
         assert_same(got[t][2], ref2a[t] if t < restart else ref2b[t - restart], f"step {t} slot 2")
 
 
+def test_qd_single_sequence_idle_step(tiny):
+    """n_seq = 1 has no gate: a step without an active sequence launches nothing, so the sequence goes on as a tracker that skipped
+    that frame."""
+    eng, (va, _, _, _) = tiny
+    steps = [{"start": [0] if t == 0 else [], "frames": [None if t == 3 else va[t]]} for t in range(STEPS)]
+    ref = reference(eng, [va[t] for t in range(STEPS) if t != 3])
+    _, got = run_batch(eng, 1, steps, use_graph=True, pipelined=True)
+    k = 0
+    for t in range(STEPS):
+        if t == 3:
+            assert got[t][0] is None
+            continue
+        assert_same(got[t][0], ref[k], f"step {t}")
+        k += 1
+
+
 def test_qd_batch_unstarted_slot_and_first_frame_without_detections(tiny):
     """Slot 1 is never started: its result is None and the others are unaffected.  Slot 2's first frame has no detections (a black
     frame), so its pre_dict is taken from its second frame, as a separate tracker does."""

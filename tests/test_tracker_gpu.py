@@ -184,6 +184,29 @@ def test_mot_byte_arm_three_frames_in_flight_matches_one_stream():
     assert len(ref.rows) == len(got.rows) == 10 and sum(r.shape[0] for r in ref.rows) > 10
     for t, (r, g) in enumerate(zip(ref.rows, got.rows)):
         assert r.shape == g.shape and torch.equal(r, g), f"frame {t}"
+    # n_seq = 2, three steps in flight: the second sequence is the first one's frames in reverse order
+    from unicorn_b200.mot import UnicornMOTBatch
+    steps = torch.stack([u8, u8.flip(0)], 1)  # [10, 2, H, W, 3]
+    seqs, pipes = [Recorder(), Recorder()], [Recorder(), Recorder()]
+    seq2 = UnicornMOTBatch(eng, (320, 320), 2, conf=0.01, nms=0.7, assoc="byte")
+    pipe2 = UnicornMOTBatch(eng, (320, 320), 2, conf=0.01, nms=0.7, assoc="byte", use_graph=True, depth=3)
+    for i in range(2):
+        seq2.start(i, seqs[i])
+        pipe2.start(i, pipes[i])
+    for t in range(10):
+        seq2.step_tensor(steps[t], img_infos=[(320, 320)] * 2)
+    sub = 0
+    for t in range(10):
+        while sub < 10 and sub - t < 3:
+            pipe2.submit(steps[sub].pin_memory())
+            sub += 1
+        pipe2.collect([(320, 320)] * 2)
+    assert all(c.graph is not None for c in pipe2._ctxs)
+    for i in range(2):
+        assert len(seqs[i].rows) == len(pipes[i].rows) == 10
+        for t, (r, g) in enumerate(zip(seqs[i].rows, pipes[i].rows)):
+            assert r.shape == g.shape and torch.equal(r, g), f"sequence {i} frame {t}"
+    assert all(torch.equal(r, g) for r, g in zip(ref.rows, seqs[0].rows))
 
 
 def test_byte_tracker_matches_reference_logic():

@@ -82,8 +82,12 @@ class Ring:
         self.collected += 1
         return self.slots[(self.collected - 1) % len(self.slots)]
 
-    def reset(self):
-        """Forget the frames in flight and drop every slot's graph (a new reference frame changes what the frame reads)."""
+    def forget(self):
+        """Forget the frames in flight: the next submit() hands out the first slot again."""
         self.submitted = self.collected = 0
+
+    def reset(self):
+        """forget() and drop every slot's graph (a new reference frame changes what the frame reads)."""
+        self.forget()
         for s in self.slots:
             s.graph = None

@@ -4,23 +4,23 @@ interaction with the previous frame -> embedding upsample (current frame only) -
 centres -> QuasiDenseEmbedTracker.match; with `assoc="byte"` the association is BYTETracker.update on the NMS output
 (mot_evaluator.py:177-209, the ByteTrack arm of the evaluator) and the embedding branch is skipped.
 
-The reference's per-box Python grid_sample loop, deepcopy of the frame dict and empty_cache() calls are gone.  The frame
-is split in a device half and a host half:
+The reference's per-box Python grid_sample loop, deepcopy of the frame dict and empty_cache() calls are gone.  UnicornMOTBatch runs
+`n_seq` sequences in lock step (one batched frame per step, every kernel computing each image as its B = 1 launch does) and splits a
+step in a device half and a host half:
 
-  submit(frame)  enqueues every kernel of the frame (optionally as ONE CUDA-graph replay), then asynchronous copies of
-                 (count, detections, sampled embeddings) into a pinned result slot, and records an event;
-  collect()      waits for the oldest slot's event and runs the association on the host.
+  submit(frames)  enqueues every kernel of the step (optionally as ONE CUDA-graph replay), then asynchronous copies of
+                  (counts, detections, sampled embeddings) into a pinned result slot, and records an event;
+  collect()       waits for the oldest slot's event and runs each sequence's association on the host.
 
 Nothing on the device depends on the association (the previous frame's s16 feature is the only carried state), so
-`submit(t+1); collect(t)` overlaps the host association of frame t with the device work of frame t+1 — same results as
+`submit(t+1); collect(t)` overlaps the host association of step t with the device work of step t+1 — same results as
 the sequential `step_tensor`, throughput max(device, host) instead of their sum.
 
-With `assoc="byte"` the frames do not even share the s16 feature: `depth` > 1 keeps that many frames in flight ON THE DEVICE, each on
-its own stream and engine context (UnicornEngine.fork(): same weights, own activations) like UnicornSOTTrack(depth=...); the detections
-are identical to the one-stream driver's (tests/test_tracker_gpu.py), collect() still returns them in frame order.
+With `assoc="byte"` the frames do not even share the s16 feature: `depth` > 1 keeps that many steps in flight ON THE DEVICE, each on
+its own stream and engine context (UnicornEngine.fork(): same weights, own activations) like UnicornSOTBatch(depth=...); the detections
+are identical to the one-stream driver's (tests/test_tracker_gpu.py), collect() still returns them in step order.
 
-UnicornMOTBatch runs several MOT sequences in lock step: one batched frame per step (every kernel computes each image as its B = 1 launch
-does), one host association per sequence."""
+UnicornMOTTracker is the n_seq = 1 case under the reference's one-sequence protocol."""
 import warnings
 
 import torch
@@ -49,199 +49,107 @@ def _qd_match(tracker, d, f, scale, score_thr, frame_id):
 
 
 class QDEmbedding:
-    """The QDTrack embedding step of a frame, on the device: interaction of the frame's s16 feature with pre_dict's, embedding
-    upsample, sampling at the detections' centres into `feats`.  pre_dict (mot_evaluator.py:1014-1020, :812-818) is the s16 feature
-    of the last frame THAT HAD DETECTIONS, kept in its own buffer and updated by device-side conditional copies (no host decision
-    inside the frame), so a frame that runs this step must run exactly once."""
+    """The QDTrack embedding step of a frame of B images, on the device: interaction of each image's s16 feature with its pre_dict,
+    embedding upsample, sampling at the image's detection centres into `feats` [B, n_keep, 128].  pre_dict (mot_evaluator.py:1014-1020,
+    :812-818) is the s16 feature of the last frame THAT HAD DETECTIONS, kept in its own buffer and updated by device-side conditional
+    copies (no host decision inside the frame), so a frame that runs this step must run exactly once.  gate (int32 [B]): image b's
+    pre_dict and first-frame flag change only where gate[b] != 0 (an idle sequence keeps its state)."""
 
-    def __init__(self, eng, H, W, max_dets, tag):
+    def __init__(self, eng, H, W, n_keep, tag, batch=1):
         dev = eng.dev
-        self.prev_feat = torch.zeros(1, H // 16, W // 16, eng.inc[1], dtype=torch.bfloat16, device=dev)
-        self.has_prev = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.feats = torch.zeros(max_dets, 128, dtype=torch.float32, device=dev)
-        self.max_dets, self.tag = max_dets, tag
+        self.prev_feat = torch.zeros(batch, H // 16, W // 16, eng.inc[1], dtype=torch.bfloat16, device=dev)
+        self.has_prev = torch.zeros(batch, dtype=torch.int32, device=dev)
+        self.feats = torch.zeros(batch, n_keep, 128, dtype=torch.float32, device=dev)
+        self.n_keep, self.tag = n_keep, tag
 
-    def __call__(self, e, feat, dets, cnt):
-        """feat: the frame's s16 feature, (dets, cnt): its NMS output.  Returns the embedding map."""
+    def __call__(self, e, feat, dets, cnt, gate=None):
+        """feat: the frame's s16 features [B,h,w,C], (dets, cnt): their NMS output.  Returns the embedding maps."""
+        B = feat.shape[0]
         # first frame with detections: pre_dict = cur_dict (:1014-1015); afterwards pre_dict advances only on frames that
         # produced detections (the reference skips its whole tracking block when outputs[0] is None, :1005)
-        ops.copy_rows_if(self.has_prev, feat, self.prev_feat, invert=True)
+        ops.copy_rows_if(self.has_prev, feat, self.prev_feat, invert=True, gate=gate)
         _, f_cur = e.interaction(self.prev_feat, feat)
         emb = e.upsample(f_cur, self.tag)
-        ops.sample_embed(emb, dets, self.max_dets, 8.0, count=cnt, out=self.feats)
-        ops.copy_rows_if(cnt, feat, self.prev_feat)
-        self.has_prev.bitwise_or_((cnt > 0).to(torch.int32))
+        if B == 1:  # the one-image launch on the [A, 7] NMS rows
+            ops.sample_embed(emb, dets.view(-1, 7), self.n_keep, 8.0, count=cnt, out=self.feats[0])
+        else:
+            ops.sample_embed(emb, dets.view(B, -1, 7), self.n_keep, 8.0, count=cnt, out=self.feats)
+        ops.copy_rows_if(cnt, feat, self.prev_feat, gate=gate)
+        started = cnt > 0
+        if gate is not None:
+            started &= gate != 0
+        self.has_prev.bitwise_or_(started.to(torch.int32))
         return emb
 
 
 class _Slot(FrameSlot):
-    """One MOT frame in flight: a frame slot plus its engine buffer tag and its pinned result."""
+    """One MOT step in flight: a frame slot of n_seq images, its engine buffer tag, its pinned results and the step's inputs (which
+    sequences are active, their scales, frame numbers and trackers), staged per slot so that a step in flight never reads the next
+    step's values."""
 
-    def __init__(self, eng, H, W, stream, tag, max_dets, feats):
-        super().__init__(eng, H, W, stream)
-        self.tag = tag
-        self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self.host_dets = torch.zeros(max_dets, 7).pin_memory()
-        self.host_feats = torch.zeros(max_dets, 128).pin_memory() if feats else None
-        self.scale, self.frame_id = 1.0, 0
-        self.warm_u8 = None  # input dtype the slot last ran eagerly with: its next frame with it is captured
-
-
-class UnicornMOTTracker:
-    def __init__(self, engine: UnicornEngine, input_size, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, tracker=None,
-                 assoc="qd", use_graph=False, depth=1):
-        assert assoc in ("qd", "byte")
-        assert depth == 1 or assoc == "byte", "only the ByteTrack arm has independent frames (the QD arm carries the previous s16 feature)"
-        self.eng, self.input_size = engine, tuple(input_size)
-        self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets  # bench.py reads max_dets
-        self.assoc = assoc
-        self.tracker = tracker if tracker is not None else (QuasiDenseEmbedTracker(device=engine.dev) if assoc == "qd" else None)
-        assert self.tracker is not None, "assoc='byte' needs a BYTETracker instance"
-        H, W = self.input_size
-        self._qd = QDEmbedding(engine, H, W, max_dets, "mot.emb") if assoc == "qd" else None
-        self.use_graph, self.depth = use_graph, depth
-        self.frame_id = 0  # frames submitted
-        self._warned = False
-        self.last = {}
-        make = lambda eng, stream, tag="mot": _Slot(eng, H, W, stream, tag, max_dets, assoc == "qd")  # noqa: E731
-        if depth == 1:
-            # two slots on this engine and the current stream, so that submit(t+1) may precede collect(t); they read one input
-            # buffer and share the NMS workspace, each has its own backbone buffers (tag).  Their graphs serve odd / even frames.
-            slots = [make(engine, None, "mot%d" % i) for i in range(2)]
-            slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
-        else:
-            slots = in_flight(engine, depth, make)
-        self._ring = Ring(slots)
-        self._ctxs = slots  # bench.py reads trk._ctxs[i]
-
-    # bench.py writes img_in_u8 and replays _graphs[p][0] (p = 0, 1: the QD arm's parity graphs); tests read ws and feats
-    img_in_u8 = property(lambda self: self._ctxs[0].img_in_u8)
-    _graphs = property(lambda self: [(c.graph, c.last) for c in self._ctxs if c.graph is not None])
-    ws = property(lambda self: self._ctxs[0].ws)
-    feats = property(lambda self: self._qd.feats)
-
-    # ------------------------------------------------------------------------------------------ device half
-    def _frame(self, c):
-        e = c.eng
-        e.begin_frame()
-        fpn, seq = e.backbone(c.img, tag=c.tag)
-        out = e.head(fpn, None, "mot")  # whole mode: zero priors (unicorn.py:133-139)
-        dets, cnt = ops.postprocess_device(out[0], e.ncls, self.conf, self.nms, c.ws)
-        c.last = dict(embed=self._qd(e, seq["feat"], dets, cnt) if self._qd else None, head=out)
-
-    def submit(self, frame, scale=1.0):
-        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3] (4x fewer H2D bytes; the float conversion happens in the stem
-        kernel), host or device.  Enqueues the frame; returns immediately."""
-        c = self._ring.submit()
-        self.frame_id = self._ring.submitted
-        if c.stream is not None:
-            c.stream.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(c.stream):  # None: the current stream
-            c.stage(frame)
-            if c.graph is not None:
-                c.graph.replay()
-            elif self.use_graph and c.warm_u8 == c.u8:
-                # a slot's first frame ran eagerly (plan-time autotuning, buffer allocation, first-frame special case); the second
-                # is captured without a warm-up run: a QD frame advances pre_dict, so it must not run twice
-                c.graph, _ = c.capture(lambda: self._frame(c))
-            else:
-                self._frame(c)
-                c.warm_u8 = c.u8
-            c.host_count.copy_(c.ws.count, non_blocking=True)
-            c.host_dets.copy_(c.ws.dets[:self.max_dets], non_blocking=True)
-            if self._qd:
-                c.host_feats.copy_(self._qd.feats, non_blocking=True)
-            c.scale, c.frame_id = scale, self.frame_id
-            c.event.record()
-        self.last = c.last
-
-    # ------------------------------------------------------------------------------------------ host half
-    def collect(self, img_info=None):
-        """Association of the oldest submitted frame.  QDTrack: (bboxes [n,5] in original-image coordinates, ids [n]);
-        ByteTrack: the list of active STracks (img_info = (height, width) of the original image)."""
-        c = self._ring.collect()
-        c.event.synchronize()
-        total = int(c.host_count[0])
-        if total > self.max_dets and not self._warned:
-            warnings.warn(f"UnicornMOTTracker: {total} detections after NMS, only the {self.max_dets} best are associated "
-                          "(raise max_dets; the reference has no cap)")
-            self._warned = True
-        n = min(total, self.max_dets)
-        d = c.host_dets[:n].clone()
-        if self.assoc == "byte":
-            H, W = self.input_size
-            info = img_info if img_info is not None else (H / c.scale, W / c.scale)
-            return self.tracker.update(d.numpy(), info, (H, W))
-        f = c.host_feats[:n].clone()
-        self.last.update(dets=d, feats=f)
-        return _qd_match(self.tracker, d, f, c.scale, self.score_thr, c.frame_id)
-
-    def step_tensor(self, frame, scale=1.0, img_info=None):
-        """Sequential protocol of the reference: one frame in, its tracks out."""
-        self.submit(frame, scale)
-        return self.collect(img_info)
-
-
-class _BatchSlot(FrameSlot):
-    """One batched MOT step in flight: a frame slot of n_seq images, its engine buffer tag, its pinned results and the step's inputs
-    (which slots are active, their scales, frame numbers and trackers), staged per slot so that a step in flight never reads the
-    next step's values."""
-
-    def __init__(self, eng, H, W, n_seq, tag, n_keep, feats):
-        super().__init__(eng, H, W, batch=n_seq)
+    def __init__(self, eng, H, W, stream, n_seq, tag, n_keep, feats):
+        super().__init__(eng, H, W, stream, batch=n_seq)
         self.tag = tag
         self.host_count = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
         self.host_dets = torch.zeros(n_seq, n_keep, 7).pin_memory()
         self.host_feats = torch.zeros(n_seq, n_keep, 128).pin_memory() if feats else None
         self.host_active = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
-        self.active = torch.zeros(n_seq, dtype=torch.int32, device=eng.dev)  # the step's active table, read by the captured graph
+        self.active = torch.zeros(n_seq, dtype=torch.int32, device=eng.dev)  # the step's active table, read by the captured QD graph
         self.mask, self.scales, self.frame_ids, self.trackers = [False] * n_seq, [1.0] * n_seq, [0] * n_seq, [None] * n_seq
-        self.warm_u8 = None
+        self.warm_u8 = None  # input dtype the slot last ran eagerly with: its next step with it is captured
 
 
 class UnicornMOTBatch:
     """`n_seq` MOT sequences in lock step: one batched frame per step (whole-mode backbone and head, NMS, and for the QD arm the
     conditional pre_dict update, interaction with the previous features, upsample and embedding sampling, all at B = n_seq), optionally
-    captured as one CUDA graph; then each sequence's own tracker on the host.  Each sequence's results equal those of its own
-    UnicornMOTTracker (conf, nms, score_thr, max_dets, assoc and use_graph mean what they mean there).
+    captured as one CUDA graph; then each sequence's own tracker on the host.  Each sequence's results equal those of the same driver
+    at n_seq = 1.
 
     start(i, tracker=None) begins a sequence in slot i at any time (a fresh QuasiDenseEmbedTracker for the QD arm unless one is given;
     the ByteTrack arm needs a BYTETracker); it writes only slot i's state and keeps the graphs.  A slot never started, or inactive in a
     step, runs on whatever its input holds: its pre_dict, first-frame flag, tracker and frame counter are left as they were and its
     result is None, as if its own tracker had not been stepped.
 
-    Protocol as UnicornMOTTracker: submit(frames, scales, active) enqueues a step, collect(img_infos) associates the oldest one;
-    two parity slots let submit(t+1) precede collect(t), so the host association of step t overlaps the device work of step t+1."""
+    submit(frames, scales, active) enqueues a step, collect(img_infos) associates the oldest one.  depth 1: two parity slots on the
+    current stream let submit(t+1) precede collect(t), so the host association of step t overlaps the device work of step t+1.
+    depth > 1 (ByteTrack arm only): that many steps in flight, each on its own stream and engine context."""
 
     def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, assoc="qd",
-                 use_graph=False):
-        if n_seq < 1 or assoc not in ("qd", "byte"):
-            raise ValueError(f"UnicornMOTBatch: n_seq >= 1 and assoc 'qd' or 'byte' (got {n_seq}, {assoc!r})")
+                 use_graph=False, depth=1):
+        if n_seq < 1 or depth < 1 or assoc not in ("qd", "byte"):
+            raise ValueError(f"UnicornMOTBatch: n_seq >= 1, depth >= 1 and assoc 'qd' or 'byte' (got {n_seq}, {depth}, {assoc!r})")
+        if depth > 1 and assoc == "qd":
+            raise ValueError("UnicornMOTBatch: only the ByteTrack arm has independent frames (the QD arm carries the previous s16 feature)")
         self.eng, self.input_size, self.n_seq = engine, tuple(input_size), n_seq
-        self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets
-        self.assoc, self.use_graph = assoc, use_graph
+        self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets  # bench.py reads max_dets
+        self.assoc, self.use_graph, self.depth = assoc, use_graph, depth
         H, W = self.input_size
-        dev = engine.dev
         self.n_keep = min(max_dets, anchor_count(H, W))  # rows a sequence can have after NMS and that are read back
-        qd = assoc == "qd"
-        if qd:  # QDEmbedding's state, one row per sequence
-            self.prev_feat = torch.zeros(n_seq, H // 16, W // 16, engine.inc[1], dtype=torch.bfloat16, device=dev)
-            self.has_prev = torch.zeros(n_seq, dtype=torch.int32, device=dev)
-            self.feats = torch.zeros(n_seq, self.n_keep, 128, dtype=torch.float32, device=dev)
-        # two parity slots on the current stream: one input buffer and one NMS workspace, own backbone buffers (tag) and graph each
-        slots = [_BatchSlot(engine, H, W, n_seq, "motb%d" % i, self.n_keep, qd) for i in range(2)]
-        slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
+        self._qd = QDEmbedding(engine, H, W, self.n_keep, "mot.emb", batch=n_seq) if assoc == "qd" else None
+        make = lambda eng, stream, tag="mot": _Slot(eng, H, W, stream, n_seq, tag, self.n_keep, assoc == "qd")  # noqa: E731
+        if depth == 1:
+            # two parity slots on this engine and the current stream: one input buffer and one NMS workspace, own backbone buffers (tag)
+            # and graph each
+            slots = [make(engine, None, "mot%d" % i) for i in range(2)]
+            slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
+        else:
+            slots = in_flight(engine, depth, make)
         self._ring = Ring(slots)
-        self._ctxs = slots
+        self._ctxs = slots  # bench.py reads trk._ctxs[i]
         self.trackers = [None] * n_seq
         self.frame_ids = [0] * n_seq  # frames each sequence has run since its start()
         self.launches_per_frame = 0
         self.last, self.last_dets, self.last_feats = {}, [None] * n_seq, [None] * n_seq
         self._warned = False
 
+    # bench.py writes img_in_u8 and replays _graphs[p][0] (p = 0, 1: the QD arm's parity graphs)
     img_in_u8 = property(lambda self: self._ctxs[0].img_in_u8)
     _graphs = property(lambda self: [(c.graph, c.last) for c in self._ctxs if c.graph is not None])
     ws = property(lambda self: self._ctxs[0].ws)
+    # the QD arm's device state: pre_dict and first-frame flag per sequence, the sampled embeddings of the latest step
+    prev_feat = property(lambda self: self._qd.prev_feat)
+    has_prev = property(lambda self: self._qd.has_prev)
+    feats = property(lambda self: self._qd.feats)
 
     def start(self, i, tracker=None):
         """Begin a new sequence in slot i: its first-frame flag and frame counter are reset and `tracker` (default: a fresh
@@ -253,28 +161,19 @@ class UnicornMOTBatch:
             if self.assoc == "byte":
                 raise ValueError("UnicornMOTBatch.start: assoc='byte' needs a BYTETracker instance")
             tracker = QuasiDenseEmbedTracker(device=self.eng.dev)
-        if self.assoc == "qd":
-            self.has_prev[i].zero_()  # stream-ordered after the steps in flight
+        if self._qd is not None:
+            self._qd.has_prev[i].zero_()  # stream-ordered after the steps in flight
         self.trackers[i], self.frame_ids[i] = tracker, 0
 
     # ------------------------------------------------------------------------------------------ device half
     def _frame(self, c):
-        e, n = c.eng, self.n_seq
+        e = c.eng
         e.begin_frame()
         fpn, seq = e.backbone(c.img, tag=c.tag)
-        out = e.head(fpn, None, "mot")  # [n, A, 5+ncls]
-        dets, cnt = ops.postprocess_device(out, e.ncls, self.conf, self.nms, c.ws)
-        embed = None
-        if self.assoc == "qd":
-            # QDEmbedding per slot: pre_dict = cur_dict on a slot's first frame with detections, afterwards only on frames with
-            # detections; the gate keeps an idle slot's pre_dict and first-frame flag
-            feat = seq["feat"]
-            ops.copy_rows_if(self.has_prev, feat, self.prev_feat, invert=True, gate=c.active)
-            _, f_cur = e.interaction(self.prev_feat, feat)
-            embed = e.upsample(f_cur, "motb.emb")
-            ops.sample_embed(embed, dets.view(n, -1, 7), self.n_keep, 8.0, count=cnt, out=self.feats)
-            ops.copy_rows_if(cnt, feat, self.prev_feat, gate=c.active)
-            self.has_prev.bitwise_or_(((cnt > 0) & (c.active != 0)).to(torch.int32))
+        out = e.head(fpn, None, "mot")  # whole mode: zero priors (unicorn.py:133-139); [n_seq, A, 5+ncls]
+        dets, cnt = ops.postprocess_device(out if self.n_seq > 1 else out[0], e.ncls, self.conf, self.nms, c.ws)
+        # one sequence needs no gate: a step without an active sequence does not run (submit)
+        embed = self._qd(e, seq["feat"], dets, cnt, gate=c.active if self.n_seq > 1 else None) if self._qd is not None else None
         c.last = dict(embed=embed, head=out)
 
     def _check(self, frames, scales, active):
@@ -290,41 +189,52 @@ class UnicornMOTBatch:
             raise ValueError(f"UnicornMOTBatch: active has {len(active)} entries for {n} sequences")
 
     def submit(self, frames, scales=None, active=None):
-        """frames: preprocessed fp32 [n_seq,3,H,W] or uint8 [n_seq,H,W,3], host or device; scales: n_seq letterbox ratios (default
-        1); active: n_seq flags (default: every started slot).  Enqueues the step; returns immediately."""
+        """frames: preprocessed fp32 [n_seq,3,H,W] or uint8 [n_seq,H,W,3] (4x fewer H2D bytes; the float conversion happens in the stem
+        kernel), host or device; scales: n_seq letterbox ratios (default 1); active: n_seq flags (default: every started slot).
+        Enqueues the step; returns immediately."""
         self._check(frames, scales, active)
         n = self.n_seq
+        mask = [self.trackers[i] is not None and (active is None or bool(active[i])) for i in range(n)]
         c = self._ring.submit()
-        u8, graph = c.u8, c.graph
-        try:
-            c.stage(frames)  # the last step that can fail (e.g. frames on another device): nothing has changed before it
-        except BaseException:
-            self._ring.submitted -= 1
-            c.u8, c.graph = u8, graph
-            raise
-        c.mask = [self.trackers[i] is not None and (active is None or bool(active[i])) for i in range(n)]
-        for i in range(n):
-            self.frame_ids[i] += c.mask[i]
-        c.scales = [1.0] * n if scales is None else [float(s) for s in scales]
-        c.frame_ids, c.trackers = list(self.frame_ids), list(self.trackers)
-        # the slot's previous step was collected, so its pinned staging buffer is free again
-        c.host_active.copy_(torch.tensor(c.mask, dtype=torch.int32))
-        c.active.copy_(c.host_active, non_blocking=True)
-        if c.graph is not None:
-            c.graph.replay()
-        elif self.use_graph and c.warm_u8 == c.u8:
-            # first step of a slot eager, second captured without a warm-up: a QD step advances pre_dict, so it must not run twice
-            c.graph, self.launches_per_frame = c.capture(lambda: self._frame(c))
-        else:
-            l0 = _lib.LAUNCHES
-            self._frame(c)
-            self.launches_per_frame = _lib.LAUNCHES - l0
-            c.warm_u8 = c.u8
-        c.host_count.copy_(c.ws.count, non_blocking=True)
-        c.host_dets.copy_(c.ws.dets.view(n, -1, 7)[:, :self.n_keep], non_blocking=True)
-        if self.assoc == "qd":
-            c.host_feats.copy_(self.feats, non_blocking=True)
-        c.event.record()
+        if not any(mask):  # no sequence to step: nothing is launched and every result is None
+            c.mask = mask
+            c.event.record()
+            return
+        if c.stream is not None:
+            c.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(c.stream):  # None: the current stream
+            u8, graph = c.u8, c.graph
+            try:
+                c.stage(frames)  # the last step that can fail (e.g. frames on another device): nothing has changed before it
+            except BaseException:
+                self._ring.submitted -= 1
+                c.u8, c.graph = u8, graph
+                raise
+            c.mask = mask
+            for i in range(n):
+                self.frame_ids[i] += c.mask[i]
+            c.scales = [1.0] * n if scales is None else [float(s) for s in scales]
+            c.frame_ids, c.trackers = list(self.frame_ids), list(self.trackers)
+            if self._qd is not None and n > 1:
+                # the slot's previous step was collected, so its pinned staging buffer is free again
+                c.host_active.copy_(torch.tensor(c.mask, dtype=torch.int32))
+                c.active.copy_(c.host_active, non_blocking=True)
+            if c.graph is not None:
+                c.graph.replay()
+            elif self.use_graph and c.warm_u8 == c.u8:
+                # a slot's first step ran eagerly (plan-time autotuning, buffer allocation, first-frame special case); the second is
+                # captured without a warm-up run: a QD step advances pre_dict, so it must not run twice
+                c.graph, self.launches_per_frame = c.capture(lambda: self._frame(c))
+            else:
+                l0 = _lib.LAUNCHES
+                self._frame(c)
+                self.launches_per_frame = _lib.LAUNCHES - l0
+                c.warm_u8 = c.u8
+            c.host_count.copy_(c.ws.count, non_blocking=True)
+            c.host_dets.copy_(c.ws.dets.view(n, -1, 7)[:, :self.n_keep], non_blocking=True)
+            if self._qd is not None:
+                c.host_feats.copy_(self._qd.feats, non_blocking=True)
+            c.event.record()
         self.last = c.last
 
     # ------------------------------------------------------------------------------------------ host half
@@ -362,3 +272,40 @@ class UnicornMOTBatch:
         """Sequential protocol: one step in, its n_seq results out."""
         self.submit(frames, scales, active)
         return self.collect(img_infos)
+
+
+class UnicornMOTTracker:
+    """One MOT sequence: UnicornMOTBatch at n_seq = 1 (same arguments) with its slot started on `tracker`, under the reference's
+    one-sequence protocol.  last: the device tensors of the latest submitted frame (embed, head) and the NMS rows / embeddings the
+    tracker was given at the latest collect() (dets, feats)."""
+
+    def __init__(self, engine: UnicornEngine, input_size, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, tracker=None,
+                 assoc="qd", use_graph=False, depth=1):
+        self._b = UnicornMOTBatch(engine, input_size, 1, conf, nms, score_thr, max_dets, assoc, use_graph, depth)
+        self._b.start(0, tracker)
+        self.tracker = self._b.trackers[0]
+
+    max_dets = property(lambda self: self._b.max_dets)
+    _ctxs = property(lambda self: self._b._ctxs)
+    img_in_u8 = property(lambda self: self._b.img_in_u8)
+    _graphs = property(lambda self: self._b._graphs)
+    ws = property(lambda self: self._b.ws)
+    feats = property(lambda self: self._b._qd.feats[0])
+    frame_id = property(lambda self: self._b.frame_ids[0])  # frames submitted
+    last = property(lambda self: self._b.last)
+
+    def submit(self, frame, scale=1.0):
+        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device.  Enqueues the frame; returns immediately."""
+        self._b.submit(frame, [scale])
+
+    def collect(self, img_info=None):
+        """Association of the oldest submitted frame.  QDTrack: (bboxes [n,5] in original-image coordinates, ids [n]);
+        ByteTrack: the list of active STracks (img_info = (height, width) of the original image)."""
+        res = self._b.collect(None if img_info is None else [img_info])[0]
+        self.last.update(dets=self._b.last_dets[0], feats=self._b.last_feats[0])
+        return res
+
+    def step_tensor(self, frame, scale=1.0, img_info=None):
+        """Sequential protocol of the reference: one frame in, its tracks out."""
+        self.submit(frame, scale)
+        return self.collect(img_info)

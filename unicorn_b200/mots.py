@@ -141,7 +141,7 @@ class UnicornMOTSTracker:
             c.warm_u8 = c.u8
         c.host_count.copy_(c.ws.count, non_blocking=True)
         c.host_dets.copy_(c.ws.dets[:self.max_dets], non_blocking=True)
-        c.host_feats.copy_(self._qd.feats, non_blocking=True)
+        c.host_feats.copy_(self._qd.feats[0], non_blocking=True)
         c.frame_id, c.img_hw = self.frame_id, (img_h, img_w)
         c.event.record()
         self.last = c.last
