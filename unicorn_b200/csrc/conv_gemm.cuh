@@ -101,6 +101,17 @@ struct alignas(64) ConvKernelParams {
   int gn_groups, gn_gs;  // gs = Cout / groups
 };
 
+// 64-bit add to shared memory as two native 32-bit atomics.  sm_90 has no 64-bit shared-memory atomic add: atomicAdd on a 64-bit
+// shared word compiles to a compare-and-swap loop, which serializes the lanes of all warps that add to one GroupNorm slot.  The lane
+// whose add wraps the low word adds the carry to the high word, so once every adder is done (the barrier before the slot is read)
+// the slot holds the exact sum modulo 2^64, the same bits as 64-bit atomics in any order.
+__device__ __forceinline__ void smem_add_u64(unsigned long long* slot, unsigned long long v) {
+  unsigned int* w = reinterpret_cast<unsigned int*>(slot);
+  const unsigned int lo = static_cast<unsigned int>(v);
+  const unsigned int old = atomicAdd(w, lo);
+  atomicAdd(w + 1, static_cast<unsigned int>(v >> 32) + (old + lo < old ? 1u : 0u));
+}
+
 // Persistent kernel: grid = min(#tiles, SMs); every CTA (pair) walks work items item = blockIdx.x / CLUSTER + i * gridDim.x / CLUSTER
 // (N tile fastest, so CTAs running side by side share the activation tile in L2); item = (N tile, group of CLUSTER M tiles).
 template <int BLOCK_N, int STAGES, bool F16, int CLUSTER, int EPI>
@@ -318,8 +329,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           }
           if (g == 0) {
             unsigned long long* slot = gacc + s_grp[cl + j] * 2;
-            atomicAdd(slot, static_cast<unsigned long long>(__float2ll_rn(gs1[j] * kGnFixedScale)));
-            atomicAdd(slot + 1, static_cast<unsigned long long>(__float2ll_rn(gs2[j] * kGnFixedScale)));
+            smem_add_u64(slot, static_cast<unsigned long long>(__float2ll_rn(gs1[j] * kGnFixedScale)));
+            smem_add_u64(slot + 1, static_cast<unsigned long long>(__float2ll_rn(gs2[j] * kGnFixedScale)));
           }
           gs1[j] = gs2[j] = 0.f;
         }
