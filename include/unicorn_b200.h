@@ -332,6 +332,19 @@ UC_API int uc_mots_encode(const float* masks, int n_max, int Hin, int Win, const
                           double r, int H, int W, void* workspace, long workspace_bytes, char* chars, long capacity,
                           long long* offsets, void* stream);
 
+/* uc_mots_encode over the instances of B images (1 <= B <= UC_MOTS_MAX_IMAGES) in one set of launches: each image has its own
+ * original size H[b] x W[b], letterbox ratio r[b] and k[b] instances (0 <= k[b] <= n_max); k, H, W and r are HOST arrays of B.
+ * masks: f32 image b at masks + b * bs_masks, [n_max,Hin,Win] (the uc_dynamic_masks_batched output).  order / emit: device, one flat
+ * list of K = sum k[b] entries grouped by image; image b's order entries are mask rows within its own block.  Overlap removal stays
+ * within an image.  offsets: device int64 [K+1] over all images, so image b's strings are contiguous; every string is byte-identical
+ * to a uc_mots_encode call on that image alone (that call's offsets are image b's minus offsets[k[0] + ... + k[b-1]]).  chars and
+ * capacity as in uc_mots_encode.  workspace: uc_mots_encode_workspace_bytes(K, max H[b], max W[b]) bytes suffice.  No allocation,
+ * no synchronisation, graph-capturable; three launches for K > 0, one for K = 0. */
+#define UC_MOTS_MAX_IMAGES 64
+UC_API int uc_mots_encode_batched(const float* masks, long bs_masks, int n_max, int Hin, int Win, int B, const int* k, const int* H,
+                                  const int* W, const double* r, const int* order, const uint8_t* emit, float thr, void* workspace,
+                                  long workspace_bytes, char* chars, long capacity, long long* offsets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

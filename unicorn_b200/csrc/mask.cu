@@ -8,7 +8,9 @@
 #include "uc_common.h"
 #include "../../include/unicorn_b200.h"
 #include <algorithm>
+#include <climits>
 #include <cmath>
+#include <cstdio>
 
 namespace uc {
 
@@ -271,22 +273,24 @@ __global__ void __launch_bounds__(256) vos_aggregate_kernel(VosObjs o, int Hin, 
 // (x, wy) holds rows 32 wy .. 32 wy + 31 of column x.  The runs start with the zero run, so a run ends at every pixel whose bit
 // differs from the previous one (pixel -1 counts as 0) and at P; pass 1 stores exactly those boundary bits.
 constexpr int kMotsThreads = 1024;
+constexpr int kMotsMaxImages = UC_MOTS_MAX_IMAGES;
 
 struct MotsWs {
-  uint32_t* diff;      // [k][words] run boundaries of the emitted instances
+  uint32_t* diff;      // run boundaries of the emitted instances, [k_b][words_b] per image, the images one after another
   int4* state;         // [k][kMotsThreads] run state before each thread's chunk of words
   int* char_off;       // [k][kMotsThreads] chars before each thread's chunk, within the instance
   long long* nchars;   // [k] chars of each instance (0 when not emitted)
 };
 static inline long align16(long b) { return (b + 15) & ~15L; }
-static long mots_workspace_bytes(int k, long words) {
-  return align16(4L * k * words) + align16(16L * k * kMotsThreads) + align16(4L * k * kMotsThreads) + align16(8L * k);
+// k instances in all, diff_words boundary words in all
+static long mots_workspace_bytes(int k, long diff_words) {
+  return align16(4L * diff_words) + align16(16L * k * kMotsThreads) + align16(4L * k * kMotsThreads) + align16(8L * k);
 }
-static MotsWs mots_ws(void* base, int k, long words) {
+static MotsWs mots_ws(void* base, int k, long diff_words) {
   char* p = static_cast<char*>(base);
   MotsWs w;
   w.diff = reinterpret_cast<uint32_t*>(p);
-  p += align16(4L * k * words);
+  p += align16(4L * diff_words);
   w.state = reinterpret_cast<int4*>(p);
   p += align16(16L * k * kMotsThreads);
   w.char_off = reinterpret_cast<int*>(p);
@@ -295,17 +299,44 @@ static MotsWs mots_ws(void* base, int k, long words) {
   return w;
 }
 
-// Pass 1: one thread per word, looping over the instances in `order`; the 32 lanes of a warp take 32 neighbouring columns of the
-// same rows, so their bilinear taps share source rows.  The pixel before the word is resampled too, so the boundary bits of the
-// word need no neighbour.
-__global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restrict__ masks, int n_max, int Hin, int Win,
-                                                          const int* __restrict__ order, const uint8_t* __restrict__ emit, int k, float thr,
-                                                          int hm, int wm, float scale, MotsWs ws) {
+// The images of one encode, passed by value: image b owns instances [k0[b], k0[b + 1]) of the flat order / emit lists, its masks
+// are resized to hm[b] x wm[b] with source scale[b], and instance j of it keeps its boundary words at
+// diff0[b] + (j - k0[b]) * wm[b] * ceil(hm[b] / 32) in MotsWs::diff.
+struct MotsImages {
+  int n;
+  int k0[kMotsMaxImages + 1];
+  int hm[kMotsMaxImages], wm[kMotsMaxImages];
+  float scale[kMotsMaxImages];
+  long diff0[kMotsMaxImages];
+};
+// The resized size and boundary words of instance j's image; returns the instance's boundary words.
+__device__ __forceinline__ const uint32_t* mots_instance(const MotsImages& im, const MotsWs& ws, int j, int& hm, int& wm, int& hw32,
+                                                         long& words) {
+  int b = 0;
+  while (j >= im.k0[b + 1]) ++b;
+  hm = im.hm[b];
+  wm = im.wm[b];
+  hw32 = (hm + 31) / 32;
+  words = static_cast<long>(wm) * hw32;
+  return ws.diff + im.diff0[b] + (j - im.k0[b]) * words;
+}
+
+// Pass 1: one thread per word of image blockIdx.z, looping over the image's instances in `order`; the 32 lanes of a warp take 32
+// neighbouring columns of the same rows, so their bilinear taps share source rows.  The pixel before the word is resampled too, so
+// the boundary bits of the word need no neighbour.
+__global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restrict__ masks, long bs_masks, int n_max, int Hin, int Win,
+                                                          const int* __restrict__ order, const uint8_t* __restrict__ emit, float thr,
+                                                          const __grid_constant__ MotsImages im, MotsWs ws) {
   pdl_wait();
   pdl_launch_dependents();
+  const int b = blockIdx.z, hm = im.hm[b], wm = im.wm[b];
+  const float scale = im.scale[b];
   const int x = blockIdx.x * 32 + threadIdx.x, wy = blockIdx.y * 8 + threadIdx.y, hw32 = (hm + 31) / 32;
   if (x >= wm || wy >= hw32) return;
   const long words = static_cast<long>(wm) * hw32;
+  masks += b * bs_masks;
+  const int j0 = im.k0[b], j1 = im.k0[b + 1];
+  uint32_t* diff = ws.diff + im.diff0[b];
   int x0, x1;
   float lx;
   resize_src(x, scale, Win, x0, x1, lx);
@@ -320,7 +351,7 @@ __global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restric
   const uint32_t valid = nrows == 32 ? ~0u : (1u << nrows) - 1u;
   uint32_t acc = 0, accp = 0;  // pixels claimed by the original masks of the earlier instances
 #pragma unroll 1
-  for (int j = 0; j < k; ++j) {
+  for (int j = j0; j < j1; ++j) {
     const int row = order[j];
     uint32_t raw = 0, rawp = 0;
     if (row >= 0 && row < n_max) {  // a row outside the mask buffer reads as an empty mask
@@ -337,7 +368,7 @@ __global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restric
     const uint32_t fr = raw & ~acc, frp = rawp & ~accp;
     acc |= raw;
     accp |= rawp;
-    if (emit[j]) ws.diff[j * words + static_cast<long>(x) * hw32 + wy] = (fr ^ ((fr << 1) | frp)) & valid;
+    if (emit[j]) diff[(j - j0) * words + static_cast<long>(x) * hw32 + wy] = (fr ^ ((fr << 1) | frp)) & valid;
   }
 }
 
@@ -404,9 +435,10 @@ __device__ __forceinline__ int4 mots_walk(const uint32_t* __restrict__ d, long w
   return s;
 }
 
-// Pass 2: one block per instance; each thread owns a contiguous chunk of words.  Scan of the run states over the chunks, then the
-// number of chars of every count, scanned into each chunk's char offset.
-__global__ void __launch_bounds__(kMotsThreads) mots_runs_kernel(const uint8_t* __restrict__ emit, int k, int hm, int wm, MotsWs ws) {
+// Pass 2: one block per instance of any image; each thread owns a contiguous chunk of words.  Scan of the run states over the
+// chunks, then the number of chars of every count, scanned into each chunk's char offset.
+__global__ void __launch_bounds__(kMotsThreads) mots_runs_kernel(const uint8_t* __restrict__ emit, const __grid_constant__ MotsImages im,
+                                                                 MotsWs ws) {
   pdl_wait();
   pdl_launch_dependents();
   __shared__ int4 sh_state[kMotsThreads];
@@ -416,31 +448,34 @@ __global__ void __launch_bounds__(kMotsThreads) mots_runs_kernel(const uint8_t* 
     if (t == 0) ws.nchars[j] = 0;
     return;
   }
-  const int hw32 = (hm + 31) / 32;
-  const long words = static_cast<long>(wm) * hw32, chunk = (words + kMotsThreads - 1) / kMotsThreads;
+  int hm, wm, hw32;
+  long words;
+  const uint32_t* d = mots_instance(im, ws, j, hm, wm, hw32, words);
+  const long chunk = (words + kMotsThreads - 1) / kMotsThreads;
   const long w0 = std::min(words, t * chunk), w1 = std::min(words, w0 + chunk);
-  const uint32_t* d = ws.diff + j * words;
   const int4 none = make_int4(0, -1, -1, -1);
   const int4 mine = mots_walk(d, w0, w1, hm, hw32, none, [](int, int4) {});
   int4 all;
   const int4 pre = block_exclusive_scan(mine, none, [](int4 a, int4 b) { return run_cat(a, b); }, sh_state, all);
-  ws.state[j * kMotsThreads + t] = pre;
+  ws.state[static_cast<long>(j) * kMotsThreads + t] = pre;
   long long n = 0;
   mots_walk(d, w0, w1, hm, hw32, pre, [&](int pos, int4 s) { n += rle_chars(run_delta(s, pos), nullptr, 0, 0); });
   if (t == kMotsThreads - 1) n += rle_chars(run_delta(all, hm * wm), nullptr, 0, 0);  // the last run ends at P
   long long total;
   const long long off = block_exclusive_scan(n, 0LL, [](long long a, long long b) { return a + b; }, sh_chars, total);
-  ws.char_off[j * kMotsThreads + t] = static_cast<int>(off);
+  ws.char_off[static_cast<long>(j) * kMotsThreads + t] = static_cast<int>(off);
   if (t == 0) ws.nchars[j] = total;
 }
 
-// Pass 3: the offsets of the k strings (block 0) and the chars of every emitted instance (block j), clipped at the capacity.
-__global__ void __launch_bounds__(kMotsThreads) mots_chars_kernel(const uint8_t* __restrict__ emit, int k, int hm, int wm, MotsWs ws,
-                                                                  char* __restrict__ chars, long capacity, long long* __restrict__ offsets) {
+// Pass 3: the offsets of the k strings of all images (block 0) and the chars of every emitted instance (block j), clipped at the
+// capacity.
+__global__ void __launch_bounds__(kMotsThreads) mots_chars_kernel(const uint8_t* __restrict__ emit, const __grid_constant__ MotsImages im,
+                                                                  MotsWs ws, char* __restrict__ chars, long capacity,
+                                                                  long long* __restrict__ offsets) {
   pdl_wait();
   pdl_launch_dependents();
   __shared__ long long base;
-  const int j = blockIdx.x, t = threadIdx.x;
+  const int j = blockIdx.x, t = threadIdx.x, k = im.k0[im.n];
   if (t == 0) {
     long long b = 0;
     for (int i = 0; i < k; ++i) {
@@ -452,11 +487,13 @@ __global__ void __launch_bounds__(kMotsThreads) mots_chars_kernel(const uint8_t*
   }
   __syncthreads();
   if (j >= k || !emit[j]) return;
-  const int hw32 = (hm + 31) / 32;
-  const long words = static_cast<long>(wm) * hw32, chunk = (words + kMotsThreads - 1) / kMotsThreads;
+  int hm, wm, hw32;
+  long words;
+  const uint32_t* d = mots_instance(im, ws, j, hm, wm, hw32, words);
+  const long chunk = (words + kMotsThreads - 1) / kMotsThreads;
   const long w0 = std::min(words, t * chunk), w1 = std::min(words, w0 + chunk);
-  long long off = base + ws.char_off[j * kMotsThreads + t];
-  const int4 end = mots_walk(ws.diff + j * words, w0, w1, hm, hw32, ws.state[j * kMotsThreads + t],
+  long long off = base + ws.char_off[static_cast<long>(j) * kMotsThreads + t];
+  const int4 end = mots_walk(d, w0, w1, hm, hw32, ws.state[static_cast<long>(j) * kMotsThreads + t],
                              [&](int pos, int4 s) { off += rle_chars(run_delta(s, pos), chars, off, capacity); });
   if (t == kMotsThreads - 1) rle_chars(run_delta(end, hm * wm), chars, off, capacity);
 }
@@ -571,35 +608,82 @@ extern "C" int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win
   return check_launch("uc_vos_aggregate");
 }
 
+// One encode over the instances of B images (B = 1: uc_mots_encode).  Every argument is validated before any CUDA call, with errors
+// prefixed by `what`, and by the image when the call is batched.
+static int mots_encode(const char* what, bool batched, const float* masks, long bs_masks, int n_max, int Hin, int Win, int B, const int* k,
+                       const int* H, const int* W, const double* r, const int* order, const uint8_t* emit, float thr, void* workspace,
+                       long workspace_bytes, char* chars, long capacity, long long* offsets, cudaStream_t stream) {
+  if (!k || !H || !W || !r) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1 || B > kMotsMaxImages) return set_error(UC_EINVAL, "%s: B = %d must be in 1..%d", what, B, kMotsMaxImages);
+  long K = 0;
+  for (int b = 0; b < B; ++b) K += std::max(k[b], 0);
+  if (K > INT_MAX) return set_error(UC_EINVAL, "%s: more than %d instances", what, INT_MAX);
+  if (!masks || !order || !emit || !offsets || (K > 0 && !workspace) || (capacity > 0 && !chars))
+    return set_error(UC_EINVAL, "%s: null pointer", what);
+  char at[96];
+  auto image = [&](int b) {
+    if (batched) snprintf(at, sizeof(at), "%s: image %d", what, b);
+    else snprintf(at, sizeof(at), "%s", what);
+    return at;
+  };
+  if (n_max < 1 || Hin < 1 || Win < 1) return set_error(UC_EINVAL, "%s: bad sizes", what);
+  if (bs_masks < static_cast<long>(n_max) * Hin * Win)
+    return set_error(UC_EINVAL, "%s: bad per-image stride %ld (>= n_max*Hin*Win = %ld)", what, bs_masks, static_cast<long>(n_max) * Hin * Win);
+  for (int b = 0; b < B; ++b)
+    if (H[b] < 1 || W[b] < 1 || !(r[b] > 0.0)) return set_error(UC_EINVAL, "%s: bad sizes", image(b));
+  for (int b = 0; b < B; ++b)
+    if (k[b] < 0 || k[b] > n_max) return set_error(UC_EINVAL, "%s: k = %d must be in 0..n_max (%d)", image(b), k[b], n_max);
+  if (capacity < 0) return set_error(UC_EINVAL, "%s: negative capacity", what);
+  if ((reinterpret_cast<uintptr_t>(masks) | reinterpret_cast<uintptr_t>(order)) % 4 || reinterpret_cast<uintptr_t>(offsets) % 8 ||
+      reinterpret_cast<uintptr_t>(workspace) % 16)
+    return set_error(UC_EINVAL, "%s: masks / order must be 4-byte, offsets 8-byte, workspace 16-byte aligned", what);
+  MotsImages im;
+  im.n = B;
+  im.k0[0] = 0;
+  long diff_words = 0;
+  int wm_max = 0, hw32_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const FrameResize rs = frame_resize(Hin, Win, H[b], W[b], r[b]);
+    if (rs.hm < 1 || rs.wm < 1) return set_error(UC_EINVAL, "%s: the resized mask is empty (r too large)", image(b));
+    const int hw32 = (rs.hm + 31) / 32;
+    const long words = static_cast<long>(rs.wm) * hw32;
+    if (words > (1L << 31) / 32) return set_error(UC_EINVAL, "%s: frame too large", image(b));
+    im.k0[b + 1] = im.k0[b] + k[b];
+    im.hm[b] = rs.hm;
+    im.wm[b] = rs.wm;
+    im.scale[b] = rs.scale;
+    im.diff0[b] = diff_words;
+    diff_words += k[b] * words;
+    wm_max = std::max(wm_max, rs.wm);
+    hw32_max = std::max(hw32_max, hw32);
+  }
+  if (workspace_bytes < mots_workspace_bytes(static_cast<int>(K), diff_words)) return set_error(UC_EINVAL, "%s: workspace too small", what);
+  MotsWs ws = mots_ws(workspace, static_cast<int>(K), diff_words);
+  if (K > 0) {
+    launch_pdl(mots_planes_kernel, dim3((wm_max + 31) / 32, (hw32_max + 7) / 8, B), dim3(32, 8), 0, stream, masks, bs_masks, n_max, Hin, Win,
+               order, emit, thr, im, ws);
+    launch_pdl(mots_runs_kernel, static_cast<int>(K), kMotsThreads, 0, stream, emit, im, ws);
+  }
+  launch_pdl(mots_chars_kernel, std::max(static_cast<int>(K), 1), kMotsThreads, 0, stream, emit, im, ws, chars, capacity, offsets);
+  return check_launch(what);
+}
+
 extern "C" long uc_mots_encode_workspace_bytes(int k_max, int H, int W) {
   if (k_max < 0 || H < 1 || W < 1) return -1;
-  return mots_workspace_bytes(k_max, W * ((H + 31) / 32));
+  return mots_workspace_bytes(k_max, static_cast<long>(k_max) * W * ((H + 31) / 32));
 }
 
 extern "C" int uc_mots_encode(const float* masks, int n_max, int Hin, int Win, const int* order, const uint8_t* emit, int k, float thr,
                               double r, int H, int W, void* workspace, long workspace_bytes, char* chars, long capacity,
                               long long* offsets, void* stream_v) {
-  if (!masks || !order || !emit || !offsets || (k > 0 && !workspace) || (capacity > 0 && !chars))
-    return set_error(UC_EINVAL, "uc_mots_encode: null pointer");
-  if (n_max < 1 || Hin < 1 || Win < 1 || H < 1 || W < 1 || !(r > 0.0)) return set_error(UC_EINVAL, "uc_mots_encode: bad sizes");
-  if (k < 0 || k > n_max) return set_error(UC_EINVAL, "uc_mots_encode: k = %d must be in 0..n_max (%d)", k, n_max);
-  if (capacity < 0) return set_error(UC_EINVAL, "uc_mots_encode: negative capacity");
-  if ((reinterpret_cast<uintptr_t>(masks) | reinterpret_cast<uintptr_t>(order)) % 4 || reinterpret_cast<uintptr_t>(offsets) % 8 ||
-      reinterpret_cast<uintptr_t>(workspace) % 16)
-    return set_error(UC_EINVAL, "uc_mots_encode: masks / order must be 4-byte, offsets 8-byte, workspace 16-byte aligned");
-  const FrameResize rs = frame_resize(Hin, Win, H, W, r);
-  if (rs.hm < 1 || rs.wm < 1) return set_error(UC_EINVAL, "uc_mots_encode: the resized mask is empty (r too large)");
-  const int hw32 = (rs.hm + 31) / 32;
-  const long words = static_cast<long>(rs.wm) * hw32;
-  if (words > (1L << 31) / 32) return set_error(UC_EINVAL, "uc_mots_encode: frame too large");
-  if (workspace_bytes < mots_workspace_bytes(k, words)) return set_error(UC_EINVAL, "uc_mots_encode: workspace too small");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  MotsWs ws = mots_ws(workspace, k, words);
-  if (k > 0) {
-    launch_pdl(mots_planes_kernel, dim3((rs.wm + 31) / 32, (hw32 + 7) / 8), dim3(32, 8), 0, stream, masks, n_max, Hin, Win, order, emit, k, thr,
-               rs.hm, rs.wm, rs.scale, ws);
-    launch_pdl(mots_runs_kernel, k, kMotsThreads, 0, stream, emit, k, rs.hm, rs.wm, ws);
-  }
-  launch_pdl(mots_chars_kernel, std::max(k, 1), kMotsThreads, 0, stream, emit, k, rs.hm, rs.wm, ws, chars, capacity, offsets);
-  return check_launch("uc_mots_encode");
+  return mots_encode("uc_mots_encode", false, masks, static_cast<long>(std::max(n_max, 0)) * std::max(Hin, 0) * std::max(Win, 0), n_max, Hin,
+                     Win, 1, &k, &H, &W, &r, order, emit, thr, workspace, workspace_bytes, chars, capacity, offsets,
+                     static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_mots_encode_batched(const float* masks, long bs_masks, int n_max, int Hin, int Win, int B, const int* k, const int* H,
+                                      const int* W, const double* r, const int* order, const uint8_t* emit, float thr, void* workspace,
+                                      long workspace_bytes, char* chars, long capacity, long long* offsets, void* stream_v) {
+  return mots_encode("uc_mots_encode_batched", true, masks, bs_masks, n_max, Hin, Win, B, k, H, W, r, order, emit, thr, workspace,
+                     workspace_bytes, chars, capacity, offsets, static_cast<cudaStream_t>(stream_v));
 }

@@ -114,6 +114,8 @@ class UnicornMOTBatch:
     current stream let submit(t+1) precede collect(t), so the host association of step t overlaps the device work of step t+1.
     depth > 1 (ByteTrack arm only): that many steps in flight, each on its own stream and engine context."""
 
+    _tag = "mot"  # engine buffer tag of the driver's activations
+
     def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, assoc="qd",
                  use_graph=False, depth=1):
         if n_seq < 1 or depth < 1 or assoc not in ("qd", "byte"):
@@ -125,12 +127,12 @@ class UnicornMOTBatch:
         self.assoc, self.use_graph, self.depth = assoc, use_graph, depth
         H, W = self.input_size
         self.n_keep = min(max_dets, anchor_count(H, W))  # rows a sequence can have after NMS and that are read back
-        self._qd = QDEmbedding(engine, H, W, self.n_keep, "mot.emb", batch=n_seq) if assoc == "qd" else None
-        make = lambda eng, stream, tag="mot": _Slot(eng, H, W, stream, n_seq, tag, self.n_keep, assoc == "qd")  # noqa: E731
+        self._qd = QDEmbedding(engine, H, W, self.n_keep, self._tag + ".emb", batch=n_seq) if assoc == "qd" else None
+        make = lambda eng, stream, tag=self._tag: _Slot(eng, H, W, stream, n_seq, tag, self.n_keep, assoc == "qd")  # noqa: E731
         if depth == 1:
             # two parity slots on this engine and the current stream: one input buffer and one NMS workspace, own backbone buffers (tag)
             # and graph each
-            slots = [make(engine, None, "mot%d" % i) for i in range(2)]
+            slots = [make(engine, None, "%s%d" % (self._tag, i)) for i in range(2)]
             slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
         else:
             slots = in_flight(engine, depth, make)
@@ -182,11 +184,11 @@ class UnicornMOTBatch:
                                           (frames.dtype == torch.float32 and tuple(frames.shape) == (n, 3, H, W)))
         if not ok:
             got = (tuple(frames.shape), frames.dtype) if torch.is_tensor(frames) else type(frames)
-            raise ValueError(f"UnicornMOTBatch: frames must be uint8 [{n},{H},{W},3] or float32 [{n},3,{H},{W}], got {got}")
+            raise ValueError(f"{type(self).__name__}: frames must be uint8 [{n},{H},{W},3] or float32 [{n},3,{H},{W}], got {got}")
         if scales is not None and len(scales) != n:
-            raise ValueError(f"UnicornMOTBatch: {len(scales)} scales for {n} sequences")
+            raise ValueError(f"{type(self).__name__}: {len(scales)} scales for {n} sequences")
         if active is not None and len(active) != n:
-            raise ValueError(f"UnicornMOTBatch: active has {len(active)} entries for {n} sequences")
+            raise ValueError(f"{type(self).__name__}: active has {len(active)} entries for {n} sequences")
 
     def submit(self, frames, scales=None, active=None):
         """frames: preprocessed fp32 [n_seq,3,H,W] or uint8 [n_seq,H,W,3] (4x fewer H2D bytes; the float conversion happens in the stem

@@ -578,14 +578,31 @@ def mots_encode_workspace(k_max, H, W, device):
     return torch.empty(fn(int(k_max), int(H), int(W)), dtype=torch.uint8, device=device)
 
 
-def mots_encode(masks, order, emit, thr, r, H, W, ws, chars, offsets):
+def mots_encode(masks, order, emit, thr, r, H, W, ws, chars, offsets, k=None):
     """COCO RLE strings of the resized, thresholded, overlap-free masks of one MOTS frame (uc_mots_encode).  masks fp32
     [n_max,Hin,Win]; order int32 [k] / emit uint8 [k] device; chars uint8 device buffer (its size is the capacity); offsets int64
-    device [>= k+1].  Launches only: offsets[k] is the number of chars needed, chars past the capacity are not written."""
-    n_max, Hin, Win = masks.shape
-    k = order.numel()
-    assert masks.dtype == torch.float32 and masks.is_contiguous() and order.dtype == torch.int32 and emit.dtype == torch.uint8
-    assert emit.numel() == k and chars.dtype == torch.uint8 and offsets.dtype == torch.int64 and offsets.numel() >= k + 1
-    _lib.check(_L().uc_mots_encode(_p(masks), n_max, Hin, Win, _p(order), _p(emit), k, _f(thr), ctypes.c_double(r), int(H), int(W),
-                                   _p(ws), _l(ws.numel()), _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_mots_encode", 3 if k else 1)
+    device [>= k+1].  Launches only: offsets[k] is the number of chars needed, chars past the capacity are not written.
+    B images (uc_mots_encode_batched): masks [B,n_max,Hin,Win]; k, r, H, W: B instance counts, letterbox ratios and original sizes
+    (host sequences); order / emit: the sum(k) entries of all images grouped by image (mask rows within the image's own block), and
+    offsets [>= sum(k)+1] over all of them.  Each image's overlap removal is its own and its strings equal its one-image call's."""
+    if masks.dim() == 3:
+        n_max, Hin, Win = masks.shape
+        k = order.numel()
+        assert masks.dtype == torch.float32 and masks.is_contiguous() and order.dtype == torch.int32 and emit.dtype == torch.uint8
+        assert emit.numel() == k and chars.dtype == torch.uint8 and offsets.dtype == torch.int64 and offsets.numel() >= k + 1
+        _lib.check(_L().uc_mots_encode(_p(masks), n_max, Hin, Win, _p(order), _p(emit), k, _f(thr), ctypes.c_double(r), int(H), int(W),
+                                       _p(ws), _l(ws.numel()), _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_mots_encode",
+                   3 if k else 1)
+        return offsets
+    B, n_max, Hin, Win = masks.shape
+    K = order.numel()
+    assert masks.dtype == torch.float32 and masks.stride(3) == 1 and masks.stride(2) == Win and masks.stride(1) == Hin * Win
+    assert k is not None and len(k) == len(r) == len(H) == len(W) == B and sum(k) == K
+    assert order.dtype == torch.int32 and emit.dtype == torch.uint8 and emit.numel() == K
+    assert chars.dtype == torch.uint8 and offsets.dtype == torch.int64 and offsets.numel() >= K + 1
+    ints = lambda v: (ctypes.c_int * B)(*[int(x) for x in v])  # noqa: E731
+    _lib.check(_L().uc_mots_encode_batched(_p(masks), _l(masks.stride(0)), n_max, Hin, Win, B, ints(k), ints(H), ints(W),
+                                           (ctypes.c_double * B)(*[float(x) for x in r]), _p(order), _p(emit), _f(thr), _p(ws),
+                                           _l(ws.numel()), _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_mots_encode_batched",
+               3 if K else 1)
     return offsets
