@@ -159,12 +159,14 @@ UC_API int uc_layernorm(const void* x, int ldx, const void* res, int ldres, cons
 /* GroupNorm apply with the statistics accumulated by uc_conv2d (gn_stats = [B][G]{sum,sumsq}):
  * y = act((x-mean)*rstd*w+b) [+ prior[pix]*beta[c]] ; optional second output y2 = y + add2.
  * network_blocks.py:50-51 with exp/unicorn_track.py:450-470 (GN16, eps 1e-3, SiLU); unicorn.py:38 (GN32, eps 1e-5);
- * unicorn_head.py:272-275 (prior fusion).  x,y,add2,y2 bf16 NHWC with pixel strides. */
+ * unicorn_head.py:272-275 (prior fusion).  x,y,add2,y2 bf16 NHWC with pixel strides, 16-byte aligned; stats 8-byte aligned.
+ * act is UC_ACT_NONE, UC_ACT_RELU or UC_ACT_SILU; G >= 1, C % G == 0, C <= 4096 (UC_EINVAL otherwise). */
 UC_API int uc_groupnorm_apply(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y,
                               int ldy, int B, long HW, int C, int G, float eps, int act, const float* prior,
                               const float* beta, const void* add2, int ldadd2, void* y2, int ldy2, void* stream);
 
-/* dst[b,oh,ow,:C] = src[b,oh/up,ow/up,:C], up in {1,2} (nearest upsample + concat slice; yolo_pafpn_new.py:139-146). */
+/* dst[b,oh,ow,:C] = src[b,oh/up,ow/up,:C], up in {1,2} (nearest upsample + concat slice; yolo_pafpn_new.py:139-146).
+ * 16-bit NHWC; C, lds, ldd multiples of 8; src and dst 16-byte aligned. */
 UC_API int uc_copy_upsample(const void* src, int lds, void* dst, int ldd, int B, int Hs, int Ws, int C, int up, void* stream);
 /* nn.PixelShuffle(2) in NHWC (unicorn.py:41): in [B,H,W,4*Co] -> out [B,2H,2W,Co], 16-bit. */
 UC_API int uc_pixel_shuffle2(const void* in, int ldi, void* out, int ldo, int B, int H, int W, int Co, void* stream);
@@ -176,6 +178,7 @@ UC_API int uc_bilinear_f32(const float* src, float* dst, int P, int Hs, int Ws, 
  * OpenCV's 8-bit fixed-point bilinear —, the rest = pad (114); swap_rb does cv2.COLOR_RGB2BGR.  uint8 HWC, 3 channels. */
 UC_API int uc_letterbox_u8(const uint8_t* src_hwc, int Hs, int Ws, uint8_t* dst_hwc, int Hd, int Wd, int rh, int rw,
                            int swap_rb, int pad, void* stream);
+/* y = a + b on 16-bit (UC_BF16 / UC_F16) rows; C and the strides multiples of 8; a, b and y 16-byte aligned. */
 UC_API int uc_add(const void* a, int lda, const void* b, int ldb, void* y, int ldy, long M, int C, int dtype, void* stream);
 /* Conditional strided row copy decided on the device: rows are copied when (*flag_dev != 0) != invert.  The MOT drivers use it for
  * "pre_dict = cur_dict only when this frame produced detections" (unicorn/evaluators/mot_evaluator.py:1005,1014-1020) so that the

@@ -1,0 +1,77 @@
+"""Argument validation of uc_groupnorm_apply, uc_copy_upsample and uc_add: every call here is rejected with UC_EINVAL and a message
+before anything is launched, so the pointers are fake addresses that are never dereferenced and the test runs without a GPU."""
+import ctypes
+
+import pytest
+
+from unicorn_b200 import _lib
+
+P = ctypes.c_void_p
+EINVAL = -1
+A16 = [P(0x10000 * (i + 1)) for i in range(6)]  # 16-byte aligned, never dereferenced
+
+
+@pytest.fixture(scope="module")
+def lib():
+    return _lib.lib()
+
+
+def gn(lib, x=A16[0], ldx=256, stats=A16[1], w=A16[2], b=A16[3], y=A16[4], ldy=256, B=1, HW=16, C=256, G=16, eps=1e-3,
+       act=_lib.ACT_SILU, prior=None, beta=None, add2=None, ldadd2=0, y2=None, ldy2=0):
+    rc = lib.uc_groupnorm_apply(x, ldx, stats, w, b, y, ldy, B, ctypes.c_long(HW), C, G, ctypes.c_float(eps), act, prior, beta, add2,
+                                ldadd2, y2, ldy2, None)
+    return rc, lib.uc_last_error()
+
+
+def rejected(call, *words):
+    rc, msg = call
+    assert rc == EINVAL, (rc, msg)
+    for w in words:
+        assert w.encode() in msg, (w, msg)
+
+
+@pytest.mark.parametrize("act", [_lib.ACT_GELU, _lib.ACT_SIGMOID, 5, -1])
+def test_groupnorm_apply_rejects_activations_it_does_not_implement(lib, act):
+    rejected(gn(lib, act=act), "uc_groupnorm_apply", "act must be")
+
+
+def test_groupnorm_apply_rejects_bad_groups_and_sizes(lib):
+    rejected(gn(lib, G=0), "G must be >= 1")  # used to divide by zero (SIGFPE) in the host process
+    rejected(gn(lib, G=-16), "G must be >= 1")
+    rejected(gn(lib, G=24), "C % G == 0")
+    rejected(gn(lib, C=252, ldx=256, ldy=256), "multiples of 8")
+    rejected(gn(lib, ldx=260), "multiples of 8")
+    rejected(gn(lib, C=4104, G=8, ldx=4104, ldy=4104), "C too large")
+    rejected(gn(lib, C=4104, G=8, ldx=4104, ldy=4104, x=None, stats=None, w=None, b=None, y=None), "C too large")
+    # C = 4096 is accepted: with null pointers the call gets past the size checks and stops at the pointer check
+    rejected(gn(lib, C=4096, G=32, ldx=4096, ldy=4096, x=None, stats=None, w=None, b=None, y=None), "null pointer")
+
+
+def test_groupnorm_apply_rejects_bad_pointers(lib):
+    rejected(gn(lib, x=None), "null pointer")
+    rejected(gn(lib, prior=A16[5]), "prior and beta go together")
+    rejected(gn(lib, y2=A16[5]), "bad second output")
+    for k in ("x", "y"):
+        rejected(gn(lib, **{k: P(0x10008)}), "16-byte aligned")
+    # a channel slice 4 bf16 elements into a 16-byte aligned buffer: legal strides, misaligned base
+    rejected(gn(lib, x=P(0x10008), y=P(0x10008)), "16-byte aligned")
+    rejected(gn(lib, add2=P(0x50008), ldadd2=256, y2=A16[5], ldy2=256), "16-byte aligned")
+    rejected(gn(lib, add2=A16[5], ldadd2=256, y2=P(0x60004), ldy2=256), "16-byte aligned")
+    rejected(gn(lib, stats=P(0x20004)), "stats must be 8-byte aligned")
+
+
+def test_copy_upsample_rejects_misaligned_maps(lib):
+    cu = lambda src, dst, up=2, C=64: (lib.uc_copy_upsample(src, 64, dst, 160, 1, 4, 4, C, up, None), lib.uc_last_error())  # noqa: E731
+    rejected(cu(P(0x10008), A16[1]), "uc_copy_upsample", "16-byte aligned")
+    rejected(cu(A16[0], P(0x20008)), "uc_copy_upsample", "16-byte aligned")
+    rejected(cu(A16[0], A16[1], up=3), "uc_copy_upsample: bad arguments")
+    rejected(cu(A16[0], A16[1], C=60), "uc_copy_upsample: bad arguments")
+    rejected(cu(None, A16[1]), "uc_copy_upsample: bad arguments")
+
+
+def test_add_rejects_misaligned_rows_and_other_dtypes(lib):
+    add = lambda a, b, y, dtype=_lib.BF16: (lib.uc_add(a, 64, b, 64, y, 64, ctypes.c_long(10), 64, dtype, None), lib.uc_last_error())  # noqa: E731
+    for args in ((P(0x10008), A16[1], A16[2]), (A16[0], P(0x20008), A16[2]), (A16[0], A16[1], P(0x30004))):
+        rejected(add(*args), "uc_add", "16-byte aligned")
+    rejected(add(A16[0], A16[1], A16[2], dtype=_lib.F32), "uc_add", "16-bit dtypes only")
+    rejected(add(A16[0], None, A16[2]), "uc_add: bad arguments")

@@ -221,6 +221,8 @@ using namespace uc;
 
 extern "C" int uc_copy_upsample(const void* src, int lds, void* dst, int ldd, int B, int Hs, int Ws, int C, int up, void* stream_v) {
   if (!src || !dst || C % 8 || lds % 8 || ldd % 8 || (up != 1 && up != 2)) return set_error(UC_EINVAL, "uc_copy_upsample: bad arguments");
+  if ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15)
+    return set_error(UC_EINVAL, "uc_copy_upsample: src and dst must be 16-byte aligned");
   const long total = static_cast<long>(B) * Hs * up * Ws * up * (C / 8);
   launch_pdl(copy_upsample_kernel, grid_for(total), 256, 0, static_cast<cudaStream_t>(stream_v), 
       static_cast<const uint16_t*>(src), lds, static_cast<uint16_t*>(dst), ldd, B, Hs, Ws, C, up);
@@ -259,6 +261,9 @@ extern "C" int uc_letterbox_u8(const uint8_t* src_hwc, int Hs, int Ws, uint8_t* 
 
 extern "C" int uc_add(const void* a, int lda, const void* b, int ldb, void* y, int ldy, long M, int C, int dtype, void* stream_v) {
   if (!a || !b || !y || C % 8 || lda % 8 || ldb % 8 || ldy % 8) return set_error(UC_EINVAL, "uc_add: bad arguments");
+  if (dtype != UC_BF16 && dtype != UC_F16) return set_error(UC_EINVAL, "uc_add: 16-bit dtypes only");
+  if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y)) & 15)
+    return set_error(UC_EINVAL, "uc_add: a, b and y must be 16-byte aligned");
   launch_pdl(add_kernel, grid_for(M * (C / 8)), 256, 0, static_cast<cudaStream_t>(stream_v), 
       static_cast<const uint16_t*>(a), lda, static_cast<const uint16_t*>(b), ldb, static_cast<uint16_t*>(y), ldy, M, C, dtype);
   return check_launch("uc_add");

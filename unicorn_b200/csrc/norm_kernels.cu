@@ -619,14 +619,22 @@ extern "C" int uc_groupnorm_apply(const void* x, int ldx, const void* stats, con
                                   int ldy, int B, long HW, int C, int G, float eps, int act, const float* prior,
                                   const float* beta, const void* add2, int ldadd2, void* y2, int ldy2, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!x || !stats || !w || !b || !y) return set_error(UC_EINVAL, "uc_groupnorm_apply: null pointer");
+  // sizes before pointers: G is checked before it divides anything
+  if (G < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply: G must be >= 1 (got %d)", G);
   if (C % 8 || ldx % 8 || ldy % 8 || C % G) return set_error(UC_EINVAL, "uc_groupnorm_apply: C, ldx, ldy multiples of 8; C %% G == 0");
+  if (C > 4096) return set_error(UC_EINVAL, "uc_groupnorm_apply: C too large");
+  if (act != UC_ACT_NONE && act != UC_ACT_RELU && act != UC_ACT_SILU)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply: act must be UC_ACT_NONE, UC_ACT_RELU or UC_ACT_SILU (got %d)", act);
+  if (!x || !stats || !w || !b || !y) return set_error(UC_EINVAL, "uc_groupnorm_apply: null pointer");
   if ((prior != nullptr) != (beta != nullptr)) return set_error(UC_EINVAL, "uc_groupnorm_apply: prior and beta go together");
   if (y2 && (!add2 || ldadd2 % 8 || ldy2 % 8)) return set_error(UC_EINVAL, "uc_groupnorm_apply: bad second output");
+  // the kernel moves 8 channels per 128-bit access
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(add2) | reinterpret_cast<uintptr_t>(y2)) & 15)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply: x, y, add2 and y2 must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(stats) & 7) return set_error(UC_EINVAL, "uc_groupnorm_apply: stats must be 8-byte aligned");
   const long total = HW * (C / 8);
   // each block pays C scale/shift computations up front; keep ~2 elements (16 channels) per thread for parallelism
   const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
-  if (C > 4096) return set_error(UC_EINVAL, "uc_groupnorm_apply: C too large");
   launch_pdl(groupnorm_apply_kernel, dim3(gx, B), 256, 3 * C * sizeof(float), stream, 
       static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
       eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2);
