@@ -251,6 +251,21 @@ UC_API long uc_postprocess_workspace_bytes_batched(int max_anchors, int B);
 UC_API int uc_postprocess_batched(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
                                   void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream);
 
+/* Flags of the *_ex / *_nms entry points.  UC_POST_CLASS_AGNOSTIC: NMS over all classes (postprocess(..., class_agnostic=True),
+ * torchvision.ops.nms); without it NMS is class-aware as in uc_postprocess.  Unknown bits: UC_EINVAL. */
+#define UC_POST_CLASS_AGNOSTIC 1
+UC_API int uc_postprocess_batched_ex(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B, int flags,
+                                     void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream);
+/* Decode + score filter of B images read straight from the per-level head maps (the arguments of uc_head_decode_batched), without
+ * the [B, A, 5+ncls] tensor: fills the workspace (uc_postprocess_workspace_bytes_batched(A, B), A = sum h*w) with exactly the
+ * candidates, keys and anchor ids that uc_head_decode_batched followed by the filter of uc_postprocess_batched leave there.
+ * uc_postprocess_nms_batched then runs the sort, gather and greedy NMS of uc_postprocess_batched on that workspace. */
+UC_API int uc_det_candidates_batched(const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                                     int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float conf_thre, void* workspace,
+                                     long workspace_bytes, void* stream);
+UC_API int uc_postprocess_nms_batched(int A, float nms_thre, int max_keep, int B, int flags, void* workspace, long workspace_bytes,
+                                      float* out_dets, int* out_count, int* out_anchor, void* stream);
+
 /* Instance-embedding sampling at box centres (unicorn/evaluators/mot_evaluator.py:1024-1034): embed NHWC 16-bit
  * [h,w,C] (pixel stride ld), boxes f32 [n,ldb] xyxy in network-input pixels, stride = 8; grid_sample(bilinear,
  * border, align_corners=False) semantics incl. the reference's clamp/normalise step.  n = min(*count_dev, n_max)

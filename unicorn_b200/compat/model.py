@@ -27,7 +27,7 @@ import math
 
 import torch
 
-from .. import ops
+from .. import ops, post_ops
 from ..engine import UnicornEngine
 from ..weights import CONFIGS, param_shapes
 
@@ -163,6 +163,13 @@ class UnicornB200Model:
 
     def __call__(self, imgs=None, seq_dict0=None, seq_dict1=None, feat=None, mode="backbone", **unused):
         e = self._engine()
+        if self.cfg["task"] == "det":  # YOLOX.forward (models/yolox.py:28-50): NCHW fp32 [B,3,H,W] -> decoded [B, A, 5+ncls]
+            if not self.head.decode_in_inference:
+                raise ValueError("UnicornB200Model: the detector returns decoded outputs only (head.decode_in_inference=True)")
+            assert imgs.is_cuda and imgs.dim() == 4 and imgs.shape[0] >= 1, "CUDA NCHW images [B,3,H,W]"
+            e.begin_frame()
+            fpn, _ = e.backbone(imgs.float().contiguous(), tag="compat")
+            return e.head(fpn, None, "mot").clone()
         if mode == "backbone":
             fpn, seq_dict = self._backbone(imgs)
             return tuple(ops.nhwc_to_nchw(t) for t in fpn), seq_dict
@@ -192,14 +199,18 @@ def _to_corners_(prediction):
     prediction[..., :4] = c
 
 
-def postprocess(prediction, num_classes, conf_thre=0.7, nms_thre=0.45):
+def postprocess(prediction, num_classes, conf_thre=0.7, nms_thre=0.45, class_agnostic=False):
     """unicorn.utils.postprocess (utils/boxes.py:33-77): list with one (M,7) tensor of rows per image
     (x1,y1,x2,y2,obj_conf,class_conf,class_pred), descending score, or None when nothing passes — on the GPU, every image of the
-    batch in one launch sequence.  Like the reference, the boxes of `prediction` are converted to corner form in place."""
+    batch in one launch sequence.  Like the reference, the boxes of `prediction` are converted to corner form in place.
+    class_agnostic=True: NMS across classes (torchvision.ops.nms, as tools/demo.py asks for)."""
     p = prediction.float().contiguous()
     B, A = p.shape[:2]
     ws = ops.PostWorkspace(A, p.device, B)
-    dets, cnt = ops.postprocess_device(p, num_classes, conf_thre, nms_thre, ws)
+    if class_agnostic:
+        dets, cnt = post_ops.postprocess_device_ex(p, num_classes, conf_thre, nms_thre, ws, class_agnostic=True)
+    else:
+        dets, cnt = ops.postprocess_device(p, num_classes, conf_thre, nms_thre, ws)
     dets = dets.view(B, A, 7)
     out = [dets[i, :n].clone() if n > 0 else None for i, n in enumerate(cnt.tolist())]
     _to_corners_(prediction)

@@ -3,6 +3,8 @@
 //   uc_postprocess   unicorn/utils/boxes.py:33-77: cxcywh->xyxy, class_conf/pred = max/argmax over classes,
 //                    keep obj*class_conf >= conf, torchvision.ops.batched_nms (greedy, IoU > thr suppresses,
 //                    only within the same class), result ordered by descending score.
+//   uc_det_candidates_batched   the decode + filter of the two above fused, read straight from the per-level head maps
+//   UC_POST_CLASS_AGNOSTIC      postprocess(..., class_agnostic=True): torchvision.ops.nms over all classes
 // Everything stays on the GPU; the host reads back one counter.  Decision arithmetic is fp32 in the reference's
 // operation order so that thresholds flip only on exact ties.
 #include "uc_common.h"
@@ -50,6 +52,8 @@ struct PostSlices {
   int A;
   __device__ __forceinline__ uint8_t* base(int b) const { return ws + b * per_image; }
   __device__ __forceinline__ int* count(int b) const { return reinterpret_cast<int*>(base(b)); }
+  // per-tile candidate counts of det_candidates (the rest of the 256-byte count header)
+  __device__ __forceinline__ int* tile_count(int b) const { return count(b) + 1; }
   __device__ __forceinline__ float* det(int b) const { return reinterpret_cast<float*>(base(b) + 256); }
   __device__ __forceinline__ float* sorted(int b) const { return det(b) + static_cast<long>(A) * 7; }
   __device__ __forceinline__ unsigned long long* keys(int b) const {
@@ -125,6 +129,114 @@ __global__ void __launch_bounds__(1024) det_filter_kernel(const float* __restric
   if (threadIdx.x == 0) *count = min(base, cap);
 }
 
+// ---- fused decode + filter for wide heads, straight from the per-level maps (head_decode + det_filter without the [B, A, 5+ncls]
+// tensor in between).  Same fp32 operations in the same order as those two kernels (the _rn intrinsics keep nvcc from contracting
+// the decode's product into the corner's sum, which the stored intermediate prevents there), so rows, keys, anchor ids and counts
+// are bit-identical.  Two launches per image, each on ntiles CTAs:
+//   1. every CTA takes a tile of anchors, compacts its candidates in anchor order into its own region of the `sorted` rows /
+//      `sorted_anchor` (both free until the gather) and writes its candidate count into the slice header;
+//   2. every CTA sums the counts of the tiles before its own and copies its candidates to their final place, with their keys.
+constexpr int kCandThreads = 256;
+constexpr int kCandMaxTiles = 63;  // tile counts live in the 256-byte header after the count
+
+static int cand_tile(int A) {  // anchors per tile: a multiple of the CTA size, at most kCandMaxTiles tiles
+  const int per = (A + kCandMaxTiles - 1) / kCandMaxTiles;
+  return std::max(1, (per + kCandThreads - 1) / kCandThreads) * kCandThreads;
+}
+
+__global__ void __launch_bounds__(kCandThreads) det_candidates_kernel(DecodeLevels lv, int tile, float conf, PostSlices sl) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.y, t0 = blockIdx.x * tile;
+  float* const stage = sl.sorted(b) + static_cast<long>(t0) * 7;
+  int* const stage_anchor = sl.sorted_anchor(b) + t0;
+  __shared__ int warp_cnt[kCandThreads / 32];
+  __shared__ int base;
+  if (threadIdx.x == 0) base = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int end = min(t0 + tile, lv.total);
+  for (int a0 = t0; a0 < end; a0 += kCandThreads) {
+    const int i = a0 + threadIdx.x;
+    bool pass = false;
+    float r[7];
+    if (i < end) {
+      int k = 0;
+      if (i >= lv.start[1]) k = 1;
+      if (i >= lv.start[2]) k = 2;
+      const int a = i - lv.start[k];
+      const float x = static_cast<float>(a % lv.w[k]), y = static_cast<float>(a / lv.w[k]);
+      const float s = static_cast<float>(lv.stride[k]);
+      const float* ro = lv.regobj[k] + b * lv.bs_ro[k] + static_cast<long>(a) * lv.ld_ro;
+      const float* cl = lv.cls[k] + b * lv.bs_cls[k] + static_cast<long>(a) * lv.ld_cls;
+      const float cx = __fmul_rn(__fadd_rn(ro[0], x), s), cy = __fmul_rn(__fadd_rn(ro[1], y), s);
+      const float w = __fmul_rn(expf(ro[2]), s), h = __fmul_rn(expf(ro[3]), s);
+      const float obj = 1.f / (1.f + expf(-ro[4]));
+      float best = 1.f / (1.f + expf(-cl[0]));
+      int bi = 0;
+      for (int c = 1; c < lv.ncls; ++c) {  // compared after the sigmoid: saturated logits tie and the first class wins, as in torch.max
+        const float v = 1.f / (1.f + expf(-cl[c]));
+        if (v > best) { best = v; bi = c; }
+      }
+      pass = __fmul_rn(obj, best) >= conf;
+      r[0] = __fsub_rn(cx, __fmul_rn(w, 0.5f)); r[1] = __fsub_rn(cy, __fmul_rn(h, 0.5f));
+      r[2] = __fadd_rn(cx, __fmul_rn(w, 0.5f)); r[3] = __fadd_rn(cy, __fmul_rn(h, 0.5f));
+      r[4] = obj; r[5] = best; r[6] = static_cast<float>(bi);
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, pass);
+    if (lane == 0) warp_cnt[warp] = __popc(bal);
+    __syncthreads();
+    if (pass) {
+      int idx = base + __popc(bal & ((1u << lane) - 1));
+      for (int q = 0; q < warp; ++q) idx += warp_cnt[q];
+      float* d = stage + static_cast<long>(idx) * 7;
+#pragma unroll
+      for (int q = 0; q < 7; ++q) d[q] = r[q];
+      stage_anchor[idx] = i;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int n = 0;
+      for (int q = 0; q < kCandThreads / 32; ++q) n += warp_cnt[q];
+      base += n;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) sl.tile_count(b)[blockIdx.x] = base;
+}
+
+__global__ void __launch_bounds__(kCandThreads) det_candidates_compact_kernel(int tile, PostSlices sl) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.y, t = blockIdx.x;
+  const int* const tc = sl.tile_count(b);
+  __shared__ int off_s;
+  if (threadIdx.x < 32) {
+    int v = 0;
+    for (int q = threadIdx.x; q < t; q += 32) v += tc[q];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) off_s = v;
+  }
+  __syncthreads();
+  const int off = off_s, n = tc[t];
+  const float* const stage = sl.sorted(b) + static_cast<long>(t) * tile * 7;
+  const int* const stage_anchor = sl.sorted_anchor(b) + static_cast<long>(t) * tile;
+  float* const det = sl.det(b);
+  unsigned long long* const keys = sl.keys(b);
+  int* const det_anchor = sl.det_anchor(b);
+  for (int j = threadIdx.x; j < n; j += kCandThreads) {
+    const float* src = stage + static_cast<long>(j) * 7;
+    const int idx = off + j;
+    float* d = det + static_cast<long>(idx) * 7;
+#pragma unroll
+    for (int q = 0; q < 7; ++q) d[q] = src[q];
+    const float score = __fmul_rn(src[4], src[5]);
+    keys[idx] = (static_cast<unsigned long long>(__float_as_uint(score)) << 32) | (0xffffffffu - static_cast<unsigned>(idx));
+    det_anchor[idx] = stage_anchor[j];
+  }
+  if (t == gridDim.x - 1 && threadIdx.x == 0) *sl.count(b) = off + n;
+}
+
 // ---- sort keys descending (bitonic, one CTA per image, n2 = power of two >= count; pads with 0 keys)
 __global__ void __launch_bounds__(1024) sort_desc_kernel(PostSlices sl) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
@@ -178,7 +290,7 @@ __global__ void __launch_bounds__(256) det_gather_kernel(PostSlices sl) {
 //  3. one warp resolves the chunk greedily, jumping from survivor to survivor with ffs;
 //  4. the newly kept boxes are appended to the kept list (shared memory, spilling to the output rows in global).
 // Work ~ N x kept IoUs instead of N^2, and the sequential part is proportional to the number of kept boxes.
-// IoU arithmetic is torchvision's devIoU (fp32, inter / (areaA + areaB - inter) > thr), same-class pairs only.
+// IoU arithmetic is torchvision's devIoU (fp32, inter / (areaA + areaB - inter) > thr), same-class pairs only (class-aware variant).
 constexpr int kNmsChunk = 256;
 constexpr int kNmsKeepSmem = 3072;
 
@@ -191,6 +303,8 @@ __device__ __forceinline__ bool nms_hit(const float4 a, const float4 b, float th
   return inter / (sa + sb - inter) > thr;
 }
 
+// kAgnostic: every pair is tested, whatever the classes (torchvision.ops.nms of postprocess(..., class_agnostic=True)).
+template <bool kAgnostic>
 __global__ void __launch_bounds__(1024) nms_greedy_kernel(PostSlices sl, float thr, float* __restrict__ out, int* __restrict__ out_count,
                                                            int max_keep, int* __restrict__ out_anchor) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
@@ -231,7 +345,7 @@ __global__ void __launch_bounds__(1024) nms_greedy_kernel(PostSlices sl, float t
       float kc;
       if (k < kNmsKeepSmem) { kb = kept_box[k]; kc = kept_cls[k]; }
       else { const float* d = out + static_cast<long>(k) * 7; kb = make_float4(d[0], d[1], d[2], d[3]); kc = d[6]; }
-      if (kc == cl && nms_hit(kb, bx, thr)) sup = true;
+      if ((kAgnostic || kc == cl) && nms_hit(kb, bx, thr)) sup = true;
     }
     sup |= __shfl_xor_sync(0xffffffffu, sup, 1) != 0;
     sup |= __shfl_xor_sync(0xffffffffu, sup, 2) != 0;
@@ -255,7 +369,7 @@ __global__ void __launch_bounds__(1024) nms_greedy_kernel(PostSlices sl, float t
         const unsigned long long aw = alive_w[sub];
         for (int t = 0; t < 64; ++t) {
           const int o = sub * 64 + t;
-          if (o > ci && ((aw >> t) & 1ull) && ccls[o] == cl && nms_hit(bx, cbox[o], thr)) bits |= 1ull << t;
+          if (o > ci && ((aw >> t) & 1ull) && (kAgnostic || ccls[o] == cl) && nms_hit(bx, cbox[o], thr)) bits |= 1ull << t;
         }
       }
       pair_mask[ci][sub] = bits;
@@ -303,11 +417,10 @@ __global__ void __launch_bounds__(1024) nms_greedy_kernel(PostSlices sl, float t
 
 using namespace uc;
 
-static int head_decode(const char* what, const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
-                       int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float* out, void* stream_v) {
-  if (!regobj || !cls || !hw || !strides || !out || ncls < 1 || ncls > ld_cls || ld_ro < 5) return set_error(UC_EINVAL, "%s: bad arguments", what);
+static int make_levels(const char* what, const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                       int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, DecodeLevels& lv) {
+  if (!regobj || !cls || !hw || !strides || ncls < 1 || ncls > ld_cls || ld_ro < 5) return set_error(UC_EINVAL, "%s: bad arguments", what);
   if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
-  DecodeLevels lv;
   int start = 0;
   for (int k = 0; k < 3; ++k) {
     lv.regobj[k] = regobj[k]; lv.cls[k] = cls[k];
@@ -320,7 +433,15 @@ static int head_decode(const char* what, const float* const* regobj, const float
     start += lv.h[k] * lv.w[k];
   }
   lv.ld_ro = ld_ro; lv.ld_cls = ld_cls; lv.ncls = ncls; lv.total = start;
-  launch_pdl(head_decode_kernel, dim3((start + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream_v), lv, out);
+  return UC_OK;
+}
+
+static int head_decode(const char* what, const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                       int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float* out, void* stream_v) {
+  if (!out) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  DecodeLevels lv;
+  if (int e = make_levels(what, regobj, cls, hw, strides, ld_ro, ld_cls, bs_ro, bs_cls, ncls, B, lv)) return e;
+  launch_pdl(head_decode_kernel, dim3((lv.total + 255) / 256, B), 256, 0, static_cast<cudaStream_t>(stream_v), lv, out);
   return check_launch(what);
 }
 
@@ -346,14 +467,7 @@ extern "C" long uc_postprocess_workspace_bytes_batched(int max_anchors, int B) {
   return B < 1 ? 0 : B * uc_postprocess_workspace_bytes(max_anchors);
 }
 
-static int postprocess(const char* what, const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
-                       void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!pred || !workspace || !out_dets || !out_count || A < 1 || ncls < 1) return set_error(UC_EINVAL, "%s: bad arguments", what);
-  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
-  if (workspace_bytes < B * uc_postprocess_workspace_bytes(A))
-    return set_error(UC_EINVAL, "%s: workspace too small (%ld bytes for %d images of %d anchors, need %ld)", what, workspace_bytes, B, A,
-                     B * uc_postprocess_workspace_bytes(A));
+static PostSlices make_slices(void* workspace, int A) {
   long a2 = 1;
   while (a2 < A) a2 <<= 1;
   PostSlices sl;
@@ -361,29 +475,98 @@ static int postprocess(const char* what, const float* pred, int A, int ncls, flo
   sl.per_image = uc_postprocess_workspace_bytes(A);
   sl.a2 = a2;
   sl.A = A;
-  launch_pdl(det_filter_kernel, B, 1024, 0, stream, pred, A, ncls, conf_thre, sl);
-  launch_pdl(sort_desc_kernel, B, 1024, 0, stream, sl);
-  launch_pdl(det_gather_kernel, dim3(std::min(num_sms() * 4, (A + 255) / 256), B), 256, 0, stream, sl);
+  return sl;
+}
+
+static int check_workspace(const char* what, int A, int B, long workspace_bytes) {
+  if (B < 1) return set_error(UC_EINVAL, "%s: B must be >= 1 (got %d)", what, B);
+  if (workspace_bytes < B * uc_postprocess_workspace_bytes(A))
+    return set_error(UC_EINVAL, "%s: workspace too small (%ld bytes for %d images of %d anchors, need %ld)", what, workspace_bytes, B, A,
+                     B * uc_postprocess_workspace_bytes(A));
+  return UC_OK;
+}
+
+template <bool kAgnostic>
+static void launch_nms(const PostSlices& sl, int B, float nms_thre, float* out_dets, int* out_count, int max_keep, int* out_anchor,
+                       cudaStream_t stream) {
   constexpr int smem = kNmsKeepSmem * (16 + 4);
   static PerDeviceFlag attr_dev;
   bool& attr = attr_dev.get();
   if (!attr) {
-    cudaFuncSetAttribute(nms_greedy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(nms_greedy_kernel<kAgnostic>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     attr = true;
   }
-  launch_pdl(nms_greedy_kernel, B, 1024, smem, stream, sl, nms_thre, out_dets, out_count, max_keep > 0 ? max_keep : 0x7fffffff, out_anchor);
+  launch_pdl(nms_greedy_kernel<kAgnostic>, B, 1024, smem, stream, sl, nms_thre, out_dets, out_count, max_keep > 0 ? max_keep : 0x7fffffff,
+             out_anchor);
+}
+
+// sort, gather and greedy NMS of the candidates a filter left in the workspace
+static void launch_nms_stages(const PostSlices& sl, int B, float nms_thre, int max_keep, int flags, float* out_dets, int* out_count,
+                              int* out_anchor, cudaStream_t stream) {
+  launch_pdl(sort_desc_kernel, B, 1024, 0, stream, sl);
+  launch_pdl(det_gather_kernel, dim3(std::min(num_sms() * 4, (sl.A + 255) / 256), B), 256, 0, stream, sl);
+  if (flags & UC_POST_CLASS_AGNOSTIC)
+    launch_nms<true>(sl, B, nms_thre, out_dets, out_count, max_keep, out_anchor, stream);
+  else
+    launch_nms<false>(sl, B, nms_thre, out_dets, out_count, max_keep, out_anchor, stream);
+}
+
+static int postprocess(const char* what, const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B, int flags,
+                       void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!pred || !workspace || !out_dets || !out_count || A < 1 || ncls < 1) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  if (flags & ~UC_POST_CLASS_AGNOSTIC) return set_error(UC_EINVAL, "%s: unknown flags 0x%x", what, flags);
+  if (int e = check_workspace(what, A, B, workspace_bytes)) return e;
+  const PostSlices sl = make_slices(workspace, A);
+  launch_pdl(det_filter_kernel, B, 1024, 0, stream, pred, A, ncls, conf_thre, sl);
+  launch_nms_stages(sl, B, nms_thre, max_keep, flags, out_dets, out_count, out_anchor, stream);
   return check_launch(what);
 }
 
 extern "C" int uc_postprocess(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, void* workspace,
                               long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
-  return postprocess("uc_postprocess", pred, A, ncls, conf_thre, nms_thre, max_keep, 1, workspace, workspace_bytes, out_dets, out_count,
+  return postprocess("uc_postprocess", pred, A, ncls, conf_thre, nms_thre, max_keep, 1, 0, workspace, workspace_bytes, out_dets, out_count,
                      out_anchor, stream_v);
 }
 
 extern "C" int uc_postprocess_batched(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B,
                                       void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor,
                                       void* stream_v) {
-  return postprocess("uc_postprocess_batched", pred, A, ncls, conf_thre, nms_thre, max_keep, B, workspace, workspace_bytes, out_dets,
+  return postprocess("uc_postprocess_batched", pred, A, ncls, conf_thre, nms_thre, max_keep, B, 0, workspace, workspace_bytes, out_dets,
                      out_count, out_anchor, stream_v);
+}
+
+extern "C" int uc_postprocess_batched_ex(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, int B, int flags,
+                                         void* workspace, long workspace_bytes, float* out_dets, int* out_count, int* out_anchor,
+                                         void* stream_v) {
+  return postprocess("uc_postprocess_batched_ex", pred, A, ncls, conf_thre, nms_thre, max_keep, B, flags, workspace, workspace_bytes,
+                     out_dets, out_count, out_anchor, stream_v);
+}
+
+extern "C" int uc_det_candidates_batched(const float* const* regobj, const float* const* cls, const int* hw, const int* strides, int ld_ro,
+                                         int ld_cls, const long* bs_ro, const long* bs_cls, int ncls, int B, float conf_thre,
+                                         void* workspace, long workspace_bytes, void* stream_v) {
+  const char* what = "uc_det_candidates_batched";
+  if (!workspace) return set_error(UC_EINVAL, "%s: null workspace", what);
+  if (B > 1 && (!bs_ro || !bs_cls)) return set_error(UC_EINVAL, "%s: null per-image strides", what);
+  DecodeLevels lv;
+  if (int e = make_levels(what, regobj, cls, hw, strides, ld_ro, ld_cls, bs_ro, bs_cls, ncls, B, lv)) return e;
+  if (int e = check_workspace(what, lv.total, B, workspace_bytes)) return e;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const PostSlices sl = make_slices(workspace, lv.total);
+  const int tile = cand_tile(lv.total), ntiles = (lv.total + tile - 1) / tile;
+  launch_pdl(det_candidates_kernel, dim3(ntiles, B), kCandThreads, 0, stream, lv, tile, conf_thre, sl);
+  launch_pdl(det_candidates_compact_kernel, dim3(ntiles, B), kCandThreads, 0, stream, tile, sl);
+  return check_launch(what);
+}
+
+extern "C" int uc_postprocess_nms_batched(int A, float nms_thre, int max_keep, int B, int flags, void* workspace, long workspace_bytes,
+                                          float* out_dets, int* out_count, int* out_anchor, void* stream_v) {
+  const char* what = "uc_postprocess_nms_batched";
+  if (!workspace || !out_dets || !out_count || A < 1) return set_error(UC_EINVAL, "%s: bad arguments", what);
+  if (flags & ~UC_POST_CLASS_AGNOSTIC) return set_error(UC_EINVAL, "%s: unknown flags 0x%x", what, flags);
+  if (int e = check_workspace(what, A, B, workspace_bytes)) return e;
+  launch_nms_stages(make_slices(workspace, A), B, nms_thre, max_keep, flags, out_dets, out_count, out_anchor,
+                    static_cast<cudaStream_t>(stream_v));
+  return check_launch(what);
 }

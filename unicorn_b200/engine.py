@@ -76,6 +76,11 @@ class UnicornEngine:
         ctx._side_streams, ctx._fork_stream = None, None
         return ctx
 
+    def _tracking_only(self, what):
+        if self.det:
+            raise ValueError(f"UnicornEngine.{what}: {self.cfg_name} is a detector (backbone, neck and head only); "
+                             f"{what} belongs to the tracking models")
+
     # ------------------------------------------------------------------------------------------ weights
     def _load(self, sd):
         dev = self.dev
@@ -116,7 +121,15 @@ class UnicornEngine:
         P["bu_conv2"], P["bu_conv1"] = cgn(n + "bu_conv2.", 3, 2), cgn(n + "bu_conv1.", 3, 2)
         for name in ("C3_p4", "C3_p3", "C3_n3", "C3_n4"):
             P[name] = csp(n + name + ".")
-        # interaction
+        self.det = self.cfg["task"] == "det"
+        if not self.det:  # a detector (YOLOX) has no interaction, upsampling or SOT predictors
+            self._load_interaction(sd, P, f, pw)
+        # head
+        self._load_head(sd, P, f, pw, cgn, block)
+        self.P = P
+
+    def _load_interaction(self, sd, P, f, pw):
+        dev = self.dev
         P["bottleneck"] = _ConvGN(pw("bottleneck.0.weight"), f("bottleneck.1.weight"), f("bottleneck.1.bias"), 1, 1, groups=32, eps=1e-5,
                                   bias=f("bottleneck.0.bias"))
         t = "transformer.encoder.layers.0."
@@ -132,19 +145,21 @@ class UnicornEngine:
         P["pos_tab"] = (f("pos_emb.col_embed.weight"), f("pos_emb.row_embed.weight"))
         P["up1"] = (pw("upsample_layer.1.weight"), f("upsample_layer.1.bias"))
         P["up3"] = (pw("upsample_layer.3.weight"), f("upsample_layer.3.bias"))
-        # head
+
+    def _load_head(self, sd, P, f, pw, cgn, block):
+        dev = self.dev
         h = "head."
         P["head"] = []
         for k in range(3):
-            lvl = dict(stem=cgn(h + f"stems.{k}.", 1), beta=f(h + f"beta_{k}").reshape(-1).contiguous(),
+            lvl = dict(stem=cgn(h + f"stems.{k}.", 1), beta=None if self.det else f(h + f"beta_{k}").reshape(-1).contiguous(),
                        att=[block(h + f"att_layers.{k}.{i}.") for i in range(3)],
                        cls=[cgn(h + f"cls_convs.{k}.{i}.", 3) for i in range(4)], reg=[cgn(h + f"reg_convs.{k}.{i}.", 3) for i in range(4)])
-            for sfx in ("", "_sot"):
+            for sfx in ("",) if self.det else ("", "_sot"):
                 ro_w = torch.cat([sd[h + f"reg_preds{sfx}.{k}.weight"], sd[h + f"obj_preds{sfx}.{k}.weight"]], 0).to(dev, F32)
                 ro_b = torch.zeros(8, device=dev)
                 ro_b[:5] = torch.cat([sd[h + f"reg_preds{sfx}.{k}.bias"], sd[h + f"obj_preds{sfx}.{k}.bias"]]).to(dev)
                 cw = sd[h + f"cls_preds{sfx}.{k}.weight"].to(dev, F32)
-                cb = torch.zeros(8, device=dev)
+                cb = torch.zeros(_cls_cols(cw.shape[0]), device=dev)  # bias of the packed (8-row padded) class conv
                 cb[:cw.shape[0]] = sd[h + f"cls_preds{sfx}.{k}.bias"].to(dev)
                 lvl["pred" + sfx] = (ops.pack_conv_weight(ro_w), ro_b, ops.pack_conv_weight(cw), cb, cw.shape[0])
             if self.cfg["mask"]:  # controller conv3x3 256 -> 169 dynamic-conv parameters (unicorn_head_mask.py:238-247,333-334)
@@ -159,7 +174,6 @@ class UnicornEngine:
                              out=(pw(mb + "tower.4.weight"), f(mb + "tower.4.bias")),
                              up0=(pw(mb + "up_mask_layer.0.weight"), f(mb + "up_mask_layer.0.bias")),
                              up2=(pw(mb + "up_mask_layer.2.weight"), f(mb + "up_mask_layer.2.bias")))
-        self.P = P
 
     def _load_convnext(self, sd, P, b, f, pw, block):
         dev = self.dev
@@ -546,6 +560,7 @@ class UnicornEngine:
         """Projection of a fixed reference frame (level 0 of the encoder input), computed once and OWNED BY THE CALLER: several
         trackers may share one engine, each keeps its own reference (the reference repo keeps `out_dict_pre` per tracker,
         unicorn_sot.py:47).  Pass the result to interaction(ref_proj=...).  feat [B,h,w,C] -> (src, q) [B*h*w, 256] each."""
+        self._tracking_only("project_ref")
         B, h, w = feat.shape[:3]
         src = torch.empty(B * h * w, 256, dtype=BF16, device=self.dev)
         q = torch.empty(B * h * w, 256, dtype=BF16, device=self.dev)
@@ -574,6 +589,7 @@ class UnicornEngine:
         [B,h,w,256].  ref_proj = project_ref(feat0) of fixed reference frames ([B*h*w, 256] each): its rows are copied in instead
         of being recomputed.  Token rows are [2][B][h*w] (all reference rows, then all current rows): every projection is one
         batched conv, and the deformable attention samples each image's own rows."""
+        self._tracking_only("interaction")
         B, h, w = feat1.shape[:3]
         n = B * h * w
         src, q = self.buf("enc.src", (2 * n, 256)), self.buf("enc.q", (2 * n, 256))
@@ -588,6 +604,7 @@ class UnicornEngine:
 
     def upsample(self, feat, tag):
         """Unicorn.forward_upsample (unicorn.py:41-44,311-313): [B,h,w,256] -> embedding [B,2h,2w,128] fp16."""
+        self._tracking_only("upsample")
         B, h, w, _ = feat.shape
         ps = ops.pixel_shuffle2(feat, out=self.buf(tag + ".ps", (B, 2 * h, 2 * w, 64)))
         t = self.conv(ps, self.P["up1"][0], 3, 1, 1, bias=self.P["up1"][1], act=ACT_RELU, out=self.buf(tag + ".u1", (B, 2 * h, 2 * w, 256)))
@@ -597,6 +614,7 @@ class UnicornEngine:
     def propagate(self, embed_ref, embed_cur, values):
         """unicorn_sot.py:88-105: label propagation + prior pyramid.  B = 1: values fp32 [K, h8*w8] -> 3 fp32 maps [K,h,w].
         B > 1 (embeddings [B,h,w,C]): values [B, K, h8*w8] -> 3 maps [B,K,h,w], every sequence against its own reference."""
+        self._tracking_only("propagate")
         B, hh, ww, C = embed_cur.shape
         if B == 1:
             K = values.shape[0]
@@ -616,6 +634,7 @@ class UnicornEngine:
     def mask_branch(self, fpn):
         """MaskBranch.forward with use_raft (condinst/mask_branch.py:77-96,158-162) of B images: -> (mask_feats fp32 [B,h8,w8,8],
         up_masks fp32 [B,h8,w8,144])."""
+        self._tracking_only("mask_branch")
         M = self.P["mask"]
         B, h, w, _ = fpn[0].shape
         x = self.conv_gn(fpn[0], M["refine"][0], self.buf("mask.x", (B, h, w, 128)), act=ACT_RELU)
@@ -631,11 +650,15 @@ class UnicornEngine:
         um = self.conv(u, M["up2"][0], 1, bias=M["up2"][1], out=self.buf("mask.up", (B, h, w, 144), F32))
         return mf, um
 
-    def head(self, fpn, priors, mode, with_masks=False):
+    def head(self, fpn, priors, mode, with_masks=False, decode=True):
         """UnicornHead.forward eval branch (unicorn_head.py:267-336) + decode_outputs (:467-482) of B images.
         fpn: 3 NHWC bf16 maps [B,h,w,C]; priors: 3 fp32 maps with B*h*w elements each ([B,h,w], or [B,1,h,w] from propagate) or None
         (MOT: zero prior == no fusion term).  Returns fp32 [B, A, 5+ncls_mode].  with_masks=True (UnicornHeadMask, unicorn_head_mask.py:333-343) also runs the
-        controller convs; their outputs are left in self.dyn_levels (3 x fp32 [B,h,w,176]) for ops.dynamic_masks."""
+        controller convs; their outputs are left in self.dyn_levels (3 x fp32 [B,h,w,176]) for ops.dynamic_masks.
+        The per-level prediction maps (reg+obj fp32 [B,h,w,8], class logits fp32 [B,h,w,round_up(ncls, 8)]) and their sizes are left in
+        self.head_maps for post_ops.det_candidates; decode=False skips the decoded tensor and returns None."""
+        if self.det and (mode == "sot" or priors is not None or with_masks):
+            raise ValueError(f"UnicornEngine.head: {self.cfg_name} is a detector: mode 'mot' (or 'whole'), no priors, no masks")
         B = fpn[0].shape[0]
         self._with_masks = with_masks
         self.dyn_levels = [None] * 3
@@ -655,6 +678,9 @@ class UnicornEngine:
         self._head_level(0, fpn, priors, sfx, ro_outs, cls_outs, hw)
         for s_ in self._side_streams:  # join
             main.wait_stream(s_)
+        self.head_maps = (ro_outs, cls_outs, hw)
+        if not decode:
+            return None
         A = sum(h * w for h, w in hw)
         return ops.head_decode(ro_outs, cls_outs, hw, STRIDES, ncls, out=self.buf(f"head.out{ncls}", (B, A, 5 + ncls), F32))
 
@@ -674,12 +700,17 @@ class UnicornEngine:
                     cur = self.conv_gn(cur, c, self.buf(f"head{k}.{name}{i % 2}", (B, h, w, 256)))
                 feats.append(cur)
             row, rob, cw, cb, _ = L["pred" + sfx]
-            cls_outs[k] = ops.conv2d(feats[0], cw, 1, 1, bias=cb, out=self.buf(f"head{k}.clso", (B, h, w, 8), F32))
+            cls_outs[k] = ops.conv2d(feats[0], cw, 1, 1, bias=cb, out=self.buf(f"head{k}.clso", (B, h, w, cb.numel()), F32))
             ro_outs[k] = ops.conv2d(feats[1], row, 1, 1, bias=rob, out=self.buf(f"head{k}.roo", (B, h, w, 8), F32))
             hw[k] = (h, w)
             if self._with_masks:
                 cw_, cb_ = L["ctrl"]
                 self.dyn_levels[k] = self.conv(feats[1], cw_, 3, 1, 1, bias=cb_, out=self.buf(f"head{k}.dyn", (B, h, w, 176), F32))
+
+
+def _cls_cols(ncls):
+    """Columns of a class-logit map: the class count rounded up to the 8-row padding of the packed weights (8 for every tracking head)."""
+    return (ncls + 7) // 8 * 8
 
 
 def _rows(t):

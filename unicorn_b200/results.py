@@ -122,3 +122,20 @@ def mots_frame_result(frame_id, boxes, ids, masks, img_h, img_w, min_box_area=10
             rles.append(rle_encode(free[i]))
             out_ids.append(tid + 1)  # 1-based ids for the MOTS files
     return frame_id, out_ids, cat_id, img_h, img_w, rles
+
+
+def coco_detections(rows, r, image_id, class_ids):
+    """COCOEvaluator.convert_to_coco_format (unicorn/evaluators/coco_evaluator.py:128-158) for one image: rows fp32 [n, 7] (postprocess
+    output in network-input pixels), r = the letterbox scale min(H / h, W / w), class_ids = the dataset's COCO category id of each
+    contiguous class.  Returns the evaluator's dicts: bbox xywh in original pixels, score = obj * cls_conf."""
+    if rows is None:
+        return []
+    rows = torch.as_tensor(rows).cpu()
+    bboxes = rows[:, 0:4].clone()
+    bboxes /= r
+    bboxes[:, 2] = bboxes[:, 2] - bboxes[:, 0]
+    bboxes[:, 3] = bboxes[:, 3] - bboxes[:, 1]
+    cls = rows[:, 6]
+    scores = rows[:, 4] * rows[:, 5]
+    return [{"image_id": int(image_id), "category_id": class_ids[int(cls[i])], "bbox": bboxes[i].numpy().tolist(),
+             "score": scores[i].numpy().item(), "segmentation": []} for i in range(bboxes.shape[0])]

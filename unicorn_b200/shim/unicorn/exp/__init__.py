@@ -17,6 +17,9 @@ class Exp:
             raise KeyError(f"unicorn_b200 has no config {exp_name!r} (known: {sorted(CONFIGS)})")
         cfg = CONFIGS[exp_name]
         self.exp_name = exp_name
+        if cfg["task"] == "det":
+            self._init_det(cfg)
+            return
         self.num_classes = cfg["num_classes"]       # unicorn_track.py:36 (8) / *_mot_challenge.py:18 (1)
         if cfg["backbone"] == "resnet50":
             self.backbone_name = "resnet50"          # exps/default/unicorn_track_r50*.py
@@ -35,6 +38,24 @@ class Exp:
             self.use_raft = True                    # unicorn_track_mask.py:44
             self.d_rate = 2                         # unicorn_track_mask.py:45
             self.ctrl_loc = "reg"                   # unicorn_track_mask.py:38
+        self.model = None
+
+    def _init_det(self, cfg):
+        """exp/unicorn_det.py:22-92 with exps/default/unicorn_det_*_800x1280.py: the COCO detector (YOLOX + YOLOXHeadDet)."""
+        self.task = "det"
+        self.num_classes = cfg["num_classes"]      # unicorn_det.py:25 (COCO)
+        if cfg["backbone"] == "resnet50":
+            self.backbone_name = "resnet50"         # unicorn_det_r50_800x1280.py
+        else:
+            self.backbone_name = "convnext_large" if "large" in self.exp_name else "convnext"  # unicorn_det.py:30
+        self.in_channels = list(cfg["in_channels"])
+        self.normalize = False                     # unicorn_det.py:62
+        self.test_size = (800, 1280)               # exps/default/unicorn_det_*_800x1280.py
+        self.input_size = (800, 1280)
+        self.test_conf = 0.01                      # unicorn_det.py:88-89
+        self.nmsthre = 0.65
+        self.output_dir = "./Unicorn_outputs"
+        self.mask = False
         self.model = None
 
     def get_model(self, load_pretrain=True):
@@ -68,4 +89,6 @@ def get_exp(exp_file=None, exp_name=None):
     """unicorn/exp/build.py:35-50."""
     assert exp_file is not None or exp_name is not None, "plz provide exp file or exp name."
     name = os.path.basename(exp_file).split(".")[0] if exp_file is not None else exp_name
+    if name.startswith("unicorn_det_") and name.endswith("_800x1280"):  # exps/default/unicorn_det_*_800x1280.py: the input size is an
+        name = name[:-len("_800x1280")]                                  # attribute of the Exp, not part of the config
     return Exp(name)

@@ -23,8 +23,14 @@ CONFIGS = {
     # exps/default/unicorn_track_r50*.py: torchvision ResNet-50 (v1.5 Bottlenecks); dims = the stage output widths (4 x 64/128/256/512)
     "unicorn_track_r50": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=False),
     "unicorn_track_r50_mask": dict(backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=8, mask=True),
+    # the COCO detectors (exps/default/unicorn_det_*_800x1280.py, YOLOX + YOLOXHeadDet): backbone, neck and an 80-class head without the
+    # prior term, the SOT predictors and the interaction modules; the first stage of the tracking models of the same backbone
+    "unicorn_det_convnext_tiny": dict(task="det", depths=(3, 3, 9, 3), dims=(96, 192, 384, 768), num_classes=80, mask=False),
+    "unicorn_det_convnext_large": dict(task="det", depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=80, mask=False),
+    "unicorn_det_r50": dict(task="det", backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=80, mask=False),
 }
 for _c in CONFIGS.values():
+    _c.setdefault("task", "track")
     _c.setdefault("backbone", "convnext")
     _c["in_channels"] = tuple(_c["dims"][1:])  # channels of the s8 / s16 / s32 maps the neck, heads and interaction read
 
@@ -57,7 +63,7 @@ def param_shapes(cfg_name):
                 cin = 4 * w
     else:
         _convnext_shapes(S, b, depths, dims)
-    _neck_and_heads(S, inc, ncls, cfg["mask"])
+    _neck_and_heads(S, inc, ncls, cfg["mask"], cfg["task"] == "det")
     return S
 
 
@@ -82,7 +88,9 @@ def _convnext_shapes(S, b, depths, dims):
         S[b + f"norm{i}.weight"] = (dims[i],); S[b + f"norm{i}.bias"] = (dims[i],)
 
 
-def _neck_and_heads(S, inc, ncls, mask):
+def _neck_and_heads(S, inc, ncls, mask, det=False):
+    """The neck and the head; det=True: YOLOXHeadDet (yolo_head_det.py:53-190), the head without the prior scales (`beta_*`), the
+    SOT predictors and the interaction / upsampling modules that follow it."""
     def baseconv(p, cin, cout, k):
         S[p + "conv.weight"] = (cout, cin, k, k)
         S[p + "bn.weight"] = (cout,); S[p + "bn.bias"] = (cout,)
@@ -106,7 +114,7 @@ def _neck_and_heads(S, inc, ncls, mask):
     baseconv(p + "bu_conv1.", inc[1], inc[1], 3)
     csp(p + "C3_n4.", 2 * inc[1], inc[2])
     h = "head."
-    for k in range(3):
+    for k in range(3 if not det else 0):
         S[h + f"beta_{k}"] = (256, 1, 1)
     for k in range(3):
         for i in range(4):
@@ -114,8 +122,8 @@ def _neck_and_heads(S, inc, ncls, mask):
     for k in range(3):
         for i in range(4):
             baseconv(h + f"reg_convs.{k}.{i}.", 256, 256, 3)
-    for name, co in (("cls_preds", ncls), ("reg_preds", 4), ("obj_preds", 1), ("cls_preds_sot", 1), ("obj_preds_sot", 1),
-                     ("reg_preds_sot", 4)):
+    preds = (("cls_preds", ncls), ("reg_preds", 4), ("obj_preds", 1))
+    for name, co in preds + (() if det else (("cls_preds_sot", 1), ("obj_preds_sot", 1), ("reg_preds_sot", 4))):
         for k in range(3):
             S[h + f"{name}.{k}.weight"] = (co, 256, 1, 1); S[h + f"{name}.{k}.bias"] = (co,)
     if mask:
@@ -137,6 +145,8 @@ def _neck_and_heads(S, inc, ncls, mask):
     for k in range(3):
         for n in range(3):
             _convnext_block(S, h + f"att_layers.{k}.{n}.", 256)
+    if det:
+        return
     S["bottleneck.0.weight"] = (256, inc[1], 1, 1); S["bottleneck.0.bias"] = (256,)
     S["bottleneck.1.weight"] = (256,); S["bottleneck.1.bias"] = (256,)
     S["upsample_layer.1.weight"] = (256, 64, 3, 3); S["upsample_layer.1.bias"] = (256,)
