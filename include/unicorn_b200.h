@@ -363,6 +363,21 @@ UC_API int uc_mots_encode_batched(const float* masks, long bs_masks, int n_max, 
                                   const int* W, const double* r, const int* order, const uint8_t* emit, float thr, void* workspace,
                                   long workspace_bytes, char* chars, long capacity, long long* offsets, void* stream);
 
+/* COCO instance-segmentation result encoding on the device (unicorn/evaluators/coco_inst_evaluator.py convert_to_coco_format): one
+ * COCO compressed RLE string per (image, row) slot of B images (1 <= B <= UC_MOTS_MAX_IMAGES), without the full-resolution masks.
+ * maps: f32 image b at maps + b * bs_maps, [n_max, hs, ws], the sigmoid masks uc_dynamic_masks_batched writes with d_rate = 1 for
+ * NMS rows row0 .. row0 + n_max - 1.  Slot j = b * n_max + i holds row row0 + i of image b; it is emitted (emit[j] = 1, written by
+ * the call: device uint8 [B * n_max]) when row0 + i < count_dev[b] (device int32 [B], read on the device), else it gets an empty
+ * string.  Each emitted mask is upsampled by aligned_bilinear(x d_rate) to the network input (hs * d_rate) x (ws * d_rate), bit for
+ * bit as uc_dynamic_masks stores it, resized by 1/r[b] to the original frame as in uc_mots_encode, thresholded (> thr) and encoded
+ * over the whole H[b] x W[b] frame: pixels outside the hm x wm corner the resize covers are background.  There is no overlap removal.
+ * H, W, r: HOST arrays of B.  offsets: device int64 [B * n_max + 1]; chars / capacity as in uc_mots_encode (idempotent: re-run with a
+ * larger buffer).  workspace: uc_mots_encode_workspace_bytes(B * n_max, max H[b], max W[b]) bytes, 16-byte aligned.  B * n_max <= 65535.
+ * Every argument is validated before any CUDA call; no allocation, no synchronisation, graph-capturable; three launches. */
+UC_API int uc_inst_encode_batched(const float* maps, long bs_maps, int n_max, int hs, int ws, int d_rate, int B, const int* count_dev,
+                                  int row0, const int* H, const int* W, const double* r, float thr, void* workspace, long workspace_bytes,
+                                  uint8_t* emit, char* chars, long capacity, long long* offsets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

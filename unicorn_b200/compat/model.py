@@ -169,7 +169,21 @@ class UnicornB200Model:
             assert imgs.is_cuda and imgs.dim() == 4 and imgs.shape[0] >= 1, "CUDA NCHW images [B,3,H,W]"
             e.begin_frame()
             fpn, _ = e.backbone(imgs.float().contiguous(), tag="compat")
-            return e.head(fpn, None, "mot").clone()
+            if not self.cfg["mask"]:
+                return e.head(fpn, None, "mot").clone()
+            # YOLOXHeadDetMask (yolo_head_det_mask.py:344-363, use_raft): (decoded [B,A,85], locations [A,2], dynamic_params [B,A,169],
+            # fpn_levels [B,A], mask_feats [B,8,h,w], up_masks [B,144,h,w])
+            out = e.head(fpn, None, "mot", with_masks=True).clone()
+            B = out.shape[0]
+            dyn = torch.cat([d[..., :169].reshape(B, -1, 169) for d in e.dyn_levels], 1).contiguous()
+            locs, lvls = [], []
+            for k, d in enumerate(e.dyn_levels):
+                h, w = d.shape[1:3]
+                yv, xv = torch.meshgrid(torch.arange(h, device=d.device), torch.arange(w, device=d.device), indexing="ij")
+                locs.append((torch.stack((xv, yv), 2).view(-1, 2).float() + 0.5) * STRIDES[k])  # decode_outputs :404
+                lvls.append(torch.full((B, h * w), k, device=d.device, dtype=torch.long))
+            mf, um = e.mask_branch(fpn)
+            return out, torch.cat(locs, 0), dyn, torch.cat(lvls, 1), mf.permute(0, 3, 1, 2).contiguous(), um.permute(0, 3, 1, 2).contiguous()
         if mode == "backbone":
             fpn, seq_dict = self._backbone(imgs)
             return tuple(ops.nhwc_to_nchw(t) for t in fpn), seq_dict

@@ -372,6 +372,120 @@ __global__ void __launch_bounds__(256) mots_planes_kernel(const float* __restric
   }
 }
 
+// ------------------------------------------------------------------------------------------------ COCO instance encoding
+// COCOInstEvaluator.convert_to_coco_format (unicorn/evaluators/coco_inst_evaluator.py): every NMS row's mask
+// aligned_bilinear(x f)-upsampled to the network input (utils/boxes.py:138-145), resized by 1/r to the original frame
+// (F.interpolate(scale_factor=1/r, bilinear)[:, 0, :H, :W]) and thresholded, without writing the full-resolution mask.  The encoded
+// mask is the whole H x W frame: pixels outside the hm x wm corner the resize produces are background.
+//
+// The sample of mask_final_up_kernel at full-resolution pixel (Y, X), with the operation order nvcc gives that kernel (its SASS:
+// one product per source row, fused with the other column's term, then the rows the same way): bit-identical to what it stores.
+// fy == 0 (every other row at f = 2, the same for the whole warp) skips the second source row: the maps are sigmoid outputs in
+// [0, 1], so fma(1, top, 0 * bot) == top exactly.
+__device__ __forceinline__ float final_up_at(const float* __restrict__ s, int ws, int y0, int y1, float fy, int x0, int x1, float fx) {
+  const float gx = 1.f - fx;
+  const float top = __fmaf_rn(fx, s[y0 * ws + x1], __fmul_rn(gx, s[y0 * ws + x0]));
+  if (fy == 0.f) return top;
+  const float bot = __fmaf_rn(fx, s[y1 * ws + x1], __fmul_rn(gx, s[y1 * ws + x0]));
+  return __fmaf_rn(1.f - fy, top, __fmul_rn(fy, bot));
+}
+// resize_sample's order of operations in mots_planes_kernel (its SASS), on the four taps of the resize
+__device__ __forceinline__ float resize_mix(float a, float b, float c, float d, float ly, float lx) {
+  const float gx = 1.f - lx;
+  const float top = __fmaf_rn(gx, a, __fmul_rn(lx, b));
+  const float bot = __fmaf_rn(gx, c, __fmul_rn(lx, d));
+  return __fmaf_rn(1.f - ly, top, __fmul_rn(ly, bot));
+}
+// The aligned_bilinear taps of the two full-resolution indices i0, i1 the resize reads.
+struct AbTaps {
+  int a0, a1, b0, b1;
+  float fa, fb;
+};
+// ab_coord's taps; for a power-of-two f the fraction k / f is exact, so k * (1 / f) is the same float without the division.
+__device__ __forceinline__ void ab_coord_fast(int i, int f, float inv_f, int n, int& i0, int& i1, float& frac) {
+  if (inv_f == 0.f) {
+    ab_coord(i, f, n, i0, i1, frac);
+    return;
+  }
+  const int ii = max(i - f / 2, 0);
+  i0 = ii / f;
+  frac = static_cast<float>(ii - i0 * f) * inv_f;
+  i1 = min(i0 + 1, n - 1);
+  i0 = min(i0, n - 1);
+}
+__device__ __forceinline__ AbTaps ab_taps(int i0, int i1, int f, float inv_f, int n) {
+  AbTaps t;
+  ab_coord_fast(i0, f, inv_f, n, t.a0, t.a1, t.fa);
+  ab_coord_fast(i1, f, inv_f, n, t.b0, t.b1, t.fb);
+  return t;
+}
+// The resized, upsampled mask at original-frame pixel (y, x) of the column taps tx (x resized to lx).
+__device__ __forceinline__ float inst_sample(const float* __restrict__ s, int hs, int ws, int f, float inv_f, int Hin, float scale, int y,
+                                            const AbTaps& tx, float lx) {
+  int Y0, Y1;
+  float ly;
+  resize_src(y, scale, Hin, Y0, Y1, ly);
+  const AbTaps ty = ab_taps(Y0, Y1, f, inv_f, hs);
+  return resize_mix(final_up_at(s, ws, ty.a0, ty.a1, ty.fa, tx.a0, tx.a1, tx.fa), final_up_at(s, ws, ty.a0, ty.a1, ty.fa, tx.b0, tx.b1, tx.fb),
+                    final_up_at(s, ws, ty.b0, ty.b1, ty.fb, tx.a0, tx.a1, tx.fa), final_up_at(s, ws, ty.b0, ty.b1, ty.fb, tx.b0, tx.b1, tx.fb),
+                    ly, lx);
+}
+
+// The part of each image's H x W frame the resize covers (rows < hv, columns < wv).
+struct InstCover {
+  int hv[kMotsMaxImages], wv[kMotsMaxImages];
+};
+
+// Pass 1 of the instance encode: slot j = blockIdx.z (image b = j / n_max, row row0 + j % n_max of its NMS output) is emitted when
+// that row exists (count[b] on the device); one thread per word of the slot's H x W frame, as in mots_planes_kernel, with no state
+// between instances.  maps: the d_rate = 1 output of uc_dynamic_masks_batched, [B, n_max, hs, ws] (image b at b * bs_maps).
+__global__ void __launch_bounds__(256) inst_planes_kernel(const float* __restrict__ maps, long bs_maps, int n_max, int hs, int ws, int f,
+                                                          const int* __restrict__ count, int row0, float thr,
+                                                          const __grid_constant__ MotsImages im, const __grid_constant__ InstCover cv,
+                                                          MotsWs wsp, uint8_t* __restrict__ emit) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int j = blockIdx.z, b = j / n_max, i = j - b * n_max;
+  const bool on = i < count[b] - row0;
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0) emit[j] = on;
+  if (!on) return;
+  const int H = im.hm[b], W = im.wm[b], hv = cv.hv[b], wv = cv.wv[b];
+  const float scale = im.scale[b];
+  const int x = blockIdx.x * 32 + threadIdx.x, wy = blockIdx.y * 8 + threadIdx.y, hw32 = (H + 31) / 32;
+  if (x >= W || wy >= hw32) return;
+  const int Hin = hs * f, Win = ws * f;
+  const float inv_f = (f & (f - 1)) == 0 ? 1.f / f : 0.f;  // 0: divide
+  const float* s = maps + b * bs_maps + static_cast<long>(i) * hs * ws;
+  AbTaps tx{}, tp{};
+  float lx = 0.f, lp = 0.f;
+  if (x < wv) {
+    int X0, X1;
+    resize_src(x, scale, Win, X0, X1, lx);
+    tx = ab_taps(X0, X1, f, inv_f, ws);
+  }
+  // the pixel before this word in column-major order: row 32 wy - 1 of column x, or the last row of column x - 1
+  const int py = wy > 0 ? 32 * wy - 1 : H - 1, px = wy > 0 ? x : x - 1;
+  const bool prev_in = px >= 0 && px < wv && py < hv;
+  if (prev_in && px != x) {
+    int X0, X1;
+    resize_src(px, scale, Win, X0, X1, lp);
+    tp = ab_taps(X0, X1, f, inv_f, ws);
+  } else if (prev_in) {
+    tp = tx;
+    lp = lx;
+  }
+  const int ybase = 32 * wy, nrows = min(32, H - ybase);
+  const uint32_t valid = nrows == 32 ? ~0u : (1u << nrows) - 1u;
+  uint32_t raw = 0;
+  if (x < wv) {
+    const int rows = min(nrows, hv - ybase);
+#pragma unroll 4
+    for (int r = 0; r < rows; ++r) raw |= static_cast<uint32_t>(inst_sample(s, hs, ws, f, inv_f, Hin, scale, ybase + r, tx, lx) > thr) << r;
+  }
+  const uint32_t rawp = prev_in ? inst_sample(s, hs, ws, f, inv_f, Hin, scale, py, tp, lp) > thr : 0u;
+  wsp.diff[im.diff0[b] + static_cast<long>(i) * W * hw32 + static_cast<long>(x) * hw32 + wy] = (raw ^ ((raw << 1) | rawp)) & valid;
+}
+
 // Run state after a prefix of the boundaries: their number and the last three boundary positions (-1: none).
 __device__ __forceinline__ int4 run_push(int4 s, int pos) { return make_int4(s.x + 1, pos, s.y, s.z); }
 __device__ __forceinline__ int4 run_cat(int4 a, int4 b) {
@@ -686,4 +800,60 @@ extern "C" int uc_mots_encode_batched(const float* masks, long bs_masks, int n_m
                                       long workspace_bytes, char* chars, long capacity, long long* offsets, void* stream_v) {
   return mots_encode("uc_mots_encode_batched", true, masks, bs_masks, n_max, Hin, Win, B, k, H, W, r, order, emit, thr, workspace,
                      workspace_bytes, chars, capacity, offsets, static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_inst_encode_batched(const float* maps, long bs_maps, int n_max, int hs, int ws, int d_rate, int B, const int* count_dev,
+                                      int row0, const int* H, const int* W, const double* r, float thr, void* workspace,
+                                      long workspace_bytes, uint8_t* emit, char* chars, long capacity, long long* offsets, void* stream_v) {
+  const char* what = "uc_inst_encode_batched";
+  if (!H || !W || !r) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1 || B > kMotsMaxImages) return set_error(UC_EINVAL, "%s: B = %d must be in 1..%d", what, B, kMotsMaxImages);
+  if (!maps || !count_dev || !workspace || !emit || !offsets || (capacity > 0 && !chars)) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (n_max < 1 || hs < 1 || ws < 1 || d_rate < 1) return set_error(UC_EINVAL, "%s: bad sizes", what);
+  if (static_cast<long>(B) * n_max > 65535) return set_error(UC_EINVAL, "%s: B * n_max = %ld slots must be <= 65535", what, static_cast<long>(B) * n_max);
+  if (row0 < 0) return set_error(UC_EINVAL, "%s: row0 = %d must be >= 0", what, row0);
+  if (bs_maps < static_cast<long>(n_max) * hs * ws)
+    return set_error(UC_EINVAL, "%s: bad per-image stride %ld (>= n_max*hs*ws = %ld)", what, bs_maps, static_cast<long>(n_max) * hs * ws);
+  char at[96];
+  for (int b = 0; b < B; ++b) {
+    snprintf(at, sizeof(at), "%s: image %d", what, b);
+    if (H[b] < 1 || W[b] < 1 || !(r[b] > 0.0)) return set_error(UC_EINVAL, "%s: bad sizes", at);
+  }
+  if (capacity < 0) return set_error(UC_EINVAL, "%s: negative capacity", what);
+  if ((reinterpret_cast<uintptr_t>(maps) | reinterpret_cast<uintptr_t>(count_dev)) % 4 || reinterpret_cast<uintptr_t>(offsets) % 8 ||
+      reinterpret_cast<uintptr_t>(workspace) % 16)
+    return set_error(UC_EINVAL, "%s: maps / count must be 4-byte, offsets 8-byte, workspace 16-byte aligned", what);
+  const int K = B * n_max;
+  MotsImages im;
+  InstCover cv;
+  im.n = B;
+  im.k0[0] = 0;
+  long diff_words = 0;
+  int w_max = 0, hw32_max = 0;
+  for (int b = 0; b < B; ++b) {
+    snprintf(at, sizeof(at), "%s: image %d", what, b);
+    const FrameResize rs = frame_resize(hs * d_rate, ws * d_rate, H[b], W[b], r[b]);
+    if (rs.hm < 1 || rs.wm < 1) return set_error(UC_EINVAL, "%s: the resized mask is empty (r too large)", at);
+    const int hw32 = (H[b] + 31) / 32;
+    const long words = static_cast<long>(W[b]) * hw32;
+    if (words > (1L << 31) / 32) return set_error(UC_EINVAL, "%s: frame too large", at);
+    im.k0[b + 1] = im.k0[b] + n_max;
+    im.hm[b] = H[b];
+    im.wm[b] = W[b];
+    im.scale[b] = rs.scale;
+    im.diff0[b] = diff_words;
+    cv.hv[b] = rs.hm;
+    cv.wv[b] = rs.wm;
+    diff_words += n_max * words;
+    w_max = std::max(w_max, W[b]);
+    hw32_max = std::max(hw32_max, hw32);
+  }
+  if (workspace_bytes < mots_workspace_bytes(K, diff_words)) return set_error(UC_EINVAL, "%s: workspace too small", what);
+  MotsWs wsp = mots_ws(workspace, K, diff_words);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  launch_pdl(inst_planes_kernel, dim3((w_max + 31) / 32, (hw32_max + 7) / 8, K), dim3(32, 8), 0, stream, maps, bs_maps, n_max, hs, ws, d_rate,
+             count_dev, row0, thr, im, cv, wsp, emit);
+  launch_pdl(mots_runs_kernel, K, kMotsThreads, 0, stream, static_cast<const uint8_t*>(emit), im, wsp);
+  launch_pdl(mots_chars_kernel, K, kMotsThreads, 0, stream, static_cast<const uint8_t*>(emit), im, wsp, chars, capacity, offsets);
+  return check_launch(what);
 }

@@ -10,6 +10,7 @@ import torch
 from . import _lib, ops, post_ops
 from .engine import STRIDES, UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count, in_flight
+from .mots import MaskEncoder
 
 
 class UnicornDetector:
@@ -40,14 +41,17 @@ class UnicornDetector:
         self._ring = Ring(in_flight(eng, depth, make))
         self.launches_per_step = 0
 
+    with_masks = False  # the head also runs the controller convs (UnicornInstanceSegmenter)
+
     def _frame(self, c):
         e = c.eng
         e.begin_frame()
         fpn, _ = e.backbone(c.img, tag="det")
-        e.head(fpn, None, "mot", decode=False)
+        e.head(fpn, None, "mot", decode=False, with_masks=self.with_masks)
         ro, cl, hw = e.head_maps
         post_ops.det_candidates(ro, cl, hw, STRIDES, e.ncls, self.conf, c.ws)
         post_ops.postprocess_nms(self.nms, c.ws, class_agnostic=self.class_agnostic)
+        return fpn
 
     def submit(self, images, rgb=False):
         """images: list of 1..max_batch uint8 HWC images (numpy arrays or tensors, host or device), BGR as cv2 loads them (rgb=True:
@@ -67,6 +71,7 @@ class UnicornDetector:
         with torch.cuda.stream(c.stream):
             c.ratios = []
             c.n = n
+            c.sizes = [(int(t.shape[0]), int(t.shape[1])) for t in srcs]
             for i, t in enumerate(srcs):
                 src = t.to(c.eng.dev, non_blocking=True).contiguous()
                 c.last[i] = src  # the upload stays alive until the step is collected
@@ -80,8 +85,12 @@ class UnicornDetector:
                 self._frame(c)
                 self.launches_per_step = _lib.LAUNCHES - l0
             c.warm = True
+            self._after_frame(c)
             c.count_host = c.ws.count.to("cpu", non_blocking=True)
             c.event.record()
+
+    def _after_frame(self, c):
+        """Work of a step that follows its graph (or eager frame) on the step's stream, before the counts are copied back."""
 
     def collect(self):
         """Rows of the oldest submitted step: a list of (rows fp32 [n, 7] CPU tensor in descending score order, r), one per image."""
@@ -96,3 +105,88 @@ class UnicornDetector:
         """One step: submit(images) then collect()."""
         self.submit(images, rgb)
         return self.collect()
+
+
+class UnicornInstanceSegmenter(UnicornDetector):
+    """UnicornInstanceSegmenter(eng, input_size, max_batch, conf, nms, use_graph, depth, mask_thres, d_rate, chunk, capacity): the
+    COCO instance segmenter (unicorn_inst_convnext_tiny: YOLOX + YOLOXHeadDetMask) on the letterbox, batching and submit / collect
+    protocol of UnicornDetector, with class-aware NMS.
+
+    collect() returns, per image, (rows fp32 [n, 7] as UnicornDetector gives them, r, rles): rles[i] is the COCO compressed RLE of row
+    i's mask over the image's original h x w, as COCOInstEvaluator.convert_to_coco_format makes it (utils/boxes.py postprocess_inst:
+    the dynamic-conv mask of every NMS row, aligned_bilinear x d_rate; then resized by 1/r and thresholded > mask_thres);
+    unicorn_b200.results.coco_instances turns them into the evaluator's dicts.
+
+    The masks of NMS rows are made `chunk` rows at a time (dynamic masks at 1/d_rate of the input, then uc_inst_encode_batched, which
+    folds the final upsample into the resize, so the full-resolution masks are never stored).  The step's graph ends with the masks
+    of rows [0, chunk); their encode follows it on the step's stream.  collect() reads the row counts and, while an image has more
+    rows, runs the next chunk eagerly for all such images at once.  With seeded weights about 15000 rows per image survive NMS at
+    conf 0.01 (DESIGN.md section 4.11): that is 150 chunks per image."""
+
+    with_masks = True
+
+    def __init__(self, eng: UnicornEngine, input_size=(800, 1280), max_batch=1, conf=0.01, nms=0.65, use_graph=True, depth=1, mask_thres=0.3,
+                 d_rate=2, chunk=100, capacity=1 << 20):
+        if eng.cfg["task"] != "det" or not eng.cfg["mask"]:
+            raise ValueError(f"UnicornInstanceSegmenter: {eng.cfg_name} is not an instance-segmentation config")
+        if d_rate != 2 or chunk < 1 or max_batch > 64 or max_batch * chunk > 65535:
+            raise ValueError(f"UnicornInstanceSegmenter: d_rate 2 (the 144-channel up-mask layer upsamples x4), chunk >= 1, max_batch <= 64 "
+                             f"and max_batch * chunk <= 65535 (got {d_rate}, {chunk}, {max_batch})")
+        super().__init__(eng, input_size, max_batch, conf, nms, False, use_graph, depth)
+        self.mask_thres, self.d_rate, self.chunk = mask_thres, d_rate, chunk
+        H, W = self.input_size
+        up, h, w, dev = 8 // d_rate, H // 8, W // 8, eng.dev
+        self._up = up
+        self._image_of = torch.arange(max_batch, dtype=torch.int32, device=dev)
+        for c in self._ring.slots:
+            c.maps = torch.empty(max_batch, chunk, h * up, w * up, dtype=torch.float32, device=dev)
+            c.scratch = torch.empty(max_batch * chunk * h * w, dtype=torch.float32, device=dev)
+            c.window = torch.zeros(max_batch, dtype=torch.int32, device=dev)  # each image's rows in the current chunk
+            c.enc = MaskEncoder(max_batch * chunk, dev, capacity)
+
+    def _frame(self, c):
+        fpn = super()._frame(c)
+        c.mf, c.um = c.eng.mask_branch(fpn)
+        c.dyn = list(c.eng.dyn_levels)
+        self._masks(c, 0)
+
+    def _masks(self, c, row0):
+        """The d_rate = 1 masks of NMS rows row0 .. row0 + chunk - 1 of every image into c.maps."""
+        torch.sub(c.ws.count, row0, out=c.window).clamp_(0, self.chunk)
+        anchors = c.ws.anchors.view(self.max_batch, self.A)[:, row0:]
+        post_ops.dynamic_masks_rows(c.mf, c.um, c.dyn, [(t.shape[1], t.shape[2]) for t in c.dyn], anchors, c.window, self._image_of,
+                                    self.chunk, self._up, c.maps, c.scratch)
+
+    def _encode(self, c, row0):
+        post_ops.inst_encode(c.maps[:c.n], c.ws.count, row0, self.d_rate, self.mask_thres, c.ratios, [h for h, _ in c.sizes],
+                             [w for _, w in c.sizes], c.enc.ws, c.enc.d_emit, c.enc.d_chars, c.enc.d_offsets)
+
+    def _after_frame(self, c):
+        if c.n < self.max_batch:
+            c.ws.count[c.n:].zero_()  # idle slots have no rows
+        c.enc.reserve(max(h for h, _ in c.sizes), max(w for _, w in c.sizes))
+        c.enc.enqueue(c.n * self.chunk, lambda: self._encode(c, 0))
+
+    def collect(self):
+        """Rows and masks of the oldest submitted step: a list of (rows fp32 [n, 7] CPU tensor in descending score order, r, rles [n]),
+        one per image."""
+        c = self._ring.collect()
+        n, k, K = c.n, self.chunk, c.n * self.chunk
+        with torch.cuda.stream(c.stream):
+            c.event.synchronize()
+            counts = [int(v) for v in c.count_host[:n]]
+            flat = c.enc.strings(K, lambda: self._encode(c, 0))
+            rles = [flat[b * k:b * k + min(k, counts[b])] for b in range(n)]
+            row0 = k
+            while any(m > row0 for m in counts):
+                self._masks(c, row0)
+                run = lambda r=row0: self._encode(c, r)  # noqa: E731
+                c.enc.enqueue(K, run)
+                flat = c.enc.strings(K, run)
+                for b in range(n):
+                    rles[b] += flat[b * k:b * k + max(0, min(k, counts[b] - row0))]
+                row0 += k
+        dets = c.ws.dets.view(self.max_batch, self.A, 7)
+        out = [(dets[i, :counts[i]].cpu(), c.ratios[i], rles[i]) for i in range(n)]
+        c.last.clear()
+        return out

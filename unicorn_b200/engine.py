@@ -634,7 +634,8 @@ class UnicornEngine:
     def mask_branch(self, fpn):
         """MaskBranch.forward with use_raft (condinst/mask_branch.py:77-96,158-162) of B images: -> (mask_feats fp32 [B,h8,w8,8],
         up_masks fp32 [B,h8,w8,144])."""
-        self._tracking_only("mask_branch")
+        if not self.cfg["mask"]:
+            self._tracking_only("mask_branch")
         M = self.P["mask"]
         B, h, w, _ = fpn[0].shape
         x = self.conv_gn(fpn[0], M["refine"][0], self.buf("mask.x", (B, h, w, 128)), act=ACT_RELU)
@@ -657,8 +658,9 @@ class UnicornEngine:
         controller convs; their outputs are left in self.dyn_levels (3 x fp32 [B,h,w,176]) for ops.dynamic_masks.
         The per-level prediction maps (reg+obj fp32 [B,h,w,8], class logits fp32 [B,h,w,round_up(ncls, 8)]) and their sizes are left in
         self.head_maps for post_ops.det_candidates; decode=False skips the decoded tensor and returns None."""
-        if self.det and (mode == "sot" or priors is not None or with_masks):
-            raise ValueError(f"UnicornEngine.head: {self.cfg_name} is a detector: mode 'mot' (or 'whole'), no priors, no masks")
+        if self.det and (mode == "sot" or priors is not None or (with_masks and not self.cfg["mask"])):
+            raise ValueError(f"UnicornEngine.head: {self.cfg_name} is a detector: mode 'mot' (or 'whole'), no priors"
+                             + ("" if self.cfg["mask"] else ", no masks"))
         B = fpn[0].shape[0]
         self._with_masks = with_masks
         self.dyn_levels = [None] * 3

@@ -53,22 +53,38 @@ class MaskEncoder:
         waits for the k strings."""
         k = len(order)
         assert 0 < k <= self.k_max
-        if self.ws is None or img_h > self.ws_hw[0] or img_w > self.ws_hw[1]:
-            self.ws_hw = (max(img_h, self.ws_hw[0]), max(img_w, self.ws_hw[1]))
-            self.ws = ops.mots_encode_workspace(self.k_max, *self.ws_hw, self.dev)
+        self.reserve(img_h, img_w)
         self.h_order[:k] = torch.as_tensor(order, dtype=torch.int32)
         self.h_emit[:k] = torch.as_tensor(emit, dtype=torch.uint8)
         self.d_order[:k].copy_(self.h_order[:k], non_blocking=True)
         self.d_emit[:k].copy_(self.h_emit[:k], non_blocking=True)
+        run = lambda: encode(self.d_order[:k], self.d_emit[:k])  # noqa: E731
+        self.enqueue(k, run)
+        return self.strings(k, run)
+
+    def reserve(self, img_h, img_w):
+        """Grows the workspace to k_max instances on an img_h x img_w frame."""
+        if self.ws is None or img_h > self.ws_hw[0] or img_w > self.ws_hw[1]:
+            self.ws_hw = (max(img_h, self.ws_hw[0]), max(img_w, self.ws_hw[1]))
+            self.ws = ops.mots_encode_workspace(self.k_max, *self.ws_hw, self.dev)
+
+    def enqueue(self, k, encode):
+        """Runs encode() (launches that leave k strings in d_chars / d_offsets) on the current stream and queues the copy of the
+        offsets; strings() then waits for them."""
+        encode()
+        self.h_offsets[:k + 1].copy_(self.d_offsets[:k + 1], non_blocking=True)
+
+    def strings(self, k, encode):
+        """The k strings of the encode enqueue(k, encode) queued on the current stream: waits for it, re-runs encode() with larger
+        buffers while the chars do not fit, and reads the chars back."""
         stream = torch.cuda.current_stream()
         while True:
-            encode(self.d_order[:k], self.d_emit[:k])
-            self.h_offsets[:k + 1].copy_(self.d_offsets[:k + 1], non_blocking=True)
             stream.synchronize()
             total = int(self.h_offsets[k])
             if total <= self.d_chars.numel():
                 break
             self._alloc(max(total, 2 * self.d_chars.numel()))
+            self.enqueue(k, encode)
         self.h_chars[:total].copy_(self.d_chars[:total], non_blocking=True)
         stream.synchronize()
         s = self.h_chars[:total].numpy().tobytes().decode("ascii")

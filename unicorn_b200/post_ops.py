@@ -1,5 +1,6 @@
 """Wrappers of the detector's post-processing entry points (include/unicorn_b200.h: uc_postprocess_batched_ex,
-uc_det_candidates_batched, uc_postprocess_nms_batched), next to the ones of unicorn_b200.ops that the tracking frames use.  Their
+uc_det_candidates_batched, uc_postprocess_nms_batched, and for the instance segmenter uc_dynamic_masks_batched over a window of NMS
+rows and uc_inst_encode_batched), next to the ones of unicorn_b200.ops that the tracking frames use.  Their
 results are pinned bit for bit to head_decode + postprocess_device (tests/test_det_gpu.py)."""
 import ctypes
 
@@ -47,3 +48,42 @@ def postprocess_nms(nms, ws, max_keep=0, class_agnostic=False):
                                                _p(ws.buf), _l(ws.nbytes), _p(ws.dets), _p(ws.count), _p(ws.anchors), _S()),
                "uc_postprocess_nms_batched")
     return ws.dets, ws.count
+
+
+def dynamic_masks_rows(mask_feats, up_masks, dyn_levels, level_hw, anchors, count, image_of, n_max, up_rate, out, scratch,
+                       soi=(64.0, 128.0, 256.0)):
+    """uc_dynamic_masks_batched with d_rate = 1 for a window of NMS rows: image b's masks of rows row0 .. row0 + count[b] - 1, where
+    `anchors` is the [B, A] NMS anchor buffer viewed from column row0 (its image stride stays A) and count device int32 [B] holds
+    each image's rows in the window (at most n_max); image_of: device int32 [0, 1, ..., B-1].  mask_feats fp32 [B,h,w,8], up_masks fp32 [B,h,w,9*up^2]; out fp32
+    [B, n_max, h*up, w*up]; scratch >= B*n_max*h*w floats (the logits; d_rate = 1 needs no upsampling buffer)."""
+    B, h, w, _ = mask_feats.shape
+    assert mask_feats.is_contiguous() and up_masks.is_contiguous() and up_masks.shape[:3] == (B, h, w)
+    assert all(t.shape[0] == B and t.stride(-1) == 1 for t in dyn_levels) and anchors.dim() == 2 and anchors.shape[0] == B
+    assert count.dtype == torch.int32 and count.numel() == B and scratch.numel() >= B * n_max * h * w
+    assert out.shape == (B, n_max, h * up_rate, w * up_rate) and out.is_contiguous() and out.dtype == torch.float32
+    dl = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in dyn_levels])
+    hw = (ctypes.c_int * 6)(*[v for pair in level_hw for v in pair])
+    bs = (ctypes.c_long * 3)(*[t.stride(0) for t in dyn_levels])
+    assert image_of.dtype == torch.int32 and image_of.numel() == B
+    _lib.check(_L().uc_dynamic_masks_batched(_p(mask_feats), _p(up_masks), B, h, w, up_rate, 1, dl, dyn_levels[0].shape[-1], bs, hw,
+                                             (ctypes.c_int * 3)(8, 16, 32), (ctypes.c_float * 3)(*soi), _p(anchors), _l(anchors.stride(0)),
+                                             _p(count), _p(image_of), B, n_max, _p(scratch), _p(out), _S()), "uc_dynamic_masks_batched", 2)
+    return out
+
+
+def inst_encode(maps, count, row0, d_rate, thr, r, H, W, ws, emit, chars, offsets):
+    """COCO RLE strings of the masks of NMS rows row0 .. row0 + n_max - 1 of B images (uc_inst_encode_batched): maps fp32
+    [B, n_max, hs, ws], the d_rate = 1 output of dynamic_masks_rows, upsampled x d_rate, resized by 1/r[b] to the original H[b] x W[b],
+    thresholded at thr and encoded over the whole frame.  count: device int32 [B], every image's NMS row count.  r, H, W: B host
+    values.  emit uint8 [>= B*n_max], offsets int64 [>= B*n_max + 1] device outputs; chars: uint8 device buffer (its size is the
+    capacity), nothing past it is written.  Launches only: offsets[B*n_max] is the number of chars needed."""
+    B, n_max, hs, wsz = maps.shape
+    assert maps.dtype == torch.float32 and maps.stride(3) == 1 and maps.stride(2) == wsz and maps.stride(1) == hs * wsz
+    assert count.dtype == torch.int32 and count.numel() >= B and len(r) == len(H) == len(W) == B
+    assert emit.dtype == torch.uint8 and emit.numel() >= B * n_max and offsets.dtype == torch.int64 and offsets.numel() >= B * n_max + 1
+    assert chars.dtype == torch.uint8 and ws.dtype == torch.uint8
+    ints = lambda v: (ctypes.c_int * B)(*[int(x) for x in v])  # noqa: E731
+    _lib.check(_L().uc_inst_encode_batched(_p(maps), _l(maps.stride(0)), n_max, hs, wsz, int(d_rate), B, _p(count), int(row0), ints(H), ints(W),
+                                           (ctypes.c_double * B)(*[float(x) for x in r]), _f(thr), _p(ws), _l(ws.numel()), _p(emit),
+                                           _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_inst_encode_batched", 3)
+    return offsets

@@ -139,3 +139,29 @@ def coco_detections(rows, r, image_id, class_ids):
     scores = rows[:, 4] * rows[:, 5]
     return [{"image_id": int(image_id), "category_id": class_ids[int(cls[i])], "bbox": bboxes[i].numpy().tolist(),
              "score": scores[i].numpy().item(), "segmentation": []} for i in range(bboxes.shape[0])]
+
+
+def coco_instances(rows, rles, r, img_h, img_w, image_id, class_ids, polygons=True):
+    """COCOInstEvaluator.convert_to_coco_format (unicorn/evaluators/coco_inst_evaluator.py) for one image: rows fp32 [n, 7] and rles [n]
+    as UnicornInstanceSegmenter.collect() returns them (the masks already resized to img_h x img_w and thresholded), r the letterbox
+    scale.  bbox, score and category_id are those of coco_detections.  polygons=True: "segmentation" holds the contours
+    cv2.findContours(RETR_TREE, CHAIN_APPROX_SIMPLE) finds in the mask, flattened, those with more than 4 coordinates, and an
+    instance left with none is dropped, as in the evaluator.  polygons=False: "segmentation" is the compressed RLE
+    {"size": [img_h, img_w], "counts": rle} (pycocotools' format), and instances with an empty mask are dropped."""
+    dets = coco_detections(rows, r, image_id, class_ids)
+    assert len(dets) == len(rles)
+    out = []
+    for d, rle in zip(dets, rles):
+        m = rle_decode(rle, img_h, img_w)
+        if polygons:
+            import cv2
+            contours, _ = cv2.findContours(np.ascontiguousarray(m, dtype=np.uint8), cv2.RETR_TREE, cv2.CHAIN_APPROX_SIMPLE)
+            d["segmentation"] = [c for c in (ct.flatten().tolist() for ct in contours) if len(c) > 4]
+            if not d["segmentation"]:
+                continue
+        else:
+            if not m.any():
+                continue
+            d["segmentation"] = {"size": [int(img_h), int(img_w)], "counts": rle}
+        out.append(d)
+    return out

@@ -41,7 +41,8 @@ class Exp:
         self.model = None
 
     def _init_det(self, cfg):
-        """exp/unicorn_det.py:22-92 with exps/default/unicorn_det_*_800x1280.py: the COCO detector (YOLOX + YOLOXHeadDet)."""
+        """exp/unicorn_det.py:22-92 with exps/default/unicorn_det_*_800x1280.py: the COCO detector (YOLOX + YOLOXHeadDet); with
+        exp/unicorn_det_mask.py (exps/default/unicorn_inst_convnext_tiny_800x1280.py) the instance segmenter (YOLOXHeadDetMask)."""
         self.task = "det"
         self.num_classes = cfg["num_classes"]      # unicorn_det.py:25 (COCO)
         if cfg["backbone"] == "resnet50":
@@ -55,7 +56,14 @@ class Exp:
         self.test_conf = 0.01                      # unicorn_det.py:88-89
         self.nmsthre = 0.65
         self.output_dir = "./Unicorn_outputs"
-        self.mask = False
+        self.mask_thres = 0.3                      # unicorn_det.py:92
+        self.mask = cfg["mask"]
+        if cfg["mask"]:                            # exp/unicorn_det_mask.py:22-44 (ExpDetMask): CondInst with the RAFT upsampler
+            self.task = "inst"
+            self.ctrl_loc = "reg"
+            self.use_raft = True
+            self.d_rate = 2
+            self.sem_loss_on = False
         self.model = None
 
     def get_model(self, load_pretrain=True):
@@ -82,13 +90,14 @@ class Exp:
                 setattr(self, k, v)
 
 
-ExpTrack = ExpTrackMask = Exp
+ExpTrack = ExpTrackMask = ExpDet = ExpDetMask = Exp
 
 
 def get_exp(exp_file=None, exp_name=None):
     """unicorn/exp/build.py:35-50."""
     assert exp_file is not None or exp_name is not None, "plz provide exp file or exp name."
     name = os.path.basename(exp_file).split(".")[0] if exp_file is not None else exp_name
-    if name.startswith("unicorn_det_") and name.endswith("_800x1280"):  # exps/default/unicorn_det_*_800x1280.py: the input size is an
-        name = name[:-len("_800x1280")]                                  # attribute of the Exp, not part of the config
+    # exps/default/unicorn_det_*_800x1280.py and unicorn_inst_*_800x1280.py: the input size is an attribute of the Exp, not part of the config
+    if name.startswith(("unicorn_det_", "unicorn_inst_")) and name.endswith("_800x1280"):
+        name = name[:-len("_800x1280")]
     return Exp(name)

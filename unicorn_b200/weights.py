@@ -28,6 +28,9 @@ CONFIGS = {
     "unicorn_det_convnext_tiny": dict(task="det", depths=(3, 3, 9, 3), dims=(96, 192, 384, 768), num_classes=80, mask=False),
     "unicorn_det_convnext_large": dict(task="det", depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536), num_classes=80, mask=False),
     "unicorn_det_r50": dict(task="det", backbone="resnet50", depths=(3, 4, 6, 3), dims=(256, 512, 1024, 2048), num_classes=80, mask=False),
+    # the COCO instance segmenter (exps/default/unicorn_inst_convnext_tiny_800x1280.py, YOLOX + YOLOXHeadDetMask, CondInst): the
+    # ConvNeXt-T detector plus the per-level controllers and the RAFT mask branch of the tracking *_mask heads
+    "unicorn_inst_convnext_tiny": dict(task="det", depths=(3, 3, 9, 3), dims=(96, 192, 384, 768), num_classes=80, mask=True),
 }
 for _c in CONFIGS.values():
     _c.setdefault("task", "track")
