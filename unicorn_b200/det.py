@@ -134,59 +134,83 @@ class UnicornInstanceSegmenter(UnicornDetector):
                              f"and max_batch * chunk <= 65535 (got {d_rate}, {chunk}, {max_batch})")
         super().__init__(eng, input_size, max_batch, conf, nms, False, use_graph, depth)
         self.mask_thres, self.d_rate, self.chunk = mask_thres, d_rate, chunk
-        H, W = self.input_size
-        up, h, w, dev = 8 // d_rate, H // 8, W // 8, eng.dev
-        self._up = up
-        self._image_of = torch.arange(max_batch, dtype=torch.int32, device=dev)
         for c in self._ring.slots:
-            c.maps = torch.empty(max_batch, chunk, h * up, w * up, dtype=torch.float32, device=dev)
-            c.scratch = torch.empty(max_batch * chunk * h * w, dtype=torch.float32, device=dev)
-            c.window = torch.zeros(max_batch, dtype=torch.int32, device=dev)  # each image's rows in the current chunk
-            c.enc = MaskEncoder(max_batch * chunk, dev, capacity)
+            c.rows = RowMasks(max_batch, self.A, self.input_size, chunk, d_rate, mask_thres, eng.dev, capacity)
 
     def _frame(self, c):
         fpn = super()._frame(c)
         c.mf, c.um = c.eng.mask_branch(fpn)
         c.dyn = list(c.eng.dyn_levels)
-        self._masks(c, 0)
-
-    def _masks(self, c, row0):
-        """The d_rate = 1 masks of NMS rows row0 .. row0 + chunk - 1 of every image into c.maps."""
-        torch.sub(c.ws.count, row0, out=c.window).clamp_(0, self.chunk)
-        anchors = c.ws.anchors.view(self.max_batch, self.A)[:, row0:]
-        post_ops.dynamic_masks_rows(c.mf, c.um, c.dyn, [(t.shape[1], t.shape[2]) for t in c.dyn], anchors, c.window, self._image_of,
-                                    self.chunk, self._up, c.maps, c.scratch)
-
-    def _encode(self, c, row0):
-        post_ops.inst_encode(c.maps[:c.n], c.ws.count, row0, self.d_rate, self.mask_thres, c.ratios, [h for h, _ in c.sizes],
-                             [w for _, w in c.sizes], c.enc.ws, c.enc.d_emit, c.enc.d_chars, c.enc.d_offsets)
+        c.rows.masks(c.mf, c.um, c.dyn, c.ws, 0)
 
     def _after_frame(self, c):
         if c.n < self.max_batch:
             c.ws.count[c.n:].zero_()  # idle slots have no rows
-        c.enc.reserve(max(h for h, _ in c.sizes), max(w for _, w in c.sizes))
-        c.enc.enqueue(c.n * self.chunk, lambda: self._encode(c, 0))
+        c.rows.enqueue(c.n, c.ws, c.ratios, c.sizes)
 
     def collect(self):
         """Rows and masks of the oldest submitted step: a list of (rows fp32 [n, 7] CPU tensor in descending score order, r, rles [n]),
         one per image."""
         c = self._ring.collect()
-        n, k, K = c.n, self.chunk, c.n * self.chunk
         with torch.cuda.stream(c.stream):
             c.event.synchronize()
-            counts = [int(v) for v in c.count_host[:n]]
-            flat = c.enc.strings(K, lambda: self._encode(c, 0))
-            rles = [flat[b * k:b * k + min(k, counts[b])] for b in range(n)]
-            row0 = k
-            while any(m > row0 for m in counts):
-                self._masks(c, row0)
-                run = lambda r=row0: self._encode(c, r)  # noqa: E731
-                c.enc.enqueue(K, run)
-                flat = c.enc.strings(K, run)
-                for b in range(n):
-                    rles[b] += flat[b * k:b * k + max(0, min(k, counts[b] - row0))]
-                row0 += k
+            counts = [int(v) for v in c.count_host[:c.n]]
+            rles = c.rows.strings(counts, c.mf, c.um, c.dyn, c.ws, c.ratios, c.sizes)
         dets = c.ws.dets.view(self.max_batch, self.A, 7)
-        out = [(dets[i, :counts[i]].cpu(), c.ratios[i], rles[i]) for i in range(n)]
+        out = [(dets[i, :counts[i]].cpu(), c.ratios[i], rles[i]) for i in range(c.n)]
         c.last.clear()
         return out
+
+
+class RowMasks:
+    """The masks of every NMS row of B images as COCO RLE strings over each image's original frame, `chunk` rows at a time (utils/
+    boxes.py postprocess_inst: the dynamic-conv mask of every row, aligned_bilinear x d_rate, resized by 1/r, thresholded > thr).  Each
+    chunk is dynamic_masks_rows at d_rate = 1 into `maps` [B, chunk, H/d_rate, W/d_rate], then uc_inst_encode_batched, which folds the
+    final upsample into the resize, so the full-resolution masks are never stored.  Holds the buffers of one frame slot.
+
+    masks(..., row0=0) may run inside the frame's CUDA graph; enqueue() queues the encode of rows [0, chunk) on the current stream, and
+    strings() waits for it and runs the further chunks eagerly, one batch per chunk for all images that still have rows."""
+
+    def __init__(self, B, A, input_size, chunk, d_rate, thr, device, capacity):
+        H, W = input_size
+        up, h, w = 8 // d_rate, H // 8, W // 8
+        self.B, self.A, self.chunk, self.d_rate, self.thr, self.up = B, A, chunk, d_rate, thr, up
+        self.image_of = torch.arange(B, dtype=torch.int32, device=device)
+        self.maps = torch.empty(B, chunk, h * up, w * up, dtype=torch.float32, device=device)
+        self.scratch = torch.empty(B * chunk * h * w, dtype=torch.float32, device=device)
+        self.window = torch.zeros(B, dtype=torch.int32, device=device)  # each image's rows in the current chunk
+        self.enc = MaskEncoder(B * chunk, device, capacity)
+
+    def masks(self, mf, um, dyn, ws, row0):
+        """The d_rate = 1 masks of NMS rows row0 .. row0 + chunk - 1 of every image into maps."""
+        torch.sub(ws.count, row0, out=self.window).clamp_(0, self.chunk)
+        anchors = ws.anchors.view(self.B, self.A)[:, row0:]
+        post_ops.dynamic_masks_rows(mf, um, dyn, [(t.shape[1], t.shape[2]) for t in dyn], anchors, self.window, self.image_of, self.chunk,
+                                    self.up, self.maps, self.scratch)
+
+    def _encode(self, n, ws, row0, ratios, sizes):
+        post_ops.inst_encode(self.maps[:n], ws.count, row0, self.d_rate, self.thr, ratios, [h for h, _ in sizes], [w for _, w in sizes],
+                             self.enc.ws, self.enc.d_emit, self.enc.d_chars, self.enc.d_offsets)
+
+    def enqueue(self, n, ws, ratios, sizes):
+        """Queues the encode of the first n images' rows [0, chunk) (their masks are in maps) on the current stream; sizes: n original
+        (h, w), ratios: their letterbox scales."""
+        self.enc.reserve(max(h for h, _ in sizes), max(w for _, w in sizes))
+        self.enc.enqueue(n * self.chunk, lambda: self._encode(n, ws, 0, ratios, sizes))
+
+    def strings(self, counts, mf, um, dyn, ws, ratios, sizes):
+        """After enqueue(): the strings of rows [0, counts[b]) of each of the n = len(counts) images, a list per image."""
+        n, k = len(counts), self.chunk
+        K = n * k
+        flat = self.enc.strings(K, lambda: self._encode(n, ws, 0, ratios, sizes))
+        rles = [flat[b * k:b * k + min(k, counts[b])] for b in range(n)]
+        row0 = k
+        while any(m > row0 for m in counts):
+            self.masks(mf, um, dyn, ws, row0)
+            run = lambda r=row0: self._encode(n, ws, r, ratios, sizes)  # noqa: E731
+            self.enc.enqueue(K, run)
+            flat = self.enc.strings(K, run)
+            for b in range(n):
+                rles[b] += flat[b * k:b * k + max(0, min(k, counts[b] - row0))]
+            row0 += k
+        return rles

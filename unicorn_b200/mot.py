@@ -53,14 +53,17 @@ class QDEmbedding:
     embedding upsample, sampling at the image's detection centres into `feats` [B, n_keep, 128].  pre_dict (mot_evaluator.py:1014-1020,
     :812-818) is the s16 feature of the last frame THAT HAD DETECTIONS, kept in its own buffer and updated by device-side conditional
     copies (no host decision inside the frame), so a frame that runs this step must run exactly once.  gate (int32 [B]): image b's
-    pre_dict and first-frame flag change only where gate[b] != 0 (an idle sequence keeps its state)."""
+    pre_dict and first-frame flag change only where gate[b] != 0 (an idle sequence keeps its state).
 
-    def __init__(self, eng, H, W, n_keep, tag, batch=1):
+    first_step=True is the rule of qdtrack's test_omni.py:97-98 instead: pre_dict is set by a sequence's first step whether or not it
+    had detections, then advances only on steps with detections."""
+
+    def __init__(self, eng, H, W, n_keep, tag, batch=1, first_step=False):
         dev = eng.dev
         self.prev_feat = torch.zeros(batch, H // 16, W // 16, eng.inc[1], dtype=torch.bfloat16, device=dev)
         self.has_prev = torch.zeros(batch, dtype=torch.int32, device=dev)
         self.feats = torch.zeros(batch, n_keep, 128, dtype=torch.float32, device=dev)
-        self.n_keep, self.tag = n_keep, tag
+        self.n_keep, self.tag, self.first_step = n_keep, tag, first_step
 
     def __call__(self, e, feat, dets, cnt, gate=None):
         """feat: the frame's s16 features [B,h,w,C], (dets, cnt): their NMS output.  Returns the embedding maps."""
@@ -75,7 +78,7 @@ class QDEmbedding:
         else:
             ops.sample_embed(emb, dets.view(B, -1, 7), self.n_keep, 8.0, count=cnt, out=self.feats)
         ops.copy_rows_if(cnt, feat, self.prev_feat, gate=gate)
-        started = cnt > 0
+        started = cnt >= 0 if self.first_step else cnt > 0  # cnt >= 0: every image (the flag stays a device-side update)
         if gate is not None:
             started &= gate != 0
         self.has_prev.bitwise_or_(started.to(torch.int32))
@@ -115,6 +118,7 @@ class UnicornMOTBatch:
     depth > 1 (ByteTrack arm only): that many steps in flight, each on its own stream and engine context."""
 
     _tag = "mot"  # engine buffer tag of the driver's activations
+    _first_step = False  # QDEmbedding's pre_dict rule
 
     def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.01, nms=0.7, score_thr=0.1, max_dets=1024, assoc="qd",
                  use_graph=False, depth=1):
@@ -127,7 +131,7 @@ class UnicornMOTBatch:
         self.assoc, self.use_graph, self.depth = assoc, use_graph, depth
         H, W = self.input_size
         self.n_keep = min(max_dets, anchor_count(H, W))  # rows a sequence can have after NMS and that are read back
-        self._qd = QDEmbedding(engine, H, W, self.n_keep, self._tag + ".emb", batch=n_seq) if assoc == "qd" else None
+        self._qd = QDEmbedding(engine, H, W, self.n_keep, self._tag + ".emb", batch=n_seq, first_step=self._first_step) if assoc == "qd" else None
         make = lambda eng, stream, tag=self._tag: _Slot(eng, H, W, stream, n_seq, tag, self.n_keep, assoc == "qd")  # noqa: E731
         if depth == 1:
             # two parity slots on this engine and the current stream: one input buffer and one NMS workspace, own backbone buffers (tag)
@@ -168,15 +172,21 @@ class UnicornMOTBatch:
         self.trackers[i], self.frame_ids[i] = tracker, 0
 
     # ------------------------------------------------------------------------------------------ device half
+    _with_masks = False  # the head also runs the controller convs (UnicornBDDMOTSBatch)
+
     def _frame(self, c):
         e = c.eng
         e.begin_frame()
         fpn, seq = e.backbone(c.img, tag=c.tag)
-        out = e.head(fpn, None, "mot")  # whole mode: zero priors (unicorn.py:133-139); [n_seq, A, 5+ncls]
+        out = e.head(fpn, None, "mot", with_masks=self._with_masks)  # whole mode: zero priors (unicorn.py:133-139); [n_seq, A, 5+ncls]
         dets, cnt = ops.postprocess_device(out if self.n_seq > 1 else out[0], e.ncls, self.conf, self.nms, c.ws)
+        self._after_nms(c, fpn)
         # one sequence needs no gate: a step without an active sequence does not run (submit)
         embed = self._qd(e, seq["feat"], dets, cnt, gate=c.active if self.n_seq > 1 else None) if self._qd is not None else None
         c.last = dict(embed=embed, head=out)
+
+    def _after_nms(self, c, fpn):
+        """Work of the step between NMS and the embedding step, inside its graph (UnicornBDDMOTSBatch: the masks)."""
 
     def _check(self, frames, scales, active):
         n, (H, W) = self.n_seq, self.input_size

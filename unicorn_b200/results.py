@@ -6,7 +6,12 @@ pycocotools is a third-party dependency of the reference that is absent from thi
 published COCO mask API (cocoapi/common/maskApi.c: rleEncode + rleToString — column-major run lengths starting with the
 zero run, then 5 data bits per character with a continuation bit, chars offset by 48, counts after the second stored as
 differences to the count two positions earlier).  Its parity is UNPINNED (no pycocotools here, no vectors in the reference);
-tests check the round trip with `rle_decode` and a hand-computed example."""
+tests check the round trip with `rle_decode` and a hand-computed example.
+
+bbox2result / track2result / segtrack2result are the per-frame result builders of the BDD100K test loop (qdtrack's test_omni.py),
+with the dtypes of mmdet and qdtrack."""
+from collections import defaultdict
+
 import numpy as np
 import torch
 
@@ -164,4 +169,41 @@ def coco_instances(rows, rles, r, img_h, img_w, image_id, class_ids, polygons=Tr
                 continue
             d["segmentation"] = {"size": [int(img_h), int(img_w)], "counts": rle}
         out.append(d)
+    return out
+
+
+def rle_dict(rle, img_h, img_w):
+    """The dict pycocotools.mask.encode returns for one mask: {"size": [h, w], "counts": compressed RLE bytes}."""
+    return {"size": [int(img_h), int(img_w)], "counts": rle.encode("ascii")}
+
+
+def bbox2result(bboxes, labels, num_classes):
+    """mmdet's bbox2result: bboxes [n, 5] (x1, y1, x2, y2, score), labels [n] -> num_classes float32 arrays [k, 5], each class's rows
+    in their input order; [0, 5] arrays when n = 0."""
+    if bboxes.shape[0] == 0:
+        return [np.zeros((0, 5), dtype=np.float32) for _ in range(num_classes)]
+    bboxes, labels = torch.as_tensor(bboxes).cpu().numpy(), torch.as_tensor(labels).cpu().numpy()
+    return [bboxes[labels == i, :] for i in range(num_classes)]
+
+
+def track2result(bboxes, labels, ids, num_classes):
+    """qdtrack's track2result (core/track/transforms.py): the rows of valid ids (> -1) per class as [id, x1, y1, x2, y2, score].  The
+    int64 ids joined to the float32 boxes make float64 arrays; a frame without a valid id gives float32 [0, 6] arrays."""
+    valid = ids > -1
+    bboxes, labels, ids = bboxes[valid], labels[valid], ids[valid]
+    if bboxes.shape[0] == 0:
+        return [np.zeros((0, 6), dtype=np.float32) for _ in range(num_classes)]
+    bboxes, labels, ids = bboxes.cpu().numpy(), labels.cpu().numpy(), ids.cpu().numpy()
+    return [np.concatenate((ids[labels == i, None], bboxes[labels == i, :]), axis=1) for i in range(num_classes)]
+
+
+def segtrack2result(bboxes, labels, segms, ids):
+    """qdtrack's segtrack2result (core/track/transforms_mots.py): {id: {"bbox", "label", "segm"}} of the valid ids (> -1), in row
+    order; ids are numpy int64 keys, bbox float32 [5], label a numpy scalar of the labels' dtype, segm as given."""
+    valid = ids > -1
+    bboxes, labels, ids = bboxes[valid].cpu().numpy(), labels[valid].cpu().numpy(), ids[valid].cpu().numpy()
+    segms = [s for s, v in zip(segms, valid.tolist()) if v]
+    out = defaultdict(list)
+    for bbox, label, segm, tid in zip(bboxes, labels, segms, ids):
+        out[tid] = dict(bbox=bbox, label=label, segm=segm)
     return out

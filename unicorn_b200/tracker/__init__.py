@@ -1,2 +1,2 @@
-from .quasi_dense import QuasiDenseEmbedTracker  # noqa: F401
+from .quasi_dense import QuasiDenseEmbedTracker, bdd_tracker  # noqa: F401
 from .byte_tracker import BYTETracker  # noqa: F401

@@ -135,3 +135,16 @@ class QuasiDenseEmbedTracker:
             self._ids_host = [t for t, ok in zip(self._ids_host, alive_host.tolist()) if ok]
         if len(self.backdrops) > self.memo_backdrop_frames:
             self.backdrops.pop()
+
+
+# The tracker settings of the BDD100K test protocol (qdtrack's test_omni.py): configs/bdd100k/unicorn.py (MOT) and
+# configs/bdd100k_mots/segtrack-frcnn_r50_fpn_12e_bdd10k_fixed_pcan.py (MOTS).
+BDD_TRACKER = dict(init_score_thr=0.4, obj_score_thr=0.2, match_score_thr=0.5, memo_tracklet_frames=10, memo_backdrop_frames=1,
+                   memo_momentum=1.0, nms_conf_thr=0.5, nms_backdrop_iou_thr=0.3, nms_class_iou_thr=0.7, with_cats=True,
+                   match_metric="bisoftmax")
+BDD_MOTS_TRACKER = dict(BDD_TRACKER, init_score_thr=0.5, obj_score_thr=0.3)
+
+
+def bdd_tracker(mots=False, device="cuda"):
+    """A QuasiDenseEmbedTracker with the BDD100K MOT (mots=False) or MOTS (mots=True) test settings."""
+    return QuasiDenseEmbedTracker(**(BDD_MOTS_TRACKER if mots else BDD_TRACKER), device=device)
