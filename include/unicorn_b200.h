@@ -164,6 +164,15 @@ UC_API int uc_layernorm(const void* x, int ldx, const void* res, int ldres, cons
 UC_API int uc_groupnorm_apply(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y,
                               int ldy, int B, long HW, int C, int G, float eps, int act, const float* prior,
                               const float* beta, const void* add2, int ldadd2, void* y2, int ldy2, void* stream);
+/* The same normalisation of ONE conv output written as B images (a head stem shared by several head images): x [HW pixels] and
+ * stats [G]{sum,sumsq} of one image; y [B][HW pixels], image stride HW * ldy.  Image b < n_plain = act((x-mean)*rstd*w+b) (the no-prior
+ * path: adding a zero prior would turn a -0 into +0); image b >= n_plain adds prior[(b - n_plain) * HW + pix] * beta[c].  Every image
+ * equals uc_groupnorm_apply at B = 1 on x, with or without its prior, bit for bit.  1 <= B <= 65535, 0 <= n_plain <= B; prior (4-byte
+ * aligned) and beta are given exactly when n_plain < B; x and y must not overlap; otherwise the conventions of uc_groupnorm_apply
+ * (UC_EINVAL before any launch). */
+UC_API int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y, int ldy,
+                                    int B, int n_plain, long HW, int C, int G, float eps, int act, const float* prior, const float* beta,
+                                    void* stream);
 
 /* dst[b,oh,ow,:C] = src[b,oh/up,ow/up,:C], up in {1,2} (nearest upsample + concat slice; yolo_pafpn_new.py:139-146).
  * 16-bit NHWC; C, lds, ldd multiples of 8; src and dst 16-byte aligned. */

@@ -1,0 +1,141 @@
+"""SOT targets plus a MOT arm on one video: UnicornUnifiedTracker (one backbone pass per frame) against the same work done by today's
+two drivers in the same process, UnicornSOTBatch(n_seq=K) fed K copies of the frame plus UnicornMOTTracker.
+
+    python tools/bench_unified.py [--configs unicorn_track_large unicorn_track_r50] [--targets 1 2 4] [--mot qd byte none] [--steps 20]
+
+800x1280, seeded weights, make_video(..., n_obj=6) frames resident on the device as uint8, CUDA graphs everywhere.  K targets are
+added on frame 0, one per object.  Both sides run the MOT driver's protocol (submit(t + 1) before collect(t), the association
+included); the two-driver side collects the SOT batch of step t before submitting its next one.  A step is timed end to end: host
+clock around `steps` steps that end in a device synchronise, three rounds alternating between the two sides; median and min-max.
+Also printed: the device-only step (CUDA events around graph replays of the step with its input copy), the kernels launched per
+step through the C ABI, and the device memory each side added on top of what was already allocated (peak allocation while it was
+built and warmed up, minus the allocation before).  The card's name and power limit are printed first.  One JSON line per
+(config, K, mot)."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+import types
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--configs", nargs="+", default=["unicorn_track_large", "unicorn_track_r50"])
+    ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
+    ap.add_argument("--targets", type=int, nargs="+", default=[1, 2, 4])
+    ap.add_argument("--mot", nargs="+", default=["qd", "byte", "none"], choices=["qd", "byte", "none"])
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=3)
+    args = ap.parse_args()
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mot import UnicornMOTTracker
+    from unicorn_b200.sot import UnicornSOTBatch
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.tracker import QuasiDenseEmbedTracker
+    from unicorn_b200.tracker.byte_tracker import BYTETracker
+    from unicorn_b200.unified import UnicornUnifiedTracker
+    from unicorn_b200.weights import make_state_dict
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
+    H, W = args.size
+    bargs = types.SimpleNamespace(track_thresh=0.5, track_buffer=30, match_thresh=0.8, mot20=False)
+    new_tracker = {"qd": lambda: QuasiDenseEmbedTracker(), "byte": lambda: BYTETracker(bargs), None: lambda: None}
+    to_u8 = lambda f: f.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()  # noqa: E731
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        frames, boxes = make_video(5, H, W, seed=0, n_obj=6)
+        ref = to_u8(frames[0:1]).cuda()
+        steps_u8 = [to_u8(frames[1 + t:2 + t]).cuda() for t in range(4)]  # [1,H,W,3]
+        for K in args.targets:
+            copies = [f.expand(K, -1, -1, -1).contiguous() for f in steps_u8]
+            for mot in [None if m == "none" else m for m in args.mot]:
+                sides = {}
+                # ---- one backbone pass per frame
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                un = UnicornUnifiedTracker(eng, (H, W), K, mot=mot, tracker=new_tracker[mot]())
+                for k in range(K):
+                    un.add_target(k, boxes[0, k])
+                un.step_tensor(ref)
+
+                def un_round(steps, un=un):
+                    un.submit(steps_u8[0])
+                    for t in range(steps):
+                        if t + 1 < steps:
+                            un.submit(steps_u8[(t + 1) % 4])
+                        un.collect((H, W))
+
+                def un_replay(t, un=un):
+                    un._slot.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
+                    un._slot.graph.replay()
+                un_round(4)
+                sides["unified"] = (un_round, un_replay, un.launches_per_frame, torch.cuda.max_memory_allocated() - m0)
+                # ---- today's drivers, each with its own backbone pass
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                sb = UnicornSOTBatch(eng, (H, W), K)
+                for k in range(K):
+                    sb.initialize_tensor(k, ref, boxes[0, k])
+                mt = UnicornMOTTracker(eng, (H, W), assoc=mot, tracker=new_tracker[mot](), use_graph=True) if mot else None
+
+                def two_round(steps, sb=sb, mt=mt):
+                    if mt:
+                        mt.submit(steps_u8[0])
+                    for t in range(steps):
+                        sb.submit(copies[t % 4])
+                        if mt and t + 1 < steps:
+                            mt.submit(steps_u8[(t + 1) % 4])
+                        sb.collect()
+                        if mt:
+                            mt.collect((H, W))
+
+                def two_replay(t, sb=sb, mt=mt):
+                    sb.slot.img_in_u8.copy_(copies[t % 4], non_blocking=True)
+                    sb.slot.graph.replay()
+                    if mt:
+                        c = mt._ctxs[t % 2]
+                        c.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
+                        c.graph.replay()
+                two_round(4)
+                launches = sb.launches_per_frame + (mt._b.launches_per_frame if mt else 0)
+                sides["two_drivers"] = (two_round, two_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                times = {key: [] for key in sides}
+                for _ in range(args.rounds):
+                    for key, (run, *_rest) in sides.items():
+                        torch.cuda.synchronize()
+                        t0 = time.perf_counter()
+                        run(args.steps)
+                        torch.cuda.synchronize()
+                        times[key].append(time.perf_counter() - t0)
+                line = {"config": cfg, "size": [H, W], "targets": K, "mot": mot or "none"}
+                for key, (_, replay, launches, mem) in sides.items():
+                    torch.cuda.synchronize()
+                    e0.record()
+                    for t in range(args.steps):
+                        replay(t)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    ms = [1e3 * t / args.steps for t in times[key]]
+                    line[key] = {"ms_per_step": round(statistics.median(ms), 2), "ms_per_step_min_max": [round(min(ms), 2), round(max(ms), 2)],
+                                 "device_ms_per_step": round(e0.elapsed_time(e1) / args.steps, 2), "launches_per_step": launches,
+                                 "added_peak_alloc_gib": round(mem / 2 ** 30, 2)}
+                line["two_drivers_over_unified"] = round(line["two_drivers"]["ms_per_step"] / line["unified"]["ms_per_step"], 3)
+                line.update(steps=args.steps, rounds=args.rounds)
+                print(json.dumps(line), flush=True)
+                del sides, un, sb, mt, un_round, un_replay, two_round, two_replay
+                torch.cuda.empty_cache()
+        del eng
+        torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()

@@ -449,23 +449,28 @@ __global__ void __launch_bounds__(256) layernorm_v8_kernel(const uint16_t* __res
 // y = act(x * scale[c] + shift[c]) (+ prior[pix] * beta[c]); optional second output y2 = y + add2.
 // scale/shift fold the group statistics (int64 fixed point {sum, sumsq} accumulated by uc_conv2d) with the affine
 // parameters; they are computed once per block into shared memory.  x/y bf16 NHWC (strided); 8 channels / thread.
+// kBcast: every output image b (blockIdx.y) reads image 0 of x and of the statistics, and only the images b >= prior_from add the
+// prior, reading its plane b - prior_from; the others take the no-prior path.  y2 is unused.
+template <bool kBcast>
 __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __restrict__ x, int ldx,
                                                                const long long* __restrict__ stats, const float* __restrict__ w,
                                                                const float* __restrict__ bvec, uint16_t* __restrict__ y, int ldy,
                                                                long HW, int C, int G, float eps, int act,
                                                                const float* __restrict__ prior, const float* __restrict__ beta,
                                                                const uint16_t* __restrict__ add2, int ldadd2,
-                                                               uint16_t* __restrict__ y2, int ldy2) {
+                                                               uint16_t* __restrict__ y2, int ldy2, int prior_from) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
   extern __shared__ float sc[];  // [2][C] scale, shift (+ [C] beta)
   const int b = blockIdx.y;
+  const int bx = kBcast ? 0 : b;  // image of x and of the statistics
+  const bool with_prior = prior != nullptr && (!kBcast || b >= prior_from);
   const int gs = C / G;
   const double inv_n = 1.0 / (static_cast<double>(HW) * gs);
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / gs;
-    const double sum = static_cast<double>(stats[(static_cast<long>(b) * G + g) * 2]) * (1.0 / kGnFixedScale);
-    const double sq = static_cast<double>(stats[(static_cast<long>(b) * G + g) * 2 + 1]) * (1.0 / kGnFixedScale);
+    const double sum = static_cast<double>(stats[(static_cast<long>(bx) * G + g) * 2]) * (1.0 / kGnFixedScale);
+    const double sq = static_cast<double>(stats[(static_cast<long>(bx) * G + g) * 2 + 1]) * (1.0 / kGnFixedScale);
     const double mean = sum * inv_n;
     const float var = fmaxf(static_cast<float>(sq * inv_n - mean * mean), 0.f);
     const float rstd = rsqrtf(var + eps);
@@ -481,7 +486,8 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
   for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int c0 = static_cast<int>(i % C8) * 8;
     const long pix = static_cast<long>(b) * HW + i / C8;
-    const uint4 u = *reinterpret_cast<const uint4*>(x + pix * ldx + c0);
+    const long xpix = kBcast ? i / C8 : pix;
+    const uint4 u = *reinterpret_cast<const uint4*>(x + xpix * ldx + c0);
     const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
     // per-channel coefficients as 128-bit shared-memory loads (c0 is a multiple of 8 -> 32-byte aligned)
     const float4 s0 = *reinterpret_cast<const float4*>(sc + c0), s1 = *reinterpret_cast<const float4*>(sc + c0 + 4);
@@ -506,8 +512,8 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
 #pragma unroll
       for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.f);
     }
-    if (prior) {
-      const float pr = __ldg(prior + pix);
+    if (with_prior) {
+      const float pr = __ldg(prior + (kBcast ? static_cast<long>(b - prior_from) * HW + i / C8 : pix));
       const float4 b0 = *reinterpret_cast<const float4*>(sc + 2 * C + c0), b1 = *reinterpret_cast<const float4*>(sc + 2 * C + c0 + 4);
       const float bt[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
@@ -516,7 +522,7 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
     uint4 o;
     o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]); o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
     *reinterpret_cast<uint4*>(y + pix * ldy + c0) = o;
-    if (y2) {
+    if (!kBcast && y2) {
       const uint4 a = *reinterpret_cast<const uint4*>(add2 + pix * ldadd2 + c0);
       const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
       uint4 o2;
@@ -635,8 +641,42 @@ extern "C" int uc_groupnorm_apply(const void* x, int ldx, const void* stats, con
   const long total = HW * (C / 8);
   // each block pays C scale/shift computations up front; keep ~2 elements (16 channels) per thread for parallelism
   const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
-  launch_pdl(groupnorm_apply_kernel, dim3(gx, B), 256, 3 * C * sizeof(float), stream, 
+  launch_pdl(groupnorm_apply_kernel<false>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
       static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
-      eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2);
+      eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2, 0);
   return check_launch("uc_groupnorm_apply");
+}
+
+extern "C" int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y, int ldy,
+                                        int B, int n_plain, long HW, int C, int G, float eps, int act, const float* prior,
+                                        const float* beta, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (B < 1 || B > 65535) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: B must be in [1, 65535] (got %d)", B);
+  if (n_plain < 0 || n_plain > B) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: n_plain must be in [0, B] (got %d, B = %d)", n_plain, B);
+  if (HW < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: HW must be >= 1");
+  if (G < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: G must be >= 1 (got %d)", G);
+  if (C % 8 || ldx % 8 || ldy % 8 || C % G || ldx < C || ldy < C)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: C, ldx, ldy multiples of 8, ldx, ldy >= C; C %% G == 0");
+  if (C > 4096) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: C too large");
+  if (act != UC_ACT_NONE && act != UC_ACT_RELU && act != UC_ACT_SILU)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: act must be UC_ACT_NONE, UC_ACT_RELU or UC_ACT_SILU (got %d)", act);
+  if (!x || !stats || !w || !b || !y) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: null pointer");
+  if ((prior != nullptr) != (beta != nullptr)) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior and beta go together");
+  if ((prior != nullptr) != (n_plain < B))
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior and beta are needed exactly when n_plain < B");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: x and y must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(stats) & 7) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: stats must be 8-byte aligned");
+  if (reinterpret_cast<uintptr_t>(prior) & 3) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior must be 4-byte aligned");
+  // every output image reads all of x: writing any of them over x would race with the other images' reads
+  const uintptr_t x0 = reinterpret_cast<uintptr_t>(x), y0 = reinterpret_cast<uintptr_t>(y);
+  const uintptr_t x1 = x0 + (static_cast<uintptr_t>(HW - 1) * ldx + C) * 2;  // one past the last element read or written
+  const uintptr_t y1 = y0 + (static_cast<uintptr_t>(B) * HW - 1) * ldy * 2 + static_cast<uintptr_t>(C) * 2;
+  if (x0 < y1 && y0 < x1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: x and y overlap (not an in-place operation)");
+  const long total = HW * (C / 8);
+  const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
+  launch_pdl(groupnorm_apply_kernel<true>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
+      static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
+      eps, act, prior, beta, static_cast<const uint16_t*>(nullptr), 0, static_cast<uint16_t*>(nullptr), 0, n_plain);
+  return check_launch("uc_groupnorm_apply_bcast");
 }

@@ -18,7 +18,7 @@ import os
 
 import torch
 
-from . import ops
+from . import ops, shared_ops
 from .weights import CONFIGS, fold_bn
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = ops.ACT_NONE, ops.ACT_RELU, ops.ACT_GELU, ops.ACT_SILU
@@ -693,14 +693,7 @@ class UnicornEngine:
             x = self.buf(f"head{k}.x", (B, h, w, 256))
             pr = priors[k].reshape(-1) if priors is not None else None
             self.conv_gn(fpn[k], L["stem"], x, prior=pr, beta=L["beta"] if pr is not None else None)
-            for i in range(3):
-                self.convnext_block(x, L["att"][i], f"head{k}.att")
-            feats = []
-            for name in ("cls", "reg"):
-                cur = x
-                for i, c in enumerate(L[name]):
-                    cur = self.conv_gn(cur, c, self.buf(f"head{k}.{name}{i % 2}", (B, h, w, 256)))
-                feats.append(cur)
+            feats = self._head_trunk(k, x)
             row, rob, cw, cb, _ = L["pred" + sfx]
             cls_outs[k] = ops.conv2d(feats[0], cw, 1, 1, bias=cb, out=self.buf(f"head{k}.clso", (B, h, w, cb.numel()), F32))
             ro_outs[k] = ops.conv2d(feats[1], row, 1, 1, bias=rob, out=self.buf(f"head{k}.roo", (B, h, w, 8), F32))
@@ -708,6 +701,72 @@ class UnicornEngine:
             if self._with_masks:
                 cw_, cb_ = L["ctrl"]
                 self.dyn_levels[k] = self.conv(feats[1], cw_, 3, 1, 1, bias=cb_, out=self.buf(f"head{k}.dyn", (B, h, w, 176), F32))
+
+    def _head_trunk(self, k, x):
+        """Level k of the head after the stem, on its output x [B,h,w,256] (in place): the three ConvNeXt blocks, then the cls and reg
+        towers.  Returns their outputs (cls, reg)."""
+        L = self.P["head"][k]
+        B, h, w, _ = x.shape
+        for i in range(3):
+            self.convnext_block(x, L["att"][i], f"head{k}.att")
+        feats = []
+        for name in ("cls", "reg"):
+            cur = x
+            for i, c in enumerate(L[name]):
+                cur = self.conv_gn(cur, c, self.buf(f"head{k}.{name}{i % 2}", (B, h, w, 256)))
+            feats.append(cur)
+        return feats
+
+    def head_shared(self, fpn, priors, mot=True):
+        """The head of one image's pyramid for several head images at once: with mot=True image 0 is the MOT image (mode "mot", no
+        prior), then one SOT image (mode "sot") per prior plane.  fpn: 3 NHWC bf16 maps [1,h,w,C]; priors: the 3 fp32 maps of
+        propagate ([K,h,w] planes in any leading shape, K >= 1).  The stem conv and its statistics run once at B = 1 and
+        uc_groupnorm_apply_bcast writes all 1 + K (or K) stem outputs; the ConvNeXt blocks and towers run on all images together, the
+        predictors of each mode on its batch slice.  Returns (MOT decoded [1, A, 5+ncls] or None, SOT decoded [K, A, 6]); every image
+        equals head(fpn, its prior or None, its mode) at B = 1, bit for bit."""
+        self._tracking_only("head_shared")
+        assert fpn[0].shape[0] == 1, "head_shared: the pyramid of one image"
+        n_mot = int(bool(mot))
+        n_sot = priors[0].numel() // (fpn[0].shape[1] * fpn[0].shape[2])
+        assert n_sot >= 1 and all(p.numel() == n_sot * f.shape[1] * f.shape[2] for p, f in zip(priors, fpn))
+        outs = {m: ([None] * 3, [None] * 3) for m in ("", "_sot")}  # (reg+obj, cls) maps per level of each mode
+        hw = [None] * 3
+
+        def level(k):
+            L = self.P["head"][k]
+            _, h, w, _ = fpn[k].shape
+            c = L["stem"]
+            st = self._stats(c.groups)
+            t = self.conv(fpn[k], c.w, c.k, c.stride, (c.k - 1) // 2, bias=c.bias, out=self.buf(f"shared{k}.stem", (1, h, w, 256)),
+                          gn_stats=st, gn_groups=c.groups)
+            x = self.buf(f"head{k}.x", (n_mot + n_sot, h, w, 256))
+            shared_ops.groupnorm_apply_bcast(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, prior=priors[k].reshape(-1), beta=L["beta"])
+            feats = self._head_trunk(k, x)
+            for sfx, i0, n in (("", 0, n_mot), ("_sot", n_mot, n_sot)):
+                if n == 0:
+                    continue
+                row, rob, cw, cb, _ = L["pred" + sfx]
+                cls, reg = feats[0][i0:i0 + n], feats[1][i0:i0 + n]
+                outs[sfx][1][k] = ops.conv2d(cls, cw, 1, 1, bias=cb, out=self.buf(f"shared{k}.clso{sfx}", (n, h, w, cb.numel()), F32))
+                outs[sfx][0][k] = ops.conv2d(reg, row, 1, 1, bias=rob, out=self.buf(f"shared{k}.roo{sfx}", (n, h, w, 8), F32))
+            hw[k] = (h, w)
+
+        # the three levels on three streams, as in head()
+        main = torch.cuda.current_stream()
+        if self._side_streams is None:
+            self._side_streams = [torch.cuda.Stream(device=self.dev) for _ in range(2)]
+        for s_ in self._side_streams:
+            s_.wait_stream(main)
+        for k in (1, 2):
+            with torch.cuda.stream(self._side_streams[k - 1]):
+                level(k)
+        level(0)
+        for s_ in self._side_streams:
+            main.wait_stream(s_)
+        A = sum(h * w for h, w in hw)
+        out_mot = ops.head_decode(*outs[""], hw, STRIDES, self.ncls, out=self.buf("shared.out_mot", (1, A, 5 + self.ncls), F32)) if mot else None
+        out_sot = ops.head_decode(*outs["_sot"], hw, STRIDES, 1, out=self.buf("shared.out_sot", (n_sot, A, 6), F32))
+        return out_mot, out_sot
 
 
 def _cls_cols(ncls):
