@@ -10,7 +10,18 @@ clock around `steps` steps that end in a device synchronise, three rounds altern
 Also printed: the device-only step (CUDA events around graph replays of the step with its input copy), the kernels launched per
 step through the C ABI, and the device memory each side added on top of what was already allocated (peak allocation while it was
 built and warmed up, minus the allocation before).  The card's name and power limit are printed first.  One JSON line per
-(config, K, mot)."""
+(config, K, mot).
+
+    python tools/bench_unified.py --workload mask [--configs ...] [--objects 1 3] [--mots on off] [--steps 20]
+
+The mask workload: VOS objects plus a MOTS arm on one video, UnicornUnifiedMaskTracker against UnicornVOSTrack(use_graph=True,
+depth=2) plus UnicornMOTSTracker(use_graph=True), both pipelined (submit(t + 1) before collect(t)), on unicorn_track_large_mask and
+unicorn_track_large_mot_challenge_mask.  The video is 1080x1920: its frames are letterboxed once on the host to 800x1280 uint8 and kept
+on the device, and the label map, soft masks and MOTS strings are produced at 1080x1920.  The objects are added on frame 0, in one
+group.  A step includes the VOS result assembly, the MOTS association and the mask encode.  The device-only step is the graph
+replays with their input copies, plus the unified tracker's result assembly, which runs after its graph (UnicornVOSTrack captures
+its own).  Launches per step count the kernels of the graphs plus the launches outside them (assembly, encode).  One JSON line per
+(config, objects, mots)."""
 import argparse
 import json
 import os
@@ -27,13 +38,23 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--configs", nargs="+", default=["unicorn_track_large", "unicorn_track_r50"])
+    ap.add_argument("--workload", choices=["box", "mask"], default="box")
+    ap.add_argument("--configs", nargs="+", default=None)
     ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
     ap.add_argument("--targets", type=int, nargs="+", default=[1, 2, 4])
     ap.add_argument("--mot", nargs="+", default=["qd", "byte", "none"], choices=["qd", "byte", "none"])
+    ap.add_argument("--objects", type=int, nargs="+", default=[1, 3])
+    ap.add_argument("--mots", nargs="+", default=["on", "off"], choices=["on", "off"])
+    ap.add_argument("--orig", type=int, nargs=2, default=(1080, 1920))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
+    if args.workload == "mask":
+        args.configs = args.configs or ["unicorn_track_large_mask", "unicorn_track_large_mot_challenge_mask"]
+        return mask(args)
+    args.configs = args.configs or ["unicorn_track_large", "unicorn_track_r50"]
     from unicorn_b200.engine import UnicornEngine
     from unicorn_b200.mot import UnicornMOTTracker
     from unicorn_b200.sot import UnicornSOTBatch
@@ -43,8 +64,6 @@ def main():
     from unicorn_b200.unified import UnicornUnifiedTracker
     from unicorn_b200.weights import make_state_dict
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
     H, W = args.size
     bargs = types.SimpleNamespace(track_thresh=0.5, track_buffer=30, match_thresh=0.8, mot20=False)
     new_tracker = {"qd": lambda: QuasiDenseEmbedTracker(), "byte": lambda: BYTETracker(bargs), None: lambda: None}
@@ -108,30 +127,144 @@ def main():
                 two_round(4)
                 launches = sb.launches_per_frame + (mt._b.launches_per_frame if mt else 0)
                 sides["two_drivers"] = (two_round, two_replay, launches, torch.cuda.max_memory_allocated() - m0)
-                times = {key: [] for key in sides}
-                for _ in range(args.rounds):
-                    for key, (run, *_rest) in sides.items():
-                        torch.cuda.synchronize()
-                        t0 = time.perf_counter()
-                        run(args.steps)
-                        torch.cuda.synchronize()
-                        times[key].append(time.perf_counter() - t0)
                 line = {"config": cfg, "size": [H, W], "targets": K, "mot": mot or "none"}
-                for key, (_, replay, launches, mem) in sides.items():
-                    torch.cuda.synchronize()
-                    e0.record()
-                    for t in range(args.steps):
-                        replay(t)
-                    e1.record()
-                    torch.cuda.synchronize()
-                    ms = [1e3 * t / args.steps for t in times[key]]
-                    line[key] = {"ms_per_step": round(statistics.median(ms), 2), "ms_per_step_min_max": [round(min(ms), 2), round(max(ms), 2)],
-                                 "device_ms_per_step": round(e0.elapsed_time(e1) / args.steps, 2), "launches_per_step": launches,
-                                 "added_peak_alloc_gib": round(mem / 2 ** 30, 2)}
-                line["two_drivers_over_unified"] = round(line["two_drivers"]["ms_per_step"] / line["unified"]["ms_per_step"], 3)
-                line.update(steps=args.steps, rounds=args.rounds)
+                line.update(compare(sides, args, e0, e1))
                 print(json.dumps(line), flush=True)
                 del sides, un, sb, mt, un_round, un_replay, two_round, two_replay
+                torch.cuda.empty_cache()
+        del eng
+        torch.cuda.empty_cache()
+
+
+def compare(sides, args, e0, e1):
+    """Times every side of `sides` {name: (round(steps), replay(t), launches, added bytes)}: rounds alternate between the sides."""
+    times = {key: [] for key in sides}
+    for _ in range(args.rounds):
+        for key, (run, *_rest) in sides.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            run(args.steps)
+            torch.cuda.synchronize()
+            times[key].append(time.perf_counter() - t0)
+    line = {}
+    for key, (_, replay, launches, mem) in sides.items():
+        torch.cuda.synchronize()
+        e0.record()
+        for t in range(args.steps):
+            replay(t)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = [1e3 * t / args.steps for t in times[key]]
+        line[key] = {"ms_per_step": round(statistics.median(ms), 2), "ms_per_step_min_max": [round(min(ms), 2), round(max(ms), 2)],
+                     "device_ms_per_step": round(e0.elapsed_time(e1) / args.steps, 2), "launches_per_step": launches,
+                     "added_peak_alloc_gib": round(mem / 2 ** 30, 2)}
+    line["two_drivers_over_unified"] = round(line["two_drivers"]["ms_per_step"] / line["unified"]["ms_per_step"], 3)
+    line.update(steps=args.steps, rounds=args.rounds)
+    return line
+
+
+def mask(args):
+    from unicorn_b200 import _lib, ops
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mots import UnicornMOTSTracker
+    from unicorn_b200.sot import preprocess
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.unified import UnicornUnifiedMaskTracker
+    from unicorn_b200.vos import UnicornVOSTrack
+    from unicorn_b200.weights import make_state_dict
+
+    H, W = args.size
+    h0, w0 = args.orig
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    frames, boxes = make_video(5, h0, w0, seed=0, n_obj=6)
+    rgb = [f.permute(1, 2, 0).flip(-1).round().clamp(0, 255).to(torch.uint8).numpy().copy() for f in frames]
+    lb = [preprocess(im, (H, W)) for im in rgb]
+    r = lb[0][1]
+    ref = lb[0][0].cuda()
+    steps_u8 = [f.cuda() for f, _ in lb[1:]]  # [1,H,W,3] letterboxed, resident on the device
+
+    def outside(step, n=4):
+        """Launches per step outside the graphs (result assembly, encode), counted over n steps."""
+        l0 = _lib.LAUNCHES
+        for t in range(n):
+            step(t)
+        return (_lib.LAUNCHES - l0) / n
+
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        for K in args.objects:
+            objs = {k + 1: boxes[0, k] * r for k in range(K)}
+            for mots in [m == "on" for m in args.mots]:
+                sides = {}
+                # ---- one backbone pass per frame
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                un = UnicornUnifiedMaskTracker(eng, (H, W), (h0, w0), K, 1, mots=mots)
+                un.add_objects(objs)
+                un.step_tensor(ref)
+
+                def un_round(steps, un=un):
+                    un.submit(steps_u8[0])
+                    for t in range(steps):
+                        if t + 1 < steps:
+                            un.submit(steps_u8[(t + 1) % 4])
+                        un.collect()
+
+                def un_replay(t, un=un):
+                    s = un._ring.slots[t % 2]
+                    s.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
+                    s.graph.replay()
+                    ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], None, [o for o, _ in s.objs], H, W, un.r, s.soft, s.seg)
+                un_round(4)
+                launches = un.launches_per_frame + outside(lambda t: un.step_tensor(steps_u8[t % 4]))
+                sides["unified"] = (un_round, un_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                # ---- today's drivers, each with its own backbone and mask-branch pass
+                m0 = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                vt = UnicornVOSTrack(eng, (H, W), use_graph=True, depth=2)
+                vt.initialize_tensor(ref, objs, orig_size=(h0, w0), r=r)
+                mt = UnicornMOTSTracker(eng, (H, W), use_graph=True) if mots else None
+                mots_launches = 0
+                if mt:  # the first MOTS step runs eagerly: its launches are those its graphs replay
+                    l0 = _lib.LAUNCHES
+                    mt.submit(ref, h0, w0)
+                    mots_launches = _lib.LAUNCHES - l0
+                    mt.collect()
+
+                def two_round(steps, vt=vt, mt=mt):
+                    vt.submit(steps_u8[0])
+                    if mt:
+                        mt.submit(steps_u8[0], h0, w0)
+                    for t in range(steps):
+                        if t + 1 < steps:
+                            vt.submit(steps_u8[(t + 1) % 4])
+                            if mt:
+                                mt.submit(steps_u8[(t + 1) % 4], h0, w0)
+                        vt.collect()
+                        if mt:
+                            mt.collect()
+
+                def two_replay(t, vt=vt, mt=mt):
+                    s = vt._workers[t % 2]
+                    s.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
+                    s.graph.replay()
+                    if mt:
+                        c = mt._slots[t % 2]
+                        c.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
+                        c.graph.replay()
+                two_round(6)
+
+                def two_step(t, vt=vt, mt=mt):
+                    vt.submit(steps_u8[t % 4])
+                    vt.collect()
+                    if mt:
+                        mt.step_tensor(steps_u8[t % 4], h0, w0)
+                launches = vt.launches_per_frame + mots_launches + outside(two_step)
+                sides["two_drivers"] = (two_round, two_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                line = {"config": cfg, "size": [H, W], "orig": [h0, w0], "objects": K, "mots": mots}
+                line.update(compare(sides, args, e0, e1))
+                print(json.dumps(line), flush=True)
+                del sides, un, vt, mt, un_round, un_replay, two_round, two_replay, two_step
                 torch.cuda.empty_cache()
         del eng
         torch.cuda.empty_cache()

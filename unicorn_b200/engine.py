@@ -717,14 +717,19 @@ class UnicornEngine:
             feats.append(cur)
         return feats
 
-    def head_shared(self, fpn, priors, mot=True):
+    def head_shared(self, fpn, priors, mot=True, with_masks=False):
         """The head of one image's pyramid for several head images at once: with mot=True image 0 is the MOT image (mode "mot", no
         prior), then one SOT image (mode "sot") per prior plane.  fpn: 3 NHWC bf16 maps [1,h,w,C]; priors: the 3 fp32 maps of
         propagate ([K,h,w] planes in any leading shape, K >= 1).  The stem conv and its statistics run once at B = 1 and
         uc_groupnorm_apply_bcast writes all 1 + K (or K) stem outputs; the ConvNeXt blocks and towers run on all images together, the
         predictors of each mode on its batch slice.  Returns (MOT decoded [1, A, 5+ncls] or None, SOT decoded [K, A, 6]); every image
-        equals head(fpn, its prior or None, its mode) at B = 1, bit for bit."""
+        equals head(fpn, its prior or None, its mode) at B = 1, bit for bit.
+        with_masks=True (a *_mask config) also runs each level's controller conv on all images at once (the controllers are shared by
+        both modes, unicorn_head_mask.py:334): self.dyn_levels holds 3 fp32 [1 + K (or K), h, w, 176] maps in image order, each image's
+        equal to that of head(..., with_masks=True) at B = 1."""
         self._tracking_only("head_shared")
+        if with_masks and not self.cfg["mask"]:
+            raise ValueError(f"UnicornEngine.head_shared: {self.cfg_name} has no mask head (with_masks needs a *_mask config)")
         assert fpn[0].shape[0] == 1, "head_shared: the pyramid of one image"
         n_mot = int(bool(mot))
         n_sot = priors[0].numel() // (fpn[0].shape[1] * fpn[0].shape[2])
@@ -749,8 +754,13 @@ class UnicornEngine:
                 cls, reg = feats[0][i0:i0 + n], feats[1][i0:i0 + n]
                 outs[sfx][1][k] = ops.conv2d(cls, cw, 1, 1, bias=cb, out=self.buf(f"shared{k}.clso{sfx}", (n, h, w, cb.numel()), F32))
                 outs[sfx][0][k] = ops.conv2d(reg, row, 1, 1, bias=rob, out=self.buf(f"shared{k}.roo{sfx}", (n, h, w, 8), F32))
+            if with_masks:
+                cw_, cb_ = L["ctrl"]
+                self.dyn_levels[k] = self.conv(feats[1], cw_, 3, 1, 1, bias=cb_, out=self.buf(f"shared{k}.dyn", (n_mot + n_sot, h, w, 176), F32))
             hw[k] = (h, w)
 
+        if with_masks:
+            self.dyn_levels = [None] * 3
         # the three levels on three streams, as in head()
         main = torch.cuda.current_stream()
         if self._side_streams is None:

@@ -1,4 +1,4 @@
-"""SOT targets and MOT objects of one video with one backbone pass per frame.
+"""SOT targets and MOT objects, or VOS objects and MOTS instances, of one video with one backbone pass per frame.
 
 Unicorn's tracking checkpoints (unicorn_track_tiny / _large / _large_mot_challenge / _r50) serve SOT and MOT with one set of weights.
 Run as two drivers (UnicornSOTTrack per target, UnicornMOTTracker), every frame computes the backbone and neck once per driver;
@@ -16,7 +16,10 @@ equals UnicornMOTTracker's on the same frames, bit for bit.
 
 The step protocol is the MOT driver's: submit(t + 1) may precede collect(t), so the host association of step t overlaps the device
 work of step t + 1; with use_graph the first step runs eagerly and the second is captured.  The target slots are static buffers the
-graph reads: adding or removing a target writes them in place and never re-captures."""
+graph reads: adding or removing a target writes them in place and never re-captures.
+
+UnicornUnifiedMaskTracker does the same for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS object slots
+in place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both."""
 import warnings
 
 import torch
@@ -25,8 +28,11 @@ from . import _lib, ops
 from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count
 from .mot import QDEmbedding, _qd_match
+from .mots import MaskEncoder, _mots_match, _mots_result
 from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
 from .tracker import QuasiDenseEmbedTracker
+from .tracker._stream import assoc_stream
+from .vos import MAX_OBJECTS_PER_SEQUENCE, ROWS_PER_GROUP_SLOT, label_values
 
 
 class _Step:
@@ -42,7 +48,49 @@ class _Step:
         self.tids, self.scale, self.frame_id, self.tracker = [], 1.0, 0, None
 
 
-class UnicornUnifiedTracker:
+class _OneVideo:
+    """What the one-video drivers share: the frame check, a step ring whose submit stages the frame or changes nothing, and the
+    eager / capture / replay choice of a step."""
+
+    def _check(self, frame):
+        H, W = self.input_size
+        ok = torch.is_tensor(frame) and ((frame.dtype == torch.uint8 and tuple(frame.shape) == (1, H, W, 3)) or
+                                         (frame.dtype == torch.float32 and tuple(frame.shape) == (1, 3, H, W)))
+        if not ok:
+            got = (tuple(frame.shape), frame.dtype) if torch.is_tensor(frame) else type(frame)
+            raise ValueError(f"{type(self).__name__}: frame must be uint8 [1,{H},{W},3] or float32 [1,3,{H},{W}], got {got}")
+
+    def _next_step(self, frame, slot_of):
+        """Checks `frame`, takes the ring's next step s and stages the frame into the frame slot slot_of(s).  Returns (s, slot).  A
+        frame that fails leaves the ring and the slot as they were."""
+        self._check(frame)
+        s = self._ring.submit()
+        c = slot_of(s)
+        u8, graph = c.u8, c.graph
+        try:
+            c.stage(frame)  # the last step that can fail: nothing has changed before it
+        except BaseException:
+            self._ring.submitted -= 1
+            c.u8, c.graph = u8, graph
+            raise
+        return s, c
+
+    def _run(self, c, frame_fn):
+        """Runs frame_fn() in frame slot c: replays c's graph, or captures it, or runs eagerly."""
+        if c.graph is not None:
+            c.graph.replay()
+        elif self.use_graph and self._warm_u8 == c.u8:
+            # the first step ran eagerly (plan-time autotuning, buffer allocation); this one is captured without a warm-up run: a QD
+            # step advances pre_dict, so it must not run twice
+            c.graph, self.launches_per_frame = c.capture(frame_fn)
+        else:
+            l0 = _lib.LAUNCHES
+            frame_fn()
+            self.launches_per_frame = _lib.LAUNCHES - l0
+            self._warm_u8 = c.u8
+
+
+class UnicornUnifiedTracker(_OneVideo):
     """Up to `max_targets` SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None) on one video, one backbone pass per frame.
 
     SOT settings (conf, nms, max_inst) default to UnicornSOTTrack's, MOT settings (mot_conf, mot_nms, score_thr, max_dets) to
@@ -165,42 +213,15 @@ class UnicornUnifiedTracker:
                 embed = self._qd(e, seq["feat"], dets, cnt)
         self.last = dict(fpn=fpn, feat=seq["feat"], priors=priors, head_mot=head_mot, head_sot=head_sot, embed=embed)
 
-    def _check(self, frame):
-        H, W = self.input_size
-        ok = torch.is_tensor(frame) and ((frame.dtype == torch.uint8 and tuple(frame.shape) == (1, H, W, 3)) or
-                                         (frame.dtype == torch.float32 and tuple(frame.shape) == (1, 3, H, W)))
-        if not ok:
-            got = (tuple(frame.shape), frame.dtype) if torch.is_tensor(frame) else type(frame)
-            raise ValueError(f"UnicornUnifiedTracker: frame must be uint8 [1,{H},{W},3] or float32 [1,3,{H},{W}], got {got}")
-
     def submit(self, frame, scale=1.0):
         """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; scale: its letterbox ratio.  Enqueues the step on
         the current stream; returns immediately."""
-        self._check(frame)
-        c = self._slot
-        s = self._ring.submit()
-        u8, graph = c.u8, c.graph
-        try:
-            c.stage(frame)  # the last step that can fail: nothing has changed before it
-        except BaseException:
-            self._ring.submitted -= 1
-            c.u8, c.graph = u8, graph
-            raise
+        s, c = self._next_step(frame, lambda s: self._slot)
         s.tids = [None if i in self._pending else t for i, t in enumerate(self._tid)]
         if self.mot is not None:
             self.frame_id += 1
         s.scale, s.frame_id, s.tracker = float(scale), self.frame_id, self.tracker
-        if c.graph is not None:
-            c.graph.replay()
-        elif self.use_graph and self._warm_u8 == c.u8:
-            # the first step ran eagerly (plan-time autotuning, buffer allocation); this one is captured without a warm-up run: a QD
-            # step advances pre_dict, so it must not run twice
-            c.graph, self.launches_per_frame = c.capture(self._frame)
-        else:
-            l0 = _lib.LAUNCHES
-            self._frame()
-            self.launches_per_frame = _lib.LAUNCHES - l0
-            self._warm_u8 = c.u8
+        self._run(c, self._frame)
         K = self.max_targets
         s.sot_count.copy_(self.sot_ws.count, non_blocking=True)
         s.sot_dets.copy_(self.sot_ws.dets.view(K, -1, 7)[:, :self.max_inst], non_blocking=True)
@@ -268,3 +289,317 @@ class UnicornUnifiedTracker:
             if n > 0 and tid in self.states:
                 self.states[tid] = state_xywh(dets[0], r, self.input_size)
         return {"targets": {tid: self.states[tid] for tid in self.targets}, "mot": out["mot"]}
+
+
+# ---------------------------------------------------------------------------------------------------------- VOS objects + MOTS
+class _MaskStep(FrameSlot):
+    """One step of UnicornUnifiedMaskTracker in flight: its frame slot and graph, the device buffers its results live in until the
+    next step of the same parity (the masks of both arms, the label map and soft masks), its pinned read-back and the host values it
+    was submitted with."""
+
+    def __init__(self, eng, H, W, O, max_dets, mots, share=None):
+        super().__init__(eng, H, W)
+        if share is not None:  # one set of input buffers and one MOTS NMS workspace for both parities
+            self.img_in, self.img_in_u8, self.ws = share.img_in, share.img_in_u8, share.ws
+        dev = eng.dev
+        self.vos_masks = torch.zeros(O, 1, H, W, dtype=torch.float32, device=dev)
+        self.host_rows = torch.zeros(O, 8).pin_memory()  # best detection row + count of every object slot
+        self.seg = self.soft = None
+        self.mots_masks = torch.zeros(max_dets, H, W, dtype=torch.float32, device=dev) if mots else None
+        self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory() if mots else None
+        self.host_dets = torch.zeros(max_dets, 7).pin_memory() if mots else None
+        self.host_feats = torch.zeros(max_dets, 128).pin_memory() if mots else None
+        self.objs, self.new_ids, self.frame_id = [], [], 0  # (id, object slot) of the live objects, ids entering from init_mask
+
+
+class UnicornUnifiedMaskTracker(_OneVideo):
+    """Up to `max_objects` VOS objects plus optionally the MOTS arm (mots=True) on one video of original size `orig_size` (h, w), one
+    backbone, neck and mask-branch pass per frame.  For the *_mask checkpoints, which serve VOS and MOTS with one set of weights.
+
+    VOS settings (conf, nms, max_inst, d_rate) default to UnicornVOSTrack's, MOTS settings (mots_conf, mots_nms, score_thr, max_dets,
+    mask_thres, mots_d_rate, min_box_area) to UnicornMOTSTracker's; `tracker`: the MOTS arm's QuasiDenseEmbedTracker (default a fresh
+    one).  Both arms use the letterbox ratio r = min(H / h, W / w).
+
+    The device half of a step is one CUDA graph per parity slot: backbone + neck at B = 1 with the VOS arm of the `max_groups` group
+    slots on the side stream (UnicornVOSBatch._frame with one sequence), the mask branch once, UnicornEngine.head_shared with the
+    controllers (image 0 the MOTS image, then one image per object slot), NMS of both arms, uc_dynamic_masks of both on the one
+    mask-branch image, and the MOTS arm's QDEmbedding.  ops.vos_aggregate of the step's objects follows the graph.  Each object's
+    rows, mask, the label map and soft masks equal those of one UnicornVOSTrack, the MOTS results those of UnicornMOTSTracker, bit
+    for bit.
+
+    add_objects({id: box_xyxy}, init_mask=None): the next submitted frame becomes the reference of these objects (one group).  With
+    init_mask (uint8 [h, w] label map) they enter that step's label map from it (UnicornVOSTrack.track_tensor with new objects);
+    without, they appear from the following step on (UnicornVOSTrack.initialize_tensor).  remove_object(id) frees the object's slot.
+    Object and group slots are static buffers the graphs read: adding or removing objects writes them in place and never
+    re-captures.  A free slot computes on stale buffers: the device `active` table zeroes its detection count, so its mask is
+    zero, and its result is dropped.  Steps already submitted report the objects they were submitted with."""
+
+    def __init__(self, engine: UnicornEngine, input_size, orig_size, max_objects, max_groups=None, mots=True, tracker=None,
+                 conf=0.001, nms=0.65, max_inst=1, d_rate=2,
+                 mots_conf=0.01, mots_nms=0.7, score_thr=0.1, max_dets=64,
+                 mask_thres=0.3, mots_d_rate=2, min_box_area=100, use_graph=True):
+        if engine.det or not engine.cfg["mask"]:
+            raise ValueError(f"UnicornUnifiedMaskTracker: {engine.cfg_name} has no tracking mask head; VOS and MOTS need a *_mask tracking config")
+        max_groups = max_objects if max_groups is None else max_groups
+        if max_objects < 1 or max_groups < 1:
+            raise ValueError(f"UnicornUnifiedMaskTracker: max_objects and max_groups must be >= 1 (got {max_objects}, {max_groups})")
+        self.eng, self.input_size, self.orig_size = engine, tuple(input_size), tuple(int(v) for v in orig_size)
+        self.max_objects, self.max_groups, self.mots = max_objects, max_groups, bool(mots)
+        self.tracker = (tracker or QuasiDenseEmbedTracker(device=engine.dev)) if mots else None
+        self.conf, self.nms, self.max_inst, self.d_rate = conf, nms, max_inst, d_rate
+        self.mots_conf, self.mots_nms, self.score_thr, self.max_dets = mots_conf, mots_nms, score_thr, max_dets
+        self.mask_thres, self.mots_d_rate, self.min_box_area = mask_thres, mots_d_rate, min_box_area
+        self.use_graph = use_graph
+        H, W = self.input_size
+        h0, w0 = self.orig_size
+        self.r = min(H / h0, W / w0)
+        dev, O, G = engine.dev, max_objects, max_groups
+        self.R = min(ROWS_PER_GROUP_SLOT, max_objects)  # label rows of every group slot
+        n8, n16 = (H // 8) * (W // 8), (H // 16) * (W // 16)
+        self.vos_ws = ops.PostWorkspace(anchor_count(H, W), dev, O)
+        self._qd = QDEmbedding(engine, H, W, max_dets, "unifiedm.emb") if mots else None
+        up, up_m = 8 // d_rate, 8 // mots_d_rate
+        self._scratch = torch.empty(max(O * (1 + up * up), max_dets * (1 + up_m * up_m) if mots else 0) * n8, dtype=torch.float32, device=dev)
+        self._enc = MaskEncoder(max_dets, dev) if mots else None
+        # the group and object slots as UnicornVOSBatch keeps them, with the device active table
+        self.ref_proj = tuple(torch.zeros(G * n16, 256, dtype=torch.bfloat16, device=dev) for _ in range(2))
+        self.lbs = torch.zeros(G, self.R, n8, dtype=torch.float32, device=dev)
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.obj_row = torch.zeros(O, **i32)  # group slot * R + label row of each object slot
+        self.active = torch.zeros(O, **i32)
+        self.image_of = torch.zeros(O, **i32)  # every object image reads the one mask-branch image
+        self.rows = torch.zeros(O, 8, dtype=torch.float32, device=dev)
+        self._gs = [0] * G  # objects (live or pending) per group slot
+        self._os = [None] * O  # (id, group slot, label row) per object slot
+        self._order = []  # live objects in group order (UnicornVOSTrack.obj_ids)
+        self._pending = []  # groups whose reference is the next submitted frame: (boxes {id: box}, init_mask or None)
+        # two parity steps: submit(t + 1) writes one while collect(t) reads the other; each has its own graph and result buffers
+        first = _MaskStep(engine, H, W, O, max_dets, mots)
+        self._ring = Ring([first, _MaskStep(engine, H, W, O, max_dets, mots, share=first)])
+        self._warm_u8 = None
+        self._host_in = torch.full((1, H, W, 3), 114, dtype=torch.uint8).pin_memory()
+        self.frame_id = 0
+        self.state_pre_dict = {}  # track(): the reference-protocol state of every object
+        self.launches_per_frame = 0
+        self.last = {}
+        self.last_rows = self.last_dets = self.last_feats = None
+
+    graphs = property(lambda self: [s.graph for s in self._ring.slots])
+    objects = property(lambda self: self._order + [o for b, _ in self._pending for o in b])
+
+    # ------------------------------------------------------------------------------------------ objects
+    def _slot_of(self, oid):
+        return next(k for k, o in enumerate(self._os) if o is not None and o[0] == oid)
+
+    def add_objects(self, boxes_xyxy, init_mask=None):
+        """Track the objects {id: [x1, y1, x2, y2]} (resized-image coordinates; ids 1..255) from the next submitted frame on.
+        init_mask: uint8 [h, w] label map of that frame in which they appear (at most one per step)."""
+        boxes = {oid: torch.as_tensor(b, dtype=torch.float32).view(-1) for oid, b in dict(boxes_xyxy).items()}
+        known = self.objects
+        try:
+            vals = [int(o) for o in boxes]
+        except (TypeError, ValueError):
+            vals = None
+        if not boxes or vals is None or any(not 1 <= v <= 255 for v in vals):
+            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: ids must be 1..255 (got {list(boxes)})")
+        if len(set(vals)) != len(vals) or set(vals) & {int(o) for o in known}:
+            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: duplicate object id in {list(boxes)} (tracked: {known})")
+        if any(b.numel() != 4 for b in boxes.values()):
+            raise ValueError("UnicornUnifiedMaskTracker.add_objects: every box needs 4 values")
+        n = len(known) + len(boxes)
+        if n > self.max_objects:
+            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {n} objects exceed max_objects = {self.max_objects}")
+        if n > MAX_OBJECTS_PER_SEQUENCE:
+            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {n} objects (at most {MAX_OBJECTS_PER_SEQUENCE} in one video)")
+        need_g = -(-len(boxes) // ROWS_PER_GROUP_SLOT)
+        if need_g > self._gs.count(0):
+            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {need_g} new group slots but {self._gs.count(0)} of max_groups = "
+                             f"{self.max_groups} are free")
+        if init_mask is not None:
+            init_mask = torch.as_tensor(init_mask)
+            if init_mask.dtype != torch.uint8 or tuple(init_mask.shape) != self.orig_size:
+                raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: init_mask must be uint8 {list(self.orig_size)}, got "
+                                 f"{init_mask.dtype} {list(init_mask.shape)}")
+            if any(m is not None for _, m in self._pending):
+                raise ValueError("UnicornUnifiedMaskTracker.add_objects: the next step already has an init_mask")
+            init_mask = init_mask.to(self.eng.dev).contiguous()
+        ids = list(boxes)
+        for c0 in range(0, len(ids), ROWS_PER_GROUP_SLOT):
+            g = self._gs.index(0)
+            chunk = ids[c0:c0 + ROWS_PER_GROUP_SLOT]
+            self._gs[g] = len(chunk)
+            for row, oid in enumerate(chunk):
+                self._os[self._os.index(None)] = (oid, g, row)
+        self._pending.append((boxes, init_mask))
+
+    def remove_object(self, oid):
+        """Stop tracking `oid` and free its object slot, and its group slot with the group's last object (steps already submitted
+        still report it)."""
+        if oid not in self.objects:
+            raise ValueError(f"UnicornUnifiedMaskTracker.remove_object: unknown object id {oid!r}")
+        k = self._slot_of(oid)
+        g = self._os[k][1]
+        self._os[k] = None
+        self._gs[g] -= 1
+        if oid in self._order:
+            self._order.remove(oid)
+            self.active[k].fill_(0)  # stream-ordered after the steps in flight
+        else:
+            i = next(i for i, (b, _) in enumerate(self._pending) if oid in b)
+            del self._pending[i][0][oid]
+            if not self._pending[i][0]:
+                del self._pending[i]
+        self.state_pre_dict.pop(oid, None)
+
+    def _write_references(self):
+        """The pending groups take the step just enqueued as their reference frame: its stride-16 feature is projected once, and the
+        projection and the boxes' label values go into the groups' slots (UnicornVOSBatch._add_group)."""
+        e = self.eng
+        n16 = self.ref_proj[0].shape[0] // self.max_groups
+        src, q = e.project_ref(self.last["feat"])
+        for boxes, _ in self._pending:
+            ids = list(boxes)
+            lbs = label_values([boxes[o] for o in ids], self.input_size, e.dev)
+            written = set()
+            for i, oid in enumerate(ids):
+                k = self._slot_of(oid)
+                _, g, row = self._os[k]
+                if g not in written:  # row 0 of a group slot may have been removed before the reference frame
+                    written.add(g)
+                    self.ref_proj[0][g * n16:(g + 1) * n16].copy_(src)
+                    self.ref_proj[1][g * n16:(g + 1) * n16].copy_(q)
+                    self.lbs[g].zero_()
+                self.lbs[g, row].copy_(lbs[i])
+                self.obj_row[k].fill_(g * self.R + row)
+                self.active[k].fill_(1)
+            self._order += ids
+        self._pending = []
+
+    # ------------------------------------------------------------------------------------------ device half
+    def _frame(self, s):
+        e = self.eng
+        H, W = self.input_size
+        hh, ww = H // 8, W // 8
+        G, O, R = self.max_groups, self.max_objects, self.R
+        F32 = torch.float32
+        e.begin_frame()
+
+        def correlate(seq):  # the VOS arm, on the stream that overlaps the neck (UnicornVOSBatch._frame with one sequence)
+            feat = seq["feat"]
+            if G > 1:
+                feat = e.buf("unifiedm.featG", (G,) + tuple(feat.shape[1:]))
+                feat.copy_(seq["feat"].expand(G, -1, -1, -1))
+            f_pre, f_cur = e.interaction(None, feat, ref_proj=self.ref_proj)
+            e_pre, e_cur = e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc")
+            coarse = ops.corr_propagate(e_pre.view(G, -1, 128), e_cur.view(G, -1, 128), self.lbs, out=e.buf("unifiedm.coarse", (G, R, hh * ww), F32))
+            c0 = torch.index_select(coarse.view(G * R, hh * ww), 0, self.obj_row, out=e.buf("unifiedm.c0", (O, hh * ww), F32)).view(O, hh, ww)
+            return (c0, ops.bilinear(c0, hh // 2, ww // 2, 2.0, 2.0, out=e.buf("unifiedm.p1", (O, hh // 2, ww // 2), F32)),
+                    ops.bilinear(c0, hh // 4, ww // 4, 4.0, 4.0, out=e.buf("unifiedm.p2", (O, hh // 4, ww // 4), F32)))
+
+        fpn, seq, priors = e.backbone(s.img, tag="unifiedm", side=correlate)
+        mf, um = e.mask_branch(fpn)  # once: every head image reads it
+        head_mots, head_vos = e.head_shared(fpn, priors, mot=self.mots, with_masks=True)
+        n_mot = int(self.mots)
+        dyn = list(e.dyn_levels)
+        hw = [(t.shape[1], t.shape[2]) for t in dyn]
+        _, cnt = ops.postprocess_device(head_vos, 1, self.conf, self.nms, self.vos_ws, max_keep=self.max_inst)
+        cnt.mul_(self.active)
+        s.vos_masks.zero_()  # an object without a detection contributes an all-zero mask (unicorn_vos.py:154-155)
+        up = 8 // self.d_rate
+        ops.dynamic_masks(mf, um, [t[n_mot:] for t in dyn], hw, self.vos_ws, 1, up_rate=up, d_rate=self.d_rate, out=s.vos_masks,
+                          scratch=self._scratch, image_of=self.image_of)
+        self.rows[:, :7].copy_(self.vos_ws.dets.view(O, -1, 7)[:, 0])
+        self.rows[:, 7].copy_(self.vos_ws.count)
+        if self.mots:
+            dets, cnt = ops.postprocess_device(head_mots[0], e.ncls, self.mots_conf, self.mots_nms, s.ws)
+            ops.dynamic_masks(mf, um, [t[:1] for t in dyn], hw, s.ws, self.max_dets, up_rate=8 // self.mots_d_rate, d_rate=self.mots_d_rate,
+                              out=s.mots_masks, scratch=self._scratch)
+            self._qd(e, seq["feat"], dets, cnt)
+        self.last = dict(feat=seq["feat"], mask_feats=mf, up_masks=um, priors=priors, head_mots=head_mots, head_vos=head_vos, dyn=dyn)
+
+    def submit(self, frame):
+        """frame: the letterboxed frame, preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device.  Enqueues the step on the
+        current stream; returns immediately."""
+        s, _ = self._next_step(frame, lambda s: s)
+        s.objs = [(oid, self._slot_of(oid)) for oid in self._order]
+        new = [(list(b), m) for b, m in self._pending if m is not None]
+        s.new_ids, init_mask = (new[0][0], new[0][1]) if new else ([], None)
+        self.frame_id += 1
+        s.frame_id = self.frame_id
+        self._run(s, lambda: self._frame(s))
+        s.host_rows.copy_(self.rows, non_blocking=True)
+        if self.mots:
+            s.host_count.copy_(s.ws.count, non_blocking=True)
+            s.host_dets.copy_(s.ws.dets[:self.max_dets], non_blocking=True)
+            s.host_feats.copy_(self._qd.feats[0], non_blocking=True)
+        # the result assembly at the original size: the object list changes with additions, so it stays outside the graph
+        ids = [oid for oid, _ in s.objs] + s.new_ids
+        H0, W0 = self.orig_size
+        if s.seg is None:
+            s.seg = torch.zeros(H0, W0, dtype=torch.uint8, device=self.eng.dev)
+        if s.soft is None or s.soft.shape[0] < len(ids):
+            s.soft = torch.zeros(max(len(ids), 4), H0, W0, dtype=torch.float32, device=self.eng.dev)
+        if ids:
+            ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], init_mask, ids, *self.input_size, self.r, s.soft, s.seg)
+        else:
+            s.seg.zero_()
+        s.event.record()
+        if self._pending:
+            self._write_references()
+
+    # ------------------------------------------------------------------------------------------ host half
+    def collect(self):
+        """Results of the oldest submitted step: {"vos": {"segmentation": uint8 [h, w], "soft": fp32 [n, h, w] (device), "objects":
+        {id: (det_row [7] | None, mask fp32 [H, W] at network resolution | None)}, "ids": [...]}, "mots": the write_results_mots()
+        tuple UnicornMOTSTracker.collect returns, or None without the MOTS arm}.  The device tensors stay valid until the step after
+        the next one is submitted."""
+        s = self._ring.collect()
+        s.event.synchronize()
+        objects, self.last_rows = {}, {}
+        for oid, k in s.objs:
+            row = s.host_rows[k].clone()
+            self.last_rows[oid] = row
+            objects[oid] = (row[:7], s.vos_masks[k, 0]) if row[7] > 0 else (None, None)
+        ids = [oid for oid, _ in s.objs] + s.new_ids
+        vos = dict(segmentation=s.seg, soft=s.soft[:len(ids)], objects=objects, ids=ids)
+        mots = None
+        self.last_dets = self.last_feats = None
+        if self.mots:
+            h0, w0 = self.orig_size
+            n = min(int(s.host_count[0]), self.max_dets)
+            d, f = s.host_dets[:n].clone(), s.host_feats[:n].clone()
+            self.last_dets, self.last_feats = d, f
+            _, oid, rows, emit = _mots_match(self.tracker, d, f, self.r, self.score_thr, s.frame_id, self.min_box_area)
+            stream = assoc_stream(self.eng.dev)
+            with torch.cuda.stream(stream):  # not behind the next step's kernels on the main stream
+                stream.wait_event(s.event)
+                rles = self._enc(s.mots_masks, rows.tolist(), emit, self.mask_thres, self.r, h0, w0)
+            mots = _mots_result(s.frame_id, oid, emit, rles, h0, w0)
+        return {"vos": vos, "mots": mots}
+
+    def step_tensor(self, frame):
+        """Sequential protocol: one step in, its results out."""
+        self.submit(frame)
+        return self.collect()
+
+    # ------------------------------------------------------------------------------------------ reference protocol
+    def track(self, image_rgb, info=None):
+        """image_rgb: an RGB frame (HWC uint8) of the original size, letterboxed once for both arms.  info: UnicornVOSTrack's dict
+        (init_object_ids, init_bbox {id: [x, y, w, h]}, optionally init_mask) for objects that start on this frame.  Returns
+        {"segmentation": uint8 [h, w] numpy, "mots": write_results_mots() tuple or None}; state_pre_dict is kept as
+        UnicornVOSTrack.track keeps it."""
+        if tuple(image_rgb.shape[:2]) != self.orig_size:
+            raise ValueError(f"UnicornUnifiedMaskTracker.track: frame size {tuple(image_rgb.shape[:2])}, the video's is {self.orig_size}")
+        info = info or {}
+        if "init_object_ids" in info:
+            boxes = {oid: xyxy_resized(info["init_bbox"][oid], self.r) for oid in info["init_object_ids"]}
+            mask = info.get("init_mask")
+            self.add_objects(boxes, None if mask is None else torch.as_tensor(mask).to(torch.uint8))
+            for oid in info["init_object_ids"]:
+                self.state_pre_dict[oid] = info["init_bbox"][oid]
+        frame, r = preprocess(image_rgb, self.input_size, out=self._host_in)
+        out = self.step_tensor(frame)
+        for oid, (det, _) in out["vos"]["objects"].items():  # unicorn_vos.py:137-149 (state of the best instance, xywh ints)
+            if det is not None:
+                self.state_pre_dict[oid] = state_xywh(det, r, self.input_size)
+        return {"segmentation": out["vos"]["segmentation"].cpu().numpy(), "mots": out["mots"]}
