@@ -173,6 +173,18 @@ UC_API int uc_groupnorm_apply(const void* x, int ldx, const void* stats, const f
 UC_API int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y, int ldy,
                                     int B, int n_plain, long HW, int C, int G, float eps, int act, const float* prior, const float* beta,
                                     void* stream);
+/* The same normalisation with the source image of each output image taken from a device table (a head stem shared by the head
+ * images of several videos): x holds n_src images [n_src][HW pixels] (row stride ldx, image stride HW * ldx) and stats their
+ * [n_src][G]{sum,sumsq}; src_of is a device int32 [B] table read when the kernel runs, so a captured graph follows its current
+ * contents.  Output image b normalises image src_of[b] with that image's statistics; b < n_plain takes the no-prior path, b >= n_plain
+ * adds prior[(b - n_plain) * HW + pix] * beta[c], as uc_groupnorm_apply_bcast.  Every image equals uc_groupnorm_apply at B = 1 on
+ * image src_of[b], bit for bit.  A table entry outside [0, n_src) leaves output image b untouched and reads nothing of x, stats or
+ * prior.  1 <= n_src, B <= 65535, 0 <= n_plain <= B; src_of non-null and 4-byte aligned; prior (4-byte aligned) and beta are given
+ * exactly when n_plain < B; x (all n_src images) and y must not overlap; otherwise the conventions of uc_groupnorm_apply (UC_EINVAL
+ * before any launch). */
+UC_API int uc_groupnorm_apply_gather(const void* x, int ldx, int n_src, const void* stats, const float* w, const float* b, void* y,
+                                     int ldy, int B, int n_plain, const int* src_of, long HW, int C, int G, float eps, int act,
+                                     const float* prior, const float* beta, void* stream);
 
 /* dst[b,oh,ow,:C] = src[b,oh/up,ow/up,:C], up in {1,2} (nearest upsample + concat slice; yolo_pafpn_new.py:139-146).
  * 16-bit NHWC; C, lds, ldd multiples of 8; src and dst 16-byte aligned. */

@@ -21,7 +21,16 @@ on the device, and the label map, soft masks and MOTS strings are produced at 10
 group.  A step includes the VOS result assembly, the MOTS association and the mask encode.  The device-only step is the graph
 replays with their input copies, plus the unified tracker's result assembly, which runs after its graph (UnicornVOSTrack captures
 its own).  Launches per step count the kernels of the graphs plus the launches outside them (assembly, encode).  One JSON line per
-(config, objects, mots)."""
+(config, objects, mots).
+
+    python tools/bench_unified.py --workload batch [--configs ...] [--n-seq 2 4] [--per-video 1 2] [--mot qd byte none] [--steps 20]
+
+The batch workload: n_seq videos (make_video seeds 0..n_seq-1), each with `per_video` targets (one per object, added on frame 0) and
+the MOT arm, three sides in the same process, all pipelined (submit(t + 1) before collect(t), the association included):
+UnicornUnifiedBatch over all videos; n_seq UnicornUnifiedTrackers stepped in turn; UnicornSOTBatch over all targets (each fed its
+video's frame) plus UnicornMOTBatch(n_seq) (the SOT batch of step t is collected before its next submit).  The device-only step is
+the graph replays of every side's drivers with their input copies.  Besides the ms per step, each side reports the aggregate
+video-frames/s (n_seq / step time).  One JSON line per (config, n_seq, per_video, mot)."""
 import argparse
 import json
 import os
@@ -38,7 +47,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["box", "mask"], default="box")
+    ap.add_argument("--workload", choices=["box", "mask", "batch"], default="box")
     ap.add_argument("--configs", nargs="+", default=None)
     ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
     ap.add_argument("--targets", type=int, nargs="+", default=[1, 2, 4])
@@ -46,6 +55,8 @@ def main():
     ap.add_argument("--objects", type=int, nargs="+", default=[1, 3])
     ap.add_argument("--mots", nargs="+", default=["on", "off"], choices=["on", "off"])
     ap.add_argument("--orig", type=int, nargs=2, default=(1080, 1920))
+    ap.add_argument("--n-seq", type=int, nargs="+", default=[2, 4])
+    ap.add_argument("--per-video", type=int, nargs="+", default=[1, 2])
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
@@ -55,6 +66,8 @@ def main():
         args.configs = args.configs or ["unicorn_track_large_mask", "unicorn_track_large_mot_challenge_mask"]
         return mask(args)
     args.configs = args.configs or ["unicorn_track_large", "unicorn_track_r50"]
+    if args.workload == "batch":
+        return batch(args)
     from unicorn_b200.engine import UnicornEngine
     from unicorn_b200.mot import UnicornMOTTracker
     from unicorn_b200.sot import UnicornSOTBatch
@@ -158,7 +171,9 @@ def compare(sides, args, e0, e1):
         line[key] = {"ms_per_step": round(statistics.median(ms), 2), "ms_per_step_min_max": [round(min(ms), 2), round(max(ms), 2)],
                      "device_ms_per_step": round(e0.elapsed_time(e1) / args.steps, 2), "launches_per_step": launches,
                      "added_peak_alloc_gib": round(mem / 2 ** 30, 2)}
-    line["two_drivers_over_unified"] = round(line["two_drivers"]["ms_per_step"] / line["unified"]["ms_per_step"], 3)
+    first, *others = sides
+    for key in others:  # each other side's step time over the first side's
+        line[f"{key}_over_{first}"] = round(line[key]["ms_per_step"] / line[first]["ms_per_step"], 3)
     line.update(steps=args.steps, rounds=args.rounds)
     return line
 
@@ -266,6 +281,129 @@ def mask(args):
                 print(json.dumps(line), flush=True)
                 del sides, un, vt, mt, un_round, un_replay, two_round, two_replay, two_step
                 torch.cuda.empty_cache()
+        del eng
+        torch.cuda.empty_cache()
+
+
+def batch(args):
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mot import UnicornMOTBatch
+    from unicorn_b200.sot import UnicornSOTBatch
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.tracker import QuasiDenseEmbedTracker
+    from unicorn_b200.tracker.byte_tracker import BYTETracker
+    from unicorn_b200.unified import UnicornUnifiedBatch, UnicornUnifiedTracker
+    from unicorn_b200.weights import make_state_dict
+
+    H, W = args.size
+    bargs = types.SimpleNamespace(track_thresh=0.5, track_buffer=30, match_thresh=0.8, mot20=False)
+    new_tracker = {"qd": lambda: QuasiDenseEmbedTracker(), "byte": lambda: BYTETracker(bargs), None: lambda: None}
+    to_u8 = lambda f: f.round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()  # noqa: E731
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    vids = [make_video(5, H, W, seed=i, n_obj=6) for i in range(max(args.n_seq))]
+    refs_all = [to_u8(f[0:1]).cuda() for f, _ in vids]  # [1,H,W,3] per video
+    steps_all = [[to_u8(f[1 + t:2 + t]).cuda() for t in range(4)] for f, _ in vids]
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        for n in args.n_seq:
+            refs, steps = refs_all[:n], steps_all[:n]
+            ref_b = torch.cat(refs)
+            steps_b = [torch.cat([steps[i][t] for i in range(n)]) for t in range(4)]  # [n,H,W,3]
+            for T in args.per_video:
+                targets = [(i, k) for i in range(n) for k in range(T)]  # (video, object) per target
+                copies = [torch.cat([steps[i][t] for i, _ in targets]) for t in range(4)]  # one frame copy per target
+                for mot in [None if m == "none" else m for m in args.mot]:
+                    sides = {}
+                    # ---- one step for every video: UnicornUnifiedBatch
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    ub = UnicornUnifiedBatch(eng, (H, W), n, n * T, mot=mot)
+                    for i in range(n):
+                        ub.start(i, new_tracker[mot]())
+                    for i, k in targets:
+                        ub.add_target(i, k, vids[i][1][0, k])
+                    ub.step_tensor(ref_b)
+
+                    def ub_round(nsteps, ub=ub):
+                        ub.submit(steps_b[0])
+                        for t in range(nsteps):
+                            if t + 1 < nsteps:
+                                ub.submit(steps_b[(t + 1) % 4])
+                            ub.collect([(H, W)] * n)
+
+                    def ub_replay(t, ub=ub):
+                        ub._slot.img_in_u8.copy_(steps_b[t % 4], non_blocking=True)
+                        ub._slot.graph.replay()
+                    ub_round(4)
+                    sides["batch"] = (ub_round, ub_replay, ub.launches_per_frame, torch.cuda.max_memory_allocated() - m0)
+                    # ---- one UnicornUnifiedTracker per video, stepped in turn
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    uts = []
+                    for i in range(n):
+                        ut = UnicornUnifiedTracker(eng, (H, W), T, mot=mot, tracker=new_tracker[mot]())
+                        for k in range(T):
+                            ut.add_target(k, vids[i][1][0, k])
+                        ut.step_tensor(refs[i])
+                        uts.append(ut)
+
+                    def ut_round(nsteps, uts=uts):
+                        for i, ut in enumerate(uts):
+                            ut.submit(steps[i][0])
+                        for t in range(nsteps):
+                            for i, ut in enumerate(uts):
+                                if t + 1 < nsteps:
+                                    ut.submit(steps[i][(t + 1) % 4])
+                                ut.collect((H, W))
+
+                    def ut_replay(t, uts=uts):
+                        for i, ut in enumerate(uts):
+                            ut._slot.img_in_u8.copy_(steps[i][t % 4], non_blocking=True)
+                            ut._slot.graph.replay()
+                    ut_round(4)
+                    sides["trackers"] = (ut_round, ut_replay, sum(ut.launches_per_frame for ut in uts),
+                                         torch.cuda.max_memory_allocated() - m0)
+                    # ---- UnicornSOTBatch over all targets plus UnicornMOTBatch over the videos
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    sb = UnicornSOTBatch(eng, (H, W), len(targets))
+                    for j, (i, k) in enumerate(targets):
+                        sb.initialize_tensor(j, refs[i], vids[i][1][0, k])
+                    mt = None
+                    if mot:
+                        mt = UnicornMOTBatch(eng, (H, W), n, assoc=mot, use_graph=True)
+                        for i in range(n):
+                            mt.start(i, new_tracker[mot]())
+                        mt.step_tensor(ref_b)
+
+                    def sm_round(nsteps, sb=sb, mt=mt):
+                        if mt:
+                            mt.submit(steps_b[0])
+                        for t in range(nsteps):
+                            sb.submit(copies[t % 4])
+                            if mt and t + 1 < nsteps:
+                                mt.submit(steps_b[(t + 1) % 4])
+                            sb.collect()
+                            if mt:
+                                mt.collect([(H, W)] * n)
+
+                    def sm_replay(t, sb=sb, mt=mt):
+                        sb.slot.img_in_u8.copy_(copies[t % 4], non_blocking=True)
+                        sb.slot.graph.replay()
+                        if mt:
+                            c = mt._ctxs[t % 2]
+                            c.img_in_u8.copy_(steps_b[t % 4], non_blocking=True)
+                            c.graph.replay()
+                    sm_round(4)
+                    launches = sb.launches_per_frame + (mt.launches_per_frame if mt else 0)
+                    sides["sot_mot"] = (sm_round, sm_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                    line = {"config": cfg, "size": [H, W], "n_seq": n, "per_video": T, "mot": mot or "none"}
+                    line.update(compare(sides, args, e0, e1))
+                    for key in sides:
+                        line[key]["video_frames_per_s"] = round(1e3 * n / line[key]["ms_per_step"], 1)
+                    print(json.dumps(line), flush=True)
+                    del sides, ub, uts, sb, mt, ub_round, ub_replay, ut_round, ut_replay, sm_round, sm_replay
+                    torch.cuda.empty_cache()
         del eng
         torch.cuda.empty_cache()
 

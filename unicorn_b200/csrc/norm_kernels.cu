@@ -449,22 +449,29 @@ __global__ void __launch_bounds__(256) layernorm_v8_kernel(const uint16_t* __res
 // y = act(x * scale[c] + shift[c]) (+ prior[pix] * beta[c]); optional second output y2 = y + add2.
 // scale/shift fold the group statistics (int64 fixed point {sum, sumsq} accumulated by uc_conv2d) with the affine
 // parameters; they are computed once per block into shared memory.  x/y bf16 NHWC (strided); 8 channels / thread.
-// kBcast: every output image b (blockIdx.y) reads image 0 of x and of the statistics, and only the images b >= prior_from add the
-// prior, reading its plane b - prior_from; the others take the no-prior path.  y2 is unused.
-template <bool kBcast>
+// kMode says which image of x and of the statistics output image b (blockIdx.y) reads:
+//   kGnEach    image b (uc_groupnorm_apply);
+//   kGnBcast   image 0, and only the images b >= prior_from add the prior, reading its plane b - prior_from; the others take the
+//              no-prior path.  y2 is unused;
+//   kGnGather  image src_of[b] of the n_src images of x, read once per CTA; the prior as kGnBcast.  An entry outside [0, n_src)
+//              leaves image b untouched.  y2 is unused.
+enum GnApplyMode { kGnEach, kGnBcast, kGnGather };
+template <int kMode>
 __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __restrict__ x, int ldx,
                                                                const long long* __restrict__ stats, const float* __restrict__ w,
                                                                const float* __restrict__ bvec, uint16_t* __restrict__ y, int ldy,
                                                                long HW, int C, int G, float eps, int act,
                                                                const float* __restrict__ prior, const float* __restrict__ beta,
                                                                const uint16_t* __restrict__ add2, int ldadd2,
-                                                               uint16_t* __restrict__ y2, int ldy2, int prior_from) {
+                                                               uint16_t* __restrict__ y2, int ldy2, int prior_from,
+                                                               const int* __restrict__ src_of, int n_src) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
   extern __shared__ float sc[];  // [2][C] scale, shift (+ [C] beta)
   const int b = blockIdx.y;
-  const int bx = kBcast ? 0 : b;  // image of x and of the statistics
-  const bool with_prior = prior != nullptr && (!kBcast || b >= prior_from);
+  const int bx = kMode == kGnEach ? b : kMode == kGnBcast ? 0 : src_of[b];  // image of x and of the statistics
+  if (kMode == kGnGather && (bx < 0 || bx >= n_src)) return;  // uniform over the CTA, before any barrier
+  const bool with_prior = prior != nullptr && (kMode == kGnEach || b >= prior_from);
   const int gs = C / G;
   const double inv_n = 1.0 / (static_cast<double>(HW) * gs);
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -486,7 +493,7 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
   for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int c0 = static_cast<int>(i % C8) * 8;
     const long pix = static_cast<long>(b) * HW + i / C8;
-    const long xpix = kBcast ? i / C8 : pix;
+    const long xpix = kMode == kGnEach ? pix : static_cast<long>(bx) * HW + i / C8;
     const uint4 u = *reinterpret_cast<const uint4*>(x + xpix * ldx + c0);
     const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
     // per-channel coefficients as 128-bit shared-memory loads (c0 is a multiple of 8 -> 32-byte aligned)
@@ -513,7 +520,7 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
       for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.f);
     }
     if (with_prior) {
-      const float pr = __ldg(prior + (kBcast ? static_cast<long>(b - prior_from) * HW + i / C8 : pix));
+      const float pr = __ldg(prior + (kMode != kGnEach ? static_cast<long>(b - prior_from) * HW + i / C8 : pix));
       const float4 b0 = *reinterpret_cast<const float4*>(sc + 2 * C + c0), b1 = *reinterpret_cast<const float4*>(sc + 2 * C + c0 + 4);
       const float bt[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
@@ -522,7 +529,7 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
     uint4 o;
     o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]); o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
     *reinterpret_cast<uint4*>(y + pix * ldy + c0) = o;
-    if (!kBcast && y2) {
+    if (kMode == kGnEach && y2) {
       const uint4 a = *reinterpret_cast<const uint4*>(add2 + pix * ldadd2 + c0);
       const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
       uint4 o2;
@@ -641,9 +648,10 @@ extern "C" int uc_groupnorm_apply(const void* x, int ldx, const void* stats, con
   const long total = HW * (C / 8);
   // each block pays C scale/shift computations up front; keep ~2 elements (16 channels) per thread for parallelism
   const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
-  launch_pdl(groupnorm_apply_kernel<false>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
+  launch_pdl(groupnorm_apply_kernel<kGnEach>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
       static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
-      eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2, 0);
+      eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2, 0,
+      static_cast<const int*>(nullptr), 0);
   return check_launch("uc_groupnorm_apply");
 }
 
@@ -675,8 +683,45 @@ extern "C" int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stat
   if (x0 < y1 && y0 < x1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: x and y overlap (not an in-place operation)");
   const long total = HW * (C / 8);
   const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
-  launch_pdl(groupnorm_apply_kernel<true>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
+  launch_pdl(groupnorm_apply_kernel<kGnBcast>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
       static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
-      eps, act, prior, beta, static_cast<const uint16_t*>(nullptr), 0, static_cast<uint16_t*>(nullptr), 0, n_plain);
+      eps, act, prior, beta, static_cast<const uint16_t*>(nullptr), 0, static_cast<uint16_t*>(nullptr), 0, n_plain,
+      static_cast<const int*>(nullptr), 0);
   return check_launch("uc_groupnorm_apply_bcast");
+}
+
+extern "C" int uc_groupnorm_apply_gather(const void* x, int ldx, int n_src, const void* stats, const float* w, const float* b, void* y,
+                                         int ldy, int B, int n_plain, const int* src_of, long HW, int C, int G, float eps, int act,
+                                         const float* prior, const float* beta, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (n_src < 1 || n_src > 65535) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: n_src must be in [1, 65535] (got %d)", n_src);
+  if (B < 1 || B > 65535) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: B must be in [1, 65535] (got %d)", B);
+  if (n_plain < 0 || n_plain > B) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: n_plain must be in [0, B] (got %d, B = %d)", n_plain, B);
+  if (HW < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: HW must be >= 1");
+  if (G < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: G must be >= 1 (got %d)", G);
+  if (C % 8 || ldx % 8 || ldy % 8 || C % G || ldx < C || ldy < C)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: C, ldx, ldy multiples of 8, ldx, ldy >= C; C %% G == 0");
+  if (C > 4096) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: C too large");
+  if (act != UC_ACT_NONE && act != UC_ACT_RELU && act != UC_ACT_SILU)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: act must be UC_ACT_NONE, UC_ACT_RELU or UC_ACT_SILU (got %d)", act);
+  if (!x || !stats || !w || !b || !y || !src_of) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: null pointer");
+  if ((prior != nullptr) != (beta != nullptr)) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: prior and beta go together");
+  if ((prior != nullptr) != (n_plain < B))
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: prior and beta are needed exactly when n_plain < B");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15)
+    return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: x and y must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(stats) & 7) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: stats must be 8-byte aligned");
+  if (reinterpret_cast<uintptr_t>(prior) & 3) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: prior must be 4-byte aligned");
+  if (reinterpret_cast<uintptr_t>(src_of) & 3) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: src_of must be 4-byte aligned");
+  // an output image may read any of the n_src images: writing any of them over x would race with the other images' reads
+  const uintptr_t x0 = reinterpret_cast<uintptr_t>(x), y0 = reinterpret_cast<uintptr_t>(y);
+  const uintptr_t x1 = x0 + (static_cast<uintptr_t>(n_src) * HW - 1) * ldx * 2 + static_cast<uintptr_t>(C) * 2;  // one past the last element
+  const uintptr_t y1 = y0 + (static_cast<uintptr_t>(B) * HW - 1) * ldy * 2 + static_cast<uintptr_t>(C) * 2;
+  if (x0 < y1 && y0 < x1) return set_error(UC_EINVAL, "uc_groupnorm_apply_gather: x and y overlap (not an in-place operation)");
+  const long total = HW * (C / 8);
+  const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
+  launch_pdl(groupnorm_apply_kernel<kGnGather>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
+      static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
+      eps, act, prior, beta, static_cast<const uint16_t*>(nullptr), 0, static_cast<uint16_t*>(nullptr), 0, n_plain, src_of, n_src);
+  return check_launch("uc_groupnorm_apply_gather");
 }

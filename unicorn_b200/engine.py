@@ -717,7 +717,7 @@ class UnicornEngine:
             feats.append(cur)
         return feats
 
-    def head_shared(self, fpn, priors, mot=True, with_masks=False):
+    def head_shared(self, fpn, priors, mot=True, with_masks=False, src_of=None):
         """The head of one image's pyramid for several head images at once: with mot=True image 0 is the MOT image (mode "mot", no
         prior), then one SOT image (mode "sot") per prior plane.  fpn: 3 NHWC bf16 maps [1,h,w,C]; priors: the 3 fp32 maps of
         propagate ([K,h,w] planes in any leading shape, K >= 1).  The stem conv and its statistics run once at B = 1 and
@@ -726,14 +726,26 @@ class UnicornEngine:
         equals head(fpn, its prior or None, its mode) at B = 1, bit for bit.
         with_masks=True (a *_mask config) also runs each level's controller conv on all images at once (the controllers are shared by
         both modes, unicorn_head_mask.py:334): self.dyn_levels holds 3 fp32 [1 + K (or K), h, w, 176] maps in image order, each image's
-        equal to that of head(..., with_masks=True) at B = 1."""
+        equal to that of head(..., with_masks=True) at B = 1.
+        src_of (a device int32 [K] table): the pyramids of n_seq images (fpn [n_seq,h,w,C]), and SOT image k reads image src_of[k].  The
+        stem conv and its statistics run once at B = n_seq and uc_groupnorm_apply_gather writes the n_seq MOT images (with mot=True;
+        image i reads image i) followed by the K SOT images; the table is read on the device, so a captured graph follows its
+        contents.  Returns (MOT decoded [n_seq, A, 5+ncls] or None, SOT decoded [K, A, 6]); every image equals head(fpn[i:i+1], its
+        prior or None, its mode) at B = 1 on its source image i, bit for bit."""
         self._tracking_only("head_shared")
         if with_masks and not self.cfg["mask"]:
             raise ValueError(f"UnicornEngine.head_shared: {self.cfg_name} has no mask head (with_masks needs a *_mask config)")
-        assert fpn[0].shape[0] == 1, "head_shared: the pyramid of one image"
-        n_mot = int(bool(mot))
+        n_src = fpn[0].shape[0]
+        assert src_of is not None or n_src == 1, "head_shared: the pyramid of one image unless src_of maps the SOT images to theirs"
+        n_mot = (n_src if src_of is not None else 1) if mot else 0
         n_sot = priors[0].numel() // (fpn[0].shape[1] * fpn[0].shape[2])
         assert n_sot >= 1 and all(p.numel() == n_sot * f.shape[1] * f.shape[2] for p, f in zip(priors, fpn))
+        if src_of is not None:
+            assert src_of.dtype == torch.int32 and src_of.numel() == n_sot
+            table = self.buf("shared.src_of", (n_mot + n_sot,), torch.int32)  # MOT image i reads image i, then the SOT images' sources
+            if n_mot:
+                torch.arange(n_mot, out=table[:n_mot])
+            table[n_mot:].copy_(src_of.view(-1))
         outs = {m: ([None] * 3, [None] * 3) for m in ("", "_sot")}  # (reg+obj, cls) maps per level of each mode
         hw = [None] * 3
 
@@ -741,11 +753,15 @@ class UnicornEngine:
             L = self.P["head"][k]
             _, h, w, _ = fpn[k].shape
             c = L["stem"]
-            st = self._stats(c.groups)
-            t = self.conv(fpn[k], c.w, c.k, c.stride, (c.k - 1) // 2, bias=c.bias, out=self.buf(f"shared{k}.stem", (1, h, w, 256)),
+            st = self._stats(c.groups, n_src)
+            t = self.conv(fpn[k], c.w, c.k, c.stride, (c.k - 1) // 2, bias=c.bias, out=self.buf(f"shared{k}.stem", (n_src, h, w, 256)),
                           gn_stats=st, gn_groups=c.groups)
             x = self.buf(f"head{k}.x", (n_mot + n_sot, h, w, 256))
-            shared_ops.groupnorm_apply_bcast(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, prior=priors[k].reshape(-1), beta=L["beta"])
+            if src_of is None:
+                shared_ops.groupnorm_apply_bcast(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, prior=priors[k].reshape(-1), beta=L["beta"])
+            else:
+                shared_ops.groupnorm_apply_gather(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, table, prior=priors[k].reshape(-1),
+                                                  beta=L["beta"])
             feats = self._head_trunk(k, x)
             for sfx, i0, n in (("", 0, n_mot), ("_sot", n_mot, n_sot)):
                 if n == 0:
@@ -774,7 +790,7 @@ class UnicornEngine:
         for s_ in self._side_streams:
             main.wait_stream(s_)
         A = sum(h * w for h, w in hw)
-        out_mot = ops.head_decode(*outs[""], hw, STRIDES, self.ncls, out=self.buf("shared.out_mot", (1, A, 5 + self.ncls), F32)) if mot else None
+        out_mot = ops.head_decode(*outs[""], hw, STRIDES, self.ncls, out=self.buf("shared.out_mot", (n_mot, A, 5 + self.ncls), F32)) if mot else None
         out_sot = ops.head_decode(*outs["_sot"], hw, STRIDES, 1, out=self.buf("shared.out_sot", (n_sot, A, 6), F32))
         return out_mot, out_sot
 

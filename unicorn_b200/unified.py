@@ -18,10 +18,15 @@ The step protocol is the MOT driver's: submit(t + 1) may precede collect(t), so 
 work of step t + 1; with use_graph the first step runs eagerly and the second is captured.  The target slots are static buffers the
 graph reads: adding or removing a target writes them in place and never re-captures.
 
+UnicornUnifiedBatch does the same for n_seq videos in one step: the backbone and neck at B = n_seq, one pool of target slots shared
+by all videos (a device table gives each slot's video), and head_shared over the n_seq pyramids, with the MOT arm batched as in
+UnicornMOTBatch.  Each video's results equal those of its own UnicornUnifiedTracker, bit for bit.
+
 UnicornUnifiedMaskTracker does the same for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS object slots
 in place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both."""
 import warnings
 
+import numpy as np
 import torch
 
 from . import _lib, ops
@@ -48,17 +53,19 @@ class _Step:
         self.tids, self.scale, self.frame_id, self.tracker = [], 1.0, 0, None
 
 
-class _OneVideo:
-    """What the one-video drivers share: the frame check, a step ring whose submit stages the frame or changes nothing, and the
-    eager / capture / replay choice of a step."""
+class _Unified:
+    """What the unified drivers share: the frame check (one frame per video, n_seq videos), a step ring whose submit stages the
+    frames or changes nothing, and the eager / capture / replay choice of a step."""
+
+    n_seq = 1
 
     def _check(self, frame):
-        H, W = self.input_size
-        ok = torch.is_tensor(frame) and ((frame.dtype == torch.uint8 and tuple(frame.shape) == (1, H, W, 3)) or
-                                         (frame.dtype == torch.float32 and tuple(frame.shape) == (1, 3, H, W)))
+        n, (H, W) = self.n_seq, self.input_size
+        ok = torch.is_tensor(frame) and ((frame.dtype == torch.uint8 and tuple(frame.shape) == (n, H, W, 3)) or
+                                         (frame.dtype == torch.float32 and tuple(frame.shape) == (n, 3, H, W)))
         if not ok:
             got = (tuple(frame.shape), frame.dtype) if torch.is_tensor(frame) else type(frame)
-            raise ValueError(f"{type(self).__name__}: frame must be uint8 [1,{H},{W},3] or float32 [1,3,{H},{W}], got {got}")
+            raise ValueError(f"{type(self).__name__}: frame must be uint8 [{n},{H},{W},3] or float32 [{n},3,{H},{W}], got {got}")
 
     def _next_step(self, frame, slot_of):
         """Checks `frame`, takes the ring's next step s and stages the frame into the frame slot slot_of(s).  Returns (s, slot).  A
@@ -90,7 +97,7 @@ class _OneVideo:
             self._warm_u8 = c.u8
 
 
-class UnicornUnifiedTracker(_OneVideo):
+class UnicornUnifiedTracker(_Unified):
     """Up to `max_targets` SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None) on one video, one backbone pass per frame.
 
     SOT settings (conf, nms, max_inst) default to UnicornSOTTrack's, MOT settings (mot_conf, mot_nms, score_thr, max_dets) to
@@ -291,6 +298,310 @@ class UnicornUnifiedTracker(_OneVideo):
         return {"targets": {tid: self.states[tid] for tid in self.targets}, "mot": out["mot"]}
 
 
+# ---------------------------------------------------------------------------------------------------------- several videos
+class _BatchStep:
+    """The pinned read-back of one submitted step of UnicornUnifiedBatch and the host values it was submitted with."""
+
+    def __init__(self, n_seq, K, max_inst, n_keep, feats):
+        self.sot_dets = torch.zeros(K, max_inst, 7).pin_memory()
+        self.sot_count = torch.zeros(K, dtype=torch.int32).pin_memory()
+        self.count = torch.zeros(n_seq, dtype=torch.int32).pin_memory()
+        self.dets = torch.zeros(n_seq, n_keep, 7).pin_memory()
+        self.feats = torch.zeros(n_seq, n_keep, 128).pin_memory() if feats else None
+        self.host_active = torch.zeros(n_seq, dtype=torch.int32).pin_memory()  # staging of the step's active table
+        self.event = torch.cuda.Event()
+        self.mask, self.tids = [False] * n_seq, []
+        self.scales, self.frame_ids, self.trackers = [1.0] * n_seq, [0] * n_seq, [None] * n_seq
+
+
+class UnicornUnifiedBatch(_Unified):
+    """`n_seq` videos in one step, each with any number of SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None), one
+    backbone pass per video frame.  Settings default as UnicornUnifiedTracker's.
+
+    start(i, tracker=None) opens video slot i (a fresh QuasiDenseEmbedTracker for the QD arm unless one is given; the ByteTrack arm
+    needs a BYTETracker): its MOT state is reset and the targets of the slot's previous video are removed.
+
+    The `max_targets` target slots are one pool shared by all videos; the device table `seq_of` gives each slot's video.
+    add_target(i, tid, box_xyxy): the next frame of video i submitted in a step where video i is active becomes the target's reference
+    frame; the target gives results from the following step on.  remove_target(i, tid) frees its slot.  Target ids are unique within
+    a video.  Both write the slot buffers, seq_of and the device `active` table in stream order and never re-capture the graph.
+
+    The device half of a step is one CUDA graph: backbone + neck at B = n_seq; on the side stream the SOT arm of the target slots at
+    B = max_targets, each slot's stride-16 feature gathered from its video through seq_of; head_shared(..., src_of=seq_of); NMS of the
+    n_seq MOT images and of the target images; the QD arm's QDEmbedding at B = n_seq, gated by the step's active videos.
+
+    submit(frames, scales, active) / collect(img_infos) follow UnicornMOTBatch at depth 1: submit(t + 1) may precede collect(t).  A
+    video idle in a step keeps its MOT state (pre_dict, first-frame flag, tracker, frame counter), its targets report nothing and a
+    pending reference waits for its next active step.  Steps already submitted report the targets that were live when they were
+    submitted."""
+
+    def __init__(self, engine: UnicornEngine, input_size, n_seq, max_targets, mot="qd", conf=0.001, nms=0.65, max_inst=3,
+                 mot_conf=0.01, mot_nms=0.7, score_thr=0.1, max_dets=1024, use_graph=True):
+        if engine.det:
+            raise ValueError(f"UnicornUnifiedBatch: {engine.cfg_name} is a detector; SOT and MOT need a tracking config")
+        if mot not in ("qd", "byte", None):
+            raise ValueError(f"UnicornUnifiedBatch: mot must be 'qd', 'byte' or None (got {mot!r})")
+        if n_seq < 1 or max_targets < 1:
+            raise ValueError(f"UnicornUnifiedBatch: n_seq and max_targets must be >= 1 (got {n_seq}, {max_targets})")
+        self.eng, self.input_size, self.n_seq, self.max_targets, self.mot = engine, tuple(input_size), n_seq, max_targets, mot
+        self.conf, self.nms, self.max_inst = conf, nms, max_inst
+        self.mot_conf, self.mot_nms, self.score_thr, self.max_dets = mot_conf, mot_nms, score_thr, max_dets
+        self.use_graph = use_graph
+        H, W = self.input_size
+        dev, K = engine.dev, max_targets
+        A = anchor_count(H, W)
+        self.n_keep = min(max_dets, A)
+        self._slot = FrameSlot(engine, H, W, batch=n_seq)  # input buffers, the MOT images' NMS workspace, the graph
+        self.sot_ws = ops.PostWorkspace(A, dev, K)
+        self._qd = QDEmbedding(engine, H, W, self.n_keep, "unifiedb.emb", batch=n_seq) if mot == "qd" else None
+        # the target slots as UnicornUnifiedTracker keeps them, plus each slot's video
+        n16 = (H // 16) * (W // 16)
+        self.ref_proj = (torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev), torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev))
+        self.lbs_pre = torch.zeros(K, 1, (H // 8) * (W // 8), dtype=torch.float32, device=dev)
+        self.active = torch.zeros(K, dtype=torch.int32, device=dev)
+        self.seq_of = torch.zeros(K, dtype=torch.int32, device=dev)
+        self.gate = torch.zeros(n_seq, dtype=torch.int32, device=dev)  # the step's active videos, read by the QD arm
+        self._tid = [None] * K  # (video, target id) per slot, live or waiting for its reference frame
+        self._pending = {}  # slot -> box (resized-image xyxy) of the targets whose reference is their video's next active frame
+        self._ring = Ring([_BatchStep(n_seq, K, max_inst, self.n_keep, mot == "qd") for _ in range(2)])
+        self._warm_u8 = None
+        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()
+        self.started = [False] * n_seq
+        self.trackers = [None] * n_seq
+        self.frame_ids = [0] * n_seq  # steps the MOT arm has run per video since its start()
+        self.states = [{} for _ in range(n_seq)]  # track(): the reference-protocol state of every target of each video
+        self.launches_per_frame = 0
+        self.last = {}
+        self.last_dets, self.last_feats = [None] * n_seq, [None] * n_seq
+        self._warned = False
+
+    graph = property(lambda self: self._slot.graph)
+
+    def targets(self, i):
+        """The target ids of video i, live or waiting for their reference frame, in slot order."""
+        return [t[1] for t in self._tid if t is not None and t[0] == i]
+
+    # ------------------------------------------------------------------------------------------ videos and targets
+    def _check_video(self, i, what):
+        if not (isinstance(i, (int, np.integer)) and 0 <= i < self.n_seq):
+            raise ValueError(f"UnicornUnifiedBatch.{what}: unknown video {i!r} (n_seq = {self.n_seq})")
+        if what != "start" and not self.started[i]:
+            raise ValueError(f"UnicornUnifiedBatch.{what}: video {i} has not been started")
+
+    def start(self, i, tracker=None):
+        """Open video slot i: its MOT state is reset, `tracker` installed and the targets of the slot's previous video removed.  Steps
+        already submitted finish with the previous video's tracker and targets."""
+        self._check_video(i, "start")
+        if self.mot == "byte" and tracker is None:
+            raise ValueError("UnicornUnifiedBatch.start: mot='byte' needs a BYTETracker instance")
+        if self.mot == "qd" and tracker is None:
+            tracker = QuasiDenseEmbedTracker(device=self.eng.dev)
+        for tid in self.targets(i):
+            self.remove_target(i, tid)
+        if self._qd is not None:
+            self._qd.has_prev[i].zero_()  # stream-ordered after the steps in flight
+        self.started[i], self.trackers[i], self.frame_ids[i] = True, tracker if self.mot is not None else None, 0
+        self.states[i] = {}
+
+    def _check_new(self, new):
+        """new: {video: [target ids]} about to be added."""
+        for i, tids in new.items():
+            self._check_video(i, "add_target")
+            known = set(self.targets(i))
+            if len(set(tids)) != len(tids) or known & set(tids):
+                raise ValueError(f"UnicornUnifiedBatch: duplicate target id of video {i} in {tids} (live: {sorted(known, key=str)})")
+        n_live, n_new = sum(t is not None for t in self._tid), sum(len(t) for t in new.values())
+        if n_live + n_new > self.max_targets:
+            raise ValueError(f"UnicornUnifiedBatch: {n_live} + {n_new} targets exceed max_targets = {self.max_targets}")
+
+    def add_target(self, i, tid, box_xyxy):
+        """Track `tid` in video i from the box [x1, y1, x2, y2] (resized-image coordinates) in video i's next active frame."""
+        self._check_new({i: [tid]})
+        box = torch.as_tensor(box_xyxy, dtype=torch.float32).view(-1)
+        if box.numel() != 4:
+            raise ValueError(f"UnicornUnifiedBatch.add_target: box_xyxy needs 4 values (got {box.numel()})")
+        k = self._tid.index(None)
+        self._tid[k], self._pending[k] = (i, tid), box
+        self.seq_of[k].fill_(i)  # stream-ordered after the steps in flight, which read the slot's previous video
+
+    def remove_target(self, i, tid):
+        """Stop tracking `tid` of video i and free its slot (steps already submitted still report it)."""
+        self._check_video(i, "remove_target")
+        if (i, tid) not in self._tid:
+            raise ValueError(f"UnicornUnifiedBatch.remove_target: unknown target id {tid!r} of video {i}")
+        k = self._tid.index((i, tid))
+        self._tid[k] = None
+        if self._pending.pop(k, None) is None:
+            self.active[k].fill_(0)  # stream-ordered after the steps in flight
+        self.states[i].pop(tid, None)
+
+    def _write_references(self, boxes):
+        """The targets of `boxes` (slot -> box) take their video's frame of the step just enqueued as their reference frame: the
+        frame's stride-16 feature is projected once per video and written into the slots (UnicornUnifiedTracker._write_references)."""
+        e = self.eng
+        H, W = self.input_size
+        n16 = (H // 16) * (W // 16)
+        for i in sorted({self._tid[k][0] for k in boxes}):
+            src, q = e.project_ref(self.last["feat"][i:i + 1])
+            for k, box in boxes.items():
+                if self._tid[k][0] != i:
+                    continue
+                self.ref_proj[0][k * n16:(k + 1) * n16].copy_(src)
+                self.ref_proj[1][k * n16:(k + 1) * n16].copy_(q)
+                lab = get_label_map(box, H, W, e.dev)
+                self.lbs_pre[k].copy_(ops.bilinear(lab, H // 8, W // 8, 8.0, 8.0).reshape(1, -1))
+                self.active[k].fill_(1)
+
+    # ------------------------------------------------------------------------------------------ device half
+    def _frame(self):
+        e, c, K, n = self.eng, self._slot, self.max_targets, self.n_seq
+        e.begin_frame()
+        values = self.lbs_pre if K > 1 else self.lbs_pre[0]
+
+        def correlate(seq):  # the SOT arm, on the stream that overlaps the neck: each slot pairs its reference with its video's frame
+            f = seq["feat"]
+            feat = torch.index_select(f, 0, self.seq_of, out=e.buf("unifiedb.featK", (K,) + tuple(f.shape[1:])))
+            f_pre, f_cur = e.interaction(None, feat, ref_proj=self.ref_proj)
+            return e.propagate(e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc"), values)
+
+        fpn, seq, priors = e.backbone(c.img, tag="unifiedb", side=correlate)
+        head_mot, head_sot = e.head_shared(fpn, priors, mot=self.mot is not None, src_of=self.seq_of)
+        _, cnt = ops.postprocess_device(head_sot, 1, self.conf, self.nms, self.sot_ws, max_keep=self.max_inst)
+        cnt.mul_(self.active)
+        embed = None
+        if head_mot is not None:
+            dets, cnt = ops.postprocess_device(head_mot if n > 1 else head_mot[0], e.ncls, self.mot_conf, self.mot_nms, c.ws)
+            if self._qd is not None:
+                # one video needs no gate: a step without an active video does not run (submit)
+                embed = self._qd(e, seq["feat"], dets, cnt, gate=self.gate if n > 1 else None)
+        self.last = dict(fpn=fpn, feat=seq["feat"], priors=priors, head_mot=head_mot, head_sot=head_sot, embed=embed)
+
+    def submit(self, frames, scales=None, active=None):
+        """frames: preprocessed fp32 [n_seq,3,H,W] or uint8 [n_seq,H,W,3], host or device; scales: n_seq letterbox ratios (default 1);
+        active: n_seq flags (default: every started video).  Enqueues the step on the current stream; returns immediately."""
+        n = self.n_seq
+        self._check(frames)
+        if scales is not None and len(scales) != n:
+            raise ValueError(f"UnicornUnifiedBatch: {len(scales)} scales for {n} videos")
+        if active is not None and len(active) != n:
+            raise ValueError(f"UnicornUnifiedBatch: active has {len(active)} entries for {n} videos")
+        if active is not None and any(bool(a) and not self.started[i] for i, a in enumerate(active)):
+            raise ValueError(f"UnicornUnifiedBatch: active names a video that has not been started ({list(active)}, started {self.started})")
+        mask = [self.started[i] and (active is None or bool(active[i])) for i in range(n)]
+        if not any(mask):  # no video to step: nothing is launched and every result is None
+            s = self._ring.submit()
+            s.mask = mask
+            s.event.record()
+            return
+        s, c = self._next_step(frames, lambda s: self._slot)
+        s.mask = mask
+        s.tids = [None if k in self._pending or t is None or not mask[t[0]] else t for k, t in enumerate(self._tid)]
+        for i in range(n):
+            self.frame_ids[i] += mask[i]
+        s.scales = [1.0] * n if scales is None else [float(v) for v in scales]
+        s.frame_ids, s.trackers = list(self.frame_ids), list(self.trackers)
+        if self._qd is not None and n > 1:
+            # this parity's previous step was collected, so its pinned staging buffer is free again
+            s.host_active.copy_(torch.tensor(mask, dtype=torch.int32))
+            self.gate.copy_(s.host_active, non_blocking=True)
+        self._run(c, self._frame)
+        s.sot_count.copy_(self.sot_ws.count, non_blocking=True)
+        s.sot_dets.copy_(self.sot_ws.dets.view(self.max_targets, -1, 7)[:, :self.max_inst], non_blocking=True)
+        if self.mot is not None:
+            s.count.copy_(c.ws.count, non_blocking=True)
+            s.dets.copy_(c.ws.dets.view(n, -1, 7)[:, :self.n_keep], non_blocking=True)
+        if self._qd is not None:
+            s.feats.copy_(self._qd.feats, non_blocking=True)
+        s.event.record()
+        ready = {k: box for k, box in self._pending.items() if mask[self._tid[k][0]]}
+        if ready:
+            self._write_references(ready)
+            for k in ready:
+                del self._pending[k]
+
+    # ------------------------------------------------------------------------------------------ host half
+    def collect(self, img_infos=None):
+        """Results of the oldest submitted step: one entry per video, None for a video idle in that step, otherwise {"targets": {tid:
+        (dets [<= max_inst, 7], count)}, "mot": ...} as UnicornUnifiedTracker.collect returns it (img_infos[i]: (height, width) of
+        video i's original image, for the ByteTrack arm).  last_dets[i] / last_feats[i] then hold the NMS rows / embeddings video i's
+        tracker was given in this step."""
+        s = self._ring.collect()
+        s.event.synchronize()
+        H, W = self.input_size
+        res = [None] * self.n_seq
+        self.last_dets, self.last_feats = [None] * self.n_seq, [None] * self.n_seq
+        for i in range(self.n_seq):
+            if not s.mask[i]:
+                continue
+            targets = {}
+            for k, t in enumerate(s.tids):
+                if t is not None and t[0] == i:
+                    cnt = int(s.sot_count[k])
+                    targets[t[1]] = (s.sot_dets[k, :min(cnt, self.max_inst)].clone(), cnt)
+            mot = None
+            if self.mot is not None:
+                total = int(s.count[i])
+                if total > self.max_dets and not self._warned:
+                    warnings.warn(f"UnicornUnifiedBatch: {total} detections after NMS in video {i}, only the {self.max_dets} best are "
+                                  "associated (raise max_dets; the reference has no cap)")
+                    self._warned = True
+                d = s.dets[i, :min(total, self.n_keep)].clone()
+                self.last_dets[i] = d
+                if self.mot == "byte":
+                    info = img_infos[i] if img_infos is not None and img_infos[i] is not None else (H / s.scales[i], W / s.scales[i])
+                    mot = s.trackers[i].update(d.numpy(), info, (H, W))
+                else:
+                    f = s.feats[i, :d.shape[0]].clone()
+                    self.last_feats[i] = f
+                    mot = _qd_match(s.trackers[i], d, f, s.scales[i], self.score_thr, s.frame_ids[i])
+            res[i] = {"targets": targets, "mot": mot}
+        return res
+
+    def step_tensor(self, frames, scales=None, active=None, img_infos=None):
+        """Sequential protocol: one step in, its results out."""
+        self.submit(frames, scales, active)
+        return self.collect(img_infos)
+
+    # ------------------------------------------------------------------------------------------ reference protocol
+    def track(self, images, new_targets=None, img_infos=None):
+        """images: n_seq RGB frames (HWC uint8, any original sizes), None for an idle video; each is letterboxed once for both arms.
+        new_targets {video: {tid: [x, y, w, h]}} (original-image pixels) start on this step's frame of their video.  Returns one entry
+        per video, None for an idle one, otherwise {"targets": {tid: [x, y, w, h]}, "mot": ...} with UnicornUnifiedTracker.track's
+        state rules; img_infos[i] defaults to video i's frame (height, width)."""
+        n = self.n_seq
+        if len(images) != n:
+            raise ValueError(f"UnicornUnifiedBatch.track: {len(images)} frames for {n} videos")
+        for i, im in enumerate(images):
+            if im is None:
+                continue
+            if not (getattr(im, "ndim", 0) == 3 and im.shape[2] == 3 and im.dtype == np.uint8):
+                raise ValueError(f"UnicornUnifiedBatch.track: frame {i} must be an RGB uint8 [h, w, 3] array")
+            if not self.started[i]:
+                raise ValueError(f"UnicornUnifiedBatch.track: video {i} has not been started")
+        new_targets = {i: dict(v) for i, v in (new_targets or {}).items()}
+        self._check_new({i: list(v) for i, v in new_targets.items()})
+        for i, v in new_targets.items():
+            if images[i] is None and v:
+                raise ValueError(f"UnicornUnifiedBatch.track: new targets of video {i} need its frame")
+        ratios = [None if im is None else preprocess(im, self.input_size, out=self._host_in[i:i + 1])[1] for i, im in enumerate(images)]
+        for i, v in new_targets.items():
+            for tid, xywh in v.items():
+                self.add_target(i, tid, xyxy_resized(xywh, ratios[i]))
+                self.states[i][tid] = list(xywh)
+        infos = [None if im is None else (img_infos[i] if img_infos is not None and img_infos[i] is not None else tuple(im.shape[:2]))
+                 for i, im in enumerate(images)]
+        out = self.step_tensor(self._host_in, [r or 1.0 for r in ratios], [im is not None for im in images], infos)
+        res = [None] * n
+        for i, o in enumerate(out):
+            if o is None:
+                continue
+            for tid, (dets, cnt) in o["targets"].items():
+                if cnt > 0 and tid in self.states[i]:
+                    self.states[i][tid] = state_xywh(dets[0], ratios[i], self.input_size)
+            res[i] = {"targets": {tid: self.states[i][tid] for tid in self.targets(i)}, "mot": o["mot"]}
+        return res
+
+
 # ---------------------------------------------------------------------------------------------------------- VOS objects + MOTS
 class _MaskStep(FrameSlot):
     """One step of UnicornUnifiedMaskTracker in flight: its frame slot and graph, the device buffers its results live in until the
@@ -312,7 +623,7 @@ class _MaskStep(FrameSlot):
         self.objs, self.new_ids, self.frame_id = [], [], 0  # (id, object slot) of the live objects, ids entering from init_mask
 
 
-class UnicornUnifiedMaskTracker(_OneVideo):
+class UnicornUnifiedMaskTracker(_Unified):
     """Up to `max_objects` VOS objects plus optionally the MOTS arm (mots=True) on one video of original size `orig_size` (h, w), one
     backbone, neck and mask-branch pass per frame.  For the *_mask checkpoints, which serve VOS and MOTS with one set of weights.
 
