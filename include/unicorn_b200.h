@@ -164,21 +164,13 @@ UC_API int uc_layernorm(const void* x, int ldx, const void* res, int ldres, cons
 UC_API int uc_groupnorm_apply(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y,
                               int ldy, int B, long HW, int C, int G, float eps, int act, const float* prior,
                               const float* beta, const void* add2, int ldadd2, void* y2, int ldy2, void* stream);
-/* The same normalisation of ONE conv output written as B images (a head stem shared by several head images): x [HW pixels] and
- * stats [G]{sum,sumsq} of one image; y [B][HW pixels], image stride HW * ldy.  Image b < n_plain = act((x-mean)*rstd*w+b) (the no-prior
- * path: adding a zero prior would turn a -0 into +0); image b >= n_plain adds prior[(b - n_plain) * HW + pix] * beta[c].  Every image
- * equals uc_groupnorm_apply at B = 1 on x, with or without its prior, bit for bit.  1 <= B <= 65535, 0 <= n_plain <= B; prior (4-byte
- * aligned) and beta are given exactly when n_plain < B; x and y must not overlap; otherwise the conventions of uc_groupnorm_apply
- * (UC_EINVAL before any launch). */
-UC_API int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y, int ldy,
-                                    int B, int n_plain, long HW, int C, int G, float eps, int act, const float* prior, const float* beta,
-                                    void* stream);
-/* The same normalisation with the source image of each output image taken from a device table (a head stem shared by the head
- * images of several videos): x holds n_src images [n_src][HW pixels] (row stride ldx, image stride HW * ldx) and stats their
- * [n_src][G]{sum,sumsq}; src_of is a device int32 [B] table read when the kernel runs, so a captured graph follows its current
- * contents.  Output image b normalises image src_of[b] with that image's statistics; b < n_plain takes the no-prior path, b >= n_plain
- * adds prior[(b - n_plain) * HW + pix] * beta[c], as uc_groupnorm_apply_bcast.  Every image equals uc_groupnorm_apply at B = 1 on
- * image src_of[b], bit for bit.  A table entry outside [0, n_src) leaves output image b untouched and reads nothing of x, stats or
+/* The same normalisation with the source image of each output image taken from a device table (a head stem shared by several head
+ * images, of one video or of several): x holds n_src images [n_src][HW pixels] (row stride ldx, image stride HW * ldx) and stats
+ * their [n_src][G]{sum,sumsq}; src_of is a device int32 [B] table read when the kernel runs, so a captured graph follows its current
+ * contents.  y holds B images [B][HW pixels], image stride HW * ldy.  Output image b normalises image src_of[b] with that image's
+ * statistics; b < n_plain = act((x-mean)*rstd*w+b) (the no-prior path: adding a zero prior would turn a -0 into +0), b >= n_plain
+ * adds prior[(b - n_plain) * HW + pix] * beta[c].  Every image equals uc_groupnorm_apply at B = 1 on image src_of[b], with or
+ * without its prior, bit for bit.  A table entry outside [0, n_src) leaves output image b untouched and reads nothing of x, stats or
  * prior.  1 <= n_src, B <= 65535, 0 <= n_plain <= B; src_of non-null and 4-byte aligned; prior (4-byte aligned) and beta are given
  * exactly when n_plain < B; x (all n_src images) and y must not overlap; otherwise the conventions of uc_groupnorm_apply (UC_EINVAL
  * before any launch). */

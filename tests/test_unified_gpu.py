@@ -1,6 +1,7 @@
-"""One backbone pass per frame for SOT targets and a MOT arm: the broadcast stem GroupNorm against uc_groupnorm_apply, the shared-trunk
-head against head() at B = 1, and UnicornUnifiedTracker against one UnicornSOTTrack per target plus one UnicornMOTTracker, bit for bit
-on every frame (detections, counts, priors, raw head outputs, MOT boxes / ids / NMS rows / embeddings or ByteTrack tracks)."""
+"""One backbone pass per frame for SOT targets and a MOT arm: the one-image stem GroupNorm (the gather with a table of zeros) against
+uc_groupnorm_apply, the shared-trunk head against head() at B = 1, and UnicornUnifiedTracker (UnicornUnifiedBatch at n_seq = 1) against
+one UnicornSOTTrack per target plus one UnicornMOTTracker, bit for bit on every frame (detections, counts, priors, raw head outputs,
+MOT boxes / ids / NMS rows / embeddings or ByteTrack tracks)."""
 import types
 
 import numpy as np
@@ -66,7 +67,7 @@ def byte_rows(tracks):
 
 # ------------------------------------------------------------------------------------------------ kernel
 @pytest.mark.parametrize("act", [0, 1, 3])
-def test_broadcast_stem_matches_groupnorm_apply(act):
+def test_zero_table_gather_matches_groupnorm_apply(act):
     from unicorn_b200 import ops, shared_ops
     g = torch.Generator(device="cuda").manual_seed(1)
     h, w, C, G_, n_plain, n_prior = 12, 20, 256, 16, 2, 3
@@ -85,7 +86,8 @@ def test_broadcast_stem_matches_groupnorm_apply(act):
     prior = torch.rand(n_prior, 1, h, w, device="cuda", generator=g)
     prior[1] = 0.0  # a zero prior plane still takes the prior path, as its own B = 1 call does
     out = torch.full((n_plain + n_prior, h, w, C), 7.0, dtype=torch.bfloat16, device="cuda")
-    shared_ops.groupnorm_apply_bcast(x, st, gw, gb, G_, 1e-3, act, out, n_plain, prior=prior.reshape(-1), beta=beta)
+    zeros = torch.zeros(n_plain + n_prior, dtype=torch.int32, device="cuda")  # every image reads the one source image
+    shared_ops.groupnorm_apply_gather(x, st, gw, gb, G_, 1e-3, act, out, n_plain, zeros, prior=prior.reshape(-1), beta=beta)
     for b in range(n_plain + n_prior):
         ref = torch.empty(1, h, w, C, dtype=torch.bfloat16, device="cuda")
         pr = prior[b - n_plain].reshape(-1).contiguous() if b >= n_plain else None

@@ -451,11 +451,10 @@ __global__ void __launch_bounds__(256) layernorm_v8_kernel(const uint16_t* __res
 // parameters; they are computed once per block into shared memory.  x/y bf16 NHWC (strided); 8 channels / thread.
 // kMode says which image of x and of the statistics output image b (blockIdx.y) reads:
 //   kGnEach    image b (uc_groupnorm_apply);
-//   kGnBcast   image 0, and only the images b >= prior_from add the prior, reading its plane b - prior_from; the others take the
-//              no-prior path.  y2 is unused;
-//   kGnGather  image src_of[b] of the n_src images of x, read once per CTA; the prior as kGnBcast.  An entry outside [0, n_src)
-//              leaves image b untouched.  y2 is unused.
-enum GnApplyMode { kGnEach, kGnBcast, kGnGather };
+//   kGnGather  image src_of[b] of the n_src images of x, read once per CTA; only the images b >= prior_from add the prior, reading
+//              its plane b - prior_from; the others take the no-prior path.  An entry outside [0, n_src) leaves image b untouched.
+//              y2 is unused.
+enum GnApplyMode { kGnEach, kGnGather };
 template <int kMode>
 __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __restrict__ x, int ldx,
                                                                const long long* __restrict__ stats, const float* __restrict__ w,
@@ -469,7 +468,7 @@ __global__ void __launch_bounds__(256) groupnorm_apply_kernel(const uint16_t* __
   pdl_launch_dependents();  // ... and the next kernel in the stream may become resident / run its prologue from here on
   extern __shared__ float sc[];  // [2][C] scale, shift (+ [C] beta)
   const int b = blockIdx.y;
-  const int bx = kMode == kGnEach ? b : kMode == kGnBcast ? 0 : src_of[b];  // image of x and of the statistics
+  const int bx = kMode == kGnEach ? b : src_of[b];  // image of x and of the statistics
   if (kMode == kGnGather && (bx < 0 || bx >= n_src)) return;  // uniform over the CTA, before any barrier
   const bool with_prior = prior != nullptr && (kMode == kGnEach || b >= prior_from);
   const int gs = C / G;
@@ -653,41 +652,6 @@ extern "C" int uc_groupnorm_apply(const void* x, int ldx, const void* stats, con
       eps, act, prior, beta, static_cast<const uint16_t*>(add2), ldadd2, static_cast<uint16_t*>(y2), ldy2, 0,
       static_cast<const int*>(nullptr), 0);
   return check_launch("uc_groupnorm_apply");
-}
-
-extern "C" int uc_groupnorm_apply_bcast(const void* x, int ldx, const void* stats, const float* w, const float* b, void* y, int ldy,
-                                        int B, int n_plain, long HW, int C, int G, float eps, int act, const float* prior,
-                                        const float* beta, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (B < 1 || B > 65535) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: B must be in [1, 65535] (got %d)", B);
-  if (n_plain < 0 || n_plain > B) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: n_plain must be in [0, B] (got %d, B = %d)", n_plain, B);
-  if (HW < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: HW must be >= 1");
-  if (G < 1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: G must be >= 1 (got %d)", G);
-  if (C % 8 || ldx % 8 || ldy % 8 || C % G || ldx < C || ldy < C)
-    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: C, ldx, ldy multiples of 8, ldx, ldy >= C; C %% G == 0");
-  if (C > 4096) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: C too large");
-  if (act != UC_ACT_NONE && act != UC_ACT_RELU && act != UC_ACT_SILU)
-    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: act must be UC_ACT_NONE, UC_ACT_RELU or UC_ACT_SILU (got %d)", act);
-  if (!x || !stats || !w || !b || !y) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: null pointer");
-  if ((prior != nullptr) != (beta != nullptr)) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior and beta go together");
-  if ((prior != nullptr) != (n_plain < B))
-    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior and beta are needed exactly when n_plain < B");
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15)
-    return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: x and y must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(stats) & 7) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: stats must be 8-byte aligned");
-  if (reinterpret_cast<uintptr_t>(prior) & 3) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: prior must be 4-byte aligned");
-  // every output image reads all of x: writing any of them over x would race with the other images' reads
-  const uintptr_t x0 = reinterpret_cast<uintptr_t>(x), y0 = reinterpret_cast<uintptr_t>(y);
-  const uintptr_t x1 = x0 + (static_cast<uintptr_t>(HW - 1) * ldx + C) * 2;  // one past the last element read or written
-  const uintptr_t y1 = y0 + (static_cast<uintptr_t>(B) * HW - 1) * ldy * 2 + static_cast<uintptr_t>(C) * 2;
-  if (x0 < y1 && y0 < x1) return set_error(UC_EINVAL, "uc_groupnorm_apply_bcast: x and y overlap (not an in-place operation)");
-  const long total = HW * (C / 8);
-  const int gx = static_cast<int>(std::max<long>(1, std::min<long>((total + 256 * 2 - 1) / (256 * 2), static_cast<long>(num_sms()) * 8)));
-  launch_pdl(groupnorm_apply_kernel<kGnBcast>, dim3(gx, B), 256, 3 * C * sizeof(float), stream,
-      static_cast<const uint16_t*>(x), ldx, reinterpret_cast<const long long*>(stats), w, b, static_cast<uint16_t*>(y), ldy, HW, C, G,
-      eps, act, prior, beta, static_cast<const uint16_t*>(nullptr), 0, static_cast<uint16_t*>(nullptr), 0, n_plain,
-      static_cast<const int*>(nullptr), 0);
-  return check_launch("uc_groupnorm_apply_bcast");
 }
 
 extern "C" int uc_groupnorm_apply_gather(const void* x, int ldx, int n_src, const void* stats, const float* w, const float* b, void* y,

@@ -721,9 +721,9 @@ class UnicornEngine:
         """The head of one image's pyramid for several head images at once: with mot=True image 0 is the MOT image (mode "mot", no
         prior), then one SOT image (mode "sot") per prior plane.  fpn: 3 NHWC bf16 maps [1,h,w,C]; priors: the 3 fp32 maps of
         propagate ([K,h,w] planes in any leading shape, K >= 1).  The stem conv and its statistics run once at B = 1 and
-        uc_groupnorm_apply_bcast writes all 1 + K (or K) stem outputs; the ConvNeXt blocks and towers run on all images together, the
-        predictors of each mode on its batch slice.  Returns (MOT decoded [1, A, 5+ncls] or None, SOT decoded [K, A, 6]); every image
-        equals head(fpn, its prior or None, its mode) at B = 1, bit for bit.
+        uc_groupnorm_apply_gather, with a table of zeros, writes all 1 + K (or K) stem outputs; the ConvNeXt blocks and towers run on
+        all images together, the predictors of each mode on its batch slice.  Returns (MOT decoded [1, A, 5+ncls] or None, SOT
+        decoded [K, A, 6]); every image equals head(fpn, its prior or None, its mode) at B = 1, bit for bit.
         with_masks=True (a *_mask config) also runs each level's controller conv on all images at once (the controllers are shared by
         both modes, unicorn_head_mask.py:334): self.dyn_levels holds 3 fp32 [1 + K (or K), h, w, 176] maps in image order, each image's
         equal to that of head(..., with_masks=True) at B = 1.
@@ -740,7 +740,9 @@ class UnicornEngine:
         n_mot = (n_src if src_of is not None else 1) if mot else 0
         n_sot = priors[0].numel() // (fpn[0].shape[1] * fpn[0].shape[2])
         assert n_sot >= 1 and all(p.numel() == n_sot * f.shape[1] * f.shape[2] for p, f in zip(priors, fpn))
-        if src_of is not None:
+        if src_of is None:  # every image reads image 0: zeroed when allocated, never written
+            table = self.buf("shared.src0", (n_mot + n_sot,), torch.int32, zero=True)
+        else:
             assert src_of.dtype == torch.int32 and src_of.numel() == n_sot
             table = self.buf("shared.src_of", (n_mot + n_sot,), torch.int32)  # MOT image i reads image i, then the SOT images' sources
             if n_mot:
@@ -757,11 +759,8 @@ class UnicornEngine:
             t = self.conv(fpn[k], c.w, c.k, c.stride, (c.k - 1) // 2, bias=c.bias, out=self.buf(f"shared{k}.stem", (n_src, h, w, 256)),
                           gn_stats=st, gn_groups=c.groups)
             x = self.buf(f"head{k}.x", (n_mot + n_sot, h, w, 256))
-            if src_of is None:
-                shared_ops.groupnorm_apply_bcast(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, prior=priors[k].reshape(-1), beta=L["beta"])
-            else:
-                shared_ops.groupnorm_apply_gather(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, table, prior=priors[k].reshape(-1),
-                                                  beta=L["beta"])
+            shared_ops.groupnorm_apply_gather(t, st, c.gw, c.gb, c.groups, c.eps, ACT_SILU, x, n_mot, table, prior=priors[k].reshape(-1),
+                                              beta=L["beta"])
             feats = self._head_trunk(k, x)
             for sfx, i0, n in (("", 0, n_mot), ("_sot", n_mot, n_sot)):
                 if n == 0:

@@ -1,29 +1,29 @@
-"""SOT targets and MOT objects, or VOS objects and MOTS instances, of one video with one backbone pass per frame.
+"""SOT targets and MOT objects, or VOS objects and MOTS instances, with one backbone pass per video frame.
 
 Unicorn's tracking checkpoints (unicorn_track_tiny / _large / _large_mot_challenge / _r50) serve SOT and MOT with one set of weights.
 Run as two drivers (UnicornSOTTrack per target, UnicornMOTTracker), every frame computes the backbone and neck once per driver;
-UnicornUnifiedTracker computes them once and shares them:
+UnicornUnifiedBatch computes them once per video frame and shares them, for n_seq videos in one step:
 
-  1. backbone + neck of the frame at B = 1;
+  1. backbone + neck of the n_seq frames at B = n_seq;
   2. on the side stream that overlaps the neck, the SOT arm of the `max_targets` target slots at B = max_targets, as
-     UnicornSOTBatch._frame runs it: interaction with each slot's reference projection, the two upsamples, propagate;
-  3. UnicornEngine.head_shared: one stem conv for the MOT image and every SOT image, the rest of the head on all of them at once;
-  4. NMS of the MOT image (whole mode, ncls classes) and of the SOT images (one class, the first max_inst rows);
-  5. QD arm: QDEmbedding, the device half of UnicornMOTTracker's QDTrack step, unchanged.
+     UnicornSOTBatch._frame runs it on each slot's video frame: interaction with the slot's reference projection, the two upsamples,
+     propagate;
+  3. UnicornEngine.head_shared: one stem conv per video frame for its MOT image and its targets' SOT images, the rest of the head on
+     all of them at once;
+  4. NMS of the MOT images (whole mode, ncls classes) and of the SOT images (one class, the first max_inst rows);
+  5. QD arm: QDEmbedding, the device half of UnicornMOTBatch's QDTrack step, unchanged.
 
-Each target's (dets, count) equals that of a UnicornSOTTrack initialised on the target's reference frame and box, and the MOT output
-equals UnicornMOTTracker's on the same frames, bit for bit.
+Each target's (dets, count) equals that of a UnicornSOTTrack initialised on the target's reference frame and box, and each video's
+MOT output equals UnicornMOTTracker's on the same frames, bit for bit.
 
 The step protocol is the MOT driver's: submit(t + 1) may precede collect(t), so the host association of step t overlaps the device
 work of step t + 1; with use_graph the first step runs eagerly and the second is captured.  The target slots are static buffers the
 graph reads: adding or removing a target writes them in place and never re-captures.
 
-UnicornUnifiedBatch does the same for n_seq videos in one step: the backbone and neck at B = n_seq, one pool of target slots shared
-by all videos (a device table gives each slot's video), and head_shared over the n_seq pyramids, with the MOT arm batched as in
-UnicornMOTBatch.  Each video's results equal those of its own UnicornUnifiedTracker, bit for bit.
+UnicornUnifiedTracker is UnicornUnifiedBatch at n_seq = 1 under the one-video protocol.
 
-UnicornUnifiedMaskTracker does the same for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS object slots
-in place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both."""
+UnicornUnifiedMaskTracker does the same on one video for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS
+object slots in place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both."""
 import warnings
 
 import numpy as np
@@ -38,19 +38,6 @@ from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
 from .tracker import QuasiDenseEmbedTracker
 from .tracker._stream import assoc_stream
 from .vos import MAX_OBJECTS_PER_SEQUENCE, ROWS_PER_GROUP_SLOT, label_values
-
-
-class _Step:
-    """The pinned read-back of one submitted step and the host values it was submitted with."""
-
-    def __init__(self, K, max_inst, n_keep, feats):
-        self.sot_dets = torch.zeros(K, max_inst, 7).pin_memory()
-        self.sot_count = torch.zeros(K, dtype=torch.int32).pin_memory()
-        self.count = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self.dets = torch.zeros(n_keep, 7).pin_memory()
-        self.feats = torch.zeros(n_keep, 128).pin_memory() if feats else None
-        self.event = torch.cuda.Event()
-        self.tids, self.scale, self.frame_id, self.tracker = [], 1.0, 0, None
 
 
 class _Unified:
@@ -97,207 +84,6 @@ class _Unified:
             self._warm_u8 = c.u8
 
 
-class UnicornUnifiedTracker(_Unified):
-    """Up to `max_targets` SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None) on one video, one backbone pass per frame.
-
-    SOT settings (conf, nms, max_inst) default to UnicornSOTTrack's, MOT settings (mot_conf, mot_nms, score_thr, max_dets) to
-    UnicornMOTTracker's.  `tracker`: the MOT arm's host tracker (default a fresh QuasiDenseEmbedTracker; the ByteTrack arm needs a
-    BYTETracker).
-
-    add_target(tid, box_xyxy): the next submitted frame becomes the target's reference frame.  Right after that step, its stride-16
-    feature is projected (project_ref) and the box's label map resized into the target's slot; the target gives results from the
-    following frame on.  remove_target(tid) frees the slot.  A free slot computes on stale buffers: the device `active` table zeroes its
-    detection count and its result is dropped.  Steps already submitted report the targets that were live when they were submitted."""
-
-    def __init__(self, engine: UnicornEngine, input_size, max_targets, mot="qd", tracker=None, conf=0.001, nms=0.65, max_inst=3,
-                 mot_conf=0.01, mot_nms=0.7, score_thr=0.1, max_dets=1024, use_graph=True):
-        if engine.det:
-            raise ValueError(f"UnicornUnifiedTracker: {engine.cfg_name} is a detector; SOT and MOT need a tracking config")
-        if mot not in ("qd", "byte", None):
-            raise ValueError(f"UnicornUnifiedTracker: mot must be 'qd', 'byte' or None (got {mot!r})")
-        if max_targets < 1:
-            raise ValueError(f"UnicornUnifiedTracker: max_targets must be >= 1 (got {max_targets})")
-        if mot == "byte" and tracker is None:
-            raise ValueError("UnicornUnifiedTracker: mot='byte' needs a BYTETracker instance")
-        if mot == "qd" and tracker is None:
-            tracker = QuasiDenseEmbedTracker(device=engine.dev)
-        self.eng, self.input_size, self.max_targets, self.mot = engine, tuple(input_size), max_targets, mot
-        self.tracker = tracker if mot is not None else None
-        self.conf, self.nms, self.max_inst = conf, nms, max_inst
-        self.mot_conf, self.mot_nms, self.score_thr, self.max_dets = mot_conf, mot_nms, score_thr, max_dets
-        self.use_graph = use_graph
-        H, W = self.input_size
-        dev, K = engine.dev, max_targets
-        A = anchor_count(H, W)
-        self.n_keep = min(max_dets, A)
-        self._slot = FrameSlot(engine, H, W)  # input buffers, the MOT image's NMS workspace, the graph
-        self.sot_ws = ops.PostWorkspace(A, dev, K)
-        self._qd = QDEmbedding(engine, H, W, self.n_keep, "unified.emb") if mot == "qd" else None
-        # the target slots: reference projection and label values as UnicornSOTBatch keeps them, and the device active table
-        n16 = (H // 16) * (W // 16)
-        self.ref_proj = (torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev), torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev))
-        self.lbs_pre = torch.zeros(K, 1, (H // 8) * (W // 8), dtype=torch.float32, device=dev)
-        self.active = torch.zeros(K, dtype=torch.int32, device=dev)
-        self._tid = [None] * K  # target id per slot, live or waiting for its reference frame
-        self._pending = {}  # slot -> box (resized-image xyxy) of the targets whose reference is the next submitted frame
-        # two parity steps: submit(t + 1) writes one while collect(t) reads the other
-        self._ring = Ring([_Step(K, max_inst, self.n_keep, mot == "qd") for _ in range(2)])
-        self._warm_u8 = None  # input dtype the last eager step ran with: the next step with it is captured
-        self._host_in = torch.full((1, H, W, 3), 114, dtype=torch.uint8).pin_memory()
-        self.frame_id = 0  # steps the MOT arm has run
-        self.states = {}  # track(): the reference-protocol state of every target
-        self.launches_per_frame = 0
-        self.last = {}
-        self._warned = False
-
-    graph = property(lambda self: self._slot.graph)
-    targets = property(lambda self: [t for t in self._tid if t is not None])
-
-    # ------------------------------------------------------------------------------------------ targets
-    def _check_new(self, tids):
-        tids = list(tids)
-        known = set(self.targets)
-        if len(set(tids)) != len(tids) or known & set(tids):
-            raise ValueError(f"UnicornUnifiedTracker: duplicate target id in {tids} (live: {sorted(known, key=str)})")
-        if len(known) + len(tids) > self.max_targets:
-            raise ValueError(f"UnicornUnifiedTracker: {len(known)} + {len(tids)} targets exceed max_targets = {self.max_targets}")
-
-    def add_target(self, tid, box_xyxy):
-        """Track `tid` from the box [x1, y1, x2, y2] (resized-image coordinates) in the next submitted frame."""
-        self._check_new([tid])
-        box = torch.as_tensor(box_xyxy, dtype=torch.float32).view(-1)
-        if box.numel() != 4:
-            raise ValueError(f"UnicornUnifiedTracker.add_target: box_xyxy needs 4 values (got {box.numel()})")
-        i = self._tid.index(None)
-        self._tid[i], self._pending[i] = tid, box
-
-    def remove_target(self, tid):
-        """Stop tracking `tid` and free its slot (steps already submitted still report it)."""
-        if tid not in self._tid:
-            raise ValueError(f"UnicornUnifiedTracker.remove_target: unknown target id {tid!r}")
-        i = self._tid.index(tid)
-        self._tid[i] = None
-        if self._pending.pop(i, None) is None:
-            self.active[i].fill_(0)  # stream-ordered after the steps in flight
-        self.states.pop(tid, None)
-
-    def _write_references(self, boxes):
-        """The targets of `boxes` (slot -> box) take the step just enqueued as their reference frame (UnicornSOTBatch.initialize_tensor
-        on that frame's stride-16 feature)."""
-        e = self.eng
-        H, W = self.input_size
-        n16 = (H // 16) * (W // 16)
-        src, q = e.project_ref(self.last["feat"])
-        for i, box in boxes.items():
-            self.ref_proj[0][i * n16:(i + 1) * n16].copy_(src)
-            self.ref_proj[1][i * n16:(i + 1) * n16].copy_(q)
-            lab = get_label_map(box, H, W, e.dev)
-            self.lbs_pre[i].copy_(ops.bilinear(lab, H // 8, W // 8, 8.0, 8.0).reshape(1, -1))
-            self.active[i].fill_(1)
-
-    # ------------------------------------------------------------------------------------------ device half
-    def _frame(self):
-        e, c, K = self.eng, self._slot, self.max_targets
-        e.begin_frame()
-        values = self.lbs_pre if K > 1 else self.lbs_pre[0]
-
-        def correlate(seq):  # the SOT arm, on the stream that overlaps the neck: each target slot pairs its reference with the frame
-            feat = seq["feat"]
-            if K > 1:
-                feat = e.buf("unified.featK", (K,) + tuple(feat.shape[1:]))
-                feat.copy_(seq["feat"].expand(K, -1, -1, -1))
-            f_pre, f_cur = e.interaction(None, feat, ref_proj=self.ref_proj)
-            return e.propagate(e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc"), values)
-
-        fpn, seq, priors = e.backbone(c.img, tag="unified", side=correlate)
-        head_mot, head_sot = e.head_shared(fpn, priors, mot=self.mot is not None)
-        _, cnt = ops.postprocess_device(head_sot, 1, self.conf, self.nms, self.sot_ws, max_keep=self.max_inst)
-        cnt.mul_(self.active)
-        embed = None
-        if head_mot is not None:
-            dets, cnt = ops.postprocess_device(head_mot[0], e.ncls, self.mot_conf, self.mot_nms, c.ws)
-            if self._qd is not None:
-                embed = self._qd(e, seq["feat"], dets, cnt)
-        self.last = dict(fpn=fpn, feat=seq["feat"], priors=priors, head_mot=head_mot, head_sot=head_sot, embed=embed)
-
-    def submit(self, frame, scale=1.0):
-        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; scale: its letterbox ratio.  Enqueues the step on
-        the current stream; returns immediately."""
-        s, c = self._next_step(frame, lambda s: self._slot)
-        s.tids = [None if i in self._pending else t for i, t in enumerate(self._tid)]
-        if self.mot is not None:
-            self.frame_id += 1
-        s.scale, s.frame_id, s.tracker = float(scale), self.frame_id, self.tracker
-        self._run(c, self._frame)
-        K = self.max_targets
-        s.sot_count.copy_(self.sot_ws.count, non_blocking=True)
-        s.sot_dets.copy_(self.sot_ws.dets.view(K, -1, 7)[:, :self.max_inst], non_blocking=True)
-        if self.mot is not None:
-            s.count.copy_(c.ws.count, non_blocking=True)
-            s.dets.copy_(c.ws.dets[:self.n_keep], non_blocking=True)
-        if self._qd is not None:
-            s.feats.copy_(self._qd.feats[0], non_blocking=True)
-        s.event.record()
-        if self._pending:
-            self._write_references(self._pending)
-            self._pending = {}
-
-    # ------------------------------------------------------------------------------------------ host half
-    def collect(self, img_info=None):
-        """Results of the oldest submitted step: {"targets": {tid: (dets [<= max_inst, 7], count)}, "mot": ...}.  "mot" is what
-        UnicornMOTTracker.collect returns (QDTrack: (bboxes [n,5] in original-image coordinates, ids [n]); ByteTrack: the active
-        STracks, img_info = (height, width) of the original image), None without a MOT arm."""
-        s = self._ring.collect()
-        s.event.synchronize()
-        targets = {}
-        for i, tid in enumerate(s.tids):
-            if tid is not None:
-                n = int(s.sot_count[i])
-                targets[tid] = (s.sot_dets[i, :min(n, self.max_inst)].clone(), n)
-        res = None
-        self.last_dets = self.last_feats = None
-        if self.mot is not None:
-            total = int(s.count[0])
-            if total > self.max_dets and not self._warned:
-                warnings.warn(f"UnicornUnifiedTracker: {total} detections after NMS, only the {self.max_dets} best are associated "
-                              "(raise max_dets; the reference has no cap)")
-                self._warned = True
-            d = s.dets[:min(total, self.n_keep)].clone()
-            self.last_dets = d
-            if self.mot == "byte":
-                H, W = self.input_size
-                info = img_info if img_info is not None else (H / s.scale, W / s.scale)
-                res = s.tracker.update(d.numpy(), info, (H, W))
-            else:
-                f = s.feats[:d.shape[0]].clone()
-                self.last_feats = f
-                res = _qd_match(s.tracker, d, f, s.scale, self.score_thr, s.frame_id)
-        return {"targets": targets, "mot": res}
-
-    def step_tensor(self, frame, scale=1.0, img_info=None):
-        """Sequential protocol: one step in, its results out."""
-        self.submit(frame, scale)
-        return self.collect(img_info)
-
-    # ------------------------------------------------------------------------------------------ reference protocol
-    def track(self, image_rgb, new_targets=None, img_info=None):
-        """image_rgb: an RGB frame (HWC uint8), letterboxed once for both arms.  new_targets {tid: [x, y, w, h]} (original-image pixels)
-        start on this frame.  Returns {"targets": {tid: [x, y, w, h]}, "mot": ...}: each target's state as UnicornSOTTrack.track keeps it
-        (a new target's is its box; a target with no detection keeps its previous state), and the MOT arm's result with img_info
-        defaulting to the frame's (height, width)."""
-        new_targets = dict(new_targets or {})
-        self._check_new(new_targets)
-        frame, r = preprocess(image_rgb, self.input_size, out=self._host_in)
-        for tid, xywh in new_targets.items():
-            self.add_target(tid, xyxy_resized(xywh, r))
-            self.states[tid] = list(xywh)
-        out = self.step_tensor(frame, r, img_info if img_info is not None else tuple(image_rgb.shape[:2]))
-        for tid, (dets, n) in out["targets"].items():
-            if n > 0 and tid in self.states:
-                self.states[tid] = state_xywh(dets[0], r, self.input_size)
-        return {"targets": {tid: self.states[tid] for tid in self.targets}, "mot": out["mot"]}
-
-
 # ---------------------------------------------------------------------------------------------------------- several videos
 class _BatchStep:
     """The pinned read-back of one submitted step of UnicornUnifiedBatch and the host values it was submitted with."""
@@ -316,7 +102,8 @@ class _BatchStep:
 
 class UnicornUnifiedBatch(_Unified):
     """`n_seq` videos in one step, each with any number of SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None), one
-    backbone pass per video frame.  Settings default as UnicornUnifiedTracker's.
+    backbone pass per video frame.  SOT settings (conf, nms, max_inst) default to UnicornSOTTrack's, MOT settings (mot_conf, mot_nms,
+    score_thr, max_dets) to UnicornMOTTracker's.
 
     start(i, tracker=None) opens video slot i (a fresh QuasiDenseEmbedTracker for the QD arm unless one is given; the ByteTrack arm
     needs a BYTETracker): its MOT state is reset and the targets of the slot's previous video are removed.
@@ -324,7 +111,8 @@ class UnicornUnifiedBatch(_Unified):
     The `max_targets` target slots are one pool shared by all videos; the device table `seq_of` gives each slot's video.
     add_target(i, tid, box_xyxy): the next frame of video i submitted in a step where video i is active becomes the target's reference
     frame; the target gives results from the following step on.  remove_target(i, tid) frees its slot.  Target ids are unique within
-    a video.  Both write the slot buffers, seq_of and the device `active` table in stream order and never re-capture the graph.
+    a video.  Both write the slot buffers, seq_of and the device `active` table in stream order and never re-capture the graph.  A
+    free slot computes on stale buffers: the `active` table zeroes its detection count and its result is dropped.
 
     The device half of a step is one CUDA graph: backbone + neck at B = n_seq; on the side stream the SOT arm of the target slots at
     B = max_targets, each slot's stride-16 feature gathered from its video through seq_of; head_shared(..., src_of=seq_of); NMS of the
@@ -354,7 +142,8 @@ class UnicornUnifiedBatch(_Unified):
         self._slot = FrameSlot(engine, H, W, batch=n_seq)  # input buffers, the MOT images' NMS workspace, the graph
         self.sot_ws = ops.PostWorkspace(A, dev, K)
         self._qd = QDEmbedding(engine, H, W, self.n_keep, "unifiedb.emb", batch=n_seq) if mot == "qd" else None
-        # the target slots as UnicornUnifiedTracker keeps them, plus each slot's video
+        # the target slots: reference projection and label values as UnicornSOTBatch keeps them, the device active table and each
+        # slot's video
         n16 = (H // 16) * (W // 16)
         self.ref_proj = (torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev), torch.zeros(K * n16, 256, dtype=torch.bfloat16, device=dev))
         self.lbs_pre = torch.zeros(K, 1, (H // 8) * (W // 8), dtype=torch.float32, device=dev)
@@ -368,7 +157,7 @@ class UnicornUnifiedBatch(_Unified):
         self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()
         self.started = [False] * n_seq
         self.trackers = [None] * n_seq
-        self.frame_ids = [0] * n_seq  # steps the MOT arm has run per video since its start()
+        self.frame_ids = [0] * n_seq  # active steps per video since its start(): the QD arm's frame number
         self.states = [{} for _ in range(n_seq)]  # track(): the reference-protocol state of every target of each video
         self.launches_per_frame = 0
         self.last = {}
@@ -437,7 +226,8 @@ class UnicornUnifiedBatch(_Unified):
 
     def _write_references(self, boxes):
         """The targets of `boxes` (slot -> box) take their video's frame of the step just enqueued as their reference frame: the
-        frame's stride-16 feature is projected once per video and written into the slots (UnicornUnifiedTracker._write_references)."""
+        frame's stride-16 feature is projected once per video and written into the slots (UnicornSOTBatch.initialize_tensor on that
+        feature)."""
         e = self.eng
         H, W = self.input_size
         n16 = (H // 16) * (W // 16)
@@ -459,13 +249,17 @@ class UnicornUnifiedBatch(_Unified):
         values = self.lbs_pre if K > 1 else self.lbs_pre[0]
 
         def correlate(seq):  # the SOT arm, on the stream that overlaps the neck: each slot pairs its reference with its video's frame
-            f = seq["feat"]
-            feat = torch.index_select(f, 0, self.seq_of, out=e.buf("unifiedb.featK", (K,) + tuple(f.shape[1:])))
+            feat = seq["feat"]
+            if n > 1:  # each slot's feature from its video's frame
+                feat = torch.index_select(feat, 0, self.seq_of, out=e.buf("unifiedb.featK", (K,) + tuple(feat.shape[1:])))
+            elif K > 1:  # one video: a broadcast copy, measurably faster than index_select through a table of zeros
+                feat = e.buf("unifiedb.featK", (K,) + tuple(feat.shape[1:])).copy_(feat.expand(K, -1, -1, -1))
             f_pre, f_cur = e.interaction(None, feat, ref_proj=self.ref_proj)
             return e.propagate(e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc"), values)
 
         fpn, seq, priors = e.backbone(c.img, tag="unifiedb", side=correlate)
-        head_mot, head_sot = e.head_shared(fpn, priors, mot=self.mot is not None, src_of=self.seq_of)
+        # one video: seq_of is all zeros, which is head_shared's own fixed table (no table rebuilt every step)
+        head_mot, head_sot = e.head_shared(fpn, priors, mot=self.mot is not None, src_of=self.seq_of if n > 1 else None)
         _, cnt = ops.postprocess_device(head_sot, 1, self.conf, self.nms, self.sot_ws, max_keep=self.max_inst)
         cnt.mul_(self.active)
         embed = None
@@ -522,9 +316,10 @@ class UnicornUnifiedBatch(_Unified):
     # ------------------------------------------------------------------------------------------ host half
     def collect(self, img_infos=None):
         """Results of the oldest submitted step: one entry per video, None for a video idle in that step, otherwise {"targets": {tid:
-        (dets [<= max_inst, 7], count)}, "mot": ...} as UnicornUnifiedTracker.collect returns it (img_infos[i]: (height, width) of
-        video i's original image, for the ByteTrack arm).  last_dets[i] / last_feats[i] then hold the NMS rows / embeddings video i's
-        tracker was given in this step."""
+        (dets [<= max_inst, 7], count)}, "mot": ...}.  "mot" is what UnicornMOTTracker.collect returns (QDTrack: (bboxes [n,5] in
+        original-image coordinates, ids [n]); ByteTrack: the active STracks, img_infos[i] = (height, width) of video i's original
+        image), None without a MOT arm.  last_dets[i] / last_feats[i] then hold the NMS rows / embeddings video i's tracker was given
+        in this step."""
         s = self._ring.collect()
         s.event.synchronize()
         H, W = self.input_size
@@ -566,8 +361,9 @@ class UnicornUnifiedBatch(_Unified):
     def track(self, images, new_targets=None, img_infos=None):
         """images: n_seq RGB frames (HWC uint8, any original sizes), None for an idle video; each is letterboxed once for both arms.
         new_targets {video: {tid: [x, y, w, h]}} (original-image pixels) start on this step's frame of their video.  Returns one entry
-        per video, None for an idle one, otherwise {"targets": {tid: [x, y, w, h]}, "mot": ...} with UnicornUnifiedTracker.track's
-        state rules; img_infos[i] defaults to video i's frame (height, width)."""
+        per video, None for an idle one, otherwise {"targets": {tid: [x, y, w, h]}, "mot": ...}: each target's state as
+        UnicornSOTTrack.track keeps it (a new target's is its box; a target with no detection keeps its previous state), and the MOT
+        arm's result with img_infos[i] defaulting to video i's frame (height, width)."""
         n = self.n_seq
         if len(images) != n:
             raise ValueError(f"UnicornUnifiedBatch.track: {len(images)} frames for {n} videos")
@@ -600,6 +396,70 @@ class UnicornUnifiedBatch(_Unified):
                     self.states[i][tid] = state_xywh(dets[0], ratios[i], self.input_size)
             res[i] = {"targets": {tid: self.states[i][tid] for tid in self.targets(i)}, "mot": o["mot"]}
         return res
+
+
+# ---------------------------------------------------------------------------------------------------------- one video
+class UnicornUnifiedTracker:
+    """Up to `max_targets` SOT targets plus optionally one MOT arm (mot = "qd", "byte" or None) on one video, one backbone pass per frame:
+    UnicornUnifiedBatch at n_seq = 1 (same settings) with its video started on `tracker` (default a fresh QuasiDenseEmbedTracker; the
+    ByteTrack arm needs a BYTETracker), under the one-video protocol.
+
+    add_target(tid, box_xyxy): the next submitted frame becomes the target's reference frame.  Right after that step, its stride-16
+    feature is projected (project_ref) and the box's label map resized into the target's slot; the target gives results from the
+    following frame on.  remove_target(tid) frees the slot.  Steps already submitted report the targets that were live when they
+    were submitted.  frame_id counts the steps submitted, with or without a MOT arm."""
+
+    def __init__(self, engine: UnicornEngine, input_size, max_targets, mot="qd", tracker=None, conf=0.001, nms=0.65, max_inst=3,
+                 mot_conf=0.01, mot_nms=0.7, score_thr=0.1, max_dets=1024, use_graph=True):
+        self._b = UnicornUnifiedBatch(engine, input_size, 1, max_targets, mot, conf, nms, max_inst, mot_conf, mot_nms, score_thr,
+                                      max_dets, use_graph)
+        self._b.start(0, tracker)
+
+    graph = property(lambda self: self._b.graph)
+    targets = property(lambda self: self._b.targets(0))
+    max_targets = property(lambda self: self._b.max_targets)
+    launches_per_frame = property(lambda self: self._b.launches_per_frame)
+    last = property(lambda self: self._b.last)
+    last_dets = property(lambda self: self._b.last_dets[0])
+    last_feats = property(lambda self: self._b.last_feats[0])
+    states = property(lambda self: self._b.states[0])
+    tracker = property(lambda self: self._b.trackers[0])
+    frame_id = property(lambda self: self._b.frame_ids[0])
+    ref_proj = property(lambda self: self._b.ref_proj)
+    lbs_pre = property(lambda self: self._b.lbs_pre)
+    sot_ws = property(lambda self: self._b.sot_ws)
+    _ring = property(lambda self: self._b._ring)
+    _pending = property(lambda self: self._b._pending)
+    _slot = property(lambda self: self._b._slot)
+    _tid = property(lambda self: [None if t is None else t[1] for t in self._b._tid])  # target id per slot
+
+    def add_target(self, tid, box_xyxy):
+        """Track `tid` from the box [x1, y1, x2, y2] (resized-image coordinates) in the next submitted frame."""
+        self._b.add_target(0, tid, box_xyxy)
+
+    def remove_target(self, tid):
+        """Stop tracking `tid` and free its slot (steps already submitted still report it)."""
+        self._b.remove_target(0, tid)
+
+    def submit(self, frame, scale=1.0):
+        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; scale: its letterbox ratio.  Enqueues the step on
+        the current stream; returns immediately."""
+        self._b.submit(frame, [scale])
+
+    def collect(self, img_info=None):
+        """Results of the oldest submitted step: {"targets": {tid: (dets [<= max_inst, 7], count)}, "mot": ...} as
+        UnicornUnifiedBatch.collect gives them for one video (img_info: (height, width) of the original image)."""
+        return self._b.collect([img_info])[0]
+
+    def step_tensor(self, frame, scale=1.0, img_info=None):
+        """Sequential protocol: one step in, its results out."""
+        self.submit(frame, scale)
+        return self.collect(img_info)
+
+    def track(self, image_rgb, new_targets=None, img_info=None):
+        """image_rgb: an RGB frame (HWC uint8), letterboxed once for both arms.  new_targets {tid: [x, y, w, h]} (original-image pixels)
+        start on this frame.  Returns {"targets": {tid: [x, y, w, h]}, "mot": ...} with UnicornUnifiedBatch.track's state rules."""
+        return self._b.track([image_rgb], {0: new_targets or {}}, [img_info])[0]
 
 
 # ---------------------------------------------------------------------------------------------------------- VOS objects + MOTS
