@@ -1,4 +1,4 @@
-"""Argument validation of uc_groupnorm_apply, uc_copy_upsample and uc_add: every call here is rejected with UC_EINVAL and a message
+"""Argument validation of uc_groupnorm_apply, uc_copy_upsample, uc_add, uc_dwconv7_ln and uc_stem_ln: every call here is rejected with UC_EINVAL and a message
 before anything is launched, so the pointers are fake addresses that are never dereferenced and the test runs without a GPU."""
 import ctypes
 
@@ -75,3 +75,32 @@ def test_add_rejects_misaligned_rows_and_other_dtypes(lib):
         rejected(add(*args), "uc_add", "16-byte aligned")
     rejected(add(A16[0], A16[1], A16[2], dtype=_lib.F32), "uc_add", "16-bit dtypes only")
     rejected(add(A16[0], None, A16[2]), "uc_add: bad arguments")
+
+
+def dwln(lib, x=A16[0], w=A16[1], bias=A16[2], lnw=A16[3], lnb=A16[4], y=A16[5], B=1, H=8, W=8, C=128):
+    rc = lib.uc_dwconv7_ln(x, w, bias, lnw, lnb, y, B, H, W, C, ctypes.c_float(1e-6), None)
+    return rc, lib.uc_last_error()
+
+
+def test_dwconv7_ln_rejects_bad_channels_in_place_and_null(lib):
+    for C in (127, 1, 1538, 2048, 0):
+        rejected(dwln(lib, C=C), "uc_dwconv7_ln", "C must be even and <= 1536")
+    rejected(dwln(lib, y=A16[0]), "uc_dwconv7_ln", "not an in-place operation")
+    for k in ("x", "w", "bias", "lnw", "lnb", "y"):
+        rejected(dwln(lib, **{k: None}), "uc_dwconv7_ln", "null pointer")
+
+
+def stem(lib, img=A16[0], w=A16[1], bias=A16[2], lnw=A16[3], lnb=A16[4], out=A16[5], B=1, H=32, W=32, C0=96):
+    rc = lib.uc_stem_ln(img, 0, w, bias, lnw, lnb, out, B, H, W, C0, ctypes.c_float(1e-6), None)
+    return rc, lib.uc_last_error()
+
+
+def test_stem_ln_rejects_bad_shapes_channels_and_null(lib):
+    for H, W in ((30, 32), (32, 34), (2, 32)):
+        rejected(stem(lib, H=H, W=W), "uc_stem_ln", "H%4==0, W%4==0")
+    rejected(stem(lib, C0=288), "uc_stem_ln", "C0<=256")
+    rejected(stem(lib, C0=100), "uc_stem_ln", "C0%32==0")
+    rejected(stem(lib, C0=160), "uc_stem_ln: unsupported C0 160")  # 5 channels per lane: no kernel instantiated
+    rejected(stem(lib, C0=224), "uc_stem_ln: unsupported C0 224")
+    for k in ("img", "w", "bias", "lnw", "lnb", "out"):
+        rejected(stem(lib, **{k: None}), "uc_stem_ln", "null pointer")

@@ -384,9 +384,9 @@ def test_corr_propagate_hard_softmax(n_obj, dtype):
 
 
 # ---------------------------------------------------------------------------------------------------------------- small kernels
-@pytest.mark.parametrize("C0", [32, 64, 128, 256])
+@pytest.mark.parametrize("C0", [32, 64, 96, 128, 192, 256])
 def test_stem_ln_channel_counts(C0):
-    """stem_ln_kernel<CPL> for CPL = 1, 2, 4, 8; W / 4 = 9 leaves a partial group of 4 output pixels per row."""
+    """stem_ln_kernel<CPL> for CPL = 1, 2, 3, 4, 6, 8; W / 4 = 9 leaves a partial group of 4 output pixels per row."""
     g = G(60 + C0)
     img = (torch.rand(2, 3, 24, 36, generator=g) * 255).to(dev)
     w = (torch.randn(C0, 3, 4, 4, generator=g) / 7).to(dev)
