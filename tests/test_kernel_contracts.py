@@ -1,4 +1,4 @@
-"""Argument validation of uc_groupnorm_apply, uc_copy_upsample, uc_add, uc_dwconv7_ln and uc_stem_ln: every call here is rejected with UC_EINVAL and a message
+"""Argument validation of uc_groupnorm_apply, uc_copy_upsample, uc_add, uc_dwconv7_ln, uc_stem_ln and uc_conv2d: every call here is rejected with UC_EINVAL and a message
 before anything is launched, so the pointers are fake addresses that are never dereferenced and the test runs without a GPU."""
 import ctypes
 
@@ -104,3 +104,79 @@ def test_stem_ln_rejects_bad_shapes_channels_and_null(lib):
     rejected(stem(lib, C0=224), "uc_stem_ln: unsupported C0 224")
     for k in ("img", "w", "bias", "lnw", "lnb", "out"):
         rejected(stem(lib, **{k: None}), "uc_stem_ln", "null pointer")
+
+
+def conv(lib, **kw):
+    """uc_conv2d on a valid 3x3 / s1 / p1 bf16 conv of 1 x 16 x 16 x 64 -> 64 channels, with the fields in kw replaced."""
+    d = _lib.UcConv2d()
+    d.x, d.x_dtype, d.B, d.H, d.W, d.Cin, d.ldx = A16[0], _lib.BF16, 1, 16, 16, 64, 64
+    d.w, d.Cout, d.KH, d.KW, d.stride, d.pad = A16[1], 64, 3, 3, 1, 1
+    d.y, d.ldy, d.y_dtype, d.act = A16[2], 64, _lib.BF16, _lib.ACT_NONE
+    for k, v in kw.items():
+        setattr(d, k, v)
+    rc = lib.uc_conv2d(ctypes.byref(d), None)
+    return rc, lib.uc_last_error()
+
+
+def test_conv2d_rejects_empty_maps(lib):
+    for k in ("B", "H", "W"):
+        for v in (0, -1):
+            rejected(conv(lib, **{k: v}), "uc_conv2d: B, H and W must be >= 1")
+
+
+@pytest.mark.parametrize("KH,KW,stride,pad,H,W", [
+    (3, 3, 1, 0, 2, 16), (3, 3, 1, 0, 16, 2), (3, 1, 1, 0, 1, 16),   # stride 1: (H + 2 pad - KH) = -1
+    (2, 2, 2, 0, 1, 16), (2, 2, 2, 0, 16, 1),                        # stride 2, numerator -1: C's division gave an output of 1
+    (3, 3, 2, 0, 2, 16), (3, 3, 2, 0, 16, 2), (3, 3, 2, 0, 1, 1)])
+def test_conv2d_rejects_kernels_larger_than_the_padded_map(lib, KH, KW, stride, pad, H, W):
+    rejected(conv(lib, KH=KH, KW=KW, stride=stride, pad=pad, H=H, W=W), "uc_conv2d", "kernel larger than the padded map")
+
+
+def test_conv2d_rejects_a_conv_that_reads_only_padding(lib):
+    # 1x1 / s2 / p1 on a map one pixel high (wide): every tap falls on the empty odd phase, the output would be the bias alone
+    rejected(conv(lib, KH=1, KW=1, stride=2, pad=1, H=1, W=16), "uc_conv2d", "reads only zero padding")
+    rejected(conv(lib, KH=3, KW=1, stride=2, pad=1, H=5, W=1), "uc_conv2d", "reads only zero padding")
+
+
+def test_conv2d_rejects_bad_groupnorm_tiles(lib):
+    st = A16[3]
+    rejected(conv(lib, gn_stats=st, gn_groups=24), "uc_conv2d: bad GroupNorm grouping")  # 24 does not divide 64
+    rejected(conv(lib, gn_stats=st, gn_groups=0), "uc_conv2d: bad GroupNorm grouping")
+    rejected(conv(lib, gn_stats=st, gn_groups=-8), "uc_conv2d: bad GroupNorm grouping")
+    # group size 24 (Cout 192, 8 groups) straddles a 64-column N tile
+    rejected(conv(lib, Cout=192, ldy=192, gn_stats=st, gn_groups=8, block_n=64), "N tile 64 incompatible with GroupNorm group size 24")
+    rejected(conv(lib, Cout=192, ldy=192, gn_stats=st, gn_groups=8, block_n=1256), "N tile 256 incompatible with GroupNorm group size 24")
+    # group size 5 or 25: no N tile is a multiple of it, so the heuristic (block_n = 0) has nothing to pick
+    rejected(conv(lib, Cout=40, ldy=40, gn_stats=st, gn_groups=8), "no N tile compatible with GroupNorm group size 5")
+    rejected(conv(lib, Cout=200, ldy=200, gn_stats=st, gn_groups=8), "no N tile compatible with GroupNorm group size 25")
+    # a CTA accumulates at most 64 groups: group size 1 or 2 at wide N tiles
+    for bn, gs in ((96, 1), (128, 1), (256, 2), (192, 2), (1128, 1), (1256, 2)):
+        rejected(conv(lib, Cout=256, ldy=256, gn_stats=st, gn_groups=256 // gs, block_n=bn), f"uc_conv2d: N tile {bn % 1000} holds "
+                 f"{bn % 1000 // gs} GroupNorm groups, more than the 64")
+
+
+@pytest.mark.parametrize("block_n", [1064, 1096, 1016, 1000, 2256])
+def test_conv2d_rejects_cluster_block_n_without_a_cluster_variant(lib, block_n):
+    rejected(conv(lib, block_n=block_n), "uc_conv2d: the cluster variant exists for block_n 128/192/256 only")
+
+
+@pytest.mark.parametrize("block_n", [8, 48, 100, 112, 160, 512, 999, -16])
+def test_conv2d_rejects_unsupported_block_n(lib, block_n):
+    rejected(conv(lib, block_n=block_n), f"uc_conv2d: unsupported block_n {block_n}")
+
+
+def test_conv2d_rejects_act_after_res_combinations(lib):
+    r = dict(res=A16[4], ldres=64, act=_lib.ACT_RELU, act_after_res=1)
+    msg = "uc_conv2d: act_after_res needs act = ReLU, res and bf16 x"
+    for bad in (dict(act=_lib.ACT_NONE), dict(act=_lib.ACT_GELU), dict(res=None), dict(x_dtype=_lib.F16, y_dtype=_lib.F16),
+                dict(gamma=A16[5]), dict(gn_stats=A16[3], gn_groups=16), dict(row_stats=A16[3], col_s=A16[5], KH=1, KW=1, pad=0)):
+        rejected(conv(lib, **{**r, **bad}), msg)
+
+
+def test_conv2d_rejects_row_stats_off_a_flat_conv(lib):
+    ln = dict(row_stats=A16[3], col_s=A16[5], act=_lib.ACT_GELU)
+    msg = "uc_conv2d: row_stats (folded LayerNorm) needs a 1x1 stride-1 conv and col_s"
+    rejected(conv(lib, **ln), msg)  # 3x3
+    rejected(conv(lib, **ln, KH=1, KW=1, pad=0, stride=2), msg)
+    rejected(conv(lib, **ln, KH=1, KW=1, pad=1), msg)
+    rejected(conv(lib, **{**ln, "col_s": None}, KH=1, KW=1, pad=0), msg)

@@ -14,6 +14,7 @@ static int pick_block_n(int Cout, int m_tiles, int gn_gs) {
   double best_cost = -1.0;
   for (int bn : cands) {
     if (gn_gs > 0 && (bn % gn_gs) != 0) continue;  // GroupNorm groups must not straddle N tiles
+    if (gn_gs > 0 && bn / gn_gs > kGnMaxLocal) continue;  // nor overflow the CTA's GroupNorm slots
     const int nt = (Cout + bn - 1) / bn;
     const long waste_cols = static_cast<long>(nt) * bn - Cout;
     if (waste_cols * 3 > static_cast<long>(nt) * bn && bn > 16 && gn_gs <= 0) continue;
@@ -47,13 +48,31 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
     return set_error(UC_EINVAL, "uc_conv2d: bad GroupNorm grouping");
   if (d->act_after_res && (d->act != UC_ACT_RELU || !d->res || d->x_dtype != UC_BF16 || d->gamma || d->gn_stats || d->row_stats))
     return set_error(UC_EINVAL, "uc_conv2d: act_after_res needs act = ReLU, res and bf16 x, and excludes gamma, gn_stats and row_stats");
-  int rc = ensure_driver();
-  if (rc) return rc;
+  if (d->row_stats && (!d->col_s || d->KH != 1 || d->KW != 1 || d->stride != 1 || d->pad != 0))
+    return set_error(UC_EINVAL, "uc_conv2d: row_stats (folded LayerNorm) needs a 1x1 stride-1 conv and col_s");
+  if (d->B < 1 || d->H < 1 || d->W < 1)
+    return set_error(UC_EINVAL, "uc_conv2d: B, H and W must be >= 1 (B=%d H=%d W=%d)", d->B, d->H, d->W);
+  // PyTorch's rule: the kernel fits in the padded map.  The numerator below is then >= 0, so C's division is the floor.
+  if (d->H + 2 * d->pad < d->KH || d->W + 2 * d->pad < d->KW)
+    return set_error(UC_EINVAL, "uc_conv2d: %dx%d kernel larger than the padded map (H=%d W=%d pad=%d)", d->KH, d->KW, d->H, d->W, d->pad);
+  const int gn_gs = d->gn_stats ? d->Cout / d->gn_groups : 0;
+  // block_n >= 1000 selects the 2-CTA cluster variant with weight multicast (1128 / 1192 / 1256)
+  const bool cluster2 = d->block_n >= 1000;
+  if (d->block_n) {
+    const int bn = cluster2 ? d->block_n - 1000 : d->block_n;
+    if (cluster2 && bn != 128 && bn != 192 && bn != 256)
+      return set_error(UC_EINVAL, "uc_conv2d: the cluster variant exists for block_n 128/192/256 only");
+    if (bn != 16 && bn != 32 && bn != 64 && bn != 96 && bn != 128 && bn != 192 && bn != 256)
+      return set_error(UC_EINVAL, "uc_conv2d: unsupported block_n %d", d->block_n);
+    if (gn_gs && bn % gn_gs) return set_error(UC_EINVAL, "uc_conv2d: N tile %d incompatible with GroupNorm group size %d", bn, gn_gs);
+    if (gn_gs && bn / gn_gs > kGnMaxLocal)
+      return set_error(UC_EINVAL, "uc_conv2d: N tile %d holds %d GroupNorm groups, more than the %d a CTA accumulates", bn, bn / gn_gs,
+                       kGnMaxLocal);
+  }
 
   const int s = d->stride;
   const int Ho = (d->H + 2 * d->pad - d->KH) / s + 1;
   const int Wo = (d->W + 2 * d->pad - d->KW) / s + 1;
-  if (Ho <= 0 || Wo <= 0) return set_error(UC_EINVAL, "uc_conv2d: empty output");
 
   ConvKernelParams p;
   memset(&p, 0, sizeof(p));
@@ -81,12 +100,39 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   p.tiles_h = (p.Ho + p.tile_h - 1) / p.tile_h;
   const int m_tiles = p.tiles_w * p.tiles_h * B;
 
+  // A stride phase of a map one pixel high or wide has no pixels (phase 1 of W = 1 at stride 2): its tensor map is not encoded, and
+  // the taps that fall on it read only zero padding, so they are left out.  t.tap still indexes the packed weights.
+  auto phase_empty = [&](int ph, int pw) { return (Wm - pw + s - 1) / s <= 0 || (Hm - ph + s - 1) / s <= 0; };
+  int nt = 0;
+  for (int kh = 0; kh < d->KH; ++kh) {
+    for (int kw = 0; kw < d->KW; ++kw) {
+      const int offh = kh - d->pad, offw = kw - d->pad;
+      const int ph = ((offh % s) + s) % s, pw = ((offw % s) + s) % s;
+      if (phase_empty(ph, pw)) continue;
+      ConvTap t;
+      t.map = static_cast<int16_t>(ph * s + pw);
+      t.dh = static_cast<int16_t>((offh - ph) / s);
+      t.dw = static_cast<int16_t>((offw - pw) / s);
+      t.tap = static_cast<int16_t>(kh * d->KW + kw);
+      p.taps[nt++] = t;
+    }
+  }
+  if (nt == 0)
+    return set_error(UC_EINVAL, "uc_conv2d: every tap of this %dx%d stride-2 conv reads only zero padding (H=%d W=%d pad=%d)", d->KH,
+                     d->KW, d->H, d->W, d->pad);
+  p.ntaps = nt;
+  p.kchunks = (d->Cin + kBlockK - 1) / kBlockK;
+  const int bn = cluster2 ? d->block_n - 1000 : d->block_n ? d->block_n : pick_block_n(d->Cout, m_tiles, gn_gs);
+  if (bn == 0) return set_error(UC_EINVAL, "uc_conv2d: no N tile compatible with GroupNorm group size %d", gn_gs);
+
+  int rc = ensure_driver();
+  if (rc) return rc;
   // activation maps: one per stride phase
   const size_t es = 2;
   for (int ph = 0; ph < s; ++ph) {
     for (int pw = 0; pw < s; ++pw) {
       const int Wp = (Wm - pw + s - 1) / s, Hp = (Hm - ph + s - 1) / s;
-      if (Wp <= 0 || Hp <= 0) continue;
+      if (phase_empty(ph, pw)) continue;
       const uint8_t* base = reinterpret_cast<const uint8_t*>(d->x) + (static_cast<size_t>(ph) * Wm + pw) * d->ldx * es;
       uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(Wp), static_cast<uint64_t>(Hp), static_cast<uint64_t>(B)};
       uint64_t strides[3] = {static_cast<uint64_t>(s) * d->ldx * es, static_cast<uint64_t>(s) * Wm * d->ldx * es,
@@ -96,30 +142,11 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
       if (rc) return rc;
     }
   }
-  int nt = 0;
-  for (int kh = 0; kh < d->KH; ++kh) {
-    for (int kw = 0; kw < d->KW; ++kw) {
-      const int offh = kh - d->pad, offw = kw - d->pad;
-      const int ph = ((offh % s) + s) % s, pw = ((offw % s) + s) % s;
-      ConvTap t;
-      t.map = static_cast<int16_t>(ph * s + pw);
-      t.dh = static_cast<int16_t>((offh - ph) / s);
-      t.dw = static_cast<int16_t>((offw - pw) / s);
-      t.tap = static_cast<int16_t>(kh * d->KW + kw);
-      p.taps[nt++] = t;
-    }
-  }
-  p.ntaps = nt;
-  p.kchunks = (d->Cin + kBlockK - 1) / kBlockK;
 
-  const int gn_gs = d->gn_stats ? d->Cout / d->gn_groups : 0;
-  // block_n >= 1000 selects the 2-CTA cluster variant with weight multicast (1128 / 1192 / 1256)
-  const bool cluster2 = d->block_n >= 1000;
-  const int bn = cluster2 ? d->block_n - 1000 : d->block_n ? d->block_n : pick_block_n(d->Cout, m_tiles, gn_gs);
-  if (bn == 0) return set_error(UC_EINVAL, "uc_conv2d: no N tile compatible with GroupNorm group size %d", gn_gs);
+  const int ktaps = d->KH * d->KW;  // taps of the packed weights
   {
-    uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(nt), static_cast<uint64_t>(d->Cout)};
-    uint64_t strides[2] = {static_cast<uint64_t>(d->Cin) * es, static_cast<uint64_t>(nt) * d->Cin * es};
+    uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(ktaps), static_cast<uint64_t>(d->Cout)};
+    uint64_t strides[2] = {static_cast<uint64_t>(d->Cin) * es, static_cast<uint64_t>(ktaps) * d->Cin * es};
     uint32_t box[3] = {static_cast<uint32_t>(kBlockK), 1, static_cast<uint32_t>(bn)};
     rc = encode_tmap(&p.tmB, dt, 3, d->w, dims, strides, box);
     if (rc) return rc;
@@ -128,12 +155,8 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   p.bias = d->bias; p.gamma = d->gamma; p.res = d->res; p.ldres = d->ldres;
   p.y = d->y; p.ldy = d->ldy; p.y_dtype = d->y_dtype; p.act = d->act_after_res ? UC_ACT_NONE : d->act; p.relu_res = d->act_after_res;
   p.row_stats = static_cast<const long long*>(d->row_stats); p.col_s = d->col_s; p.row_inv = 1.f / (kGnFixedScale * static_cast<float>(d->Cin)); p.row_eps = d->row_eps;
-  if (d->row_stats && (!d->col_s || d->KH != 1 || d->KW != 1 || d->stride != 1 || d->pad != 0))
-    return set_error(UC_EINVAL, "uc_conv2d: row_stats (folded LayerNorm) needs a 1x1 stride-1 conv and col_s");
   p.gn_stats = static_cast<long long*>(d->gn_stats); p.gn_groups = d->gn_groups;
-  p.gn_gs = d->gn_stats ? d->Cout / d->gn_groups : 1 << 30;
-  if (d->gn_stats && (bn % p.gn_gs) != 0)
-    return set_error(UC_EINVAL, "uc_conv2d: N tile %d incompatible with GroupNorm group size %d", bn, p.gn_gs);
+  p.gn_gs = d->gn_stats ? gn_gs : 1 << 30;
   p.n_tiles = (d->Cout + bn - 1) / bn;
   p.m_tiles = m_tiles;
   if (d->y_dtype != UC_F32) {  // 16-bit y (and the residual, same dtype and geometry) moves by TMA through the staging tile
@@ -151,8 +174,8 @@ extern "C" int uc_conv2d(const UcConv2d* d, void* stream_v) {
   }
   const bool f16 = d->x_dtype == UC_F16;
   if (cluster2) {
-    uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(nt), static_cast<uint64_t>(d->Cout)};
-    uint64_t strides[2] = {static_cast<uint64_t>(d->Cin) * es, static_cast<uint64_t>(nt) * d->Cin * es};
+    uint64_t dims[3] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(ktaps), static_cast<uint64_t>(d->Cout)};
+    uint64_t strides[2] = {static_cast<uint64_t>(d->Cin) * es, static_cast<uint64_t>(ktaps) * d->Cin * es};
     uint32_t box[3] = {static_cast<uint32_t>(kBlockK), 1, static_cast<uint32_t>(bn / 2)};
     rc = encode_tmap(&p.tmBh, dt, 3, d->w, dims, strides, box);
     if (rc) return rc;
