@@ -348,6 +348,22 @@ typedef struct UcVosObject {
 UC_API int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win, int H, int W, float r, float* soft_out,
                             uint8_t* seg_out, void* stream);
 
+/* uc_vos_aggregate of B videos (1 <= B <= UC_VOS_MAX_VIDEOS) in one launch, all at the network resolution Hin x Win.  Video b has
+ * its own objects (objs: HOST array of n, 1 <= n <= 16, ids 1..255, in the reference's list order), original size H x W, letterbox
+ * ratio r > 0 and outputs (soft_out may be NULL; seg_out may not).  videos is a HOST array of B.  Video b's seg and soft equal those
+ * of uc_vos_aggregate called on video b alone, bit for bit; uc_vos_aggregate is this call with B = 1.  Every argument is validated
+ * before any CUDA call; no allocation, no synchronisation, one launch. */
+#define UC_VOS_MAX_VIDEOS UC_MOTS_MAX_IMAGES
+typedef struct UcVosVideo {
+  const UcVosObject* objs;
+  int n;
+  int H, W;
+  float r;
+  float* soft_out;
+  uint8_t* seg_out;
+} UcVosVideo;
+UC_API int uc_vos_aggregate_batched(const UcVosVideo* videos, int B, int Hin, int Win, void* stream);
+
 /* MOTS result encoding on the device (unicorn/evaluators/mot_evaluator.py:804-805, :858-866, :884-888): for the k instances of
  * one frame, masks f32 [n_max,Hin,Win] (the uc_dynamic_masks output) are resized to the original H x W frame as in uc_vos_aggregate
  * (only the hm x wm corner F.interpolate produces, hm = min(H, floor(Hin/r)), is encoded), thresholded (> thr), made overlap free

@@ -30,7 +30,18 @@ the MOT arm, three sides in the same process, all pipelined (submit(t + 1) befor
 UnicornUnifiedBatch over all videos; n_seq UnicornUnifiedTrackers stepped in turn; UnicornSOTBatch over all targets (each fed its
 video's frame) plus UnicornMOTBatch(n_seq) (the SOT batch of step t is collected before its next submit).  The device-only step is
 the graph replays of every side's drivers with their input copies.  Besides the ms per step, each side reports the aggregate
-video-frames/s (n_seq / step time).  One JSON line per (config, n_seq, per_video, mot)."""
+video-frames/s (n_seq / step time).  One JSON line per (config, n_seq, per_video, mot).
+
+    python tools/bench_unified.py --workload mask-batch [--configs ...] [--n-seq 2 4] [--objects 1 3] [--mots on off] [--steps 20]
+
+The mask-batch workload: n_seq videos of mixed original sizes (1080x1920 and 480x640 in turn, make_video seeds 0..n_seq-1, each
+letterboxed once on the host to 800x1280 uint8 and kept on the device), each with `objects` VOS objects (added on frame 0, in one
+group) and optionally the MOTS arm, on unicorn_track_large_mask and unicorn_track_large_mot_challenge_mask.  Three sides in the same
+process: UnicornUnifiedMaskBatch over all videos and n_seq UnicornUnifiedMaskTrackers stepped in turn, both pipelined (submit(t + 1)
+before collect(t)); UnicornVOSBatch (synchronous per step) plus UnicornMOTSBatch (pipelined).  A step includes the VOS result assembly
+of every video, the MOTS association and the mask encode.  The device-only step is every side's graph replays with their input
+copies plus the result assemblies outside the graphs.  Launches per step count the kernels of the graphs plus the launches outside
+them.  One JSON line per (config, n_seq, objects, mots)."""
 import argparse
 import json
 import os
@@ -47,7 +58,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["box", "mask", "batch"], default="box")
+    ap.add_argument("--workload", choices=["box", "mask", "batch", "mask-batch"], default="box")
     ap.add_argument("--configs", nargs="+", default=None)
     ap.add_argument("--size", type=int, nargs=2, default=(800, 1280))
     ap.add_argument("--targets", type=int, nargs="+", default=[1, 2, 4])
@@ -62,9 +73,9 @@ def main():
     args = ap.parse_args()
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print(json.dumps({"card": torch.cuda.get_device_name(), "nvidia_smi": q}), flush=True)
-    if args.workload == "mask":
+    if args.workload in ("mask", "mask-batch"):
         args.configs = args.configs or ["unicorn_track_large_mask", "unicorn_track_large_mot_challenge_mask"]
-        return mask(args)
+        return mask(args) if args.workload == "mask" else mask_batch(args)
     args.configs = args.configs or ["unicorn_track_large", "unicorn_track_r50"]
     if args.workload == "batch":
         return batch(args)
@@ -403,6 +414,157 @@ def batch(args):
                         line[key]["video_frames_per_s"] = round(1e3 * n / line[key]["ms_per_step"], 1)
                     print(json.dumps(line), flush=True)
                     del sides, ub, uts, sb, mt, ub_round, ub_replay, ut_round, ut_replay, sm_round, sm_replay
+                    torch.cuda.empty_cache()
+        del eng
+        torch.cuda.empty_cache()
+
+
+def mask_batch(args):
+    from unicorn_b200 import _lib, ops, shared_ops
+    from unicorn_b200.engine import UnicornEngine
+    from unicorn_b200.mots import UnicornMOTSBatch
+    from unicorn_b200.sot import preprocess
+    from unicorn_b200.synthetic import make_video
+    from unicorn_b200.unified import UnicornUnifiedMaskBatch, UnicornUnifiedMaskTracker
+    from unicorn_b200.vos import UnicornVOSBatch
+    from unicorn_b200.weights import make_state_dict
+
+    H, W = args.size
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    origs = [(1080, 1920), (480, 640)]
+    vids = []  # per video: (original size, r, letterboxed reference [1,H,W,3], 4 letterboxed steps, frame-0 boxes in resized coordinates)
+    for i in range(max(args.n_seq)):
+        h0, w0 = origs[i % 2]
+        frames, boxes = make_video(5, h0, w0, seed=i, n_obj=6)
+        rgb = [f.permute(1, 2, 0).flip(-1).round().clamp(0, 255).to(torch.uint8).numpy().copy() for f in frames]
+        lb = [preprocess(im, (H, W)) for im in rgb]
+        r = lb[0][1]
+        vids.append(((h0, w0), r, lb[0][0].cuda(), [f.cuda() for f, _ in lb[1:]], boxes[0] * r))
+
+    def outside(step, n=4):
+        """Launches per step outside the graphs (result assembly, encode), counted over n steps."""
+        l0 = _lib.LAUNCHES
+        for t in range(n):
+            step(t)
+        return (_lib.LAUNCHES - l0) / n
+
+    for cfg in args.configs:
+        eng = UnicornEngine(make_state_dict(cfg, 0), cfg)
+        for n in args.n_seq:
+            vs = vids[:n]
+            ref_b = torch.cat([v[2] for v in vs])
+            steps_b = [torch.cat([v[3][t] for v in vs]) for t in range(4)]  # [n,H,W,3]
+            sizes = [v[0] for v in vs]
+            for K in args.objects:
+                objs = [{k + 1: v[4][k] for k in range(K)} for v in vs]
+                for mots in [m == "on" for m in args.mots]:
+                    sides = {}
+                    # ---- one step for every video: UnicornUnifiedMaskBatch
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    ub = UnicornUnifiedMaskBatch(eng, (H, W), n, n * K, n, mots=mots)
+                    for i, v in enumerate(vs):
+                        ub.start(i, v[0])
+                        ub.add_objects(i, objs[i])
+                    ub.step_tensor(ref_b)
+
+                    def ub_round(nsteps, ub=ub):
+                        ub.submit(steps_b[0])
+                        for t in range(nsteps):
+                            if t + 1 < nsteps:
+                                ub.submit(steps_b[(t + 1) % 4])
+                            ub.collect()
+
+                    def ub_replay(t, ub=ub):
+                        s = ub._ring.slots[t % 2]
+                        s.img_in_u8.copy_(steps_b[t % 4], non_blocking=True)
+                        s.graph.replay()
+                        shared_ops.vos_aggregate_batched([([s.vos_masks[k] for _, k in s.objs[i]], None, [o for o, _ in s.objs[i]], s.r[i], s.soft[i],
+                                                    s.seg[i]) for i in range(n)], H, W)
+                    ub_round(4)
+                    launches = ub.launches_per_frame + outside(lambda t, ub=ub: ub.step_tensor(steps_b[t % 4]))
+                    sides["batch"] = (ub_round, ub_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                    # ---- one UnicornUnifiedMaskTracker per video, stepped in turn
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    uts = []
+                    for i, v in enumerate(vs):
+                        ut = UnicornUnifiedMaskTracker(eng, (H, W), v[0], K, 1, mots=mots)
+                        ut.add_objects(objs[i])
+                        ut.step_tensor(v[2])
+                        uts.append(ut)
+
+                    def ut_round(nsteps, uts=uts):
+                        for i, ut in enumerate(uts):
+                            ut.submit(vs[i][3][0])
+                        for t in range(nsteps):
+                            for i, ut in enumerate(uts):
+                                if t + 1 < nsteps:
+                                    ut.submit(vs[i][3][(t + 1) % 4])
+                                ut.collect()
+
+                    def ut_replay(t, uts=uts):
+                        for i, ut in enumerate(uts):
+                            s = ut._ring.slots[t % 2]
+                            s.img_in_u8.copy_(vs[i][3][t % 4], non_blocking=True)
+                            s.graph.replay()
+                            ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], None, [o for o, _ in s.objs], H, W, ut.r, s.soft, s.seg)
+                    ut_round(4)
+
+                    def ut_step(t, uts=uts):
+                        for i, ut in enumerate(uts):
+                            ut.step_tensor(vs[i][3][t % 4])
+                    launches = sum(ut.launches_per_frame for ut in uts) + outside(ut_step)
+                    sides["trackers"] = (ut_round, ut_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                    # ---- UnicornVOSBatch over the videos plus UnicornMOTSBatch over the videos
+                    m0 = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    vb = UnicornVOSBatch(eng, (H, W), n, n * K, n)
+                    for i, v in enumerate(vs):
+                        vb.initialize_tensor(i, v[2], objs[i], orig_size=v[0], r=v[1])
+                    vb.track_tensor(steps_b[0])  # captures the graph
+                    mb, mots_launches = None, 0
+                    if mots:
+                        mb = UnicornMOTSBatch(eng, (H, W), n, use_graph=True)
+                        for i in range(n):
+                            mb.start(i)
+                        mb.step_tensor(ref_b, sizes)  # the first step runs eagerly: its launches are those its graphs replay
+                        mots_launches = mb.launches_per_frame
+
+                    def vm_round(nsteps, vb=vb, mb=mb):
+                        if mb:
+                            mb.submit(steps_b[0], sizes)
+                        for t in range(nsteps):
+                            vb.track_tensor(steps_b[t % 4])
+                            if mb and t + 1 < nsteps:
+                                mb.submit(steps_b[(t + 1) % 4], sizes)
+                            if mb:
+                                mb.collect()
+
+                    def vm_replay(t, vb=vb, mb=mb):
+                        vb.slot.img_in_u8.copy_(steps_b[t % 4], non_blocking=True)
+                        vb.slot.graph.replay()
+                        for sq in vb.seqs:
+                            ids = sq.obj_ids
+                            ops.vos_aggregate([vb.masks[sq.obj_slot[o]] for o in ids], None, ids, H, W, sq.r, sq.soft, sq.seg)
+                        if mb:
+                            c = mb._ctxs[t % 2]
+                            c.img_in_u8.copy_(steps_b[t % 4], non_blocking=True)
+                            c.graph.replay()
+                    vm_round(4)
+
+                    def vm_step(t, vb=vb, mb=mb):
+                        vb.track_tensor(steps_b[t % 4])
+                        if mb:
+                            mb.step_tensor(steps_b[t % 4], sizes)
+                    launches = vb.launches_per_frame + mots_launches + outside(vm_step)
+                    sides["vos_mots"] = (vm_round, vm_replay, launches, torch.cuda.max_memory_allocated() - m0)
+                    line = {"config": cfg, "size": [H, W], "origs": sizes, "n_seq": n, "objects": K, "mots": mots}
+                    line.update(compare(sides, args, e0, e1))
+                    for key in sides:
+                        line[key]["video_frames_per_s"] = round(1e3 * n / line[key]["ms_per_step"], 1)
+                    print(json.dumps(line), flush=True)
+                    del sides, ub, uts, vb, mb, ub_round, ub_replay, ut_round, ut_replay, ut_step, vm_round, vm_replay, vm_step
                     torch.cuda.empty_cache()
         del eng
         torch.cuda.empty_cache()

@@ -33,6 +33,11 @@ class UcVosObject(ctypes.Structure):
     _fields_ = [("mask", ctypes.c_void_p), ("init_mask", ctypes.c_void_p), ("id", ctypes.c_int)]
 
 
+class UcVosVideo(ctypes.Structure):
+    _fields_ = [("objs", ctypes.POINTER(UcVosObject)), ("n", ctypes.c_int), ("H", ctypes.c_int), ("W", ctypes.c_int), ("r", ctypes.c_float),
+                ("soft_out", ctypes.c_void_p), ("seg_out", ctypes.c_void_p)]
+
+
 _lib = None
 
 

@@ -217,20 +217,35 @@ __device__ __forceinline__ float resize_sample(const float* s, int ld, int y0, i
 // external/lib/test/tracker/unicorn_vos.py:129-155 (resize of every object's best mask to the original frame:
 // F.interpolate(scale_factor=1/r, bilinear, align_corners=False)[:H, :W] into a zero map) and :105-121 (soft aggregation:
 // background = prod_i (1 - m_i) in float32 in list order, argmax over [background, m_id...] with the lower channel winning
-// ties, label = object id).  One thread per original-frame pixel; the resized soft masks are optional outputs.
+// ties, label = object id).  One thread per original-frame pixel; the resized soft masks are optional outputs.  blockIdx.y selects
+// the video: every video has its own objects, original size, resize and outputs, the network resolution Hin x Win is shared.
 constexpr int kVosMaxObj = 16;
-struct VosObjs {
+constexpr int kVosMaxVideos = UC_VOS_MAX_VIDEOS;
+struct VosVideo {
   const float* mask[kVosMaxObj];       // network-resolution soft mask [Hin, Win] or nullptr
   const uint8_t* init_mask[kVosMaxObj];  // original-frame label map [H, W]: object = (label == id), or nullptr
-  int id[kVosMaxObj];
-  int by_id[kVosMaxObj];  // object indices in ascending id order (argmax tie-breaking)
+  float* soft;                         // [n, H, W] or nullptr
+  uint8_t* seg;                        // [H, W]
+  int H, W, hm, wm;                    // original frame, and the corner the resize covers
+  float scale;                         // source scale of the resize
   int n;
+  uint8_t id[kVosMaxObj];
+  uint8_t by_id[kVosMaxObj];  // object indices in ascending id order (argmax tie-breaking)
 };
+struct VosVideos {
+  VosVideo v[kVosMaxVideos];
+};
+// CUDA 12.1+ guarantees 32764 bytes of kernel parameters on sm_70 and later
+static_assert(sizeof(VosVideos) <= 32764, "the VOS descriptors must fit the kernel-parameter block");
 
-__global__ void __launch_bounds__(256) vos_aggregate_kernel(VosObjs o, int Hin, int Win, int H, int W, int hm, int wm, float scale,
-                                                             float* __restrict__ soft, uint8_t* __restrict__ seg) {
+__global__ void __launch_bounds__(256) vos_aggregate_kernel(const __grid_constant__ VosVideos vs, int Hin, int Win) {
   pdl_wait();
   pdl_launch_dependents();
+  const VosVideo& o = vs.v[blockIdx.y];
+  const int H = o.H, W = o.W, hm = o.hm, wm = o.wm;
+  const float scale = o.scale;
+  float* __restrict__ soft = o.soft;
+  uint8_t* __restrict__ seg = o.seg;
   const long total = static_cast<long>(H) * W;
   for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int x = static_cast<int>(i % W), y = static_cast<int>(i / W);
@@ -703,23 +718,49 @@ extern "C" int uc_dynamic_masks_batched(const float* mask_feats, const float* up
                        static_cast<cudaStream_t>(stream_v));
 }
 
+// The assembly of B videos in one launch (B = 1: uc_vos_aggregate).  Every argument is validated before any CUDA call, with errors
+// prefixed by `what`, and by the video when the call is batched.
+static int vos_aggregate(const char* what, bool batched, const UcVosVideo* videos, int B, int Hin, int Win, cudaStream_t stream) {
+  if (!videos) return set_error(UC_EINVAL, "%s: null pointer", what);
+  if (B < 1 || B > kVosMaxVideos) return set_error(UC_EINVAL, "%s: B = %d must be in 1..%d", what, B, kVosMaxVideos);
+  char at[96];
+  VosVideos vs;
+  memset(&vs, 0, sizeof(vs));
+  long total_max = 0;
+  for (int b = 0; b < B; ++b) {
+    if (batched) snprintf(at, sizeof(at), "%s: video %d", what, b);
+    else snprintf(at, sizeof(at), "%s", what);
+    const UcVosVideo& in = videos[b];
+    if (!in.objs || !in.seg_out || in.n < 1 || in.n > kVosMaxObj) return set_error(UC_EINVAL, "%s: 1..%d objects", at, kVosMaxObj);
+    if (Hin < 1 || Win < 1 || in.H < 1 || in.W < 1 || !(in.r > 0.f)) return set_error(UC_EINVAL, "%s: bad sizes", at);
+    VosVideo& o = vs.v[b];
+    o.n = in.n;
+    for (int k = 0; k < in.n; ++k) {
+      if (in.objs[k].id < 1 || in.objs[k].id > 255) return set_error(UC_EINVAL, "%s: object ids must be 1..255", at);
+      o.mask[k] = in.objs[k].mask; o.init_mask[k] = in.objs[k].init_mask; o.id[k] = static_cast<uint8_t>(in.objs[k].id);
+      o.by_id[k] = static_cast<uint8_t>(k);
+    }
+    std::stable_sort(o.by_id, o.by_id + in.n, [&](int a, int c) { return o.id[a] < o.id[c]; });
+    const FrameResize rs = frame_resize(Hin, Win, in.H, in.W, in.r);
+    o.H = in.H; o.W = in.W; o.hm = rs.hm; o.wm = rs.wm; o.scale = rs.scale;
+    o.soft = in.soft_out;
+    o.seg = in.seg_out;
+    total_max = std::max(total_max, static_cast<long>(in.H) * in.W);
+  }
+  // the x dimension stride-loops over the largest frame; a CTA past its own video's pixels does nothing
+  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total_max + 255) / 256, static_cast<long>(num_sms()) * 16)));
+  launch_pdl(vos_aggregate_kernel, dim3(grid, B), 256, 0, stream, vs, Hin, Win);
+  return check_launch(what);
+}
+
 extern "C" int uc_vos_aggregate(const UcVosObject* objs, int n, int Hin, int Win, int H, int W, float r, float* soft_out, uint8_t* seg_out,
                                 void* stream_v) {
-  if (!objs || !seg_out || n < 1 || n > kVosMaxObj) return set_error(UC_EINVAL, "uc_vos_aggregate: 1..%d objects", kVosMaxObj);
-  if (Hin < 1 || Win < 1 || H < 1 || W < 1 || !(r > 0.f)) return set_error(UC_EINVAL, "uc_vos_aggregate: bad sizes");
-  VosObjs o;
-  memset(&o, 0, sizeof(o));
-  o.n = n;
-  for (int k = 0; k < n; ++k) {
-    if (objs[k].id < 1 || objs[k].id > 255) return set_error(UC_EINVAL, "uc_vos_aggregate: object ids must be 1..255");
-    o.mask[k] = objs[k].mask; o.init_mask[k] = objs[k].init_mask; o.id[k] = objs[k].id; o.by_id[k] = k;
-  }
-  std::stable_sort(o.by_id, o.by_id + n, [&](int a, int b) { return o.id[a] < o.id[b]; });
-  const FrameResize rs = frame_resize(Hin, Win, H, W, r);
-  const long total = static_cast<long>(H) * W;
-  const int grid = static_cast<int>(std::max<long>(1, std::min<long>((total + 255) / 256, static_cast<long>(num_sms()) * 16)));
-  launch_pdl(vos_aggregate_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream_v), o, Hin, Win, H, W, rs.hm, rs.wm, rs.scale, soft_out, seg_out);
-  return check_launch("uc_vos_aggregate");
+  const UcVosVideo v{objs, n, H, W, r, soft_out, seg_out};
+  return vos_aggregate("uc_vos_aggregate", false, &v, 1, Hin, Win, static_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int uc_vos_aggregate_batched(const UcVosVideo* videos, int B, int Hin, int Win, void* stream_v) {
+  return vos_aggregate("uc_vos_aggregate_batched", true, videos, B, Hin, Win, static_cast<cudaStream_t>(stream_v));
 }
 
 // One encode over the instances of B images (B = 1: uc_mots_encode).  Every argument is validated before any CUDA call, with errors

@@ -554,9 +554,16 @@ def vos_aggregate(masks, init_mask, ids, Hin, Win, r, soft, seg):
     [>= n, H0, W0], and the label map seg uint8 [H0, W0] (argmax over the background product and the objects, in list order).
     masks: fp32 [1, Hin, Win] network-resolution masks of the first len(masks) ids; the remaining ids take (init_mask == id) of
     init_mask, a uint8 [H0, W0] label map."""
+    objs, n, H0, W0 = _vos_objects(masks, init_mask, ids, Hin, Win, soft, seg)
+    _lib.check(_L().uc_vos_aggregate(objs, n, Hin, Win, H0, W0, _f(r), _p(soft), _p(seg), _S()), "uc_vos_aggregate")
+    return seg
+
+
+def _vos_objects(masks, init_mask, ids, Hin, Win, soft, seg):
+    """The host object array of one video of vos_aggregate (soft may be None), with its object count and original size."""
     n = len(ids)
     H0, W0 = seg.shape
-    assert soft.dtype == torch.float32 and soft.is_contiguous() and soft.shape[0] >= n and tuple(soft.shape[1:]) == (H0, W0)
+    assert soft is None or (soft.dtype == torch.float32 and soft.is_contiguous() and soft.shape[0] >= n and tuple(soft.shape[1:]) == (H0, W0))
     assert seg.dtype == torch.uint8 and seg.is_contiguous() and len(masks) <= n
     objs = (_lib.UcVosObject * n)()
     for k, oid in enumerate(ids):
@@ -567,8 +574,7 @@ def vos_aggregate(masks, init_mask, ids, Hin, Win, r, soft, seg):
         else:
             assert init_mask is not None and init_mask.dtype == torch.uint8 and tuple(init_mask.shape) == (H0, W0)
             objs[k].init_mask = init_mask.data_ptr()
-    _lib.check(_L().uc_vos_aggregate(objs, n, Hin, Win, H0, W0, _f(r), _p(soft), _p(seg), _S()), "uc_vos_aggregate")
-    return seg
+    return objs, n, H0, W0
 
 
 def mots_encode_workspace(k_max, H, W, device):
