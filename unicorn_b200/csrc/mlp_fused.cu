@@ -17,7 +17,10 @@
 //   * C = 384: the 64 x 384 output accumulator does not fit a warpgroup's registers next to the hidden chunk, so the output columns
 //     are computed in two halves of 192, each walking all hidden chunks (GEMM1 and the GELU are evaluated twice);
 //   * after the last chunk the warpgroup adds b2 to its accumulator, multiplies by the layer scale, adds the shortcut and stores x
-//     in place — the same epilogue arithmetic and order as uc_conv2d's.
+//     in place — the same epilogue arithmetic and order as uc_conv2d's.  Every shortcut load of the tile is issued right before the
+//     last chunk's GEMM2 and ahead of the first store, so the loads run under that GEMM2: a load behind a store to the same map
+//     would wait for it, one memory round trip per 8-column group and row half.  b2 and the layer scale are read from a copy in
+//     shared memory.
 //   * the two consumer warpgroups share the weight rings and run independently otherwise, so one is in its GELU / LayerNorm while
 //     the other keeps the tensor core busy.
 //
@@ -47,7 +50,7 @@ struct MlpCfg {
   static constexpr int STEPS = NH * NCHUNK;             // weight chunks per row tile
   static constexpr int AS = C <= 192 ? 2 : 1;           // row-tile buffers (C >= 256 has room for one next to the weight rings)
   static constexpr int WS = C <= 256 ? 2 : 1;           // weight-ring stages
-  static constexpr int SMEM = AS * A_BYTES + WS * (W1_BYTES + W2_BYTES) + 1024 + 512;
+  static constexpr int SMEM = AS * A_BYTES + WS * (W1_BYTES + W2_BYTES) + 1024 + 512 + 2 * C * 4;  // + barriers, b2 / gamma
   static constexpr int CPT = C / 16;                    // 16-byte chunks of a row per LayerNorm thread (2 threads per row)
 };
 
@@ -73,6 +76,9 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
   uint8_t* sW1 = sA + Cfg::AS * Cfg::A_BYTES;         // [WS][KB][64 rows][128 B]
   uint8_t* sW2 = sW1 + Cfg::WS * Cfg::W1_BYTES;       // [WS][C rows][128 B]
   uint64_t* bar = reinterpret_cast<uint64_t*>(sW2 + Cfg::WS * Cfg::W2_BYTES);
+  // [C] b2, then [C] gamma; addressed from smem_raw so that the compiler reads them with LDS
+  float* sB2 = reinterpret_cast<float*>(smem_raw + (sW2 + Cfg::WS * Cfg::W2_BYTES + 512 - smem_raw));
+  float* sGm = sB2 + C;
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
@@ -89,9 +95,14 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
     }
     fence_barrier_init();
   }
-  __syncthreads();
   pdl_wait();
   pdl_launch_dependents();
+  static_assert(C <= kMlpThreads, "one b2 / gamma column per thread");
+  if (threadIdx.x < C) {
+    sB2[threadIdx.x] = p.b2[threadIdx.x];
+    sGm[threadIdx.x] = p.gamma[threadIdx.x];
+  }
+  __syncthreads();
 
   const int n_local = (p.m_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);  // row tiles of this CTA
   auto tile_of = [&](int i) { return static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x); };
@@ -192,6 +203,16 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
   const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(sA + c * 64 * 128)), w1_desc0 = wgmma_desc_sw128(smem_u32(sW1));
   const uint64_t w2_desc0 = wgmma_desc_sw128(smem_u32(sW2));
   float acc2[Cfg::N2 / 2];
+  uint32_t hf[4][4];  // GEMM2's A fragment: the bf16 hidden chunk
+  // ---- GEMM2 of weight step (ws, wph): output accumulator += H chunk . W2 chunk^T
+  auto gemm2 = [&](int j, int ws, int wph) {
+    mbar_wait(&bar[W2_FULL + ws], wph);
+    wgmma_fence();
+    const uint64_t bd2 = w2_desc0 + static_cast<uint64_t>((ws * Cfg::W2_BYTES) >> 4);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs_bf16<Cfg::N2>(acc2, hf[kk], bd2 + 2 * kk, (j | kk) != 0 ? 1u : 0u);
+    wgmma_commit();
+  };
   int g = 0;
   for (int i = 0; i < n_local; ++i) {
     const int ab = i % Cfg::AS;
@@ -199,8 +220,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
     layer_norm_tile(ab);
 #pragma unroll 1
    for (int nh = 0; nh < Cfg::NH; ++nh) {
-    for (int j = 0; j < Cfg::NCHUNK; ++j, ++g) {
-      const int ws = g % Cfg::WS, wph = (g / Cfg::WS) & 1;
+    int ws, wph;
+    for (int j = 0;; ++j, ++g) {
+      ws = g % Cfg::WS;
+      wph = (g / Cfg::WS) & 1;
       // ---- GEMM1: hidden chunk j of this warpgroup's 64 rows
       float acc1[kMlpHC / 2];
       mbar_wait(&bar[W1_FULL + ws], wph);
@@ -220,7 +243,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
         if (nh == Cfg::NH - 1 && j == Cfg::NCHUNK - 1) mbar_arrive(&bar[A_EMPTY + ab]);
       }
       // ---- + b1', GELU, bf16: accumulator columns 16 kk .. 16 kk + 15 are the A fragment of GEMM2's K step kk
-      uint32_t hf[4][4];
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
@@ -233,33 +255,41 @@ __global__ void __launch_bounds__(kMlpThreads, 1) convnext_mlp_kernel(const __gr
           hf[kk][2 * half + 1] = pack2_fast(lo2(h1), hi2(h1), false);
         }
       }
-      // ---- GEMM2: output accumulator += H chunk . W2 chunk^T
-      mbar_wait(&bar[W2_FULL + ws], wph);
-      wgmma_fence();
-      const uint64_t bd2 = w2_desc0 + static_cast<uint64_t>((ws * Cfg::W2_BYTES) >> 4);
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wgmma_rs_bf16<Cfg::N2>(acc2, hf[kk], bd2 + 2 * kk, (j | kk) != 0 ? 1u : 0u);
-      wgmma_commit();
+      if (j == Cfg::NCHUNK - 1) break;  // the last chunk's GEMM2 is issued below, behind the shortcut loads
+      gemm2(j, ws, wph);
       wgmma_wait<0>();
       wgmma_fence_regs(acc2);
       if (ct == 0) mbar_arrive(&bar[W2_EMPTY + ws]);
     }
-    // ---- output columns nh * N2 .. : x += gamma * (acc2 + b2)
+    // ---- output columns nh * N2 .. : x += gamma * (acc2 + b2).  The shortcut words of both row halves of every 8-column group
+    // are loaded first, all of them before the first store (rows past M are neither read nor written), and run under the last
+    // chunk's GEMM2.  They are issued ahead of it, not behind it: a register written while an RS wgmma is in flight may be one
+    // of hf's, and ptxas then waits for the wgmma before the write.
     const long grow0 = static_cast<long>(tile_of(i)) * kMlpRows + c * 64 + rl;
+    uint32_t* xr = reinterpret_cast<uint32_t*>(p.x + grow0 * C + nh * Cfg::N2 + 2 * t);
+    const bool in0 = grow0 < p.M, in1 = grow0 + 8 < p.M;
+    uint32_t rw[Cfg::N2 / 4];
+#pragma unroll
+    for (int i8 = 0; i8 < Cfg::N2 / 8; ++i8) {
+      rw[2 * i8] = in0 ? xr[4 * i8] : 0u;
+      rw[2 * i8 + 1] = in1 ? xr[4 * i8 + 4 * C] : 0u;
+    }
+    gemm2(Cfg::NCHUNK - 1, ws, wph);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc2);
+    if (ct == 0) mbar_arrive(&bar[W2_EMPTY + ws]);
+    ++g;
 #pragma unroll
     for (int i8 = 0; i8 < Cfg::N2 / 8; ++i8) {
       const int col = nh * Cfg::N2 + 8 * i8 + 2 * t;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(p.b2 + col)), gm = __ldg(reinterpret_cast<const float2*>(p.gamma + col));
+      const float2 b = *reinterpret_cast<const float2*>(sB2 + col), gm = *reinterpret_cast<const float2*>(sGm + col);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const long grow = grow0 + 8 * h;
-        if (grow < p.M) {
-          uint32_t* xp = reinterpret_cast<uint32_t*>(p.x + grow * C + col);
-          const uint32_t rw = *xp;
+        if (h == 0 ? in0 : in1) {
           f32x2 v = add2(pk2(acc2[4 * i8 + 2 * h], acc2[4 * i8 + 2 * h + 1]), pk2(b.x, b.y));
           v = mul2(v, pk2(gm.x, gm.y));
-          v = add2(v, pk2(bf16lo(rw), bf16hi(rw)));
-          *xp = pack2_fast(lo2(v), hi2(v), false);
+          v = add2(v, pk2(bf16lo(rw[2 * i8 + h]), bf16hi(rw[2 * i8 + h])));
+          xr[4 * i8 + 4 * C * h] = pack2_fast(lo2(v), hi2(v), false);
         }
       }
     }
