@@ -253,7 +253,10 @@ UC_API int uc_head_decode_batched(const float* const* regobj, const float* const
  * many boxes are kept: the rows returned are exactly the first max_keep rows of the full result (the SOT driver only
  * consumes output[:max_inst], external/lib/test/tracker/unicorn_sot.py:69-70); max_keep <= 0 = no limit.
  * out_anchor (device int[A], may be NULL) receives the anchor index of every returned row — what postprocess_inst
- * (utils/boxes.py:125-128) needs to pick each instance's location / dynamic parameters / FPN level. */
+ * (utils/boxes.py:125-128) needs to pick each instance's location / dynamic parameters / FPN level.
+ * Decisions are pinned bit for bit: a row passes when rn(obj * cls_conf) >= conf_thre (cls_conf the first maximum), and the
+ * NMS of each class equals torchvision.ops.nms on CUDA (devIoU: union = fmaf(w_later, h_later, area_earlier) - inter, IEEE
+ * divide, IoU > (float)nms_thre suppresses), rows of equal score in ascending candidate order. */
 UC_API long uc_postprocess_workspace_bytes(int max_anchors);
 UC_API int uc_postprocess(const float* pred, int A, int ncls, float conf_thre, float nms_thre, int max_keep, void* workspace,
                           long workspace_bytes, float* out_dets, int* out_count, int* out_anchor, void* stream);
@@ -304,7 +307,8 @@ UC_API int uc_qd_assign(const float* scores, int N, int M, const long long* memo
                         float obj_thr, float nms_conf_thr, long long* ids_out, uint8_t* taken_ws, void* stream);
 /* Pairwise IoU out[i,j] of xyxy f32 boxes with row strides.  plus_one = 0: torchvision.ops.box_iou
  * (quasi_dense_embed_tracker.py:80,146); plus_one = 1: cython_bbox.bbox_overlaps' inclusive-pixel convention
- * (unicorn/tracker/matching.py:65-68, ByteTrack). */
+ * (unicorn/tracker/matching.py:65-68, ByteTrack).  Every fp32 step is rounded on its own (no fused multiply-add), so
+ * plus_one = 0 equals torchvision.ops.box_iou bit for bit; plus_one = 1 is that order in fp32 where bbox_overlaps uses float64. */
 UC_API int uc_box_iou(const float* a, int lda, int N, const float* b, int ldb, int M, float* out, int plus_one, void* stream);
 
 /* dst += aligned_bilinear(src, factor) on NHWC bf16 maps (condinst/comm.py:5-27; mask_branch.py:81-96). */

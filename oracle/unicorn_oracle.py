@@ -8,8 +8,10 @@ Parity status: PINNED against the reference's own modules, imported in the build
 (oracle/ref_import.py) — tests/golden/make_golden.py runs both on the same seeded weights/inputs and
 tests/test_oracle_golden.py re-checks this file against the committed outputs on any machine.
 The MSDA core is additionally pinned to the reference's only known-answer test (unicorn/models/ops/test.py:21-56,
-seed 3 shapes) through ms_deform_attn_core_pytorch.  Unpinned: torchvision batched_nms tie-breaking (version
-unpinned upstream) — restated here as greedy per-class NMS and cross-checked against torchvision 0.26.
+seed 3 shapes) through ms_deform_attn_core_pytorch.  NMS is restated as stable greedy per-class NMS on an exact numpy
+emulation of torchvision's CUDA devIoU (fused union, float32 threshold), checked against torchvision.ops.nms on CUDA
+(torchvision 0.26) at near-threshold pairs; equal scores are visited in ascending index, which torchvision does not
+promise across versions.
 
 Every function cites the reference file:line it follows (paths relative to the reference repo root).
 """
@@ -308,23 +310,67 @@ def box_iou_np(a, b):
     return inter / (area_a[:, None] + area_b[None, :] - inter)
 
 
+def fma32(a, b, c):
+    """fmaf(a, b, c) of float32 arrays: a * b + c rounded once to float32.  The float64 product of two floats is exact; the
+    float64 sum s is off by e (TwoSum: s + e == a * b + c exactly), which changes the float32 rounding only when s is a float32
+    midpoint, where the exact sum lies on the side of e."""
+    a, b, c = (np.asarray(v, dtype=np.float32).astype(np.float64) for v in (a, b, c))
+    p = a * b
+    s = p + c
+    t = s - p
+    e = (p - (s - t)) + (c - t)
+    r = s.astype(np.float32)
+    r64 = r.astype(np.float64)
+    up = s > r64
+    other = np.nextafter(r, np.where(up, np.float32(np.inf), np.float32(-np.inf)))
+    mid = (s != r64) & ((r64 + other.astype(np.float64)) * 0.5 == s)
+    return np.where(mid & (e != 0) & ((e > 0) == up), other, r)
+
+
+def dev_iou(a, b):
+    """IoU of boxes a (earlier in the score order) and b (later), xyxy float32 [..., 4], broadcast: torchvision's CUDA devIoU
+    (csrc/ops/cuda/nms_kernel.cu) as nvcc compiles it: rounded widths, heights, intersection and a's area, b's area fused into
+    the union, union = fmaf(wb, hb, area_a) - inter, an IEEE divide."""
+    f = np.float32
+    a, b = np.asarray(a, dtype=f), np.asarray(b, dtype=f)
+    w = np.maximum(np.minimum(a[..., 2], b[..., 2]) - np.maximum(a[..., 0], b[..., 0]), f(0))
+    h = np.maximum(np.minimum(a[..., 3], b[..., 3]) - np.maximum(a[..., 1], b[..., 1]), f(0))
+    inter = w * h
+    sa = (a[..., 2] - a[..., 0]) * (a[..., 3] - a[..., 1])
+    union = fma32(b[..., 2] - b[..., 0], b[..., 3] - b[..., 1], sa) - inter
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return inter / union
+
+
+def box_iou_f32(a, b, plus_one=False):
+    """[N, M] IoU with every float32 step rounded on its own: torchvision.ops.box_iou's separate torch ops (plus_one=False),
+    and the same order with + 1 after each difference, the inclusive-pixel convention of cython_bbox.bbox_overlaps."""
+    f = np.float32
+    a, b = np.asarray(a, dtype=f), np.asarray(b, dtype=f)
+    one = f(1) if plus_one else f(0)
+    area_a = ((a[:, 2] - a[:, 0]) + one) * ((a[:, 3] - a[:, 1]) + one)
+    area_b = ((b[:, 2] - b[:, 0]) + one) * ((b[:, 3] - b[:, 1]) + one)
+    lt = np.maximum(a[:, None, :2], b[None, :, :2])
+    rb = np.minimum(a[:, None, 2:], b[None, :, 2:])
+    wh = np.maximum((rb - lt) + one, f(0))
+    inter = wh[..., 0] * wh[..., 1]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return inter / ((area_a[:, None] + area_b[None, :]) - inter)
+
+
 def nms_greedy(boxes, scores, thr):
-    """torchvision.ops.nms semantics: visit in descending score (stable), suppress IoU > thr. fp32 arithmetic."""
+    """torchvision.ops.nms on CUDA: visit in descending score (equal scores in ascending index), a kept box suppresses every
+    later box with dev_iou(kept, later) > float32(thr)."""
     boxes = np.asarray(boxes, dtype=np.float32)
     order = np.argsort(-np.asarray(scores, dtype=np.float32), kind="stable")
+    thr = np.float32(thr)
     keep = []
     suppressed = np.zeros(len(order), dtype=bool)
-    areas = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1])
     for ii, i in enumerate(order):
         if suppressed[ii]:
             continue
         keep.append(i)
-        rest = order[ii + 1:]
-        xx1 = np.maximum(boxes[i, 0], boxes[rest, 0]); yy1 = np.maximum(boxes[i, 1], boxes[rest, 1])
-        xx2 = np.minimum(boxes[i, 2], boxes[rest, 2]); yy2 = np.minimum(boxes[i, 3], boxes[rest, 3])
-        inter = np.clip(xx2 - xx1, 0, None).astype(np.float32) * np.clip(yy2 - yy1, 0, None).astype(np.float32)
-        iou = inter / (areas[i] + areas[rest] - inter)
-        suppressed[ii + 1:] |= iou > thr
+        suppressed[ii + 1:] |= dev_iou(boxes[i], boxes[order[ii + 1:]]) > thr
     return np.asarray(keep, dtype=np.int64)
 
 

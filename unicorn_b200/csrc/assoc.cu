@@ -97,7 +97,10 @@ __global__ void __launch_bounds__(256) bisoftmax_kernel(const float* __restrict_
 }
 
 // plus1 = 0: torchvision.ops.box_iou; plus1 = 1: cython_bbox.bbox_overlaps (inclusive-pixel convention used by ByteTrack,
-// unicorn/tracker/matching.py:65-68)
+// unicorn/tracker/matching.py:65-68).  Every step is rounded on its own, as torchvision's separate torch ops are
+// (union = rn(rn(area1 + area2) - inter)): the _rn intrinsics keep nvcc from fusing an area's product into the union, so
+// plus1 = 0 equals torchvision.ops.box_iou bit for bit.  plus1 = 1 is the same order with the + 1 after each difference;
+// bbox_overlaps computes in float64.
 __global__ void __launch_bounds__(256) box_iou_kernel(const float* __restrict__ a, int lda, int N, const float* __restrict__ b, int ldb,
                                                        int M, float* __restrict__ out, float plus1) {
   pdl_wait();               // programmatic dependent launch: global memory is touched only after the predecessor completed
@@ -106,10 +109,12 @@ __global__ void __launch_bounds__(256) box_iou_kernel(const float* __restrict__ 
   if (t >= static_cast<long>(N) * M) return;
   const float* p = a + (t / M) * lda;
   const float* q = b + (t % M) * ldb;
-  const float area1 = (p[2] - p[0] + plus1) * (p[3] - p[1] + plus1), area2 = (q[2] - q[0] + plus1) * (q[3] - q[1] + plus1);
-  const float w = fmaxf(fminf(p[2], q[2]) - fmaxf(p[0], q[0]) + plus1, 0.f), h = fmaxf(fminf(p[3], q[3]) - fmaxf(p[1], q[1]) + plus1, 0.f);
-  const float inter = w * h;
-  out[t] = inter / (area1 + area2 - inter);
+  const float area1 = __fmul_rn(__fadd_rn(__fsub_rn(p[2], p[0]), plus1), __fadd_rn(__fsub_rn(p[3], p[1]), plus1));
+  const float area2 = __fmul_rn(__fadd_rn(__fsub_rn(q[2], q[0]), plus1), __fadd_rn(__fsub_rn(q[3], q[1]), plus1));
+  const float w = fmaxf(__fadd_rn(__fsub_rn(fminf(p[2], q[2]), fmaxf(p[0], q[0])), plus1), 0.f);
+  const float h = fmaxf(__fadd_rn(__fsub_rn(fminf(p[3], q[3]), fmaxf(p[1], q[1])), plus1), 0.f);
+  const float inter = __fmul_rn(w, h);
+  out[t] = __fdiv_rn(inter, __fsub_rn(__fadd_rn(area1, area2), inter));
 }
 
 

@@ -5,8 +5,11 @@
 //                    only within the same class), result ordered by descending score.
 //   uc_det_candidates_batched   the decode + filter of the two above fused, read straight from the per-level head maps
 //   UC_POST_CLASS_AGNOSTIC      postprocess(..., class_agnostic=True): torchvision.ops.nms over all classes
-// Everything stays on the GPU; the host reads back one counter.  Decision arithmetic is fp32 in the reference's
-// operation order so that thresholds flip only on exact ties.
+// Everything stays on the GPU; the host reads back one counter.  Decision arithmetic is fp32 with the reference's roundings:
+// the score filter is rn(obj * class_conf) >= conf (first maximum over classes), and NMS is torchvision's CUDA devIoU with
+// the later box's area fused into the union (nms_hit), so kept sets, order and count equal torchvision.ops.nms on CUDA
+// bit for bit (class-aware: per class), equal scores kept in ascending candidate order.  Not matched: torchvision's CPU nms,
+// which compares in double, and the class offsets batched_nms adds on CUDA up to 5000 boxes, which re-round the IoU.
 #include "uc_common.h"
 #include "../../include/unicorn_b200.h"
 #include <algorithm>
@@ -290,17 +293,23 @@ __global__ void __launch_bounds__(256) det_gather_kernel(PostSlices sl) {
 //  3. one warp resolves the chunk greedily, jumping from survivor to survivor with ffs;
 //  4. the newly kept boxes are appended to the kept list (shared memory, spilling to the output rows in global).
 // Work ~ N x kept IoUs instead of N^2, and the sequential part is proportional to the number of kept boxes.
-// IoU arithmetic is torchvision's devIoU (fp32, inter / (areaA + areaB - inter) > thr), same-class pairs only (class-aware variant).
+// IoU arithmetic is torchvision's CUDA devIoU, same-class pairs only (class-aware variant); see nms_hit for its rounding.
 constexpr int kNmsChunk = 256;
 constexpr int kNmsKeepSmem = 3072;
 
+// IoU(a, b) > thr of an earlier box a (higher in the score order) and a later box b, rounded as torchvision's CUDA devIoU is
+// compiled: widths, heights, the intersection and a's area are rounded products, b's area is fused into the union
+// (union = fmaf(wb, hb, area_a) - inter), an IEEE divide and a float compare.  The _rn intrinsics pin that order: with plain
+// operators nvcc picks which area it fuses (per call site, after hoisting), and a one-ulp difference in the union flips pairs
+// within an ulp of the threshold.
 __device__ __forceinline__ bool nms_hit(const float4 a, const float4 b, float thr) {
   const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
   const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-  const float w = fmaxf(xx2 - xx1, 0.f), h = fmaxf(yy2 - yy1, 0.f);
-  const float inter = w * h;
-  const float sa = (a.z - a.x) * (a.w - a.y), sb = (b.z - b.x) * (b.w - b.y);
-  return inter / (sa + sb - inter) > thr;
+  const float w = fmaxf(__fsub_rn(xx2, xx1), 0.f), h = fmaxf(__fsub_rn(yy2, yy1), 0.f);
+  const float inter = __fmul_rn(w, h);
+  const float sa = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
+  const float uni = __fsub_rn(__fmaf_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y), sa), inter);
+  return __fdiv_rn(inter, uni) > thr;
 }
 
 // kAgnostic: every pair is tested, whatever the classes (torchvision.ops.nms of postprocess(..., class_agnostic=True)).
