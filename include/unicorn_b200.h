@@ -191,6 +191,12 @@ UC_API int uc_bilinear_f32(const float* src, float* dst, int P, int Hs, int Ws, 
  * OpenCV's 8-bit fixed-point bilinear —, the rest = pad (114); swap_rb does cv2.COLOR_RGB2BGR.  uint8 HWC, 3 channels. */
 UC_API int uc_letterbox_u8(const uint8_t* src_hwc, int Hs, int Ws, uint8_t* dst_hwc, int Hd, int Wd, int rh, int rw,
                            int swap_rb, int pad, void* stream);
+/* uc_letterbox_u8's output (swap_rb = 1) for the BGR frame cv2.cvtColor(COLOR_YUV2BGR_NV12) makes of an NV12 frame (BT.601 limited
+ * range, OpenCV's 20-bit fixed point), bit-exact, without storing that frame: y = the Hs x Ws luma plane, uv = the interleaved
+ * Hs/2 x Ws chroma plane (U, V pairs), both with row pitch ld >= Ws bytes (decoder surfaces: the planes may be apart).  Hs, Ws even;
+ * 1 <= rh <= Hd, 1 <= rw <= Wd; 0 <= pad <= 255.  BGR uint8 HWC out, top-left placement. */
+UC_API int uc_letterbox_nv12(const uint8_t* y, const uint8_t* uv, int ld, int Hs, int Ws, uint8_t* dst_hwc, int Hd, int Wd, int rh,
+                             int rw, int pad, void* stream);
 /* y = a + b on 16-bit (UC_BF16 / UC_F16) rows; C and the strides multiples of 8; a, b and y 16-byte aligned. */
 UC_API int uc_add(const void* a, int lda, const void* b, int ldb, void* y, int ldy, long M, int C, int dtype, void* stream);
 /* Conditional strided row copy decided on the device: rows are copied when (*flag_dev != 0) != invert.  The MOT drivers use it for

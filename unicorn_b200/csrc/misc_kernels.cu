@@ -95,6 +95,11 @@ __device__ __forceinline__ void resize_axis(int d, double scale, int ssize, bool
   s1 = min(max(s + 1, 0), ssize - 1);
 }
 
+// Vertical pass of OpenCV's 8-bit bilinear on the horizontal sums h0 (row sy0) and h1 (row sy1).
+__device__ __forceinline__ int resize_vert(int h0, int h1, int b0, int b1) {
+  return (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+}
+
 __global__ void __launch_bounds__(256) letterbox_u8_kernel(const uint8_t* __restrict__ src, int Hs, int Ws, uint8_t* __restrict__ dst, int Hd,
                                                             int Wd, int rh, int rw, double scale_y, double scale_x, int swap_rb, int pad) {
   pdl_wait();
@@ -113,9 +118,52 @@ __global__ void __launch_bounds__(256) letterbox_u8_kernel(const uint8_t* __rest
       for (int c = 0; c < 3; ++c) {
         const int h0 = r0[sx0 * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
         const int h1 = r1[sx0 * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
-        const int v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-        o[swap_rb ? 2 - c : c] = static_cast<uint8_t>(v);
+        o[swap_rb ? 2 - c : c] = static_cast<uint8_t>(resize_vert(h0, h1, b0, b1));
       }
+    }
+    uint8_t* d = dst + i * 3;
+    d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
+  }
+}
+
+// NV12 -> BGR as cv2.cvtColor(COLOR_YUV2BGR_NV12) computes it (OpenCV 4.x imgproc/src/color_yuv.simd.hpp: BT.601 limited range in
+// 20-bit fixed point): Y' = max(0, Y - 16) * 1220542, u = U - 128, v = V - 128,
+//   R = (Y' + 1673527 v + 2^19) >> 20,  G = (Y' - 852492 v - 409993 u + 2^19) >> 20,  B = (Y' + 2116026 u + 2^19) >> 20, each
+// clamped to 0..255; chroma is nearest, the UV pair of pixel (r, c) is at row r >> 1, column c & ~1 of the interleaved plane.
+__device__ __forceinline__ void nv12_bgr(const uint8_t* __restrict__ y, const uint8_t* __restrict__ uv, int ld, int r, int c, int bgr[3]) {
+  const int yy = max(0, static_cast<int>(__ldg(y + static_cast<long>(r) * ld + c)) - 16) * 1220542;
+  const uint8_t* p = uv + static_cast<long>(r >> 1) * ld + (c & ~1);
+  const int u = static_cast<int>(__ldg(p)) - 128, v = static_cast<int>(__ldg(p + 1)) - 128;
+  constexpr int half = 1 << 19;
+  bgr[0] = min(max((yy + 2116026 * u + half) >> 20, 0), 255);
+  bgr[1] = min(max((yy - 852492 * v - 409993 * u + half) >> 20, 0), 255);
+  bgr[2] = min(max((yy + 1673527 * v + half) >> 20, 0), 255);
+}
+
+// letterbox_u8_kernel's output (swap_rb) for the BGR frame cv2.cvtColor(COLOR_YUV2BGR_NV12) makes of an NV12 frame: the four bilinear
+// taps are converted to BGR in registers, so the BGR frame is never stored.  Y plane `y` and interleaved UV plane `uv` share the row
+// pitch ld (bytes), so pitched decoder surfaces with padding rows between the planes are read in place.
+__global__ void __launch_bounds__(256) letterbox_nv12_kernel(const uint8_t* __restrict__ y, const uint8_t* __restrict__ uv, int ld, int Hs,
+                                                              int Ws, uint8_t* __restrict__ dst, int Hd, int Wd, int rh, int rw,
+                                                              double scale_y, double scale_x, int pad) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long total = static_cast<long>(Hd) * Wd;
+  for (long i = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
+    const int x = static_cast<int>(i % Wd), yo = static_cast<int>(i / Wd);
+    uint8_t o[3] = {static_cast<uint8_t>(pad), static_cast<uint8_t>(pad), static_cast<uint8_t>(pad)};
+    if (x < rw && yo < rh) {
+      int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
+      resize_axis(x, scale_x, Ws, true, sx0, sx1, a0, a1);
+      resize_axis(yo, scale_y, Hs, false, sy0, sy1, b0, b1);
+      int p00[3], p01[3], p10[3], p11[3];
+      nv12_bgr(y, uv, ld, sy0, sx0, p00);
+      nv12_bgr(y, uv, ld, sy0, sx1, p01);
+      nv12_bgr(y, uv, ld, sy1, sx0, p10);
+      nv12_bgr(y, uv, ld, sy1, sx1, p11);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        o[c] = static_cast<uint8_t>(resize_vert(p00[c] * a0 + p01[c] * a1, p10[c] * a0 + p11[c] * a1, b0, b1));
     }
     uint8_t* d = dst + i * 3;
     d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
@@ -257,6 +305,19 @@ extern "C" int uc_letterbox_u8(const uint8_t* src_hwc, int Hs, int Ws, uint8_t* 
   launch_pdl(letterbox_u8_kernel, grid_for(static_cast<long>(Hd) * Wd), 256, 0, static_cast<cudaStream_t>(stream_v), src_hwc, Hs, Ws, dst_hwc,
              Hd, Wd, rh, rw, scale_y, scale_x, swap_rb, pad);
   return check_launch("uc_letterbox_u8");
+}
+
+extern "C" int uc_letterbox_nv12(const uint8_t* y, const uint8_t* uv, int ld, int Hs, int Ws, uint8_t* dst_hwc, int Hd, int Wd, int rh,
+                                 int rw, int pad, void* stream_v) {
+  if (!y || !uv || !dst_hwc) return set_error(UC_EINVAL, "uc_letterbox_nv12: null plane or destination");
+  if (Hs < 2 || Ws < 2 || Hs % 2 || Ws % 2) return set_error(UC_EINVAL, "uc_letterbox_nv12: Hs and Ws must be even and >= 2");
+  if (ld < Ws) return set_error(UC_EINVAL, "uc_letterbox_nv12: row pitch ld must be >= Ws");
+  if (rh < 1 || rw < 1 || rh > Hd || rw > Wd) return set_error(UC_EINVAL, "uc_letterbox_nv12: rh, rw must be in 1..Hd, 1..Wd");
+  if (pad < 0 || pad > 255) return set_error(UC_EINVAL, "uc_letterbox_nv12: pad must be in 0..255");
+  const double scale_x = 1.0 / (static_cast<double>(rw) / Ws), scale_y = 1.0 / (static_cast<double>(rh) / Hs);
+  launch_pdl(letterbox_nv12_kernel, grid_for(static_cast<long>(Hd) * Wd), 256, 0, static_cast<cudaStream_t>(stream_v), y, uv, ld, Hs, Ws,
+             dst_hwc, Hd, Wd, rh, rw, scale_y, scale_x, pad);
+  return check_launch("uc_letterbox_nv12");
 }
 
 extern "C" int uc_add(const void* a, int lda, const void* b, int ldb, void* y, int ldy, long M, int C, int dtype, void* stream_v) {

@@ -7,10 +7,11 @@ image), so each image's rows are those of its own one-image run.  The rows are i
 unicorn_b200.results.coco_detections turns them into the evaluator's COCO dicts."""
 import torch
 
-from . import _lib, ops, post_ops
+from . import _lib, post_ops
 from .engine import STRIDES, UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count, in_flight
 from .mots import MaskEncoder
+from .sot import letterbox_frame, nv12_size
 
 
 class UnicornDetector:
@@ -54,28 +55,28 @@ class UnicornDetector:
         return fpn
 
     def submit(self, images, rgb=False):
-        """images: list of 1..max_batch uint8 HWC images (numpy arrays or tensors, host or device), BGR as cv2 loads them (rgb=True:
-        RGB).  Enqueues the step; returns immediately."""
+        """images: list of 1..max_batch images (numpy arrays or tensors, host or device): uint8 HWC, BGR as cv2 loads them (rgb=True:
+        RGB), or NV12 uint8 [3h/2, w], which always gives BGR (sot.letterbox_frame); the two may be mixed.  Enqueues the step; returns
+        immediately."""
         n = len(images)
         if not 1 <= n <= self.max_batch:
             raise ValueError(f"UnicornDetector: 1..{self.max_batch} images per step (got {n})")
         srcs = []
         for im in images:
             t = torch.as_tensor(im)
-            if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
+            if nv12_size(t) is None and (t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3):
                 raise ValueError(f"UnicornDetector: images must be uint8 [h, w, 3], got {tuple(t.shape)} {t.dtype}")
             srcs.append(t)
         c = self._ring.submit()
         if c.stream is not None:
             c.stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(c.stream):
-            c.ratios = []
+            c.ratios, c.sizes = [], []
             c.n = n
-            c.sizes = [(int(t.shape[0]), int(t.shape[1])) for t in srcs]
             for i, t in enumerate(srcs):
-                src = t.to(c.eng.dev, non_blocking=True).contiguous()
-                c.last[i] = src  # the upload stays alive until the step is collected
-                c.ratios.append(ops.letterbox_u8(src, self.input_size, swap_rb=rgb, out=c.img_in_u8[i:i + 1])[1])
+                _, r, size = letterbox_frame(t, self.input_size, c.eng.dev, device_out=c.img_in_u8[i:i + 1], device_preproc=True, rgb=rgb)
+                c.ratios.append(r)
+                c.sizes.append(size)
             if c.graph is not None:
                 c.graph.replay()
             elif self.use_graph:
@@ -98,7 +99,6 @@ class UnicornDetector:
         c.event.synchronize()
         dets = c.ws.dets.view(self.max_batch, self.A, 7)
         out = [(dets[i, :int(c.count_host[i])].cpu(), c.ratios[i]) for i in range(c.n)]
-        c.last.clear()
         return out
 
     def detect(self, images, rgb=False):
@@ -158,7 +158,6 @@ class UnicornInstanceSegmenter(UnicornDetector):
             rles = c.rows.strings(counts, c.mf, c.um, c.dyn, c.ws, c.ratios, c.sizes)
         dets = c.ws.dets.view(self.max_batch, self.A, 7)
         out = [(dets[i, :counts[i]].cpu(), c.ratios[i], rles[i]) for i in range(c.n)]
-        c.last.clear()
         return out
 
 

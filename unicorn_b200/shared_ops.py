@@ -1,8 +1,9 @@
-"""Wrappers of uc_groupnorm_apply_gather, the stem of UnicornEngine.head_shared, and of uc_vos_aggregate_batched, the result
-assembly of UnicornUnifiedMaskBatch (include/unicorn_b200.h).  They sit next to unicorn_b200.ops rather than in it because every
-launcher of ops has a per-launch fp32 reference in the tracking-frame launch check (tests/test_launch_parity_gpu.py); these are
-pinned bit for bit to their B = 1 launches instead: ops.groupnorm_apply (tests/test_unified_gpu.py, tests/test_unified_batch_gpu.py)
-and ops.vos_aggregate (tests/test_unified_mask_batch_gpu.py)."""
+"""Wrappers of uc_groupnorm_apply_gather, the stem of UnicornEngine.head_shared, of uc_vos_aggregate_batched, the result
+assembly of UnicornUnifiedMaskBatch, and of uc_letterbox_nv12, the letterbox of NV12 frames (include/unicorn_b200.h).  They sit next
+to unicorn_b200.ops rather than in it because every launcher of ops has a per-launch fp32 reference in the tracking-frame launch check
+(tests/test_launch_parity_gpu.py); these are pinned bit for bit instead: to their B = 1 launches, ops.groupnorm_apply
+(tests/test_unified_gpu.py, tests/test_unified_batch_gpu.py) and ops.vos_aggregate (tests/test_unified_mask_batch_gpu.py), and to
+cv2's conversion followed by the reference's letterbox (tests/test_nv12_gpu.py)."""
 import ctypes
 
 import torch
@@ -43,3 +44,27 @@ def vos_aggregate_batched(videos, Hin, Win):
         descs[b].soft_out, descs[b].seg_out = _p(soft), _p(seg)
     _lib.check(_L().uc_vos_aggregate_batched(descs, B, Hin, Win, _S()), "uc_vos_aggregate_batched")
     return [v[5] for v in videos]
+
+
+def letterbox_nv12(src, input_size, pad=114, out=None):
+    """src: NV12 uint8 [3h/2, w] CUDA tensor (h rows of Y, then h/2 rows of interleaved U, V; unit column stride, any row stride
+    >= w, so a view of a wider decoder surface works) -> (uint8 [1,H,W,3] letterboxed frame, r): ops.letterbox_u8's output, with r and
+    the resized size computed as it computes them, for the BGR frame cv2.cvtColor(COLOR_YUV2BGR_NV12) makes of src."""
+    if not torch.is_tensor(src) or src.dtype != torch.uint8 or src.dim() != 2 or src.shape[0] < 3 or src.shape[0] % 3 or src.shape[1] < 1:
+        raise ValueError(f"letterbox_nv12: src must be an NV12 uint8 [3h/2, w] tensor, got {getattr(src, 'shape', type(src))} "
+                         f"{getattr(src, 'dtype', '')}")
+    if src.stride(1) != 1 or src.stride(0) < src.shape[1] or not src.is_cuda:
+        raise ValueError(f"letterbox_nv12: src must be a CUDA tensor with unit column stride and a row stride >= w, got {src.device}, "
+                         f"strides {src.stride()}")
+    h, w = src.shape[0] * 2 // 3, src.shape[1]
+    H, W = input_size
+    r = min(H / h, W / w)
+    if out is None:
+        out = torch.empty(1, H, W, 3, dtype=torch.uint8, device=src.device)
+    if out.dtype != torch.uint8 or tuple(out.shape) != (1, H, W, 3) or not out.is_contiguous() or out.device != src.device:
+        raise ValueError(f"letterbox_nv12: out must be a contiguous uint8 [1, {H}, {W}, 3] tensor on {src.device}, got "
+                         f"{tuple(out.shape)} {out.dtype} on {out.device}")
+    ld = src.stride(0)
+    _lib.check(_L().uc_letterbox_nv12(_p(src), ctypes.c_void_p(src.data_ptr() + h * ld), ld, h, w, _p(out), H, W, int(h * r), int(w * r),
+                                      int(pad), _S()), "uc_letterbox_nv12")
+    return out, r

@@ -10,7 +10,7 @@ UnicornSOTBatch is the driver: `n_seq` sequences in lock step, one batched frame
 UnicornSOTTrack is its n_seq = 1 case under the reference's one-sequence protocol."""
 import torch
 
-from . import ops
+from . import ops, shared_ops
 from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, in_flight
 
@@ -38,6 +38,84 @@ def preprocess(img_rgb, input_size, out=None):
     out.fill_(114)
     out[0, :int(height * r), :int(width * r)] = torch.from_numpy(rsz)
     return out, r
+
+
+def nv12_size(image):
+    """(h, w) of a 2-D frame, which is NV12: uint8 [3h/2, w] (numpy array or tensor), h rows of luma then h/2 rows of interleaved
+    U, V, with h and w even.  None for a frame that is not 2-D (an RGB frame, checked by the path that reads it).  ValueError for
+    any other 2-D frame."""
+    if getattr(image, "ndim", None) != 2:
+        return None
+    rows, w = (int(v) for v in image.shape)
+    h = rows * 2 // 3
+    if str(image.dtype) not in ("uint8", "torch.uint8") or rows % 3 or h < 2 or h % 2 or w < 2 or w % 2:
+        raise ValueError(f"a 2-D frame is NV12, uint8 [3h/2, w] with h and w even and >= 2; got {tuple(image.shape)} {image.dtype}")
+    return h, w
+
+
+def letterbox_frame(image, input_size, device, out=None, device_out=None, device_preproc=False, rgb=True):
+    """One raw frame -> (letterboxed BGR uint8 [1,H,W,3], r, (h, w) of the original frame).  The one place that knows the frame
+    formats the drivers take:
+      * uint8 [h, w, 3], RGB as the reference's frames (rgb=False: BGR, as cv2 loads images): preprocess() with cv2 on the host into
+        `out`, or with device_preproc uploaded and letterboxed on `device` (uc_letterbox_u8) into `device_out`;
+      * uint8 [3h/2, w], NV12 as hardware decoders deliver frames: always letterboxed on `device` (uc_letterbox_nv12) into
+        `device_out`, to the bytes the RGB frame cv2.cvtColor(image, COLOR_YUV2RGB_NV12) gives.  rgb does not apply.
+    A CUDA tensor on `device` is read in place on the current stream, which it is recorded on, so its memory is not reused before
+    that read even when the caller drops it right away; one on another GPU is copied over.  A host array or tensor is staged through
+    pinned memory (1.5 bytes per pixel for NV12).  A destination left None is allocated.  A malformed 2-D frame raises ValueError
+    before anything is enqueued."""
+    size = nv12_size(image)
+    if size is None and not device_preproc:
+        assert rgb, "a BGR frame is letterboxed on the device"
+        frame, r = preprocess(image, input_size, out=out)
+        return frame, r, tuple(image.shape[:2])
+    device = torch.device(device)
+    if device.index is None:
+        device = torch.device(device.type, torch.cuda.current_device())
+    src = torch.as_tensor(image)
+    if src.device == device:
+        src.record_stream(torch.cuda.current_stream(device))
+    else:
+        if not src.is_cuda and not src.is_pinned():
+            src = torch.empty(src.shape, dtype=src.dtype, pin_memory=True).copy_(src)
+        src = src.to(device, non_blocking=True)
+    if size is not None:
+        frame, r = shared_ops.letterbox_nv12(src, input_size, out=device_out)
+        return frame, r, size
+    assert src.dtype == torch.uint8 and src.dim() == 3 and src.shape[2] == 3
+    frame, r = ops.letterbox_u8(src.contiguous(), input_size, swap_rb=rgb, out=device_out)
+    return frame, r, tuple(src.shape[:2])
+
+
+class LetterboxBatch:
+    """The raw frames of one batched step, letterboxed (letterbox_frame) into one uint8 [n,H,W,3] batch.  A frame letterboxed on the
+    host lands in a pinned buffer, one letterboxed on the device in a device buffer, allocated by the first step that needs it.  The
+    batch is the pinned buffer when no frame of the step was letterboxed on the device, otherwise the device buffer with the
+    host-letterboxed frames copied up, so RGB and NV12 frames mix in one step."""
+
+    def __init__(self, n, input_size, device, device_preproc=False):
+        H, W = input_size
+        self.input_size, self.device, self.device_preproc = tuple(input_size), device, device_preproc
+        self.host = torch.full((n, H, W, 3), 114, dtype=torch.uint8).pin_memory()
+        self.dev = None
+
+    def __call__(self, images):
+        """images: n raw frames, None for an idle slot -> (frames [n,H,W,3], ratios, sizes (h, w)); None ratio and size for an idle
+        slot, whose frame in the batch is stale.  Every NV12 frame is checked before any is letterboxed."""
+        nv12 = [nv12_size(im) is not None for im in images]
+        if self.dev is None and (self.device_preproc or any(nv12)):
+            self.dev = torch.empty(self.host.shape, dtype=torch.uint8, device=self.device)
+        lb = [None if im is None else letterbox_frame(im, self.input_size, self.device, self.host[i:i + 1],
+                                                       None if self.dev is None else self.dev[i:i + 1], self.device_preproc)
+              for i, im in enumerate(images)]
+        if not any(t is not None and t[0].is_cuda for t in lb):
+            frames = self.host
+        else:
+            frames = self.dev
+            for i, t in enumerate(lb):
+                if t is not None and not t[0].is_cuda:
+                    frames[i:i + 1].copy_(t[0], non_blocking=True)
+        return frames, [None if t is None else t[1] for t in lb], [None if t is None else t[2] for t in lb]
 
 
 def xyxy_resized(xywh, r):
@@ -76,7 +154,8 @@ class UnicornSOTBatch:
 
     max_inst: detection rows read back per sequence; the greedy NMS scan stops there (the driver consumes output[:max_inst] only,
     unicorn_sot.py:69-70) unless full_nms=True, which computes the complete postprocess() list.  device_preproc: initialize() / track()
-    upload the raw RGB frame and letterbox it on the GPU (uc_letterbox_u8, a bit-exact restatement of the reference's cv2 recipe)."""
+    upload the raw RGB frame and letterbox it on the GPU (uc_letterbox_u8, a bit-exact restatement of the reference's cv2 recipe).
+    NV12 frames are always letterboxed on the GPU (letterbox_frame)."""
 
     def __init__(self, engine: UnicornEngine, input_size, n_seq, conf=0.001, nms=0.65, max_inst=3, use_graph=True, full_nms=False,
                  device_preproc=False, depth=1):
@@ -99,9 +178,7 @@ class UnicornSOTBatch:
         n16 = (H // 16) * (W // 16)
         self.ref_proj = (torch.zeros(n_seq * n16, 256, dtype=torch.bfloat16, device=dev), torch.zeros(n_seq * n16, 256, dtype=torch.bfloat16, device=dev))
         self.lbs_pre = torch.zeros(n_seq, 1, (H // 8) * (W // 8), dtype=torch.float32, device=dev)
-        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()  # host-letterboxed frames (track())
-        self._dev_in = None  # device-letterboxed frames (track() with device_preproc)
-        self._raw = [None] * n_seq
+        self._frames = LetterboxBatch(n_seq, self.input_size, dev, device_preproc)  # the letterboxed frames of track()
         self.ready = [False] * n_seq
         self.states = [None] * n_seq
         self.launches_per_frame = 0  # bench.py reads it
@@ -177,35 +254,17 @@ class UnicornSOTBatch:
         return self.collect()
 
     # -------------------------------------------------------------------------------- reference protocol
-    def _letterbox(self, i, image, out=None):
-        """Slot i's raw RGB frame (HWC uint8) -> (letterboxed uint8 [1,H,W,3], r), on the host or with device_preproc on the device."""
-        if not self.device_preproc:
-            return preprocess(image, self.input_size, out=out)
-        src = torch.from_numpy(image) if not torch.is_tensor(image) else image
-        assert src.dtype == torch.uint8 and src.dim() == 3 and src.shape[2] == 3
-        if self._raw[i] is None or self._raw[i][0].shape != src.shape:
-            self._raw[i] = (torch.empty(src.shape, dtype=torch.uint8, device=self.eng.dev), torch.empty(src.shape, dtype=torch.uint8).pin_memory())
-        dev_raw, host_raw = self._raw[i]
-        host_raw.copy_(src)
-        dev_raw.copy_(host_raw, non_blocking=True)
-        return ops.letterbox_u8(dev_raw, self.input_size, swap_rb=True, out=out)
-
     def initialize(self, i, image, info: dict):
-        ref, r = self._letterbox(i, image)
+        """Slot i: image a raw frame, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (letterbox_frame); info: init_bbox [x, y, w, h]."""
+        ref, r, _ = letterbox_frame(image, self.input_size, self.eng.dev, device_preproc=self.device_preproc)
         self.initialize_tensor(i, ref, xyxy_resized(info["init_bbox"], r))
         self.states[i] = info["init_bbox"]
 
     def track(self, images):
-        """images: n_seq RGB frames (HWC uint8), None for an idle slot.  Returns n_seq results {"target_bbox": [x, y, w, h]}, None for
-        idle or uninitialised slots."""
+        """images: n_seq raw frames, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (letterbox_frame; the two may be mixed), None for an
+        idle slot.  Returns n_seq results {"target_bbox": [x, y, w, h]}, None for idle or uninitialised slots."""
         assert len(images) == self.n_seq
-        if not self.device_preproc:
-            frames = self._host_in
-        elif self._dev_in is None:
-            frames = self._dev_in = torch.empty(self._host_in.shape, dtype=torch.uint8, device=self.eng.dev)
-        else:
-            frames = self._dev_in
-        ratios = [None if im is None else self._letterbox(i, im, frames[i:i + 1])[1] for i, im in enumerate(images)]
+        frames, ratios, _ = self._frames(images)
         dets, counts = self.track_tensor(frames)
         res = [None] * self.n_seq
         for i, r in enumerate(ratios):

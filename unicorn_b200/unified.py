@@ -37,7 +37,7 @@ from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count
 from .mot import QDEmbedding, _qd_match
 from .mots import MaskEncoder, _mots_match, _mots_result
-from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
+from .sot import LetterboxBatch, get_label_map, letterbox_frame, nv12_size, state_xywh, xyxy_resized
 from .tracker import QuasiDenseEmbedTracker
 from .tracker._stream import assoc_stream
 from .vos import MAX_OBJECTS_PER_SEQUENCE, ROWS_PER_GROUP_SLOT, label_values
@@ -157,7 +157,7 @@ class UnicornUnifiedBatch(_Unified):
         self._pending = {}  # slot -> box (resized-image xyxy) of the targets whose reference is their video's next active frame
         self._ring = Ring([_BatchStep(n_seq, K, max_inst, self.n_keep, mot == "qd") for _ in range(2)])
         self._warm_u8 = None
-        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()
+        self._frames = LetterboxBatch(n_seq, self.input_size, engine.dev)  # the letterboxed frames of track()
         self.started = [False] * n_seq
         self.trackers = [None] * n_seq
         self.frame_ids = [0] * n_seq  # active steps per video since its start(): the QD arm's frame number
@@ -362,7 +362,8 @@ class UnicornUnifiedBatch(_Unified):
 
     # ------------------------------------------------------------------------------------------ reference protocol
     def track(self, images, new_targets=None, img_infos=None):
-        """images: n_seq RGB frames (HWC uint8, any original sizes), None for an idle video; each is letterboxed once for both arms.
+        """images: n_seq raw frames (any original sizes), RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame; the two
+        may be mixed), None for an idle video; each is letterboxed once for both arms.
         new_targets {video: {tid: [x, y, w, h]}} (original-image pixels) start on this step's frame of their video.  Returns one entry
         per video, None for an idle one, otherwise {"targets": {tid: [x, y, w, h]}, "mot": ...}: each target's state as
         UnicornSOTTrack.track keeps it (a new target's is its box; a target with no detection keeps its previous state), and the MOT
@@ -373,7 +374,7 @@ class UnicornUnifiedBatch(_Unified):
         for i, im in enumerate(images):
             if im is None:
                 continue
-            if not (getattr(im, "ndim", 0) == 3 and im.shape[2] == 3 and im.dtype == np.uint8):
+            if nv12_size(im) is None and not (getattr(im, "ndim", 0) == 3 and im.shape[2] == 3 and im.dtype == np.uint8):
                 raise ValueError(f"UnicornUnifiedBatch.track: frame {i} must be an RGB uint8 [h, w, 3] array")
             if not self.started[i]:
                 raise ValueError(f"UnicornUnifiedBatch.track: video {i} has not been started")
@@ -382,14 +383,14 @@ class UnicornUnifiedBatch(_Unified):
         for i, v in new_targets.items():
             if images[i] is None and v:
                 raise ValueError(f"UnicornUnifiedBatch.track: new targets of video {i} need its frame")
-        ratios = [None if im is None else preprocess(im, self.input_size, out=self._host_in[i:i + 1])[1] for i, im in enumerate(images)]
+        frames, ratios, sizes = self._frames(images)
         for i, v in new_targets.items():
             for tid, xywh in v.items():
                 self.add_target(i, tid, xyxy_resized(xywh, ratios[i]))
                 self.states[i][tid] = list(xywh)
-        infos = [None if im is None else (img_infos[i] if img_infos is not None and img_infos[i] is not None else tuple(im.shape[:2]))
+        infos = [None if im is None else (img_infos[i] if img_infos is not None and img_infos[i] is not None else sizes[i])
                  for i, im in enumerate(images)]
-        out = self.step_tensor(self._host_in, [r or 1.0 for r in ratios], [im is not None for im in images], infos)
+        out = self.step_tensor(frames, [r or 1.0 for r in ratios], [im is not None for im in images], infos)
         res = [None] * n
         for i, o in enumerate(out):
             if o is None:
@@ -460,7 +461,8 @@ class UnicornUnifiedTracker:
         return self.collect(img_info)
 
     def track(self, image_rgb, new_targets=None, img_info=None):
-        """image_rgb: an RGB frame (HWC uint8), letterboxed once for both arms.  new_targets {tid: [x, y, w, h]} (original-image pixels)
+        """image_rgb: a raw frame, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame), letterboxed once for both
+        arms.  new_targets {tid: [x, y, w, h]} (original-image pixels)
         start on this frame.  Returns {"targets": {tid: [x, y, w, h]}, "mot": ...} with UnicornUnifiedBatch.track's state rules."""
         return self._b.track([image_rgb], {0: new_targets or {}}, [img_info])[0]
 
@@ -758,12 +760,14 @@ class UnicornUnifiedMaskTracker(_Unified):
 
     # ------------------------------------------------------------------------------------------ reference protocol
     def track(self, image_rgb, info=None):
-        """image_rgb: an RGB frame (HWC uint8) of the original size, letterboxed once for both arms.  info: UnicornVOSTrack's dict
+        """image_rgb: a raw frame of the original size, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame), letterboxed
+        once for both arms.  info: UnicornVOSTrack's dict
         (init_object_ids, init_bbox {id: [x, y, w, h]}, optionally init_mask) for objects that start on this frame.  Returns
         {"segmentation": uint8 [h, w] numpy, "mots": write_results_mots() tuple or None}; state_pre_dict is kept as
         UnicornVOSTrack.track keeps it."""
-        if tuple(image_rgb.shape[:2]) != self.orig_size:
-            raise ValueError(f"UnicornUnifiedMaskTracker.track: frame size {tuple(image_rgb.shape[:2])}, the video's is {self.orig_size}")
+        size = nv12_size(image_rgb) or tuple(image_rgb.shape[:2])
+        if size != self.orig_size:
+            raise ValueError(f"UnicornUnifiedMaskTracker.track: frame size {size}, the video's is {self.orig_size}")
         info = info or {}
         if "init_object_ids" in info:
             boxes = {oid: xyxy_resized(info["init_bbox"][oid], self.r) for oid in info["init_object_ids"]}
@@ -771,7 +775,7 @@ class UnicornUnifiedMaskTracker(_Unified):
             self.add_objects(boxes, None if mask is None else torch.as_tensor(mask).to(torch.uint8))
             for oid in info["init_object_ids"]:
                 self.state_pre_dict[oid] = info["init_bbox"][oid]
-        frame, r = preprocess(image_rgb, self.input_size, out=self._host_in)
+        frame, r, _ = letterbox_frame(image_rgb, self.input_size, self.eng.dev, out=self._host_in)
         out = self.step_tensor(frame)
         for oid, (det, _) in out["vos"]["objects"].items():  # unicorn_vos.py:137-149 (state of the best instance, xywh ints)
             if det is not None:
@@ -884,7 +888,7 @@ class UnicornUnifiedMaskBatch(_Unified):
         first = _MaskBatchStep(engine, H, W, n_seq, O, max_dets, self.n_keep, self.mots)
         self._ring = Ring([first, _MaskBatchStep(engine, H, W, n_seq, O, max_dets, self.n_keep, self.mots, share=first)])
         self._warm_u8 = None
-        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()
+        self._frames = LetterboxBatch(n_seq, self.input_size, engine.dev)  # the letterboxed frames of track()
         self.started = [False] * n_seq
         self.orig_sizes, self.r = [None] * n_seq, [1.0] * n_seq
         self.trackers = [None] * n_seq
@@ -1193,8 +1197,8 @@ class UnicornUnifiedMaskBatch(_Unified):
 
     # ------------------------------------------------------------------------------------------ reference protocol
     def track(self, images, infos=None):
-        """images: n_seq RGB frames (HWC uint8) of their videos' original sizes, None for an idle video; each is letterboxed once for
-        both arms.  infos: n_seq dicts as UnicornUnifiedMaskTracker.track takes (init_object_ids, init_bbox {id: [x, y, w, h]},
+        """images: n_seq raw frames of their videos' original sizes, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame;
+        the two may be mixed), None for an idle video; each is letterboxed once for both arms.  infos: n_seq dicts as UnicornUnifiedMaskTracker.track takes (init_object_ids, init_bbox {id: [x, y, w, h]},
         optionally init_mask) or None.  Returns one entry per video, None for an idle one, otherwise {"segmentation": uint8 [h, w]
         numpy, "mots": write_results_mots() tuple or None}; state_pre_dicts[i] is kept as UnicornVOSTrack.track keeps it."""
         n = self.n_seq
@@ -1207,11 +1211,13 @@ class UnicornUnifiedMaskBatch(_Unified):
                 if infos[i] and "init_object_ids" in infos[i]:
                     raise ValueError(f"UnicornUnifiedMaskBatch.track: new objects of video {i} need its frame")
                 continue
-            if not (getattr(im, "ndim", 0) == 3 and im.shape[2] == 3 and im.dtype == np.uint8):
+            size = nv12_size(im)
+            if size is None and not (getattr(im, "ndim", 0) == 3 and im.shape[2] == 3 and im.dtype == np.uint8):
                 raise ValueError(f"UnicornUnifiedMaskBatch.track: frame {i} must be an RGB uint8 [h, w, 3] array")
             self._check_video(i, "track")
-            if tuple(im.shape[:2]) != self.orig_sizes[i]:
-                raise ValueError(f"UnicornUnifiedMaskBatch.track: frame {i} has size {tuple(im.shape[:2])}, its video's is {self.orig_sizes[i]}")
+            size = size or tuple(im.shape[:2])
+            if size != self.orig_sizes[i]:
+                raise ValueError(f"UnicornUnifiedMaskBatch.track: frame {i} has size {size}, its video's is {self.orig_sizes[i]}")
             info = infos[i] or {}
             if "init_object_ids" in info:
                 boxes = {oid: xyxy_resized(info["init_bbox"][oid], self.r[i]) for oid in info["init_object_ids"]}
@@ -1222,10 +1228,8 @@ class UnicornUnifiedMaskBatch(_Unified):
             self._add(i, boxes, mask)
             for oid in infos[i]["init_object_ids"]:
                 self.state_pre_dicts[i][oid] = infos[i]["init_bbox"][oid]
-        for i, im in enumerate(images):
-            if im is not None:
-                preprocess(im, self.input_size, out=self._host_in[i:i + 1])
-        out = self.step_tensor(self._host_in, [im is not None for im in images])
+        frames = self._frames(images)[0]
+        out = self.step_tensor(frames, [im is not None for im in images])
         res = [None] * n
         for i, o in enumerate(out):
             if o is None:

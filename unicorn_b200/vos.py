@@ -18,7 +18,7 @@ import torch
 from . import ops
 from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count, in_flight
-from .sot import get_label_map, preprocess, state_xywh, xyxy_resized
+from .sot import LetterboxBatch, get_label_map, letterbox_frame, state_xywh, xyxy_resized
 
 
 def label_values(boxes_xyxy, input_size, device):
@@ -222,18 +222,18 @@ class UnicornVOSTrack:
 
     # ------------------------------------------------------------------------------------------ reference protocol
     def initialize(self, image, info: dict):
-        """image: RGB uint8 HWC; info: init_object_ids, init_bbox {id: [x,y,w,h]} (unicorn_vos.py:43-69)."""
-        self.H, self.W = image.shape[:2]
-        ref, r = preprocess(image, self.input_size)
+        """image: a raw frame, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (letterbox_frame); info: init_object_ids, init_bbox {id:
+        [x,y,w,h]} (unicorn_vos.py:43-69)."""
+        ref, r, (self.H, self.W) = letterbox_frame(image, self.input_size, self.eng.dev)
         for oid in info["init_object_ids"]:
             self.state_pre_dict[oid] = info["init_bbox"][oid]
         boxes = {oid: xyxy_resized(info["init_bbox"][oid], r) for oid in info["init_object_ids"]}
         self.initialize_tensor(ref, boxes, orig_size=(self.H, self.W), r=r)
 
     def track(self, image, info: dict = None):
-        """-> {"segmentation": uint8 [H,W] numpy} (unicorn_vos.py:71-127)."""
+        """image: a raw frame as initialize() takes it -> {"segmentation": uint8 [H,W] numpy} (unicorn_vos.py:71-127)."""
         info = info or {}
-        cur, r = preprocess(image, self.input_size)
+        cur, r, _ = letterbox_frame(image, self.input_size, self.eng.dev)
         new_boxes, init_mask = None, None
         if "init_object_ids" in info:
             for oid in info["init_object_ids"]:
@@ -303,7 +303,7 @@ class UnicornVOSBatch:
         self.masks = torch.zeros(max_objects, 1, H, W, dtype=torch.float32, device=dev)
         self.rows = torch.zeros(max_objects, 8, dtype=torch.float32, device=dev)  # best detection row + count of each object slot
         self.host_rows = torch.zeros(max_objects, 8).pin_memory()
-        self._host_in = torch.full((n_seq, H, W, 3), 114, dtype=torch.uint8).pin_memory()  # host-letterboxed frames (track())
+        self._frames = LetterboxBatch(n_seq, self.input_size, dev)  # the letterboxed frames of track()
         self._gs = [None] * max_groups  # host mirrors of the slot tables: sequence of a group slot, (sequence, group slot, row)
         self._os = [None] * max_objects
         self.seqs = [None] * n_seq
@@ -484,28 +484,27 @@ class UnicornVOSBatch:
 
     # -------------------------------------------------------------------------------- reference protocol
     def initialize(self, i, image, info: dict):
-        """Slot i: image RGB uint8 HWC; info: init_object_ids, init_bbox {id: [x,y,w,h]} (unicorn_vos.py:43-69)."""
-        ref, r = preprocess(image, self.input_size)
+        """Slot i: image a raw frame, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (letterbox_frame); info: init_object_ids, init_bbox
+        {id: [x,y,w,h]} (unicorn_vos.py:43-69)."""
+        ref, r, size = letterbox_frame(image, self.input_size, self.eng.dev)
         boxes = {oid: xyxy_resized(info["init_bbox"][oid], r) for oid in info["init_object_ids"]}
-        self.initialize_tensor(i, ref, boxes, orig_size=image.shape[:2], r=r)
+        self.initialize_tensor(i, ref, boxes, orig_size=size, r=r)
         self.state_pre_dicts[i] = {oid: info["init_bbox"][oid] for oid in info["init_object_ids"]}
 
     def track(self, images, infos=None):
-        """images: n_seq RGB frames (HWC uint8), None for an idle slot; infos: n_seq dicts as UnicornVOSTrack.track takes (or None).
-        Returns n_seq results {"segmentation": uint8 [H,W] numpy}, None for idle or uninitialised slots."""
+        """images: n_seq raw frames as initialize() takes them (RGB and NV12 may be mixed), None for an idle slot; infos: n_seq dicts
+        as UnicornVOSTrack.track takes (or None).  Returns n_seq results {"segmentation": uint8 [H,W] numpy}, None for idle or
+        uninitialised slots."""
         n = self.n_seq
         assert len(images) == n
         infos = infos or [None] * n
-        ratios = [None] * n
-        for i, im in enumerate(images):
-            if im is not None:
-                ratios[i] = preprocess(im, self.input_size, out=self._host_in[i:i + 1])[1]
+        frames, ratios, _ = self._frames(images)
         new = {}
         for i, info in enumerate(infos):
             if info and "init_object_ids" in info and images[i] is not None and self.seqs[i] is not None:
                 new[i] = ({oid: xyxy_resized(info["init_bbox"][oid], ratios[i]) for oid in info["init_object_ids"]},
                           torch.as_tensor(info["init_mask"]).to(torch.uint8))
-        out = self.track_tensor([self._host_in[i:i + 1] if im is not None else None for i, im in enumerate(images)], new)
+        out = self.track_tensor([frames[i:i + 1] if im is not None else None for i, im in enumerate(images)], new)
         res = [None] * n
         for i, o in enumerate(out):
             if o is None:
