@@ -196,7 +196,7 @@ def test_pipelined_graph_driver_equals_sequential_and_host_path():
         pipe_trk.submit(frames[t:t + 1], *sizes[t % 2])
         pipe.append(pipe_trk.collect())
     pipe.append(pipe_trk.collect())
-    assert all(s.graph is not None for s in pipe_trk._slots)
+    assert all(s.graph is not None for s in pipe_trk._ctxs)
     assert pipe == seq
 
 

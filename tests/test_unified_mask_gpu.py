@@ -125,9 +125,7 @@ def mots_reference(e, v, n):
     out = []
     for t in range(n):
         res = trk.step_tensor(v.frames[t:t + 1], *v.orig)
-        c = trk._ring.slots[(trk._ring.collected - 1) % 2]
-        k = c.last["dets"].shape[0]
-        out.append((res, c.last["dets"].clone(), c.host_feats[:k].clone()))
+        out.append((res, trk.last["dets"].clone(), trk.last["feats"].clone()))
     return out
 
 
@@ -347,7 +345,7 @@ def test_rejections_change_nothing():
     trk.add_objects({1: v.boxes[0, 0], 2: v.boxes[0, 1]})
 
     def state():
-        return (list(trk.objects), [(list(b), m is None) for b, m in trk._pending], list(trk._os), list(trk._gs), trk._ring.submitted,
+        return (list(trk.objects), [(list(b), m is None) for b, m in trk._b._pending[0]], list(trk._b._os), list(trk._b._gs), trk._ring.submitted,
                 trk.frame_id, trk.active.tolist(), trk.obj_row.tolist())
     before = state()
     good_mask = torch.zeros(TINY, dtype=torch.uint8)
@@ -357,7 +355,7 @@ def test_rejections_change_nothing():
         trk.add_objects({4: v.boxes[0, 2], "4": v.boxes[0, 2]})
     with pytest.raises(ValueError, match="1..255"):
         trk.add_objects({0: v.boxes[0, 2]})
-    with pytest.raises(ValueError, match="exceed max_objects"):
+    with pytest.raises(ValueError, match="3 new objects but 2 of max_objects = 4 slots are free"):
         trk.add_objects({4: v.boxes[0, 2], 5: v.boxes[0, 2], 6: v.boxes[0, 2]})
     with pytest.raises(ValueError, match="4 values"):
         trk.add_objects({4: [0.0, 1.0, 2.0]})
@@ -369,7 +367,7 @@ def test_rejections_change_nothing():
         trk.remove_object(7)
     with pytest.raises(ValueError, match="frame must be"):
         trk.submit(v.frames[0:1, :160])
-    with pytest.raises(ValueError, match="frame size"):
+    with pytest.raises(ValueError, match="has size"):
         trk.track(np.zeros((240, 400, 3), np.uint8))
     assert state() == before
     trk.add_objects({3: v.boxes[0, 2]}, init_mask=good_mask)
@@ -383,16 +381,18 @@ def test_rejections_change_nothing():
     with pytest.raises(ValueError, match="max_groups"):
         for oid in range(1, 5):
             trk2.add_objects({oid: v.boxes[0, 0]})
-    assert trk2.objects == [1, 2, 3] and trk2._gs == [1, 1, 1]
+    assert trk2.objects == [1, 2, 3] and trk2._b._gs == [1, 1, 1]
     big = UnicornUnifiedMaskTracker(e, TINY, TINY, 17, 3, mots=False)
     with pytest.raises(ValueError, match="at most 16"):
         big.add_objects({o: v.boxes[0, 0] for o in range(1, 18)})
-    assert big.objects == [] and big._gs == [0, 0, 0] and big._os == [None] * 17
+    assert big.objects == [] and big._b._gs == [0, 0, 0] and big._b._os == [None] * 17
     # the driver still runs on the state it had: frame 0 is the reference of objects 1..4, object 3 enters from its (empty) mask
     assert state() == before
     res = trk.step_tensor(v.frames[0:1])
     assert res["vos"]["ids"] == [3] and res["mots"] is None and trk.objects == [1, 2, 3, 4]
-    assert trk.active.tolist() == [1, 1, 1, 1]
+    assert trk._b.image_of.tolist() == [0, 0, 0, 0]  # the reference frame made every object slot live: it reads video 0's image
+    trk.step_tensor(v.frames[1:2])
+    assert trk.active.tolist() == [1, 1, 1, 1]  # the step's active table
 
 
 @pytest.mark.parametrize("name", ["unicorn_track_tiny", "unicorn_det_convnext_tiny"])

@@ -435,7 +435,7 @@ def main_mots(args):
             return time.perf_counter() - t0
 
         def pipe_replay(t, trk=trk):
-            c = trk._slots[t % 2]
+            c = trk._ctxs[t % 2]
             c.img_in_u8.copy_(steps_u8[t % 4][0:1], non_blocking=True)
             c.graph.replay()
         pipe_round(4)

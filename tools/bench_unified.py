@@ -190,7 +190,7 @@ def compare(sides, args, e0, e1):
 
 
 def mask(args):
-    from unicorn_b200 import _lib, ops
+    from unicorn_b200 import _lib, shared_ops
     from unicorn_b200.engine import UnicornEngine
     from unicorn_b200.mots import UnicornMOTSTracker
     from unicorn_b200.sot import preprocess
@@ -240,7 +240,8 @@ def mask(args):
                     s = un._ring.slots[t % 2]
                     s.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
                     s.graph.replay()
-                    ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], None, [o for o, _ in s.objs], H, W, un.r, s.soft, s.seg)
+                    shared_ops.vos_aggregate_batched([([s.vos_masks[k] for _, k in s.objs[0]], None, [o for o, _ in s.objs[0]], un.r, s.soft[0],
+                                                       s.seg[0])], H, W)
                 un_round(4)
                 launches = un.launches_per_frame + outside(lambda t: un.step_tensor(steps_u8[t % 4]))
                 sides["unified"] = (un_round, un_replay, launches, torch.cuda.max_memory_allocated() - m0)
@@ -275,7 +276,7 @@ def mask(args):
                     s.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
                     s.graph.replay()
                     if mt:
-                        c = mt._slots[t % 2]
+                        c = mt._ctxs[t % 2]
                         c.img_in_u8.copy_(steps_u8[t % 4], non_blocking=True)
                         c.graph.replay()
                 two_round(6)
@@ -508,7 +509,8 @@ def mask_batch(args):
                             s = ut._ring.slots[t % 2]
                             s.img_in_u8.copy_(vs[i][3][t % 4], non_blocking=True)
                             s.graph.replay()
-                            ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], None, [o for o, _ in s.objs], H, W, ut.r, s.soft, s.seg)
+                            shared_ops.vos_aggregate_batched([([s.vos_masks[k] for _, k in s.objs[0]], None, [o for o, _ in s.objs[0]], ut.r,
+                                                               s.soft[0], s.seg[0])], H, W)
                     ut_round(4)
 
                     def ut_step(t, uts=uts):

@@ -1,29 +1,28 @@
-"""MOTS per-frame driver on the H100 engine — the per-frame body of MOTEvaluator.evaluate_omni_mots
+"""MOTS driver on the H100 engine — the per-frame body of MOTEvaluator.evaluate_omni_mots
 (unicorn/evaluators/mot_evaluator.py:776-897): whole-mode detector with the CondInst controllers -> NMS -> dynamic-conv masks of the
 kept detections -> embedding sampling -> QuasiDenseEmbedTracker.match(return_index=True) -> masks of the tracked boxes in
 ascending-id order, resized to the original frame, overlap free, area filter, COCO RLE.
 
-Like the QD arm of the MOT driver (mot.py) the frame is split in a device half and a host half:
+UnicornMOTSBatch runs `n_seq` sequences in lock step under the protocol of UnicornMOTBatch (mot.py), and like the QD arm of the MOT
+driver splits a step in a device half and a host half:
 
-  submit(frame, img_h, img_w)  enqueues every kernel of the frame (with use_graph, one CUDA-graph replay from the second frame of
-                               a slot on), the masks into the slot's own buffer, and asynchronous copies of (count, detections,
-                               sampled embeddings) into pinned slot memory;
-  collect()                    waits for the oldest slot, runs the association on the host, and encodes the tracked masks on the
-                               device (uc_mots_encode on the association stream, so it does not queue behind the next frame).
+  submit(frames, img_sizes)  enqueues every kernel of the step (with use_graph, one CUDA-graph replay per parity slot from the
+                             slot's second step on), the masks into the slot's own buffer, and asynchronous copies of (counts,
+                             detections, sampled embeddings) into pinned slot memory;
+  collect()                  waits for the oldest slot, runs each active sequence's association on the host, then ONE encode of
+                             the tracked instances of every sequence on the device (uc_mots_encode_batched, uc_mots_encode for a
+                             single frame) on the association stream, so it does not queue behind the next step; one upload of
+                             order / emit and at most two host synchronises per step.
 
 Two slots: submit(t+1) may precede collect(t).  The host reads back only detections, embeddings and the RLE strings; the masks
 never leave the device.  results.mots_frame_result is the host restatement the tests compare against.
 
-UnicornMOTSBatch runs `n_seq` sequences in lock step under the protocol of UnicornMOTBatch (mot.py): one batched frame per step (one
-CUDA graph per parity slot), each active sequence's own association on the host, then ONE batched encode (uc_mots_encode_batched) of
-the tracked instances of every sequence, with one upload of order / emit and at most two host synchronises per step."""
+UnicornMOTSTracker is the n_seq = 1 case under the reference's one-sequence protocol."""
 import torch
 
 from . import ops
 from .engine import UnicornEngine
-from .frames import FrameSlot, Ring
-from .mot import QDEmbedding, UnicornMOTBatch
-from .tracker import QuasiDenseEmbedTracker
+from .mot import UnicornMOTBatch
 from .tracker._stream import assoc_stream
 
 
@@ -102,9 +101,13 @@ class MaskEncoder:
     def batch(self, masks, thr, frames):
         """masks fp32 [B,n_max,Hin,Win] (device); frames: B entries (order, emit, r, img_h, img_w) as in __call__, None for an image
         with nothing to encode.  One upload, one encode and two host synchronises for the whole batch (one more encode and
-        synchronise when the chars outgrow the buffers).  Returns B lists of strings."""
+        synchronise when the chars outgrow the buffers).  A batch of one frame takes the one-frame launch, whose strings are the same.
+        Returns B lists of strings."""
         _, _, Hin, Win = masks.shape
         frames = [f if f is not None else ([], [], 1.0, Hin, Win) for f in frames]
+        if len(frames) == 1:
+            order, emit, r, img_h, img_w = frames[0]
+            return [self(masks[0], order, emit, thr, r, img_h, img_w)]
         ks = [len(f[0]) for f in frames]
         if sum(ks) == 0:
             return [[] for _ in frames]
@@ -141,112 +144,12 @@ def _mots_result(frame_id, ids, emit, rles, img_h, img_w):
     return (frame_id, [int(t) + 1 for t, e in zip(ids.tolist(), emit) if e], 2, img_h, img_w, [s for s, e in zip(rles, emit) if e])
 
 
-class _Slot(FrameSlot):
-    """One MOTS frame in flight: a frame slot plus its engine buffer tag, its mask buffer and its pinned results."""
-
-    def __init__(self, eng, H, W, tag, max_dets):
-        super().__init__(eng, H, W)
-        self.tag = tag
-        self.masks = torch.zeros(max_dets, H, W, dtype=torch.float32, device=eng.dev)  # uc_dynamic_masks output of the slot's frame
-        self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self.host_dets = torch.zeros(max_dets, 7).pin_memory()
-        self.host_feats = torch.zeros(max_dets, 128).pin_memory()
-        self.frame_id, self.img_hw = 0, (0, 0)
-        self.warm_u8 = None  # input dtype the slot last ran eagerly with: its next frame with it is captured
-
-
-class UnicornMOTSTracker:
-    def __init__(self, engine: UnicornEngine, input_size, conf=0.01, nms=0.7, score_thr=0.1, max_dets=64, mask_thres=0.3, d_rate=2,
-                 min_box_area=100, tracker=None, use_graph=False):
-        assert engine.cfg["mask"], "MOTS needs a *_mask model"
-        self.eng, self.input_size = engine, tuple(input_size)
-        self.conf, self.nms, self.score_thr, self.max_dets = conf, nms, score_thr, max_dets
-        self.mask_thres, self.d_rate, self.min_box_area = mask_thres, d_rate, min_box_area
-        self.tracker = tracker or QuasiDenseEmbedTracker(device=engine.dev)
-        self.use_graph = use_graph
-        H, W = self.input_size
-        self._qd = QDEmbedding(engine, H, W, max_dets, "mots.emb")
-        up = 8 // d_rate
-        self._scratch = torch.empty(max_dets * (H // 8) * (W // 8) * (1 + up * up), dtype=torch.float32, device=engine.dev)
-        # two slots on this engine and the current stream, so that submit(t+1) may precede collect(t); they share the input buffers
-        # and the NMS workspace, each has its own backbone buffers (tag) and mask buffer
-        slots = [_Slot(engine, H, W, "mots%d" % i, max_dets) for i in range(2)]
-        slots[1].img_in, slots[1].img_in_u8, slots[1].ws = slots[0].img_in, slots[0].img_in_u8, slots[0].ws
-        self._ring = Ring(slots)
-        self._slots = slots
-        self._enc = MaskEncoder(max_dets, engine.dev)
-        self.frame_id = 0  # frames submitted
-        self.last = {}
-
-    # ------------------------------------------------------------------------------------------ device half
-    def _frame(self, c):
-        e = c.eng
-        e.begin_frame()
-        fpn, seq = e.backbone(c.img, tag=c.tag)
-        out = e.head(fpn, None, "mot", with_masks=True)
-        dets, cnt = ops.postprocess_device(out[0], e.ncls, self.conf, self.nms, c.ws)
-        mf, um = e.mask_branch(fpn)
-        hw = [(t.shape[1], t.shape[2]) for t in e.dyn_levels]
-        ops.dynamic_masks(mf, um, e.dyn_levels, hw, c.ws, self.max_dets, up_rate=8 // self.d_rate, d_rate=self.d_rate, out=c.masks,
-                          scratch=self._scratch)
-        self._qd(e, seq["feat"], dets, cnt)  # pre_dict as in the MOT driver (:803-818)
-        c.last = dict(head=out, mask_feats=mf, up_masks=um, dyn=list(e.dyn_levels))
-
-    def submit(self, frame, img_h, img_w):
-        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; (img_h, img_w): original image size.  Enqueues
-        the frame; returns immediately."""
-        c = self._ring.submit()
-        self.frame_id = self._ring.submitted
-        c.stage(frame)
-        if c.graph is not None:
-            c.graph.replay()
-        elif self.use_graph and c.warm_u8 == c.u8:
-            # the slot's first frame ran eagerly (plan-time autotuning, buffer allocation); the second is captured without a
-            # warm-up run: a QD frame advances pre_dict, so it must not run twice
-            c.graph, _ = c.capture(lambda: self._frame(c))
-        else:
-            self._frame(c)
-            c.warm_u8 = c.u8
-        c.host_count.copy_(c.ws.count, non_blocking=True)
-        c.host_dets.copy_(c.ws.dets[:self.max_dets], non_blocking=True)
-        c.host_feats.copy_(self._qd.feats[0], non_blocking=True)
-        c.frame_id, c.img_hw = self.frame_id, (img_h, img_w)
-        c.event.record()
-        self.last = c.last
-
-    # ------------------------------------------------------------------------------------------ host half
-    def collect(self):
-        """Association and mask encoding of the oldest submitted frame.  Returns the tuple write_results_mots() consumes:
-        (frame_id, ids (1-based), cat_id, img_h, img_w, rles)."""
-        c = self._ring.collect()
-        c.event.synchronize()
-        img_h, img_w = c.img_hw
-        H, W = self.input_size
-        n = min(int(c.host_count[0]), self.max_dets)
-        d, f = c.host_dets[:n].clone(), c.host_feats[:n].clone()
-        scale = min(H / float(img_h), W / float(img_w))
-        ob, oid, rows, emit = _mots_match(self.tracker, d, f, scale, self.score_thr, c.frame_id, self.min_box_area)
-        # the tracked boxes, their ids and mask rows (ascending id), what the frame's strings encode
-        c.last.update(dets=d, masks=c.masks[:n], boxes=ob, ids=oid, rows=rows)
-        self.last = c.last
-        stream = assoc_stream(self.eng.dev)
-        with torch.cuda.stream(stream):  # not behind the next frame's kernels on the main stream
-            stream.wait_event(c.event)
-            rles = self._enc(c.masks, rows.tolist(), emit, self.mask_thres, scale, img_h, img_w)
-        return _mots_result(c.frame_id, oid, emit, rles, img_h, img_w)
-
-    def step_tensor(self, frame, img_h, img_w):
-        """Sequential protocol of the reference: one frame in, its write_results_mots() tuple out."""
-        self.submit(frame, img_h, img_w)
-        return self.collect()
-
-
 class UnicornMOTSBatch(UnicornMOTBatch):
     """`n_seq` MOTS sequences in lock step: the QD arm of UnicornMOTBatch (same start / submit / collect protocol, CUDA graphs, idle and
     never-started slots) with the mask head in the step.  The device half at B = n_seq adds the controllers, the mask branch and the
     dynamic masks of every image's NMS rows, written into the parity slot's own mask buffer [n_seq, max_dets, H, W]; collect() runs
-    each active sequence's association as UnicornMOTSTracker does, then one batched encode of all their tracked instances.  Each
-    sequence's results equal those of its own UnicornMOTSTracker.
+    each active sequence's association, then one batched encode of all their tracked instances.  Each sequence's results equal
+    those of the same driver at n_seq = 1.
 
     submit(frames, img_sizes, active) takes the n_seq original (h, w) instead of letterbox scales; collect() returns n_seq
     write_results_mots() tuples (frame_id, ids (1-based), cat_id, img_h, img_w, rles), None for a slot not stepped."""
@@ -267,6 +170,7 @@ class UnicornMOTSBatch(UnicornMOTBatch):
             c.masks = torch.zeros(n_seq, max_dets, H, W, dtype=torch.float32, device=engine.dev)
             c.img_hw = [None] * n_seq
         self._enc = MaskEncoder(n_seq * max_dets, engine.dev)
+        self.last_tracked = [None] * n_seq
 
     # ------------------------------------------------------------------------------------------ device half
     def _frame(self, c):
@@ -274,10 +178,10 @@ class UnicornMOTSBatch(UnicornMOTBatch):
         e.begin_frame()
         fpn, seq = e.backbone(c.img, tag=c.tag)
         out = e.head(fpn, None, "mot", with_masks=True)
-        dets, cnt = ops.postprocess_device(out, e.ncls, self.conf, self.nms, c.ws)
+        # one sequence: the one-image launches; it needs no gate (a step without an active sequence does not run)
+        dets, cnt = ops.postprocess_device(out[0] if one else out, e.ncls, self.conf, self.nms, c.ws)
         mf, um = e.mask_branch(fpn)
         hw = [(t.shape[1], t.shape[2]) for t in e.dyn_levels]
-        # one sequence: the one-image launches of UnicornMOTSTracker; it needs no gate (a step without an active sequence does not run)
         ops.dynamic_masks(mf, um, e.dyn_levels, hw, c.ws, self.max_dets, up_rate=8 // self.d_rate, d_rate=self.d_rate,
                           out=c.masks[0] if one else c.masks, scratch=self._scratch, image_of=None if one else self._image_of)
         self._qd(e, seq["feat"], dets, cnt, gate=None if one else c.active)
@@ -299,11 +203,13 @@ class UnicornMOTSBatch(UnicornMOTBatch):
     # ------------------------------------------------------------------------------------------ host half
     def collect(self):
         """Association and mask encoding of the oldest submitted step: n_seq write_results_mots() tuples, None for a slot not stepped.
-        last_dets[i] / last_feats[i] then hold the NMS rows / embeddings slot i's tracker was given (None for such a slot)."""
+        last_dets[i] / last_feats[i] then hold the NMS rows / embeddings slot i's tracker was given, and last_tracked[i] {"masks": the
+        masks of those rows (device), "boxes", "ids", "rows": the tracked boxes, their ids and mask rows in ascending id} (None for such
+        a slot)."""
         c = self._ring.collect()
         c.event.synchronize()
         n_seq = self.n_seq
-        self.last_dets, self.last_feats = [None] * n_seq, [None] * n_seq
+        self.last_dets, self.last_feats, self.last_tracked = [None] * n_seq, [None] * n_seq, [None] * n_seq
         tracked, frames = {}, [None] * n_seq
         for i in range(n_seq):
             if not c.mask[i]:
@@ -311,7 +217,8 @@ class UnicornMOTSBatch(UnicornMOTBatch):
             n = min(int(c.host_count[i]), self.n_keep)
             d, f = c.host_dets[i, :n].clone(), c.host_feats[i, :n].clone()
             self.last_dets[i], self.last_feats[i] = d, f
-            _, oid, rows, emit = _mots_match(c.trackers[i], d, f, c.scales[i], self.score_thr, c.frame_ids[i], self.min_box_area)
+            ob, oid, rows, emit = _mots_match(c.trackers[i], d, f, c.scales[i], self.score_thr, c.frame_ids[i], self.min_box_area)
+            self.last_tracked[i] = dict(masks=c.masks[i, :n], boxes=ob, ids=oid, rows=rows)
             tracked[i] = oid, emit
             frames[i] = (rows.tolist(), emit, c.scales[i], *c.img_hw[i])
         stream = assoc_stream(self.eng.dev)
@@ -328,4 +235,41 @@ class UnicornMOTSBatch(UnicornMOTBatch):
     def step_tensor(self, frames, img_sizes, active=None):
         """Sequential protocol: one step in, its n_seq results out."""
         self.submit(frames, img_sizes, active)
+        return self.collect()
+
+
+class UnicornMOTSTracker:
+    """One MOTS sequence: UnicornMOTSBatch at n_seq = 1 (same arguments) with its slot started on `tracker` (default a fresh
+    QuasiDenseEmbedTracker), under the reference's one-sequence protocol.  last: the device tensors of the latest submitted frame
+    (head, mask_feats, up_masks, dyn) and, from the latest collect(), the NMS rows / embeddings the tracker was given (dets, feats),
+    the rows' masks (masks) and the tracked boxes, ids and mask rows in ascending id (boxes, ids, rows)."""
+
+    def __init__(self, engine: UnicornEngine, input_size, conf=0.01, nms=0.7, score_thr=0.1, max_dets=64, mask_thres=0.3, d_rate=2,
+                 min_box_area=100, tracker=None, use_graph=False):
+        self._b = UnicornMOTSBatch(engine, input_size, 1, conf, nms, score_thr, max_dets, mask_thres, d_rate, min_box_area, use_graph)
+        self._b.start(0, tracker)
+        self.tracker = self._b.trackers[0]
+
+    max_dets = property(lambda self: self._b.max_dets)
+    mask_thres = property(lambda self: self._b.mask_thres)
+    min_box_area = property(lambda self: self._b.min_box_area)
+    _ctxs = property(lambda self: self._b._ctxs)
+    frame_id = property(lambda self: self._b.frame_ids[0])  # frames submitted
+    last = property(lambda self: self._b.last)
+
+    def submit(self, frame, img_h, img_w):
+        """frame: preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device; (img_h, img_w): original image size.  Enqueues
+        the frame; returns immediately."""
+        self._b.submit(frame, [(img_h, img_w)])
+
+    def collect(self):
+        """Association and mask encoding of the oldest submitted frame.  Returns the tuple write_results_mots() consumes:
+        (frame_id, ids (1-based), cat_id, img_h, img_w, rles)."""
+        res = self._b.collect()[0]
+        self.last.update(dets=self._b.last_dets[0], feats=self._b.last_feats[0], **self._b.last_tracked[0])
+        return res
+
+    def step_tensor(self, frame, img_h, img_w):
+        """Sequential protocol of the reference: one frame in, its write_results_mots() tuple out."""
+        self.submit(frame, img_h, img_w)
         return self.collect()

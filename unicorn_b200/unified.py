@@ -22,11 +22,10 @@ graph reads: adding or removing a target writes them in place and never re-captu
 
 UnicornUnifiedTracker is UnicornUnifiedBatch at n_seq = 1 under the one-video protocol.
 
-UnicornUnifiedMaskTracker does the same on one video for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS
-object slots in place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both.
-UnicornUnifiedMaskBatch does it for n_seq videos in one step, as UnicornUnifiedBatch does for the box checkpoints: the object and
-group slots are one pool shared by all videos, and one uc_vos_aggregate_batched launch assembles every video's label map at its own
-original size."""
+UnicornUnifiedMaskBatch does the same for the *_mask checkpoints, which serve VOS and MOTS with one set of weights: VOS object slots in
+place of the SOT targets, the MOTS arm in place of the MOT arm, and the mask branch computed once for both.  The object and group
+slots are one pool shared by all videos, and one uc_vos_aggregate_batched launch assembles every video's label map at its own
+original size.  UnicornUnifiedMaskTracker is UnicornUnifiedMaskBatch at n_seq = 1 under the one-video protocol."""
 import warnings
 
 import numpy as np
@@ -37,7 +36,7 @@ from .engine import UnicornEngine
 from .frames import FrameSlot, Ring, anchor_count
 from .mot import QDEmbedding, _qd_match
 from .mots import MaskEncoder, _mots_match, _mots_result
-from .sot import LetterboxBatch, get_label_map, letterbox_frame, nv12_size, state_xywh, xyxy_resized
+from .sot import LetterboxBatch, get_label_map, nv12_size, state_xywh, xyxy_resized
 from .tracker import QuasiDenseEmbedTracker
 from .tracker._stream import assoc_stream
 from .vos import MAX_OBJECTS_PER_SEQUENCE, ROWS_PER_GROUP_SLOT, label_values
@@ -46,8 +45,6 @@ from .vos import MAX_OBJECTS_PER_SEQUENCE, ROWS_PER_GROUP_SLOT, label_values
 class _Unified:
     """What the unified drivers share: the frame check (one frame per video, n_seq videos), a step ring whose submit stages the
     frames or changes nothing, and the eager / capture / replay choice of a step."""
-
-    n_seq = 1
 
     def _check(self, frame):
         n, (H, W) = self.n_seq, self.input_size
@@ -467,322 +464,6 @@ class UnicornUnifiedTracker:
         return self._b.track([image_rgb], {0: new_targets or {}}, [img_info])[0]
 
 
-# ---------------------------------------------------------------------------------------------------------- VOS objects + MOTS
-class _MaskStep(FrameSlot):
-    """One step of UnicornUnifiedMaskTracker in flight: its frame slot and graph, the device buffers its results live in until the
-    next step of the same parity (the masks of both arms, the label map and soft masks), its pinned read-back and the host values it
-    was submitted with."""
-
-    def __init__(self, eng, H, W, O, max_dets, mots, share=None):
-        super().__init__(eng, H, W)
-        if share is not None:  # one set of input buffers and one MOTS NMS workspace for both parities
-            self.img_in, self.img_in_u8, self.ws = share.img_in, share.img_in_u8, share.ws
-        dev = eng.dev
-        self.vos_masks = torch.zeros(O, 1, H, W, dtype=torch.float32, device=dev)
-        self.host_rows = torch.zeros(O, 8).pin_memory()  # best detection row + count of every object slot
-        self.seg = self.soft = None
-        self.mots_masks = torch.zeros(max_dets, H, W, dtype=torch.float32, device=dev) if mots else None
-        self.host_count = torch.zeros(1, dtype=torch.int32).pin_memory() if mots else None
-        self.host_dets = torch.zeros(max_dets, 7).pin_memory() if mots else None
-        self.host_feats = torch.zeros(max_dets, 128).pin_memory() if mots else None
-        self.objs, self.new_ids, self.frame_id = [], [], 0  # (id, object slot) of the live objects, ids entering from init_mask
-
-
-class UnicornUnifiedMaskTracker(_Unified):
-    """Up to `max_objects` VOS objects plus optionally the MOTS arm (mots=True) on one video of original size `orig_size` (h, w), one
-    backbone, neck and mask-branch pass per frame.  For the *_mask checkpoints, which serve VOS and MOTS with one set of weights.
-
-    VOS settings (conf, nms, max_inst, d_rate) default to UnicornVOSTrack's, MOTS settings (mots_conf, mots_nms, score_thr, max_dets,
-    mask_thres, mots_d_rate, min_box_area) to UnicornMOTSTracker's; `tracker`: the MOTS arm's QuasiDenseEmbedTracker (default a fresh
-    one).  Both arms use the letterbox ratio r = min(H / h, W / w).
-
-    The device half of a step is one CUDA graph per parity slot: backbone + neck at B = 1 with the VOS arm of the `max_groups` group
-    slots on the side stream (UnicornVOSBatch._frame with one sequence), the mask branch once, UnicornEngine.head_shared with the
-    controllers (image 0 the MOTS image, then one image per object slot), NMS of both arms, uc_dynamic_masks of both on the one
-    mask-branch image, and the MOTS arm's QDEmbedding.  ops.vos_aggregate of the step's objects follows the graph.  Each object's
-    rows, mask, the label map and soft masks equal those of one UnicornVOSTrack, the MOTS results those of UnicornMOTSTracker, bit
-    for bit.
-
-    add_objects({id: box_xyxy}, init_mask=None): the next submitted frame becomes the reference of these objects (one group).  With
-    init_mask (uint8 [h, w] label map) they enter that step's label map from it (UnicornVOSTrack.track_tensor with new objects);
-    without, they appear from the following step on (UnicornVOSTrack.initialize_tensor).  remove_object(id) frees the object's slot.
-    Object and group slots are static buffers the graphs read: adding or removing objects writes them in place and never
-    re-captures.  A free slot computes on stale buffers: the device `active` table zeroes its detection count, so its mask is
-    zero, and its result is dropped.  Steps already submitted report the objects they were submitted with."""
-
-    def __init__(self, engine: UnicornEngine, input_size, orig_size, max_objects, max_groups=None, mots=True, tracker=None,
-                 conf=0.001, nms=0.65, max_inst=1, d_rate=2,
-                 mots_conf=0.01, mots_nms=0.7, score_thr=0.1, max_dets=64,
-                 mask_thres=0.3, mots_d_rate=2, min_box_area=100, use_graph=True):
-        if engine.det or not engine.cfg["mask"]:
-            raise ValueError(f"UnicornUnifiedMaskTracker: {engine.cfg_name} has no tracking mask head; VOS and MOTS need a *_mask tracking config")
-        max_groups = max_objects if max_groups is None else max_groups
-        if max_objects < 1 or max_groups < 1:
-            raise ValueError(f"UnicornUnifiedMaskTracker: max_objects and max_groups must be >= 1 (got {max_objects}, {max_groups})")
-        self.eng, self.input_size, self.orig_size = engine, tuple(input_size), tuple(int(v) for v in orig_size)
-        self.max_objects, self.max_groups, self.mots = max_objects, max_groups, bool(mots)
-        self.tracker = (tracker or QuasiDenseEmbedTracker(device=engine.dev)) if mots else None
-        self.conf, self.nms, self.max_inst, self.d_rate = conf, nms, max_inst, d_rate
-        self.mots_conf, self.mots_nms, self.score_thr, self.max_dets = mots_conf, mots_nms, score_thr, max_dets
-        self.mask_thres, self.mots_d_rate, self.min_box_area = mask_thres, mots_d_rate, min_box_area
-        self.use_graph = use_graph
-        H, W = self.input_size
-        h0, w0 = self.orig_size
-        self.r = min(H / h0, W / w0)
-        dev, O, G = engine.dev, max_objects, max_groups
-        self.R = min(ROWS_PER_GROUP_SLOT, max_objects)  # label rows of every group slot
-        n8, n16 = (H // 8) * (W // 8), (H // 16) * (W // 16)
-        self.vos_ws = ops.PostWorkspace(anchor_count(H, W), dev, O)
-        self._qd = QDEmbedding(engine, H, W, max_dets, "unifiedm.emb") if mots else None
-        up, up_m = 8 // d_rate, 8 // mots_d_rate
-        self._scratch = torch.empty(max(O * (1 + up * up), max_dets * (1 + up_m * up_m) if mots else 0) * n8, dtype=torch.float32, device=dev)
-        self._enc = MaskEncoder(max_dets, dev) if mots else None
-        # the group and object slots as UnicornVOSBatch keeps them, with the device active table
-        self.ref_proj = tuple(torch.zeros(G * n16, 256, dtype=torch.bfloat16, device=dev) for _ in range(2))
-        self.lbs = torch.zeros(G, self.R, n8, dtype=torch.float32, device=dev)
-        i32 = dict(dtype=torch.int32, device=dev)
-        self.obj_row = torch.zeros(O, **i32)  # group slot * R + label row of each object slot
-        self.active = torch.zeros(O, **i32)
-        self.image_of = torch.zeros(O, **i32)  # every object image reads the one mask-branch image
-        self.rows = torch.zeros(O, 8, dtype=torch.float32, device=dev)
-        self._gs = [0] * G  # objects (live or pending) per group slot
-        self._os = [None] * O  # (id, group slot, label row) per object slot
-        self._order = []  # live objects in group order (UnicornVOSTrack.obj_ids)
-        self._pending = []  # groups whose reference is the next submitted frame: (boxes {id: box}, init_mask or None)
-        # two parity steps: submit(t + 1) writes one while collect(t) reads the other; each has its own graph and result buffers
-        first = _MaskStep(engine, H, W, O, max_dets, mots)
-        self._ring = Ring([first, _MaskStep(engine, H, W, O, max_dets, mots, share=first)])
-        self._warm_u8 = None
-        self._host_in = torch.full((1, H, W, 3), 114, dtype=torch.uint8).pin_memory()
-        self.frame_id = 0
-        self.state_pre_dict = {}  # track(): the reference-protocol state of every object
-        self.launches_per_frame = 0
-        self.last = {}
-        self.last_rows = self.last_dets = self.last_feats = None
-
-    graphs = property(lambda self: [s.graph for s in self._ring.slots])
-    objects = property(lambda self: self._order + [o for b, _ in self._pending for o in b])
-
-    # ------------------------------------------------------------------------------------------ objects
-    def _slot_of(self, oid):
-        return next(k for k, o in enumerate(self._os) if o is not None and o[0] == oid)
-
-    def add_objects(self, boxes_xyxy, init_mask=None):
-        """Track the objects {id: [x1, y1, x2, y2]} (resized-image coordinates; ids 1..255) from the next submitted frame on.
-        init_mask: uint8 [h, w] label map of that frame in which they appear (at most one per step)."""
-        boxes = {oid: torch.as_tensor(b, dtype=torch.float32).view(-1) for oid, b in dict(boxes_xyxy).items()}
-        known = self.objects
-        try:
-            vals = [int(o) for o in boxes]
-        except (TypeError, ValueError):
-            vals = None
-        if not boxes or vals is None or any(not 1 <= v <= 255 for v in vals):
-            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: ids must be 1..255 (got {list(boxes)})")
-        if len(set(vals)) != len(vals) or set(vals) & {int(o) for o in known}:
-            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: duplicate object id in {list(boxes)} (tracked: {known})")
-        if any(b.numel() != 4 for b in boxes.values()):
-            raise ValueError("UnicornUnifiedMaskTracker.add_objects: every box needs 4 values")
-        n = len(known) + len(boxes)
-        if n > self.max_objects:
-            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {n} objects exceed max_objects = {self.max_objects}")
-        if n > MAX_OBJECTS_PER_SEQUENCE:
-            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {n} objects (at most {MAX_OBJECTS_PER_SEQUENCE} in one video)")
-        need_g = -(-len(boxes) // ROWS_PER_GROUP_SLOT)
-        if need_g > self._gs.count(0):
-            raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: {need_g} new group slots but {self._gs.count(0)} of max_groups = "
-                             f"{self.max_groups} are free")
-        if init_mask is not None:
-            init_mask = torch.as_tensor(init_mask)
-            if init_mask.dtype != torch.uint8 or tuple(init_mask.shape) != self.orig_size:
-                raise ValueError(f"UnicornUnifiedMaskTracker.add_objects: init_mask must be uint8 {list(self.orig_size)}, got "
-                                 f"{init_mask.dtype} {list(init_mask.shape)}")
-            if any(m is not None for _, m in self._pending):
-                raise ValueError("UnicornUnifiedMaskTracker.add_objects: the next step already has an init_mask")
-            init_mask = init_mask.to(self.eng.dev).contiguous()
-        ids = list(boxes)
-        for c0 in range(0, len(ids), ROWS_PER_GROUP_SLOT):
-            g = self._gs.index(0)
-            chunk = ids[c0:c0 + ROWS_PER_GROUP_SLOT]
-            self._gs[g] = len(chunk)
-            for row, oid in enumerate(chunk):
-                self._os[self._os.index(None)] = (oid, g, row)
-        self._pending.append((boxes, init_mask))
-
-    def remove_object(self, oid):
-        """Stop tracking `oid` and free its object slot, and its group slot with the group's last object (steps already submitted
-        still report it)."""
-        if oid not in self.objects:
-            raise ValueError(f"UnicornUnifiedMaskTracker.remove_object: unknown object id {oid!r}")
-        k = self._slot_of(oid)
-        g = self._os[k][1]
-        self._os[k] = None
-        self._gs[g] -= 1
-        if oid in self._order:
-            self._order.remove(oid)
-            self.active[k].fill_(0)  # stream-ordered after the steps in flight
-        else:
-            i = next(i for i, (b, _) in enumerate(self._pending) if oid in b)
-            del self._pending[i][0][oid]
-            if not self._pending[i][0]:
-                del self._pending[i]
-        self.state_pre_dict.pop(oid, None)
-
-    def _write_references(self):
-        """The pending groups take the step just enqueued as their reference frame: its stride-16 feature is projected once, and the
-        projection and the boxes' label values go into the groups' slots (UnicornVOSBatch._add_group)."""
-        e = self.eng
-        n16 = self.ref_proj[0].shape[0] // self.max_groups
-        src, q = e.project_ref(self.last["feat"])
-        for boxes, _ in self._pending:
-            ids = list(boxes)
-            lbs = label_values([boxes[o] for o in ids], self.input_size, e.dev)
-            written = set()
-            for i, oid in enumerate(ids):
-                k = self._slot_of(oid)
-                _, g, row = self._os[k]
-                if g not in written:  # row 0 of a group slot may have been removed before the reference frame
-                    written.add(g)
-                    self.ref_proj[0][g * n16:(g + 1) * n16].copy_(src)
-                    self.ref_proj[1][g * n16:(g + 1) * n16].copy_(q)
-                    self.lbs[g].zero_()
-                self.lbs[g, row].copy_(lbs[i])
-                self.obj_row[k].fill_(g * self.R + row)
-                self.active[k].fill_(1)
-            self._order += ids
-        self._pending = []
-
-    # ------------------------------------------------------------------------------------------ device half
-    def _frame(self, s):
-        e = self.eng
-        H, W = self.input_size
-        hh, ww = H // 8, W // 8
-        G, O, R = self.max_groups, self.max_objects, self.R
-        F32 = torch.float32
-        e.begin_frame()
-
-        def correlate(seq):  # the VOS arm, on the stream that overlaps the neck (UnicornVOSBatch._frame with one sequence)
-            feat = seq["feat"]
-            if G > 1:
-                feat = e.buf("unifiedm.featG", (G,) + tuple(feat.shape[1:]))
-                feat.copy_(seq["feat"].expand(G, -1, -1, -1))
-            f_pre, f_cur = e.interaction(None, feat, ref_proj=self.ref_proj)
-            e_pre, e_cur = e.upsample(f_pre, "embp"), e.upsample(f_cur, "embc")
-            coarse = ops.corr_propagate(e_pre.view(G, -1, 128), e_cur.view(G, -1, 128), self.lbs, out=e.buf("unifiedm.coarse", (G, R, hh * ww), F32))
-            c0 = torch.index_select(coarse.view(G * R, hh * ww), 0, self.obj_row, out=e.buf("unifiedm.c0", (O, hh * ww), F32)).view(O, hh, ww)
-            return (c0, ops.bilinear(c0, hh // 2, ww // 2, 2.0, 2.0, out=e.buf("unifiedm.p1", (O, hh // 2, ww // 2), F32)),
-                    ops.bilinear(c0, hh // 4, ww // 4, 4.0, 4.0, out=e.buf("unifiedm.p2", (O, hh // 4, ww // 4), F32)))
-
-        fpn, seq, priors = e.backbone(s.img, tag="unifiedm", side=correlate)
-        mf, um = e.mask_branch(fpn)  # once: every head image reads it
-        head_mots, head_vos = e.head_shared(fpn, priors, mot=self.mots, with_masks=True)
-        n_mot = int(self.mots)
-        dyn = list(e.dyn_levels)
-        hw = [(t.shape[1], t.shape[2]) for t in dyn]
-        _, cnt = ops.postprocess_device(head_vos, 1, self.conf, self.nms, self.vos_ws, max_keep=self.max_inst)
-        cnt.mul_(self.active)
-        s.vos_masks.zero_()  # an object without a detection contributes an all-zero mask (unicorn_vos.py:154-155)
-        up = 8 // self.d_rate
-        ops.dynamic_masks(mf, um, [t[n_mot:] for t in dyn], hw, self.vos_ws, 1, up_rate=up, d_rate=self.d_rate, out=s.vos_masks,
-                          scratch=self._scratch, image_of=self.image_of)
-        self.rows[:, :7].copy_(self.vos_ws.dets.view(O, -1, 7)[:, 0])
-        self.rows[:, 7].copy_(self.vos_ws.count)
-        if self.mots:
-            dets, cnt = ops.postprocess_device(head_mots[0], e.ncls, self.mots_conf, self.mots_nms, s.ws)
-            ops.dynamic_masks(mf, um, [t[:1] for t in dyn], hw, s.ws, self.max_dets, up_rate=8 // self.mots_d_rate, d_rate=self.mots_d_rate,
-                              out=s.mots_masks, scratch=self._scratch)
-            self._qd(e, seq["feat"], dets, cnt)
-        self.last = dict(feat=seq["feat"], mask_feats=mf, up_masks=um, priors=priors, head_mots=head_mots, head_vos=head_vos, dyn=dyn)
-
-    def submit(self, frame):
-        """frame: the letterboxed frame, preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device.  Enqueues the step on the
-        current stream; returns immediately."""
-        s, _ = self._next_step(frame, lambda s: s)
-        s.objs = [(oid, self._slot_of(oid)) for oid in self._order]
-        new = [(list(b), m) for b, m in self._pending if m is not None]
-        s.new_ids, init_mask = (new[0][0], new[0][1]) if new else ([], None)
-        self.frame_id += 1
-        s.frame_id = self.frame_id
-        self._run(s, lambda: self._frame(s))
-        s.host_rows.copy_(self.rows, non_blocking=True)
-        if self.mots:
-            s.host_count.copy_(s.ws.count, non_blocking=True)
-            s.host_dets.copy_(s.ws.dets[:self.max_dets], non_blocking=True)
-            s.host_feats.copy_(self._qd.feats[0], non_blocking=True)
-        # the result assembly at the original size: the object list changes with additions, so it stays outside the graph
-        ids = [oid for oid, _ in s.objs] + s.new_ids
-        H0, W0 = self.orig_size
-        if s.seg is None:
-            s.seg = torch.zeros(H0, W0, dtype=torch.uint8, device=self.eng.dev)
-        if s.soft is None or s.soft.shape[0] < len(ids):
-            s.soft = torch.zeros(max(len(ids), 4), H0, W0, dtype=torch.float32, device=self.eng.dev)
-        if ids:
-            ops.vos_aggregate([s.vos_masks[k] for _, k in s.objs], init_mask, ids, *self.input_size, self.r, s.soft, s.seg)
-        else:
-            s.seg.zero_()
-        s.event.record()
-        if self._pending:
-            self._write_references()
-
-    # ------------------------------------------------------------------------------------------ host half
-    def collect(self):
-        """Results of the oldest submitted step: {"vos": {"segmentation": uint8 [h, w], "soft": fp32 [n, h, w] (device), "objects":
-        {id: (det_row [7] | None, mask fp32 [H, W] at network resolution | None)}, "ids": [...]}, "mots": the write_results_mots()
-        tuple UnicornMOTSTracker.collect returns, or None without the MOTS arm}.  The device tensors stay valid until the step after
-        the next one is submitted."""
-        s = self._ring.collect()
-        s.event.synchronize()
-        objects, self.last_rows = {}, {}
-        for oid, k in s.objs:
-            row = s.host_rows[k].clone()
-            self.last_rows[oid] = row
-            objects[oid] = (row[:7], s.vos_masks[k, 0]) if row[7] > 0 else (None, None)
-        ids = [oid for oid, _ in s.objs] + s.new_ids
-        vos = dict(segmentation=s.seg, soft=s.soft[:len(ids)], objects=objects, ids=ids)
-        mots = None
-        self.last_dets = self.last_feats = None
-        if self.mots:
-            h0, w0 = self.orig_size
-            n = min(int(s.host_count[0]), self.max_dets)
-            d, f = s.host_dets[:n].clone(), s.host_feats[:n].clone()
-            self.last_dets, self.last_feats = d, f
-            _, oid, rows, emit = _mots_match(self.tracker, d, f, self.r, self.score_thr, s.frame_id, self.min_box_area)
-            stream = assoc_stream(self.eng.dev)
-            with torch.cuda.stream(stream):  # not behind the next step's kernels on the main stream
-                stream.wait_event(s.event)
-                rles = self._enc(s.mots_masks, rows.tolist(), emit, self.mask_thres, self.r, h0, w0)
-            mots = _mots_result(s.frame_id, oid, emit, rles, h0, w0)
-        return {"vos": vos, "mots": mots}
-
-    def step_tensor(self, frame):
-        """Sequential protocol: one step in, its results out."""
-        self.submit(frame)
-        return self.collect()
-
-    # ------------------------------------------------------------------------------------------ reference protocol
-    def track(self, image_rgb, info=None):
-        """image_rgb: a raw frame of the original size, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame), letterboxed
-        once for both arms.  info: UnicornVOSTrack's dict
-        (init_object_ids, init_bbox {id: [x, y, w, h]}, optionally init_mask) for objects that start on this frame.  Returns
-        {"segmentation": uint8 [h, w] numpy, "mots": write_results_mots() tuple or None}; state_pre_dict is kept as
-        UnicornVOSTrack.track keeps it."""
-        size = nv12_size(image_rgb) or tuple(image_rgb.shape[:2])
-        if size != self.orig_size:
-            raise ValueError(f"UnicornUnifiedMaskTracker.track: frame size {size}, the video's is {self.orig_size}")
-        info = info or {}
-        if "init_object_ids" in info:
-            boxes = {oid: xyxy_resized(info["init_bbox"][oid], self.r) for oid in info["init_object_ids"]}
-            mask = info.get("init_mask")
-            self.add_objects(boxes, None if mask is None else torch.as_tensor(mask).to(torch.uint8))
-            for oid in info["init_object_ids"]:
-                self.state_pre_dict[oid] = info["init_bbox"][oid]
-        frame, r, _ = letterbox_frame(image_rgb, self.input_size, self.eng.dev, out=self._host_in)
-        out = self.step_tensor(frame)
-        for oid, (det, _) in out["vos"]["objects"].items():  # unicorn_vos.py:137-149 (state of the best instance, xywh ints)
-            if det is not None:
-                self.state_pre_dict[oid] = state_xywh(det, r, self.input_size)
-        return {"segmentation": out["vos"]["segmentation"].cpu().numpy(), "mots": out["mots"]}
-
-
 # ---------------------------------------------------------------------------------------------------------- VOS objects + MOTS, several videos
 MAX_VIDEOS = 64  # UC_VOS_MAX_VIDEOS: uc_vos_aggregate_batched assembles at most this many videos in one launch
 
@@ -813,17 +494,20 @@ class _MaskBatchStep(FrameSlot):
 
 class UnicornUnifiedMaskBatch(_Unified):
     """`n_seq` videos in one step, each with up to 16 VOS objects plus optionally the MOTS arm (mots=True), one backbone, neck and
-    mask-branch pass per video frame.  For the *_mask checkpoints.  VOS and MOTS settings and their defaults are
-    UnicornUnifiedMaskTracker's.
+    mask-branch pass per video frame.  For the *_mask checkpoints.  VOS settings (conf, nms, max_inst, d_rate) default to
+    UnicornVOSTrack's, MOTS settings (mots_conf, mots_nms, score_thr, max_dets, mask_thres, mots_d_rate, min_box_area) to
+    UnicornMOTSTracker's.
 
     start(i, orig_size, tracker=None) opens video slot i with its original (h, w), which fixes its letterbox ratio r[i] = min(H / h,
     W / w): its MOTS first-frame flag is reset in stream order, `tracker` installed (default a fresh QuasiDenseEmbedTracker) and the
     objects of the slot's previous video removed.
 
     The `max_objects` object slots and `max_groups` group slots are one pool shared by all videos.  add_objects(i, {id: box_xyxy},
-    init_mask=None), remove_object(i, id) and objects(i) follow UnicornUnifiedMaskTracker's rules within each video (ids 1..255 and
-    unique within the video, at most 16 objects per video, 8 objects per group slot, at most one init_mask per video per step, shaped
-    like the video's orig_size); the objects take video i's next active frame as their reference.  The device tables group_seq,
+    init_mask=None), remove_object(i, id) and objects(i) manage the objects of each video (ids 1..255 and unique within the video, at
+    most 16 objects per video, 8 objects per group slot, at most one init_mask per video per step, shaped like the video's
+    orig_size); the objects of one add_objects call form one group and take video i's next active frame as their reference.  With
+    init_mask (uint8 [h, w] label map) they enter that step's label map from it (UnicornVOSTrack.track_tensor with new objects);
+    without, they appear from the following step on (UnicornVOSTrack.initialize_tensor).  The device tables group_seq,
     obj_seq, obj_row and image_of say which video, label row and mask-branch image every slot reads; they are written in place, in
     stream order, and never re-capture a graph.  Every entry is checked on the host before it is written.
 
@@ -834,10 +518,12 @@ class UnicornUnifiedMaskBatch(_Unified):
     arms, and the MOTS arm's QDEmbedding at B = n_seq gated by the step's active videos.  One uc_vos_aggregate_batched launch then
     assembles every active video with objects at its own original size; an active video without objects gets a zeroed label map.
 
-    submit(frames, active) / collect() follow UnicornUnifiedMaskTracker: two parity slots, so submit(t + 1) may precede collect(t); the
-    first step runs eagerly and the next is captured; a step with no active video launches nothing.  A video idle in a step keeps its
+    submit(frames, active) / collect(): two parity slots, so submit(t + 1) may precede collect(t); the first step runs eagerly and the
+    next is captured; a step with no active video launches nothing.  A free object slot computes on stale buffers, skipped by the
+    dynamic masks, and its detection count is zeroed; steps already submitted report the objects they were submitted with.  A video idle in a step keeps its
     MOTS state (pre_dict, first-frame flag, tracker, frame counter), its objects report nothing and its pending references wait for
-    its next active frame.  Each video's results equal those of its own UnicornUnifiedMaskTracker, bit for bit."""
+    its next active frame.  Each video's results equal those of the same driver at n_seq = 1, and each object's rows, mask, the label
+    map and soft masks those of one UnicornVOSTrack, the MOTS results those of UnicornMOTSTracker, bit for bit."""
 
     def __init__(self, engine: UnicornEngine, input_size, n_seq, max_objects, max_groups=None, mots=True,
                  conf=0.001, nms=0.65, max_inst=1, d_rate=2,
@@ -1021,7 +707,7 @@ class UnicornUnifiedMaskBatch(_Unified):
     def _write_references(self, videos):
         """The pending groups of `videos` take their video's frame of the step just enqueued as their reference frame: the frame's
         stride-16 feature is projected once per video, and the projection, the boxes' label values and the slot tables are written
-        into the groups' slots (UnicornUnifiedMaskTracker._write_references per video)."""
+        into the groups' slots (UnicornVOSBatch._add_group per video)."""
         e, n, G = self.eng, self.n_seq, self.max_groups
         n16 = self.ref_proj[0].shape[0] // G
         for i in videos:
@@ -1080,7 +766,7 @@ class UnicornUnifiedMaskBatch(_Unified):
         self.rows[:, :7].copy_(self.vos_ws.dets.view(O, -1, 7)[:, 0])
         self.rows[:, 7].copy_(self.vos_ws.count)
         if self.mots:
-            one = n == 1  # one video: the one-image launches of UnicornUnifiedMaskTracker; no gate (an idle step does not run)
+            one = n == 1  # one video: the one-image launches; no gate (an idle step does not run)
             dets, cnt = ops.postprocess_device(head_mots[0] if one else head_mots, e.ncls, self.mots_conf, self.mots_nms, s.ws)
             ops.dynamic_masks(mf, um, [t[:n] for t in dyn], hw, s.ws, self.max_dets, up_rate=8 // self.mots_d_rate, d_rate=self.mots_d_rate,
                               out=s.mots_masks[0] if one else s.mots_masks, scratch=self._scratch, image_of=None if one else self._mots_image_of)
@@ -1151,9 +837,10 @@ class UnicornUnifiedMaskBatch(_Unified):
 
     # ------------------------------------------------------------------------------------------ host half
     def collect(self):
-        """Results of the oldest submitted step: one entry per video, None for a video idle in that step, otherwise {"vos": ...,
-        "mots": ...} as UnicornUnifiedMaskTracker.collect gives them for that video.  The device tensors stay valid until the step
-        after the next one is submitted.  last_rows[i] / last_dets[i] / last_feats[i] then hold video i's object rows, and the NMS
+        """Results of the oldest submitted step: one entry per video, None for a video idle in that step, otherwise {"vos":
+        {"segmentation": uint8 [h, w], "soft": fp32 [n, h, w] (device), "objects": {id: (det_row [7] | None, mask fp32 [H, W] at
+        network resolution | None)}, "ids": [...]}, "mots": the write_results_mots() tuple, or None without the MOTS arm}.  The device
+        tensors stay valid until the step after the next one is submitted.  last_rows[i] / last_dets[i] / last_feats[i] then hold video i's object rows, and the NMS
         rows and embeddings its tracker was given in this step."""
         s = self._ring.collect()
         s.event.synchronize()
@@ -1198,8 +885,8 @@ class UnicornUnifiedMaskBatch(_Unified):
     # ------------------------------------------------------------------------------------------ reference protocol
     def track(self, images, infos=None):
         """images: n_seq raw frames of their videos' original sizes, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame;
-        the two may be mixed), None for an idle video; each is letterboxed once for both arms.  infos: n_seq dicts as UnicornUnifiedMaskTracker.track takes (init_object_ids, init_bbox {id: [x, y, w, h]},
-        optionally init_mask) or None.  Returns one entry per video, None for an idle one, otherwise {"segmentation": uint8 [h, w]
+        the two may be mixed), None for an idle video; each is letterboxed once for both arms.  infos: n_seq dicts as UnicornVOSTrack.track takes them (init_object_ids, init_bbox {id: [x, y, w, h]},
+        optionally init_mask) for objects that start on this frame, or None.  Returns one entry per video, None for an idle one, otherwise {"segmentation": uint8 [h, w]
         numpy, "mots": write_results_mots() tuple or None}; state_pre_dicts[i] is kept as UnicornVOSTrack.track keeps it."""
         n = self.n_seq
         infos = list(infos) if infos is not None else [None] * n
@@ -1239,3 +926,68 @@ class UnicornUnifiedMaskBatch(_Unified):
                     self.state_pre_dicts[i][oid] = state_xywh(det, self.r[i], self.input_size)
             res[i] = {"segmentation": o["vos"]["segmentation"].cpu().numpy(), "mots": o["mots"]}
         return res
+
+
+class UnicornUnifiedMaskTracker:
+    """Up to `max_objects` VOS objects plus optionally the MOTS arm (mots=True) on one video of original size `orig_size` (h, w), one
+    backbone, neck and mask-branch pass per frame: UnicornUnifiedMaskBatch at n_seq = 1 (same settings) with its video started on
+    `tracker` (the MOTS arm's QuasiDenseEmbedTracker, default a fresh one), under the one-video protocol.  Both arms use the
+    letterbox ratio r = min(H / h, W / w).  frame_id counts the steps submitted."""
+
+    def __init__(self, engine: UnicornEngine, input_size, orig_size, max_objects, max_groups=None, mots=True, tracker=None,
+                 conf=0.001, nms=0.65, max_inst=1, d_rate=2,
+                 mots_conf=0.01, mots_nms=0.7, score_thr=0.1, max_dets=64,
+                 mask_thres=0.3, mots_d_rate=2, min_box_area=100, use_graph=True):
+        self._b = UnicornUnifiedMaskBatch(engine, input_size, 1, max_objects, max_groups, mots, conf, nms, max_inst, d_rate, mots_conf,
+                                          mots_nms, score_thr, max_dets, mask_thres, mots_d_rate, min_box_area, use_graph)
+        self._b.start(0, orig_size, tracker)
+
+    objects = property(lambda self: self._b.objects(0))
+    frame_id = property(lambda self: self._b.frame_ids[0])
+    graphs = property(lambda self: self._b.graphs)
+    launches_per_frame = property(lambda self: self._b.launches_per_frame)
+    last = property(lambda self: self._b.last)
+    last_rows = property(lambda self: self._b.last_rows[0])
+    last_dets = property(lambda self: self._b.last_dets[0])
+    last_feats = property(lambda self: self._b.last_feats[0])
+    state_pre_dict = property(lambda self: self._b.state_pre_dicts[0])
+    r = property(lambda self: self._b.r[0])
+    ref_proj = property(lambda self: self._b.ref_proj)
+    lbs = property(lambda self: self._b.lbs)
+    obj_row = property(lambda self: self._b.obj_row)
+    active = property(lambda self: self._b.active)
+    vos_ws = property(lambda self: self._b.vos_ws)
+    R = property(lambda self: self._b.R)
+    _ring = property(lambda self: self._b._ring)
+
+    def add_objects(self, boxes_xyxy, init_mask=None):
+        """Track the objects {id: [x1, y1, x2, y2]} (resized-image coordinates; ids 1..255) from the next submitted frame on.
+        init_mask: uint8 [h, w] label map of that frame in which they appear (at most one per step)."""
+        self._b.add_objects(0, boxes_xyxy, init_mask)
+
+    def remove_object(self, oid):
+        """Stop tracking `oid` and free its object slot, and its group slot with the group's last object (steps already submitted
+        still report it)."""
+        self._b.remove_object(0, oid)
+
+    def submit(self, frame):
+        """frame: the letterboxed frame, preprocessed fp32 [1,3,H,W] or uint8 [1,H,W,3], host or device.  Enqueues the step on the
+        current stream; returns immediately."""
+        self._b.submit(frame)
+
+    def collect(self):
+        """Results of the oldest submitted step: {"vos": ..., "mots": ...} as UnicornUnifiedMaskBatch.collect gives them for one
+        video."""
+        return self._b.collect()[0]
+
+    def step_tensor(self, frame):
+        """Sequential protocol: one step in, its results out."""
+        self.submit(frame)
+        return self.collect()
+
+    def track(self, image_rgb, info=None):
+        """image_rgb: a raw frame of the original size, RGB uint8 [h, w, 3] or NV12 uint8 [3h/2, w] (sot.letterbox_frame), letterboxed
+        once for both arms.  info: UnicornVOSTrack's dict (init_object_ids, init_bbox {id: [x, y, w, h]}, optionally init_mask) for
+        objects that start on this frame.  Returns {"segmentation": uint8 [h, w] numpy, "mots": write_results_mots() tuple or None};
+        state_pre_dict is kept as UnicornVOSTrack.track keeps it."""
+        return self._b.track([image_rgb], [info])[0]
