@@ -417,6 +417,29 @@ UC_API int uc_inst_encode_batched(const float* maps, long bs_maps, int n_max, in
                                   int row0, const int* H, const int* W, const double* r, float thr, void* workspace, long workspace_bytes,
                                   uint8_t* emit, char* chars, long capacity, long long* offsets, void* stream);
 
+/* BDD100K MOTS bitmasks on the device (qdtrack core/to_bdd100k/utils.py:15-38, mask_prepare + mask_merge; the seg_track result of
+ * tools/to_bdd100k.py): for B frames (1 <= B <= UC_MOTS_MAX_IMAGES), frame b with k[b] tracked instances (0 <= k[b] <= 65535) and size
+ * H[b] x W[b] (H * W < 2^31), the uint8 row-major [H, W, 4] RGBA array mask_merge saves as PNG, at out + out_offsets[b] (byte offsets
+ * into the out_bytes bytes of out, 4-byte aligned, frames not overlapping).  k, H, W, out_offsets: HOST arrays of B.
+ * DEVICE inputs, one flat list of K = sum k[b] instances grouped by frame: string j = chars[offsets[j] .. offsets[j+1]) (offsets int64
+ * [K+1] into the n_chars chars) is instance j's COCO compressed RLE counts over its frame (column-major, pycocotools' string form);
+ * colors[j] its packed colour, byte 0 = R at the lowest address (label + 1, 0, id >> 8, id & 255 as uint8); ranks[j] its position in
+ * the paint order of its frame (np.argsort of the scores: 0 is painted first), a permutation of 0 .. k[b]-1.  A pixel takes the
+ * colour of the covering instance of highest rank (all four channels, zeros included); a pixel no instance covers is 0.  The ranks are
+ * used as given: the call does not sort.  A frame without instances is all zeros.
+ * status: device int32 [B], written by the call: frame b's UC_BDD_* flags, 0 when every string of the frame is well formed.  A
+ * malformed string paints nothing and never writes outside its frame.  workspace: device, 16-byte aligned,
+ * uc_bdd_bitmask_workspace_bytes(B, k, H, W, n_chars) bytes (-1 for bad arguments).  Every argument is validated before any CUDA
+ * call; no allocation, no synchronisation, graph-capturable: two memsets and three launches for K > 0, one memset and one launch
+ * for K = 0. */
+#define UC_BDD_BAD_CHARS 1 /* a char outside '0' .. 'o', a count of more than 7 chars, or a string that ends inside a count */
+#define UC_BDD_BAD_RUNS 2  /* a negative count, or counts whose sum is not H * W */
+#define UC_BDD_BAD_INDEX 4 /* offsets[j] > offsets[j+1], an offset outside [0, n_chars], or a rank outside [0, k[b]) */
+UC_API long uc_bdd_bitmask_workspace_bytes(int B, const int* k, const int* H, const int* W, long n_chars);
+UC_API int uc_bdd_bitmask_batched(int B, const int* k, const int* H, const int* W, const long* out_offsets, const char* chars, long n_chars,
+                                  const long long* offsets, const uint32_t* colors, const int* ranks, void* workspace, long workspace_bytes,
+                                  uint8_t* out, long out_bytes, int* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,14 +14,19 @@
 
 Frames come letterboxed (top-left, pad 114) as for UnicornMOTSBatch.  BDD100K frames are 720x1280, so at 800x1280 r = 1 and the
 mmdet test pipeline plus test_omni.preprocess reduce to that letterbox.  At other ratios they are not equivalent: the reference
-resizes float pixels with cv2 and truncates to uint8."""
+resizes float pixels with cv2 and truncates to uint8.
+
+BDDBitmasks and write_seg_track take the MOTS track_result dicts on to qdtrack's seg_track format (tools/to_bdd100k.py --task
+seg_track: core/to_bdd100k/transforms.py seg_track_to_bdd100k and utils.py mask_prepare / mask_merge), one RGBA "bitmask" PNG per
+frame, with the masks decoded and painted on the device (uc_bdd_bitmask_batched)."""
+import os
 import warnings
 from collections import defaultdict
 
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, post_ops
 from .det import RowMasks
 from .frames import anchor_count
 from .mot import UnicornMOTBatch
@@ -191,3 +196,142 @@ class UnicornBDDMOTSBatch(UnicornBDDMOTBatch):
                 self.last_rles[i] = rles[i]
                 res[i] = bdd_mots_result(c.trackers[i], *rows[i], c.scales[i], c.frame_ids[i] - 1, rles[i], *c.img_hw[i], self.num_classes)
         return res
+
+
+BDD_MAX_FRAMES = 64  # UC_MOTS_MAX_IMAGES: frames per uc_bdd_bitmask_batched call
+_BAD = ((post_ops.BDD_BAD_CHARS, "bad chars"), (post_ops.BDD_BAD_RUNS, "runs that do not cover the frame"),
+        (post_ops.BDD_BAD_INDEX, "bad offsets or paint order"))
+
+
+def _channel(v):
+    """What mask_merge stores in a channel where the mask is 1: bitmask * (1 - m) + m * v with m uint8, cast back to uint8 (a float
+    value is truncated, an integer one wraps).  v: one value per instance."""
+    return (np.ones(len(v), np.uint8) * v).astype(np.uint8)
+
+
+def _frame(track_dict, h, w, f):
+    """mask_prepare (utils.py:15-22) of one frame without the decode: its strings, packed colours (uint32, R in the low byte) and
+    paint ranks."""
+    strings, labels, scores = [], [], []
+    for id_, inst in track_dict.items():
+        segm = inst["segm"]
+        if [int(v) for v in segm["size"]] != [h, w]:
+            raise ValueError(f"BDDBitmasks: frame {f}, track {id_}: segm size {list(segm['size'])} is not the frame's [{h}, {w}]")
+        c = segm["counts"]
+        strings.append(c.encode("ascii") if isinstance(c, str) else bytes(c))
+        labels.append(inst["label"])
+        scores.append(inst["bbox"][-1])
+    r = np.array(labels) + 1  # segtrack2result's labels are float32: so is label + 1
+    if not (np.isfinite(r) & (r >= 0) & (r < 256)).all():
+        raise ValueError(f"BDDBitmasks: frame {f}: label + 1 = {r[~(np.isfinite(r) & (r >= 0) & (r < 256))][0]} does not fit a uint8 channel")
+    ids = np.array(list(track_dict), dtype=np.int64)  # segtrack2result's keys are int64
+    rgba = np.stack([_channel(r), np.zeros(len(ids), np.uint8), _channel(ids >> 8), _channel(ids & 255)], 1)
+    ranks = np.empty(len(strings), dtype=np.int32)
+    ranks[np.argsort(scores)] = np.arange(len(strings), dtype=np.int32)  # the reference's own sort: ties as numpy orders them
+    return strings, np.ascontiguousarray(rgba).view("<u4").reshape(-1), ranks
+
+
+class BDDBitmasks:
+    """qdtrack's seg_track bitmasks of up to BDD_MAX_FRAMES frames per call on `device`: paint(track_results, sizes) packs every
+    frame's strings, colours and paint order (np.argsort of the scores, as mask_merge) on the host, uploads them in one copy and runs
+    one uc_bdd_bitmask_batched.  The pinned and device buffers grow on demand.  A bitmask has its frame's original size; the reference
+    hard-codes 720 x 1280, the BDD100K size."""
+
+    def __init__(self, device="cuda", capacity=1 << 16):
+        self.dev, self.capacity = torch.device(device), capacity
+        self._h_in = self._d_in = self._out = self._h_out = self._ws = None  # allocated by the first paint()
+        self._status = self._h_status = None
+
+    def _grow(self, t, n, pinned=False):
+        """t, or a larger buffer (pinned host or on the device) when t holds fewer than n bytes."""
+        if t is not None and t.numel() >= n:
+            return t
+        n = max(n, 2 * t.numel() if t is not None else self.capacity)
+        return torch.empty(n, dtype=torch.uint8).pin_memory() if pinned else torch.empty(n, dtype=torch.uint8, device=self.dev)
+
+    def paint(self, track_results, sizes, host=False):
+        """track_results: 1..64 track_result dicts ({id: {"bbox", "label", "segm"}}, as UnicornBDDMOTSBatch.collect() returns them or
+        as loaded from a results pickle), sizes: each frame's original (h, w); every segm["size"] must equal it.  Returns the uint8
+        [h, w, 4] bitmasks, device views valid until the next call (host=True: numpy views of pinned memory).  A malformed RLE string
+        raises ValueError."""
+        B = len(track_results)
+        if not 1 <= B <= BDD_MAX_FRAMES or len(sizes) != B:
+            raise ValueError(f"BDDBitmasks.paint: 1..{BDD_MAX_FRAMES} frames with one (h, w) each, got {B} frames, {len(sizes)} sizes")
+        hs, ws = [int(s[0]) for s in sizes], [int(s[1]) for s in sizes]
+        if any(h < 1 or w < 1 for h, w in zip(hs, ws)):
+            raise ValueError(f"BDDBitmasks.paint: bad frame sizes {list(sizes)}")
+        strings, colors, ranks, k = [], [], [], []
+        for f, (d, h, w) in enumerate(zip(track_results, hs, ws)):
+            s, c, r = _frame(d, h, w, f)
+            strings += s
+            colors.append(c)
+            ranks.append(r)
+            k.append(len(s))
+        K = len(strings)
+        chars = b"".join(strings)
+        offsets = np.zeros(K + 1, dtype=np.int64)
+        np.cumsum([len(s) for s in strings], out=offsets[1:])
+        # one upload: offsets | colours | ranks | chars, each 16-byte aligned
+        o_col = (8 * (K + 1) + 15) & ~15
+        o_rank = o_col + ((4 * K + 15) & ~15)
+        o_chars = o_rank + ((4 * K + 15) & ~15)
+        total = o_chars + max(len(chars), 1)
+        self._h_in = self._grow(self._h_in, total, pinned=True)
+        self._d_in = self._grow(self._d_in, total)
+        h = self._h_in.numpy()
+        h[:8 * (K + 1)] = offsets.view(np.uint8)
+        h[o_col:o_col + 4 * K] = np.concatenate(colors).view(np.uint8)
+        h[o_rank:o_rank + 4 * K] = np.concatenate(ranks + [np.zeros(0, np.int32)]).view(np.uint8)
+        h[o_chars:o_chars + len(chars)] = np.frombuffer(chars, dtype=np.uint8)
+        with torch.cuda.device(self.dev):
+            out = self._launch(total, K, o_col, o_rank, o_chars, len(chars), k, hs, ws, host)
+        bad = [(f, int(v)) for f, v in enumerate(self._h_status[:B].tolist()) if v]
+        if bad:
+            raise ValueError("BDDBitmasks.paint: malformed segm RLE: " + "; ".join(
+                f"frame {f}: " + ", ".join(what for bit, what in _BAD if v & bit) for f, v in bad))
+        return out
+
+    def _launch(self, total, K, o_col, o_rank, o_chars, n_chars, k, hs, ws, host):
+        """Uploads the packed inputs, paints, reads back the status (and with host=True the bitmasks) and waits."""
+        B = len(k)
+        if self._status is None:
+            self._status = torch.zeros(BDD_MAX_FRAMES, dtype=torch.int32, device=self.dev)
+            self._h_status = torch.zeros(BDD_MAX_FRAMES, dtype=torch.int32).pin_memory()
+        d = self._d_in
+        d[:total].copy_(self._h_in[:total], non_blocking=True)
+        out_off = np.zeros(B + 1, dtype=np.int64)
+        np.cumsum([4 * h * w for h, w in zip(hs, ws)], out=out_off[1:])
+        self._out = self._grow(self._out, int(out_off[B]))
+        self._ws = self._grow(self._ws, post_ops.bdd_bitmask_workspace_bytes(k, hs, ws, n_chars))
+        n = 4 * max(K, 1)  # not empty: an empty view has no data pointer (nothing is read for K = 0)
+        post_ops.bdd_bitmask(d[o_chars:], n_chars, d[:8 * (K + 1)].view(torch.int64), d[o_col:o_col + n].view(torch.int32),
+                             d[o_rank:o_rank + n].view(torch.int32), k, hs, ws, self._out, out_off[:B].tolist(), self._ws, self._status)
+        out = self._out
+        self._h_status[:B].copy_(self._status[:B], non_blocking=True)
+        if host:
+            self._h_out = self._grow(self._h_out, int(out_off[B]), pinned=True)
+            self._h_out[:int(out_off[B])].copy_(self._out[:int(out_off[B])], non_blocking=True)
+            out = self._h_out
+        torch.cuda.current_stream().synchronize()
+        views = [out[int(out_off[f]):int(out_off[f + 1])].view(hs[f], ws[f], 4) for f in range(B)]
+        return [v.numpy() for v in views] if host else views
+
+
+def write_seg_track(track_results, img_names, out_base, sizes, painter=None, batch=BDD_MAX_FRAMES):
+    """qdtrack's seg_track_to_bdd100k (core/to_bdd100k/transforms.py): frame i's bitmask as an RGBA PNG at
+    out_base/seg_track/<img_names[i] with .jpg replaced by .png>, written with PIL as mask_merge does.  track_results, img_names and
+    sizes ((h, w) per frame) run in parallel; the bitmasks are painted `batch` frames per call.  Returns the paths written."""
+    from PIL import Image
+    if not len(track_results) == len(img_names) == len(sizes):
+        raise ValueError("write_seg_track: track_results, img_names and sizes must have one entry per frame")
+    painter = painter or BDDBitmasks()
+    base = os.path.join(out_base, "seg_track")
+    os.makedirs(base, exist_ok=True)
+    paths = []
+    for i in range(0, len(track_results), batch):
+        for name, bm in zip(img_names[i:i + batch], painter.paint(track_results[i:i + batch], sizes[i:i + batch], host=True)):
+            path = os.path.join(base, name.replace(".jpg", ".png"))
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            Image.fromarray(bm).save(path)
+            paths.append(path)
+    return paths

@@ -1,7 +1,7 @@
 """Wrappers of the detector's post-processing entry points (include/unicorn_b200.h: uc_postprocess_batched_ex,
 uc_det_candidates_batched, uc_postprocess_nms_batched, and for the instance segmenter uc_dynamic_masks_batched over a window of NMS
-rows and uc_inst_encode_batched), next to the ones of unicorn_b200.ops that the tracking frames use.  Their
-results are pinned bit for bit to head_decode + postprocess_device (tests/test_det_gpu.py)."""
+rows and uc_inst_encode_batched; for the BDD100K MOTS bitmasks uc_bdd_bitmask_batched), next to the ones of unicorn_b200.ops that the
+tracking frames use.  The detector's results are pinned bit for bit to head_decode + postprocess_device (tests/test_det_gpu.py)."""
 import ctypes
 
 import torch
@@ -87,3 +87,38 @@ def inst_encode(maps, count, row0, d_rate, thr, r, H, W, ws, emit, chars, offset
                                            (ctypes.c_double * B)(*[float(x) for x in r]), _f(thr), _p(ws), _l(ws.numel()), _p(emit),
                                            _p(chars), _l(chars.numel()), _p(offsets), _S()), "uc_inst_encode_batched", 3)
     return offsets
+
+
+BDD_BAD_CHARS, BDD_BAD_RUNS, BDD_BAD_INDEX = 1, 2, 4  # UC_BDD_* status flags
+
+
+def _ints(v, ctype=ctypes.c_int):
+    return (ctype * len(v))(*[int(x) for x in v])
+
+
+def bdd_bitmask_workspace_bytes(k, H, W, n_chars):
+    """uc_bdd_bitmask_workspace_bytes: the workspace of a uc_bdd_bitmask_batched call on frames with k[b] instances of H[b] x W[b]
+    and n_chars chars in all."""
+    n = _L().uc_bdd_bitmask_workspace_bytes
+    n.restype = ctypes.c_long
+    nbytes = n(len(k), _ints(k), _ints(H), _ints(W), _l(n_chars))
+    if nbytes < 0:
+        raise ValueError(f"bdd_bitmask_workspace_bytes: bad arguments k={list(k)}, H={list(H)}, W={list(W)}, n_chars={n_chars}")
+    return nbytes
+
+
+def bdd_bitmask(chars, n_chars, offsets, colors, ranks, k, H, W, out, out_offsets, ws, status):
+    """The RGBA bitmasks of B frames (uc_bdd_bitmask_batched): chars uint8 (the first n_chars used), offsets int64 [K+1], colors int32
+    [K] (packed R | G << 8 | B << 16 | A << 24) and ranks int32 [K] on the device, K = sum(k); k, H, W: B host ints.  Frame b is
+    written as uint8 [H[b], W[b], 4] at byte out_offsets[b] (host) of the device buffer out.  status: device int32 [>= B], frame b's
+    UC_BDD_* flags (0 = every string well formed).  ws: device uint8, bdd_bitmask_workspace_bytes(k, H, W, n_chars) bytes.  Launches
+    only."""
+    B = len(k)
+    assert len(H) == len(W) == len(out_offsets) == B and sum(k) + 1 <= offsets.numel()
+    assert chars.dtype == torch.uint8 and n_chars <= chars.numel() and offsets.dtype == torch.int64
+    assert colors.dtype == ranks.dtype == status.dtype == torch.int32 and colors.numel() >= sum(k) and ranks.numel() >= sum(k)
+    assert out.dtype == ws.dtype == torch.uint8 and status.numel() >= B
+    _lib.check(_L().uc_bdd_bitmask_batched(B, _ints(k), _ints(H), _ints(W), _ints(out_offsets, ctypes.c_long), _p(chars), _l(n_chars),
+                                           _p(offsets), _p(colors), _p(ranks), _p(ws), _l(ws.numel()), _p(out), _l(out.numel()), _p(status),
+                                           _S()), "uc_bdd_bitmask_batched", 3 if sum(k) else 1)
+    return status
